@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- steps/sec of the blub fluid step on B200 + PCG roofline + CPU baseline (contract: see DESIGN.md section 6).
+"""bench.py -- steps/sec of the blub fluid step on H100 + PCG roofline + CPU baseline (contract: see DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl blub|reference] [--workload dam_256] [--multi sharded|replicas]
+                    [--dump-outputs DIR]
 
 A "step" is one HybridFluid::step (P2G, PCG solve, G2P/advection, density rhs, PCG solve, particle correction) over the
 synthetic 256^3 / 16,387,064-particle dam break that BASELINE.json's metric is quoted on.  N > 1 (torchrun, one rank per
@@ -10,6 +11,9 @@ with the same 16.3 M particles per slab); `value` = slab-steps/s = N * steps/s. 
 same per-slab scene on one GPU.  `--multi stacked` stacks N dam_256 cubes instead, `--multi replicas` runs N independent scenes.
 `--impl reference`: the reference (Rust + wgpu/Vulkan) cannot run on this image, so this arm times the CPU restatement of
 its algorithm (oracle/) on the host cores -- the only place besides cpu_baseline where bench.py executes oracle/.
+`--dump-outputs DIR`: after the K timed steps, the state the timed path left (the ten arrays of blub_fluid_view) is written to
+DIR/<name>.npy (float32; fixed, seeded samples of arrays larger than a cap, <= 64 MB in all, N > 1: DIR/<name>_rank<k>.npy sharing
+that budget), so that two builds can be compared.
 """
 import argparse
 import json
@@ -115,6 +119,47 @@ class ClockSampler:
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons, "samples": len(sm)}
 
 
+DUMP_PARTICLES = 1 << 18  # particles sampled per particle array (4 floats each)
+DUMP_CELLS = 1 << 20      # cells sampled per grid volume
+
+
+def _sample(n, cap, seed):
+    """All indices when n <= cap, else `cap` distinct indices drawn with a fixed seed, ascending."""
+    import numpy as np
+
+    if n <= cap:
+        return np.arange(n, dtype=np.int64)
+    return np.sort(np.random.default_rng(seed).choice(n, size=cap, replace=False))
+
+
+def dump_outputs(fluid, out_dir, suffix="", parts=1):
+    """The ten arrays a renderer binds after a step (blub_fluid_view), as float32 .npy files.  Particle arrays are (n, 4) in
+    the library's particle order; grid volumes are flattened in x-fastest order.  Arrays above the caps are sampled at indices
+    drawn with a fixed seed, stored beside them in float64 (particle_index, cell_index).  At most ~50 MB in all: with `parts`
+    ranks dumping into the same directory each one gets 1/parts of the caps."""
+    import numpy as np
+
+    from blub_b200 import fluid as F
+
+    os.makedirs(out_dir, exist_ok=True)
+    fluid.synchronize()
+    n = fluid.num_particles
+    pi = _sample(n, DUMP_PARTICLES // parts, 1)
+    files = {"particle_index": pi.astype(np.float64)}
+    for name, tap in (("particles_position", F.TAP_POS), ("particles_velocity_x", F.TAP_VX), ("particles_velocity_y", F.TAP_VY),
+                      ("particles_velocity_z", F.TAP_VZ)):
+        files[name] = fluid.download_particles(tap)[pi]
+    ci = _sample(fluid.n, DUMP_CELLS // parts, 2)
+    files["cell_index"] = ci.astype(np.float64)
+    for name, tap in (("grid_velocity_x", F.TAP_UX), ("grid_velocity_y", F.TAP_UY), ("grid_velocity_z", F.TAP_UZ), ("marker", F.TAP_MARKER),
+                      ("pressure_from_velocity", F.TAP_P_VEL), ("pressure_from_density", F.TAP_P_DEN)):
+        files[name] = fluid.download_grid(tap).reshape(-1)[ci].astype(np.float32)
+    for name, a in files.items():
+        np.save(os.path.join(out_dir, name + suffix + ".npy"), np.ascontiguousarray(a))
+    return {"dir": out_dir, "particles": n, "particles_dumped": int(pi.size), "cells_dumped": int(ci.size),
+            "bytes": int(sum(a.nbytes for a in files.values()))}
+
+
 def pcg_roofline(device, n=256, reps=5):
     """SURVEY 8(d) microbench: n^3 grid, all interior cells FLUID, rhs ~ U[-1,1) (seed 1234) mean-removed, tolerance 0 so
     all 33 iterations run; algorithmic bytes = (42 * 33 + 21) * N per solve."""
@@ -140,18 +185,14 @@ def pcg_roofline(device, n=256, reps=5):
     cells = n ** 3
     bytes_alg = (42 * 33 + 21) * cells
     peaks = {}
-    src = "fallback 6650 GB/s (B200_PROFILING.md)"
-    peak = 6650.0
+    src = "H100 SXM data sheet, 3350 GB/s"
+    peak = 3350.0
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peaks = json.load(open(pk))
         peak = float(peaks.get("hbm_gbs", peak))
         src = "MEASURED_PEAKS.json hbm_gbs (burst copy)"
-    traffic = traffic_src = None
-    tp = os.path.join(ROOT, "profiles", "pcg_traffic.json")
-    if os.path.exists(tp):  # DRAM bytes of this kernel on this workload from the committed ncu --set full capture (not measurable without a profiler)
-        tj = json.load(open(tp))
-        traffic, traffic_src = tj.get("dram_bytes_per_solve"), tj.get("source")
+    traffic = traffic_src = None  # DRAM bytes actually moved need a hardware profiler: not measured
     ach = bytes_alg / t / 1e9
     e, it = f.last_solve(0)
     f.close()
@@ -285,7 +326,7 @@ def late_window_and_in_step(fluid, step, stepper, dt, steps_done, args, early_ms
     touched_cells = work["tiles"] * work["cells_per_tile"] + work["columns"] * work["cells_per_column"]
     m = fluid.download_grid(F.TAP_MARKER)
     fluid_cells = int((m == 1).sum())
-    peak = 6650.0
+    peak = 3350.0  # H100 SXM data sheet
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = float(json.load(open(pk)).get("hbm_gbs", peak))
@@ -300,8 +341,7 @@ def late_window_and_in_step(fluid, step, stepper, dt, steps_done, args, early_ms
     in_step = {"at_step": steps_done - 1, "fluid_cells": fluid_cells, "fluid_fraction": round(fluid_cells / fluid.n, 4),
                "solver_work": work, "touched_cells": touched_cells, "bytes_per_cell_and_pass": 42, "solves": solves,
                "stage_ms": {name: round(v, 4) for name, v in zip(F.STAGES, stage_ms)}, "stage_total_ms": round(float(sum(stage_ms)), 4),
-               "note": "touched = cells of the tiles and quad columns on the solver's work lists; the fluid working set of this scene is L2-resident, so the in-step solve is "
-                       "latency / instruction bound, not HBM bound -- the HBM roofline of the kernel is the dense microbench in `roofline`"}
+               "note": "touched = cells of the tiles and quad columns on the solver's work lists; the HBM roofline of the kernel is the dense microbench in `roofline`"}
     # what a consumer pays to GET the result: nothing on the device (blub_fluid_view hands out the ten device pointers the renderer binds,
     # hybrid_fluid.rs:351-369); a host copy of the particle positions is a plain D2H transfer
     t0 = time.perf_counter()
@@ -375,6 +415,8 @@ def main():
     ap.add_argument("--no-scaling-reference", action="store_true")
     ap.add_argument("--no-phases", action="store_true", help="skip the late-window timing and the in-step stage / roofline analysis (N = 1)")
     ap.add_argument("--late-start", type=int, default=100, help="first step of the late timing window (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the fluid state they produced to DIR/<name>.npy (float32, seeded samples, <= 64 MB)")
     ap.add_argument("--multi", default="sharded", choices=["sharded", "stacked", "split", "replicas"],
                     help="N > 1: one z-slab sharded simulation of a z-uniform dam (default: weak scaling, balanced), of N stacked dam_256 cubes, of the workload's "
                          "OWN grid cut into N slabs (split: strong scaling, e.g. --workload basin_512 = config C4), or N independent replicas")
@@ -396,7 +438,7 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: no CUDA device (there is no CPU fallback)")
+        raise SystemExit("bench.py needs an H100: no CUDA device (there is no CPU fallback)")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
@@ -478,6 +520,9 @@ def main():
     launches = blub_b200.kernel_launch_count() - launches0
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    dumped = None
+    if args.dump_outputs:  # the state after the last timed step, before anything else advances the simulation
+        dumped = dump_outputs(fluid, args.dump_outputs, f"_rank{rank}" if world > 1 else "", parts=world)
     t_ms = torch.tensor([ms], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(t_ms, op=dist.ReduceOp.MAX)
@@ -565,6 +610,8 @@ def main():
             line["result_handoff"] = handoff
         if scaling_ref is not None:
             line["scaling_reference"] = scaling_ref
+        if dumped is not None:
+            line["dumped_outputs"] = dumped
         if sharded is not None:
             line["pcg_sharded"] = sharded
         print(json.dumps(line), flush=True)

@@ -1,9 +1,9 @@
-"""blub_b200 -- B200-native APIC/FLIP fluid-step core (drop-in for Wumpf/blub's HybridFluid path).
+"""blub_b200 -- H100-native APIC/FLIP fluid-step core (drop-in for Wumpf/blub's HybridFluid path).
 
-The product is ``libblubcore.so`` (hand-written sm_100a CUDA behind the C ABI of ``include/blub_fluid.h``); this
+The product is ``libblubcore.so`` (hand-written sm_90a CUDA behind the C ABI of ``include/blub_fluid.h``); this
 package is only the ctypes mirror of the reference's ``HybridFluid`` interface used by tests and ``bench.py``.
 There is no CPU fallback: importing works anywhere (so that symbols can be checked), but creating a fluid without
-the built library or without a B200 raises.
+the built library or without an H100 raises.
 """
 from .fluid import (  # noqa: F401
     DT_120HZ,

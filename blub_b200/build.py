@@ -1,4 +1,4 @@
-"""Builds libblubcore.so in-tree with nvcc for sm_100a (no torch, no JIT cache).
+"""Builds libblubcore.so in-tree with nvcc for sm_90a (no torch, no JIT cache).
 
     python -m blub_b200.build [--force] [--verbose]
 """
@@ -17,7 +17,7 @@ EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"]}
 HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "voxelize_core.hpp", os.path.join("..", "..", "include", "blub_fluid.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",
 ]
 
@@ -45,7 +45,7 @@ def build(force=False, verbose=False):
             subprocess.check_call(cmd)
             rebuilt = True
     if rebuilt or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         if verbose:
             print(" ".join(cmd), flush=True)
         subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// blub_core.hpp -- C++ host side of libblubcore: the B200-native counterparts of the reference's
+// blub_core.hpp -- C++ host side of libblubcore: the H100-native counterparts of the reference's
 // `HybridFluid` (src/simulation/hybrid_fluid.rs), `PressureSolver` and `PressureField`
 // (src/simulation/pressure_solver.rs).  Same method names, argument meaning and defaults; wgpu objects are replaced by
 // device pointers and one CUDA stream.  The C ABI in include/blub_fluid.h is a thin shim over these classes.
@@ -218,7 +218,7 @@ class HybridFluid {
     struct SlabHaloItem {
         void *cell0;           // cell-0 pointer of a grid volume
         size_t bytes_per_cell;
-        int kind;              // 0 SUM (float data) / 1 MAX (int8) over the 4 overlap planes, 2 COPY of 2 owned planes into the ghost planes
+        int kind;              // 0 SUM (64-bit fixed-point data) / 1 MAX (int8) over the 4 overlap planes, 2 COPY of 2 owned planes into the ghost planes
     };
     size_t slab_extra_window_bytes() const;
     uint32_t slab_migrant_capacity() const;
@@ -273,8 +273,9 @@ class HybridFluid {
     float4 *pos_[2] = {nullptr, nullptr}; // ping-pong for the binning reorder
     int cur_ = 0;
     float4 *row_[3] = {nullptr, nullptr, nullptr};
-    GridArray<float> u_[3], density_;
-    GridArray<float2> numw_[3];        // scatter-form P2G accumulators: (sum w*value, sum w) per face (sharded step / comparison path only)
+    GridArray<float> u_[3];
+    GridArray<long long> density_;     // density scatter accumulator, 64-bit fixed point (common.cuh: to_fixed)
+    GridArray<longlong2> numw_[3];     // scatter-form P2G accumulators: (sum w*value, sum w) per face, 64-bit fixed point
     FluidBits fluid_bits_ = {nullptr, 0}; // 1 bit per cell "FLUID", rebuilt with every finished marker volume
     bool fluid_bits_stale_ = false;       // the marker volume was written through a tap since
     GridArray<int8_t> marker_;

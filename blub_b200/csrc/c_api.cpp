@@ -70,7 +70,7 @@ Tap tap_of(BlubFluid *f, int tap) {
 extern "C" {
 
 const char *blub_last_error(void) { return g_last_error.c_str(); }
-const char *blub_version(void) { return "blub-b200 0.1 (sm_100a)"; }
+const char *blub_version(void) { return "blub-b200 0.1 (sm_90a)"; }
 
 int blub_fluid_create(BlubFluid **out, uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num_particles, int device, void *cuda_stream) {
     if (!out) return fail(BLUB_ERR_INVALID_ARGUMENT, "out is NULL");

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers of libblubcore (sm_100a only).
+// common.cuh -- shared device/host helpers of libblubcore (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -30,6 +30,17 @@ struct CudaError : std::runtime_error {
     } while (0)
 
 extern std::atomic<uint64_t> g_kernel_launches;
+
+// SM count of the current device, queried once per device: grids sized "so many blocks per SM" follow the GPU they run on.
+inline int device_sm_count() {
+    static std::atomic<int> cache[64];
+    int dev = 0, n = 0;
+    BLUB_CUDA_CHECK(cudaGetDevice(&dev));
+    if (dev >= 0 && dev < 64 && (n = cache[dev].load(std::memory_order_relaxed)) > 0) return n;
+    BLUB_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    if (dev >= 0 && dev < 64) cache[dev].store(n, std::memory_order_relaxed);
+    return n;
+}
 
 // Every kernel launch of the library goes through this macro so that bench.py can report gpu_launches.
 #define BLUB_LAUNCH(kernel, grid, block, smem, stream, ...)                                                            \
@@ -141,6 +152,17 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 
 __device__ __forceinline__ float saturatef(float x) { return __saturatef(x); }
+
+// Accumulators of the scatter kernels: 64-bit fixed point.  Integer additions are associative, so a sum does not depend on the order in
+// which the atomics arrive: the same input gives the same step, bit for bit, run after run.  Sums of w * value carry 36 fractional bits
+// (range +-2^27), sums of weights 40 (range +-2^23); a contribution is rounded to 2^-36 / 2^-40, far below float resolution for the
+// weights that matter (a face with a total weight of 1e-6 keeps a relative precision of 1e-6).
+constexpr int FIXED_VALUE_BITS = 36, FIXED_WEIGHT_BITS = 40;
+template <int FRAC> __device__ __forceinline__ long long to_fixed(float v) { return __float2ll_rn(v * (float)(1ull << FRAC)); }
+template <int FRAC> __device__ __forceinline__ double from_fixed(long long a) { return (double)a / (double)(1ull << FRAC); }
+__device__ __forceinline__ void fixed_add(long long *dst, long long v) {
+    atomicAdd(reinterpret_cast<unsigned long long *>(dst), (unsigned long long)v); // two's complement: signed sums come out right
+}
 
 // RGBA16F solid voxel texel: xyz = velocity in cells/s, w != 0 => solid (src/scene/voxelization.rs:17)
 struct Voxel {

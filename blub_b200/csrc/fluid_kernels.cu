@@ -1,7 +1,7 @@
-// fluid_kernels.cu -- grid passes and grid -> particle kernels of the fluid step (sm_100a); the particle -> grid transfers
+// fluid_kernels.cu -- grid passes and grid -> particle kernels of the fluid step (sm_90a); the particle -> grid transfers
 // live in transfer_kernels.cu, the pressure solve in pcg.cu.
 //
-// Reference counterparts (relative to /root/reference/shader/simulation): divergence_compute.comp, divergence_remove.comp,
+// Reference counterparts (relative to the reference's shader/simulation): divergence_compute.comp, divergence_remove.comp,
 // extrapolate_velocity.comp, advect_particles.comp, density_projection_{position_change,correct_particles}.comp.
 #include <cstdlib>
 #include <cstring>
@@ -506,7 +506,7 @@ __global__ void __launch_bounds__(PT) correct_particles_kernel(GridDim g, const 
 
 inline int blocks_for(int64_t n, int per_block) { return (int)((n + per_block - 1) / per_block); }
 // particle kernels: at most 128 blocks per SM (small enough for a negligible tail, few enough to launch quickly), a grid-stride loop over the rest
-inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), 148 * 128); }
+inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), device_sm_count() * 128); }
 
 } // namespace
 

@@ -42,15 +42,16 @@ void launch_p2g_gather(cudaStream_t st, const GridDim &g, const StepParams *para
                        const int8_t *marker, float *const u[3]);
 // scatter form of P2G / density in two halves, for callers that exchange halos in between (z-slab sharding)
 void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float4 *const row[3],
-                        float2 *const nw[3], int8_t *marker, bool clear_accumulators);
+                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators);
 // particle_words: wpr * ny * nz words, 1 bit per cell "a particle marked this cell" (before the boundary rule); the finish pass visits and
 // re-zeroes the accumulators of the one-cell dilation of those cells only
-void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], float2 *const nw[3], int8_t *marker,
+void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,
                        const uint2 *vox, const FluidBits &bits, uint32_t *particle_words);
-void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float *density);
-void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const float *density, float *rhs);
+// density: 64-bit fixed-point accumulator volume (FIXED_WEIGHT_BITS, common.cuh)
+void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density);
+void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs);
 void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos,
-                        const int8_t *marker, float *density, float *rhs);
+                        const int8_t *marker, long long *density, float *rhs);
 void launch_boundary_marker(cudaStream_t st, const GridDim &g, int8_t *marker, const uint2 *vox, const FluidBits &bits, uint32_t *particle_words = nullptr);
 void launch_fluid_bits(cudaStream_t st, const GridDim &g, const int8_t *marker, const FluidBits &bits);
 int binning_scan_blocks(const GridDim &g);

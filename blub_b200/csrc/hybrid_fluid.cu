@@ -43,7 +43,7 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
     BLUB_CUDA_CHECK(cudaSetDevice(device));
     cudaDeviceProp prop;
     BLUB_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) throw CudaError(std::string("libblubcore is built for sm_100a only, found ") + prop.name);
+    if (prop.major != 9 || prop.minor != 0) throw CudaError(std::string("libblubcore is built for sm_90a only, found ") + prop.name);
     if (stream_ == nullptr) {
         BLUB_CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
         owns_stream_ = true;
@@ -89,8 +89,7 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
     }
     configure_transfer_kernels();
     {
-        // Default: the scatter form.  Measured on the 256^3 dam break (profiles/r02_s4_timelines.md): scatter 1.30 / 1.60 / 1.53 ms at steps
-        // 3 / 56 / 110, gather 2.20 / 3.51 / 3.36 ms -- the gather is bit-reproducible, the scatter is faster.  BLUB_P2G=gather or
+        // Default: the scatter form, faster than the gather on the 256^3 dam break; the gather is bit-reproducible.  BLUB_P2G=gather or
         // blub_fluid_set_transfer_path(f, 0) selects the gather.
         const char *tp = std::getenv("BLUB_P2G");
         set_transfer_path(tp && std::string(tp) == "gather" ? 0 : 1);
@@ -390,8 +389,8 @@ void HybridFluid::upload_step_params(float dt) {
 }
 
 // Particle binning (hybrid_fluid.rs:854-894): every `particle_rebinning_step_frequency`-th step including step 0, 0 = never -- and, because
-// a re-sort costs 0.5 ms here (positions only, deterministic) while a decayed particle order costs the scatters and the G2P kernels 0.5 ms
-// EVERY step (profiles/r02_s11_rebin_cadence.md), additionally every `internal_resort_every_`-th step (8; BLUB_RESORT_EVERY=0 turns that off).
+// a re-sort (positions only, deterministic) costs about what a decayed particle order costs the scatters and the G2P kernels in
+// EVERY step, additionally every `internal_resort_every_`-th step (8; BLUB_RESORT_EVERY=0 turns that off).
 // Binning only permutes the particle arrays: with it or without it a step computes the same sums in a different order.
 bool HybridFluid::binning_step() const {
     const uint32_t rebin = dynamic_settings_.particle_rebinning_step_frequency;
@@ -408,7 +407,7 @@ void HybridFluid::refresh_fluid_bits() {
     fluid_bits_stale_ = false;
 }
 
-// 0: gather form of P2G (default), 1: scatter form (RED.ADD.F32x2 into accumulator volumes; what the sharded step uses)
+// 0: gather form of P2G (default), 1: scatter form (fixed-point integer reductions into accumulator volumes; what the sharded step uses)
 void HybridFluid::set_transfer_path(int scatter) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     if ((scatter || slab_world_ > 1) && !numw_[0].ptr)
@@ -420,7 +419,7 @@ void HybridFluid::set_transfer_path(int scatter) {
 // Stage numbering shared with oracle/blub_oracle.c:orc_step_stages (the order of hybrid_fluid.rs:798-974).
 void HybridFluid::run_stage(int stage, float dt) {
     float *u[3] = {u_[0].ptr, u_[1].ptr, u_[2].ptr};
-    float2 *nw[3] = {numw_[0].ptr, numw_[1].ptr, numw_[2].ptr};
+    longlong2 *nw[3] = {numw_[0].ptr, numw_[1].ptr, numw_[2].ptr};
     const FluidBits &bits = fluid_bits_;
     const bool shard = slab_world_ > 1 && solver_->comm.world > 1;
     const uint32_t np = slab_world_ > 1 ? max_num_particles_ : num_particles_; // sharded: the device-side count guards the kernels
@@ -440,7 +439,7 @@ void HybridFluid::run_stage(int stage, float dt) {
             fluid_bits_stale_ = false;
         } else {
             launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, true);
-            const SlabHaloItem items[4] = {{nw[0], sizeof(float2), 0}, {nw[1], sizeof(float2), 0}, {nw[2], sizeof(float2), 0}, {marker_.ptr, 1, 1}};
+            const SlabHaloItem items[4] = {{nw[0], sizeof(longlong2), 0}, {nw[1], sizeof(longlong2), 0}, {nw[2], sizeof(longlong2), 0}, {marker_.ptr, 1, 1}};
             slab_halo_exchange(items, 4); // X1
             launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, voxels_, bits, particle_words_);
             fluid_bits_stale_ = false;
@@ -494,7 +493,7 @@ void HybridFluid::run_stage(int stage, float dt) {
             launch_density_rhs(stream_, grid_, params_dev_, np, pos_[cur_], marker_.ptr, density_.ptr, solver_->residual());
         } else {
             launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr);
-            const SlabHaloItem items[1] = {{density_.ptr, sizeof(float), 0}};
+            const SlabHaloItem items[1] = {{density_.ptr, sizeof(long long), 0}};
             slab_halo_exchange(items, 1); // X4
             launch_density_finish(stream_, grid_, params_dev_, marker_.ptr, density_.ptr, solver_->residual());
         }

@@ -1,4 +1,4 @@
-// pcg.cu -- preconditioned conjugate gradient pressure solve (sm_100a).
+// pcg.cu -- preconditioned conjugate gradient pressure solve (sm_90a).
 //
 // Replaces PressureSolver::solve (src/simulation/pressure_solver.rs:591-729) and the seven compute pipelines under
 // shader/simulation/pressure_solver/.  Same recurrence, same iteration schedule (error checks at i % freq == 0 and
@@ -536,7 +536,7 @@ __global__ void __launch_bounds__(PCG_THREADS) pcg_search_kernel(GridDim g, Tile
 // redundantly in the same fixed order (bit-identical scalars everywhere, no broadcast, deterministic); converged solves
 // stop at once instead of running out a recorded launch list.  Blocks walk the compacted list of active tiles with a
 // fixed stride, so a tile is processed by the same SM in every phase.  24 B/cell/iteration of DRAM traffic at most
-// (A: r, s, code in + s' out = 13; B: p, r, s', code in + p, r out = 21 ... minus what stays in the 126 MB L2).
+// (A: r, s, code in + s' out = 13; B: p, r, s', code in + p, r out = 21 ... minus what stays in the 50 MB L2 of an H100).
 struct PcgSolveArgs {
     GridDim g;
     TileMap t;
@@ -635,7 +635,7 @@ __device__ __forceinline__ double grid_sum(cooperative_groups::grid_group &grid,
 }
 
 // Sparsity (SKIP): the FLUID set of a real scene is a thin, ragged body -- at step 110 of the 256^3 dam break 64 % of the
-// 128x8x4 tiles hold fluid but only 16 % of the 4x1x4 thread columns do (profiles/r01_v12_sparsity.txt).  A thread of a
+// 128x8x4 tiles hold fluid but only 16 % of the 4x1x4 thread columns do (tools/sparsity.py).  A thread of a
 // sparse tile therefore reads the six code words of its column first and touches p, r, s only on planes whose quad holds a
 // FLUID cell: under the zero invariant everything it would have loaded, added or stored elsewhere is exactly 0, so the
 // result is bit-identical to the dense form.  Tiles that are at least 3/4 full (flagged by pcg_prepare_kernel, the flag
@@ -679,7 +679,7 @@ __device__ __forceinline__ void load_column_codes(const TileEnv &e, const TileCt
 // body: every value it would load is 0 (zero invariant), it would store nothing and add 0 to the partial sums -- and nobody else
 // depends on it (x-neighbours live in the same warp, y / z neighbours are read from memory).  In a dam break most warps of the
 // "active" tiles along the free surface are like that: skipping them at warp granularity removes the body's instruction skeleton,
-// which is what the sparse solve is bound by (profiles/r02_s2_pcg_step110.md: 1.16 G warp instructions, 17 of 32 lanes active).
+// which is what the sparse solve is bound by.
 __device__ __forceinline__ bool warp_has_no_fluid(const unsigned (&w)[PCG_TZ + 2]) {
     unsigned any = 0;
 #pragma unroll
@@ -944,8 +944,8 @@ __global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(Pc
 
 // ---------------------------------------------------------------------------------------------------------------
 // Grid-wide reduction of the column solver.  With the fluid working set in L2 the solve is bound by the latency of these two
-// reductions per iteration (profiles/r02_s6_pcg_overhead.md: ~8 us per phase with no work at all), so they are kept lean
-// (tools/barrier_bench.cu, profiles/r02_s7_barrier_bench.md: cooperative_groups grid.sync() + re-read 4.5 us, this form 3.7 us at 592 blocks):
+// reductions per iteration, so they are kept lean
+// (tools/barrier_bench.cu compares it with cooperative_groups grid.sync() + re-read):
 // one shared-memory pass forms the block's sum and maximum, thread 0 publishes them, arrives on a monotonically increasing counter
 // (red.release) and spins with ld.acquire until everybody of this round has arrived; then every block re-reads all partials and adds
 // them in the same fixed order in fp64: bit-identical scalars in all blocks, deterministic run to run, no broadcast step.
@@ -1106,10 +1106,10 @@ __device__ __forceinline__ void grid_allreduce(const SlabComm &c, unsigned seq, 
 // ---------------------------------------------------------------------------------------------------------------
 // Column solver (default on one GPU): the persistent solver with a work list that follows the fluid.
 //
-// What the in-step profile of the tile kernel showed (profiles/r02_s2_pcg_step110.md, step 110 of the 256^3 dam break, 12.6 % of the
-// cells FLUID): 1.16 G warp instructions per solve, and in the sparsely filled tiles only 4-5 of 32 lanes do anything -- a warp pays the
+// Why: at step 110 of the 256^3 dam break (12.6 % of the cells FLUID) the sparsely filled tiles of the tile kernel have only 4-5 of 32
+// lanes doing anything -- a warp pays the
 // whole instruction skeleton of a plane as soon as ONE of its lanes has a FLUID quad there.  The solve is bound by that skeleton and by
-// the 4-5 sequential tile passes per block and phase, not by bandwidth (the fluid working set is L2-resident).
+// the 4-5 sequential tile passes per block and phase, not by bandwidth.
 // Here tiles that are at least 3/4 full still run the branch-free tile body (an all-fluid grid costs what it cost: the roofline
 // microbench), but everything else is flattened into ONE list of active quad columns (4 cells x PCG_TZ planes, ascending index:
 // deterministic) and dealt to the warps 32 columns at a time: every lane has work, x-adjacent quads still sit in adjacent lanes
@@ -1193,7 +1193,9 @@ __device__ __forceinline__ TileCtx column_ctx(int i, int sz) {
     return c;
 }
 
-__global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_columns_kernel(PcgSolveArgs a) {
+// Three resident blocks per SM (up to 85 registers): for sm_90a, a four-block bound (64 registers) spills the column body to local memory,
+// and on an H100 SXM (700 W limit) the 256^3 dam break runs 100.9 instead of 97.7 steps/s with three blocks (profiles/h100_choices.json).
+__global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSolveArgs a) {
     __shared__ ReduceScratch sc;
     __shared__ double sh_csum[SLAB_MAX_WORLD];
     __shared__ float sh_cmax[SLAB_MAX_WORLD];

@@ -52,7 +52,7 @@ __global__ void slab_barrier_kernel(SlabComm c, int *error_flag) {
     }
 }
 
-__global__ void __launch_bounds__(256) halo_add_kernel(float *__restrict__ dst, const float *__restrict__ src, int64_t n) {
+__global__ void __launch_bounds__(256) halo_add_kernel(long long *__restrict__ dst, const long long *__restrict__ src, int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (i < n) dst[i] += src[i];
 }
@@ -105,7 +105,7 @@ inline int blocks_for(int64_t n, int per) { return (int)((n + per - 1) / per); }
 // ---------------------------------------------------------------------------------------------------------------
 size_t HybridFluid::slab_extra_window_bytes() const {
     const size_t cols = (size_t)grid_.nx * grid_.ny;
-    const size_t halo = (cols * 100 + 255) / 256 * 256;                              // 3 x float2 x 4 planes + marker x 4 planes
+    const size_t halo = (cols * 196 + 255) / 256 * 256;                              // 3 x longlong2 x 4 planes + marker x 4 planes
     const size_t part = ((size_t)slab_migrant_capacity() * sizeof(MigrantRecord) + 255) / 256 * 256;
     return 4 * halo + 2 * part + 256;
 }
@@ -115,7 +115,7 @@ uint32_t HybridFluid::slab_migrant_capacity() const { return (uint32_t)grid_.nx 
 void HybridFluid::slab_layout(void *window, char *&halo0, size_t &halo_bytes, char *&part0, size_t &part_bytes, unsigned int *&counts) const {
     const size_t vol = GridArray<float>::bytes_for(grid_);
     const size_t cols = (size_t)grid_.nx * grid_.ny;
-    halo_bytes = (cols * 100 + 255) / 256 * 256;
+    halo_bytes = (cols * 196 + 255) / 256 * 256;
     part_bytes = ((size_t)slab_migrant_capacity() * sizeof(MigrantRecord) + 255) / 256 * 256;
     char *w = static_cast<char *>(window) + 4096 + 3 * vol;
     halo0 = w;
@@ -184,8 +184,8 @@ void HybridFluid::slab_halo_exchange(const SlabHaloItem *items, int n_items) {
             const size_t bytes = (size_t)planes * plane_cells * it.bytes_per_cell;
             char *dst = static_cast<char *>(it.cell0) + (size_t)first * plane_cells * it.bytes_per_cell;
             if (it.kind == 0) {
-                const int64_t n = (int64_t)(bytes / sizeof(float));
-                BLUB_LAUNCH(halo_add_kernel, blocks_for(n, 256), 256, 0, stream_, reinterpret_cast<float *>(dst), reinterpret_cast<const float *>(src + off), n);
+                const int64_t n = (int64_t)(bytes / sizeof(long long)); // fixed-point sums: exact, the same on both sides of the face
+                BLUB_LAUNCH(halo_add_kernel, blocks_for(n, 256), 256, 0, stream_, reinterpret_cast<long long *>(dst), reinterpret_cast<const long long *>(src + off), n);
             } else if (it.kind == 1) {
                 BLUB_LAUNCH(halo_max_kernel, blocks_for((int64_t)bytes, 256), 256, 0, stream_, reinterpret_cast<int8_t *>(dst),
                             reinterpret_cast<const int8_t *>(src + off), (int64_t)bytes);

@@ -1,6 +1,6 @@
-// transfer_kernels.cu -- particle <-> grid transfers of the fluid step (sm_100a): cell lists, P2G, density error, binning.
+// transfer_kernels.cu -- particle <-> grid transfers of the fluid step (sm_90a): cell lists, P2G, density error, binning.
 //
-// Reference counterparts (relative to /root/reference/shader/simulation): transfer_clear.comp, transfer_build_linkedlist.comp,
+// Reference counterparts (relative to the reference's shader/simulation): transfer_clear.comp, transfer_build_linkedlist.comp,
 // transfer_gather_velocity.comp, density_projection_gather_error.comp:41-97, particle_binning_*.comp.
 //
 // Not a port.  The reference threads per-dual-cell linked lists through the particle buffer (atomic exchange: arbitrary order)
@@ -9,8 +9,9 @@
 //
 //   * P2G SCATTER (default; the form z-slab ranks always use): one thread per particle; the lanes of a warp that share a dual cell -- found
 //     with match.any, adjacent or not -- add their contributions up in groups of four with two shuffle steps, and the lowest lane of a
-//     group issues one 8-byte vector reduction (RED.ADD.F32x2) per face: 10.7 reductions per particle instead of 24 (17.8 with runs of
-//     adjacent lanes only).  A sparse finish pass normalises and puts the accumulators back to zero (no memsets, no dense pass).
+//     group adds (sum w*value, sum w) of each face into 64-bit fixed-point accumulators with integer atomics: 10.7 faces per particle instead
+//     of 24 (17.8 with runs of adjacent lanes only), and sums that do not depend on the arrival order of the atomics (deterministic).
+//     A sparse finish pass normalises and puts the accumulators back to zero (no memsets, no dense pass).
 //   * CELL LISTS (gather form and binning): a counting sort of particle INDICES by primal cell -- count (one integer atomic per particle),
 //     exclusive scan, fill, and a canonicalisation (rank counting) that puts every cell's slice into ascending particle index.  The
 //     lists are therefore a pure function of the particle array: the same input gives the same lists, run after run, whatever
@@ -36,7 +37,7 @@ constexpr int PT = 256; // threads per block for particle and cell kernels
 __device__ __forceinline__ int lin(const GridDim &g, int x, int y, int z) { return (z * g.ny + y) * g.nx + x; }
 inline int blocks_for(int64_t n, int per_block) { return (int)((n + per_block - 1) / per_block); }
 // particle kernels: at most 128 blocks per SM (small enough for a negligible tail, few enough to launch quickly), a grid-stride loop over the rest
-inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), 148 * 128); }
+inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), device_sm_count() * 128); }
 
 // The position a transfer sees: clamped so that every face / cell a particle touches exists (a simulated particle is always
 // inside [1.001, dim - 1.001], so this only ever changes particles handed in from outside the domain).  lo = 1.0 for the
@@ -181,10 +182,10 @@ __global__ void __launch_bounds__(PT) cell_fill_kernel(const StepParams *__restr
 // cell_start[c] + #{entries of c smaller than it}.  One thread per list entry, k loads each from one or two cache lines.
 // After this the lists no longer depend on the arrival order of the count atomics.
 // CROWDED cells (more than CROWD_T particles: a wave piling up against a wall puts thousands of particles into single cells --
-// 7380 at step 56 of the 256^3 dam break, profiles/r02_s3_p2g_parts.md -- where the reference simply stops reading its lists after 12
-// entries) keep their arrival order and are appended to the crowded-cell list instead: their sums are formed by a whole warp in exact
-// integer arithmetic (p2g_crowded_kernel), which is order independent, so the result stays deterministic without an O(k^2) rank count
-// and without one thread walking thousands of particles.
+// thousands at step 56 of the 256^3 dam break -- where the reference simply stops reading its lists after 12
+// entries) are appended to the crowded-cell list instead and put into the same order by a whole block each (crowded_canonicalize_kernel):
+// one thread per entry would walk thousands of entries there.  Their P2G sums are formed by a whole warp in exact integer arithmetic
+// (p2g_crowded_kernel).
 constexpr uint32_t CROWD_T = 32;
 __device__ __forceinline__ void cell_canonicalize_kernel_one(uint32_t j, const StepParams *__restrict__ params, const uint2 *__restrict__ cell_slot,
                                                                const uint32_t *__restrict__ cell_start, const uint32_t *__restrict__ arrival,
@@ -210,6 +211,46 @@ __global__ void __launch_bounds__(PT) cell_canonicalize_kernel(const StepParams 
     // a bounded grid strides over the particles: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
     for (uint32_t j = blockIdx.x * PT + threadIdx.x; (j & ~31u) < np_; j += gridDim.x * PT) cell_canonicalize_kernel_one(j, params, cell_slot, cell_start, arrival, order, crowd);
+}
+
+// Ascending particle index inside every crowded cell: one block per cell.  A slice of up to CROWD_SORT_SMEM entries is sorted in shared
+// memory by a bitonic network (O(k log^2 k) compare-exchanges spread over the block); a larger one (none seen in the scenes here) falls back
+// to rank counting over global memory.  The binning permutes the particles by these lists, so their order must not depend on the
+// arrival order of the count atomics either.
+constexpr uint32_t CROWD_SORT_SMEM = 8192; // entries (32 KB)
+__global__ void __launch_bounds__(PT) crowded_canonicalize_kernel(const uint32_t *__restrict__ cell_start, const uint32_t *__restrict__ arrival,
+                                                                  uint32_t *__restrict__ order, CrowdedCells crowd) {
+    __shared__ uint32_t sh[CROWD_SORT_SMEM];
+    const uint32_t ncrowded = *crowd.count;
+    for (uint32_t slot = blockIdx.x; slot < ncrowded; slot += gridDim.x) {
+        const uint32_t cell = crowd.cells[slot];
+        const uint32_t s = cell_start[cell], k = cell_start[cell + 1] - s;
+        const uint32_t *src = arrival + s;
+        if (k <= CROWD_SORT_SMEM) { // block-uniform
+            uint32_t m = 2;
+            while (m < k) m <<= 1;
+            for (uint32_t t = threadIdx.x; t < m; t += PT) sh[t] = t < k ? src[t] : 0xffffffffu; // padding sorts last
+            __syncthreads();
+            for (uint32_t size = 2; size <= m; size <<= 1)
+                for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+                    for (uint32_t t = threadIdx.x; t < (m >> 1); t += PT) {
+                        const uint32_t a = 2 * t - (t & (stride - 1)), b = a + stride;
+                        const uint32_t x = sh[a], y = sh[b];
+                        if ((x > y) == ((a & size) == 0)) { sh[a] = y; sh[b] = x; }
+                    }
+                    __syncthreads();
+                }
+            for (uint32_t t = threadIdx.x; t < k; t += PT) order[s + t] = sh[t];
+            __syncthreads(); // the slice in shared memory is read to the end before the next cell overwrites it
+        } else {
+            for (uint32_t j = threadIdx.x; j < k; j += PT) {
+                const uint32_t v = src[j];
+                uint32_t rank = 0;
+                for (uint32_t t = 0; t < k; ++t) rank += src[t] < v ? 1u : 0u;
+                order[s + rank] = v;
+            }
+        }
+    }
 }
 
 // Which cells of a 32-cell word the boundary rule makes SOLID: border cells and solid voxels (transfer_set_boundary_marker.comp:11-20)
@@ -578,10 +619,9 @@ __global__ void __launch_bounds__(PT) p2g_crowded_kernel(GridDim g, const uint32
 // axis c (transfer_build_linkedlist.comp:21-23), and contributes to the eight faces d + {0,1}^3.  (sum w*value, sum w) of a
 // face are interleaved as one float2.  Runs of adjacent lanes with the same dual cell (cell-sorted particles hit the SAME eight
 // faces) first add their contributions up with shuffles (segmented reduction in groups of four lanes); only the first lane of a group issues
-// reductions: one 8-byte RED.ADD.F32x2 per (group, face).  Measured against one reduction per (particle, face): P2G 1.92 -> 1.71 ms,
-// density 0.64 -> 0.57 ms at step 110 of the 256^3 dam break (profiles/r02_s1_tests_and_variant_timelines.md).
-// Runs are cut into groups of at most four lanes: two shuffle steps instead of five.  The full log2(32) reduction was what bound the kernel
-// (ncu: mio_throttle the top stall, 240 shuffles per particle, profiles/r02_s10_particle_kernels.md), while runs are short -- a dual cell
+// reductions: two 64-bit fixed-point integer adds per (group, face), fewer than per (particle, face).
+// Runs are cut into groups of at most four lanes: two shuffle steps instead of five.  A full log2(32) reduction costs 240 shuffles per
+// particle, while runs are short -- a dual cell
 // holds 8 particles on average and a cell-sorted warp holds them in 2-4 separate runs; a longer run simply issues one reduction per
 // group of four.  Warps in which every lane is its own run (the usual case once the particle order has decayed) skip the shuffles.
 // Since r2 session 18 this is the comparison path (BLUB_SCATTER_AGG=adjacent); the default is matched_group_sum below.
@@ -649,8 +689,8 @@ __device__ __forceinline__ bool warp_group_sum(int key, float (&v)[NV]) {
 template <bool MARK, bool MATCH>
 __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
-                                                         const float4 *__restrict__ rowz, float2 *__restrict__ nwx, float2 *__restrict__ nwy,
-                                                         float2 *__restrict__ nwz, int8_t *__restrict__ marker) {
+                                                         const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
+                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker) {
     const uint32_t np = params->num_particles;
     if ((i & ~31u) >= np) return;  // whole warp beyond the last particle (z-slab ranks launch over their capacity)
     const bool valid = i < np;     // no per-lane early return: every lane of a live warp takes part in the shuffles
@@ -658,7 +698,7 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
     if (MARK && valid) marker[cell_of_position(g, p)] = (int8_t)CELL_FLUID; // transfer_build_linkedlist.comp:17-19
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 rows[3] = {valid ? rowx[i] : zero, valid ? rowy[i] : zero, valid ? rowz[i] : zero};
-    float2 *const nw[3] = {nwx, nwy, nwz};
+    longlong2 *const nw[3] = {nwx, nwy, nwz};
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         const float ox = c == 0 ? 1.0f : 0.5f, oy = c == 1 ? 1.0f : 0.5f, oz = c == 2 ? 1.0f : 0.5f;
@@ -683,17 +723,25 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
         if (head && valid) {
 #pragma unroll
             for (int k = 0; k < 8; ++k)
-                if (acc[2 * k + 1] > 0.0f) atomicAdd(nw[c] + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz, make_float2(acc[2 * k], acc[2 * k + 1]));
+            {
+                // a contribution whose weight rounds to 0 is left out entirely (value too), so a face with weight 0 also has value 0
+                const long long wq = to_fixed<FIXED_WEIGHT_BITS>(acc[2 * k + 1]);
+                if (wq > 0) {
+                    longlong2 *const f = nw[c] + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz;
+                    const long long num = to_fixed<FIXED_VALUE_BITS>(acc[2 * k]);
+                    if (num != 0) fixed_add(&f->x, num);
+                    fixed_add(&f->y, wq);
+                }
+            }
         }
     }
 }
-// 4 resident blocks per SM (64 registers): compiled for 5 / 6 blocks (48 / 40 registers, 16 / 64 bytes of spills) the stage is slower
-// (0.697 / 0.713 / 0.768 ms at step 3 of the 256^3 dam break, profiles/r02_s19_multi_gpu_check_and_occupancy.md)
+// 4 resident blocks per SM (64 registers, no spills for sm_90a); a 5 / 6-block bound (48 / 40 registers) spills
 template <bool MARK, bool MATCH>
 __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
-                                                         const float4 *__restrict__ rowz, float2 *__restrict__ nwx, float2 *__restrict__ nwy,
-                                                         float2 *__restrict__ nwz, int8_t *__restrict__ marker) {
+                                                         const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
+                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker) {
     // a bounded grid strides over the particles: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
     for (uint32_t i = blockIdx.x * PT + threadIdx.x; (i & ~31u) < np_; i += gridDim.x * PT) p2g_scatter_kernel_one<MARK, MATCH>(i, g, params, pos, rowx, rowy, rowz, nwx, nwy, nwz, marker);
@@ -711,8 +759,8 @@ __device__ __forceinline__ unsigned pbits(const GridDim &g, const uint32_t *__re
 }
 __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, const uint32_t *__restrict__ particle_words, const StepParams *__restrict__ params,
                                                            const int8_t *__restrict__ marker, float *__restrict__ ux, float *__restrict__ uy,
-                                                           float *__restrict__ uz, float2 *__restrict__ nwx, float2 *__restrict__ nwy,
-                                                           float2 *__restrict__ nwz) {
+                                                           float *__restrict__ uz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
+                                                           longlong2 *__restrict__ nwz) {
     const int nwords = wpr * g.ny * g.nz;
     const int w = blockIdx.x * PT + threadIdx.x, lane = threadIdx.x & 31;
     unsigned touched = 0;
@@ -734,7 +782,7 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
     }
     unsigned todo = __ballot_sync(0xffffffffu, touched != 0u);
     float *const u[3] = {ux, uy, uz};
-    float2 *const nw[3] = {nwx, nwy, nwz};
+    longlong2 *const nw[3] = {nwx, nwy, nwz};
     while (todo) {
         const int src = __ffs(todo) - 1;
         todo &= todo - 1;
@@ -746,13 +794,13 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
         const int mb[3] = {marker[i + 1], marker[i + g.sy], marker[i + g.sz]};
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            const float2 a = nw[c][i];
-            if (a.x != 0.0f || a.y != 0.0f) nw[c][i] = make_float2(0.0f, 0.0f);
+            const longlong2 a = nw[c][i];
+            if (a.x != 0 || a.y != 0) nw[c][i] = make_longlong2(0, 0);
             float out = 0.0f;
             if (ma == CELL_FLUID || mb[c] == CELL_FLUID) {
                 if (ma != CELL_SOLID && mb[c] != CELL_SOLID) {
-                    float v = a.x;
-                    if (a.y > 0.0f) v /= a.y;
+                    const double num = from_fixed<FIXED_VALUE_BITS>(a.x), den = from_fixed<FIXED_WEIGHT_BITS>(a.y);
+                    const float v = a.y > 0 ? (float)(num / den) : 0.0f; // weight 0: no contribution reached this face
                     out = v + params->gravity_dt[c];
                 }
             }
@@ -766,7 +814,7 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
 // warp-aggregated like the P2G scatter.
 template <bool MATCH>
 __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
-                                                             float *__restrict__ density) {
+                                                             long long *__restrict__ density) {
     const uint32_t np = params->num_particles;
     if ((i & ~31u) >= np) return; // whole warp beyond the last particle
     const bool valid = i < np;
@@ -784,12 +832,12 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
     if (head && valid) {
 #pragma unroll
         for (int k = 0; k < 8; ++k)
-            if (acc[k] > 0.0f) atomicAdd(density + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz, acc[k]);
+            if (acc[k] > 0.0f) fixed_add(density + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz, to_fixed<FIXED_WEIGHT_BITS>(acc[k]));
     }
 }
 template <bool MATCH>
 __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
-                                                             float *__restrict__ density) {
+                                                             long long *__restrict__ density) {
     // a bounded grid strides over the particles: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
     for (uint32_t i = blockIdx.x * PT + threadIdx.x; (i & ~31u) < np_; i += gridDim.x * PT) density_scatter_kernel_one<MATCH>(i, g, params, pos, density);
@@ -797,12 +845,12 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
 
 // density_projection_gather_error.comp:99-199
 __global__ void __launch_bounds__(PT) density_rhs_kernel(GridDim g, const StepParams *__restrict__ params,
-                                                         const int8_t *__restrict__ marker, const float *__restrict__ density,
+                                                         const int8_t *__restrict__ marker, const long long *__restrict__ density,
                                                          float *__restrict__ rhs) {
     const int64_t i = (int64_t)blockIdx.x * PT + threadIdx.x;
     if (i >= g.n) return;
     if (marker[i] != CELL_FLUID) return;
-    float d = density[i];
+    float d = (float)from_fixed<FIXED_WEIGHT_BITS>(density[i]);
     const int m[6] = {marker[i + 1], marker[i + g.sy], marker[i + g.sz], marker[i - 1], marker[i - g.sy], marker[i - g.sz]};
     bool any_air = false;
 #pragma unroll
@@ -851,6 +899,7 @@ void launch_cell_lists(cudaStream_t st, const GridDim &g, const StepParams *para
     BLUB_LAUNCH(cell_fill_kernel, particle_blocks(np_upper), PT, 0, st, params, l.cell_slot, l.cell_start, l.arrival);
     BLUB_CUDA_CHECK(cudaMemsetAsync(l.crowd.count, 0, sizeof(uint32_t), st));
     BLUB_LAUNCH(cell_canonicalize_kernel, particle_blocks(np_upper), PT, 0, st, params, l.cell_slot, l.cell_start, l.arrival, l.order, l.crowd);
+    BLUB_LAUNCH(crowded_canonicalize_kernel, 2 * device_sm_count(), PT, 0, st, l.cell_start, l.arrival, l.order, l.crowd); // 2 blocks per SM
 }
 
 void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits) {
@@ -872,10 +921,11 @@ void configure_transfer_kernels() {
     BLUB_CUDA_CHECK(cudaFuncSetAttribute(p2g_gather_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GATHER_SMEM_BYTES));
 }
 
-constexpr int CROWD_BLOCKS = 296; // 2 blocks of 8 warps per SM walk the crowded-cell list (usually empty: the kernel then costs a launch)
 
 void launch_p2g_gather(cudaStream_t st, const GridDim &g, const StepParams *params, const CellLists &l, const float4 *pos, float4 *const row[3],
                        const int8_t *marker, float *const u[3]) {
+    // 2 blocks of 8 warps per SM walk the crowded-cell list (usually empty: the kernel then costs a launch)
+    const int CROWD_BLOCKS = 2 * device_sm_count();
     const dim3 grid((g.nx + GXS - 1) / GXS, (g.ny + GLY - 1) / GLY, (g.nz + GW - 1) / GW);
     // Faces no block stores (blocks without particles return at once) keep their previous value, as in the reference, which only
     // writes faces that touch a FLUID cell (transfer_gather_velocity.comp:41-47, SURVEY B6): nothing reads them before
@@ -899,38 +949,38 @@ static bool scatter_groups_by_match() {
 }
 
 void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float4 *const row[3],
-                        float2 *const nw[3], int8_t *marker, bool clear_accumulators) {
+                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators) {
     // transfer_clear.comp: marker <- AIR.  The (num, weight) volumes (they replace the linked-list head volume) are all zero here on one GPU:
     // they are allocated zeroed and launch_p2g_finish puts back to zero what the scatter touched.  A z-slab rank also receives partial sums
     // from its neighbours in the overlap planes, some of them from particles whose cells it never sees: it clears the volumes the plain way.
     BLUB_CUDA_CHECK(cudaMemsetAsync(marker, 0xFF, (size_t)g.n, st));
     if (clear_accumulators)
-        for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(nw[c], 0, (size_t)g.n * sizeof(float2), st));
+        for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(nw[c], 0, (size_t)g.n * sizeof(longlong2), st));
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? p2g_scatter_kernel<true, true> : p2g_scatter_kernel<true, false>;
     BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker);
 }
 
-void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], float2 *const nw[3], int8_t *marker,
+void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,
                        const uint2 *vox, const FluidBits &bits, uint32_t *particle_words) {
     launch_boundary_marker(st, g, marker, vox, bits, particle_words);
     BLUB_LAUNCH(p2g_normalize_kernel, blocks_for((int64_t)bits.wpr * g.ny * g.nz, PT), PT, 0, st, g, bits.wpr, particle_words, params, marker, u[0], u[1], u[2], nw[0],
                 nw[1], nw[2]);
 }
 
-void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float *density) {
-    BLUB_CUDA_CHECK(cudaMemsetAsync(density, 0, (size_t)g.n * sizeof(float), st));
+void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density) {
+    BLUB_CUDA_CHECK(cudaMemsetAsync(density, 0, (size_t)g.n * sizeof(long long), st));
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? density_scatter_kernel<true> : density_scatter_kernel<false>;
     BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, density);
 }
 
-void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const float *density, float *rhs) {
+void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs) {
     BLUB_LAUNCH(density_rhs_kernel, blocks_for(g.n, PT), PT, 0, st, g, params, marker, density, rhs);
 }
 
 void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos,
-                        const int8_t *marker, float *density, float *rhs) {
+                        const int8_t *marker, long long *density, float *rhs) {
     launch_density_scatter(st, g, params, np_upper, pos, density);
     launch_density_finish(st, g, params, marker, density, rhs);
 }

@@ -1,11 +1,11 @@
 /*
- * blub_fluid.h -- C ABI of libblubcore.so, the B200-native APIC/FLIP fluid-step core.
+ * blub_fluid.h -- C ABI of libblubcore.so, the H100-native APIC/FLIP fluid-step core.
  *
  * Drop-in boundary for Wumpf/blub's `HybridFluid` (src/simulation/hybrid_fluid.rs) and its
  * `PressureSolver`/`PressureField` (src/simulation/pressure_solver.rs).  The reference has no
  * FFI/plugin layer: its narrowest seam is the Rust method set of `HybridFluid`, whose arguments are
  * wgpu objects.  Every entry point below names the reference method it replaces (file:line relative
- * to /root/reference); wgpu handles become plain device pointers, a CUDA stream and POD structs.
+ * to the reference checkout); wgpu handles become plain device pointers, a CUDA stream and POD structs.
  * INTEGRATION.md shows the Rust `extern "C"` block a maintainer would add.
  *
  * Conventions kept from the reference:
@@ -18,7 +18,7 @@
  *     statistics read-back, which is asynchronous and may lag (pressure_solver.rs:148-209);
  *   - the reference panics on set-up failure and only logs at run time; here every fallible call
  *     returns an int code and nothing throws across the boundary.
- * There is NO CPU fallback: every call fails with BLUB_ERR_CUDA if no usable sm_100 device exists.
+ * There is NO CPU fallback: every call fails with BLUB_ERR_CUDA if no usable sm_90 (H100) device exists.
  */
 #ifndef BLUB_FLUID_H
 #define BLUB_FLUID_H

@@ -9,7 +9,7 @@
  * environment (no cargo/rustc/Vulkan/shaderc, 258 un-vendored crates, windowed app) and it
  * ships no tests, golden vectors or known-answer fixtures for this path.  This file follows
  * the reference's shaders and host code line by line (citations below, relative to
- * /root/reference) and is pinned only by analytic known-answer tests (tests/test_oracle_kat.py, tests/test_transfer_kat.py).
+ * the reference checkout) and is pinned only by analytic known-answer tests (tests/test_oracle_kat.py, tests/test_transfer_kat.py).
  *
  * Conventions (shader/simulation/hybrid_fluid.glsl:20-23):
  *   marker: SOLID = 0, FLUID = 1, AIR = -1; any out-of-domain texel/image read returns 0.
@@ -141,7 +141,7 @@ void orc_destroy(OrcFluid *f) {
 /* ------------------------------------------------------------------ particle seeding
  * hybrid_fluid.rs:609-678.  RNG = rand 0.8.5 SmallRng (xoshiro256++ seeded through SplitMix64),
  * cgmath 0.18 Standard -> Vector3<f32> draws x,y,z; f32 = (next_u32 >> 8) * 2^-24 with
- * next_u32 = high half of next_u64.  Third-party crates are absent from /root/reference
+ * next_u32 = high half of next_u64.  Third-party crates are absent from the reference checkout
  * (Cargo.lock pins rand 0.8.5, rand_core 0.6.4, cgmath 0.18.0): restated from the published
  * algorithms, unverifiable offline. */
 typedef struct { uint64_t s[4]; } Xo;

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device, an H100 (run with -m gpu)")
 
 
 # Collection order: the cheapest, most local checks first, so that a `-x` run stops at the real culprit (a broken kernel fails its

@@ -1,8 +1,8 @@
 """Writes the scene fixtures used by the tests and by bench.py.
 
-The GPU box has no /root/reference, so the scene PARAMETERS of the reference's shipped scenes are restated here
-(cited) and emitted as blub scene JSON (same schema as src/scene/mod.rs:19-43); `tests/test_host.py` checks them against
-/root/reference/scenes/*.json whenever that directory is present.  The synthetic scenes are the ones SURVEY.md section 0.1 /
+The scene PARAMETERS of the reference's shipped scenes are restated here (cited) and emitted as blub scene JSON (same schema as
+src/scene/mod.rs:19-43); `tests/test_host.py` checks them against the reference's scene files, stored unchanged under
+tests/golden/reference_scenes.  The synthetic scenes are the ones SURVEY.md section 0.1 /
 BASELINE.json ask for (256^3 with ~16M particles, 512^3 with ~64M).
 
     python tests/golden/make_scenes.py

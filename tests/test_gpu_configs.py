@@ -1,10 +1,10 @@
 """GPU parity on the configurations BASELINE.json names (SURVEY.md section 8, C2 / C3 / C5) -- oracle comparisons at full size, not only
 property checks:
 
-  C2  scenes/dam_halfhalf.json           128 x 64 x 64, 1,218,672 particles   (/root/reference/scenes/dam_halfhalf.json:13-19)
-  C3  scenes/dam_halfhalf_highres.json   256 x 128 x 128, 10,113,264 particles (/root/reference/scenes/dam_halfhalf_highres.json:13-19)
+  C2  scenes/dam_halfhalf.json           128 x 64 x 64, 1,218,672 particles   (reference scenes/dam_halfhalf.json:13-19)
+  C3  scenes/dam_halfhalf_highres.json   256 x 128 x 128, 10,113,264 particles (reference scenes/dam_halfhalf_highres.json:13-19)
   C5  the double-dam scene with a moving solid, stepped in Scene::step's order: animate, voxelize, step
-      (/root/reference/src/scene/mod.rs:192-213; the shipped meshes are git-LFS stubs, so the solid is the analytic box of bench.py)
+      (reference src/scene/mod.rs:192-213; the shipped meshes are git-LFS stubs, so the solid is the analytic box of bench.py)
 
 Each scene gets the stage-by-stage comparison of one step (all 14 stages, tests/stagewise.py) with the scene's own solver defaults, and a
 multi-step trajectory comparison under the converged-solver protocol of SURVEY 8(c).  The oracle needs seconds per step at these sizes

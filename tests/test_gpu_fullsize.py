@@ -1,4 +1,4 @@
-"""Full-size (BASELINE.json configs) property checks on the B200: things the oracle is too slow for."""
+"""Full-size (BASELINE.json configs) property checks on the H100: things the oracle is too slow for."""
 import numpy as np
 import pytest
 

@@ -135,7 +135,7 @@ def test_tma_tiled_pcg_matches_oracle(max_it, freq, tol):
                     assert e < tol / DT and np.abs(res).max() <= 1.02 * tol / DT + 1e-4, (e, np.abs(res).max())
         results[path] = gpu.download_grid(F.TAP_P_VEL)
         assert gpu.last_solve(0)[0] >= 0.0
-    if tol == 0.0:  # same arithmetic per cell; only the per-block partial sums are grouped differently (148 vs 592 blocks)
+    if tol == 0.0:  # same arithmetic per cell; only the per-block partial sums are grouped differently (the paths launch different numbers of blocks)
         grid_close(results[True], results["tma"], "tma vs register path", rel=2e-3, abs_=1e-4)
 
 

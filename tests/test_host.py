@@ -1,5 +1,5 @@
 """CPU-side tests: the C ABI library loads and exports every declared symbol, the scene loader reads blub scenes,
-fixtures match the reference's shipped scenes (when /root/reference is present).  No compute calls: no GPU here."""
+fixtures match the reference's shipped scenes (stored verbatim under tests/golden/reference_scenes).  No compute calls: no GPU here."""
 import json
 import os
 import re
@@ -12,6 +12,7 @@ from blub_b200 import fluid as F
 from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF_SCENES = os.path.join(util.HERE, "golden", "reference_scenes")  # the reference's scenes/*.json, unchanged
 
 
 def declared_symbols():
@@ -26,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     assert len(syms) >= 25
     for s in syms:
         assert hasattr(L, s), f"{s} declared in include/blub_fluid.h but not exported"
-    assert b"sm_100a" in L.blub_version()
+    assert b"sm_90a" in L.blub_version()
 
 
 def test_ctypes_mirror_binds_every_declared_symbol():
@@ -97,22 +98,22 @@ def test_scene_loader_errors(tmp_path, text):
         blub_b200.scene_info(str(tmp_path / "missing.json"))
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/scenes"), reason="reference checkout not present")
 def test_fixtures_match_reference_scenes():
     for name in ["single_cell_debug", "dam_halfhalf", "dam_halfhalf_highres", "filled_basin"]:
-        ref = json.load(open(f"/root/reference/scenes/{name}.json"))
+        ref = json.load(open(os.path.join(REF_SCENES, name + ".json")))
         mine = json.load(open(util.scene_path(name)))
         assert ref["fluid"] == mine["fluid"] and ref["gravity"] == mine["gravity"], name
-    ref = json.load(open("/root/reference/scenes/double_dam_wgpulogo.json"))  # config C5's fluid, without the LFS-stub mesh
+    ref = json.load(open(os.path.join(REF_SCENES, "double_dam_wgpulogo.json")))  # config C5's fluid, without the LFS-stub mesh
     mine = json.load(open(util.scene_path("double_dam")))
     assert ref["fluid"] == mine["fluid"] and ref["gravity"] == mine["gravity"]
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/scenes"), reason="reference checkout not present")
 def test_loader_reads_every_reference_scene_unchanged():
-    for fn in sorted(os.listdir("/root/reference/scenes")):
-        info = blub_b200.scene_info(os.path.join("/root/reference/scenes", fn))
-        ref = json.load(open(os.path.join("/root/reference/scenes", fn)))
+    names = sorted(os.listdir(REF_SCENES))
+    assert len(names) == 14, names
+    for fn in names:
+        info = blub_b200.scene_info(os.path.join(REF_SCENES, fn))
+        ref = json.load(open(os.path.join(REF_SCENES, fn)))
         d = ref["fluid"]["grid_dimension"]
         assert tuple(info.grid_dimension) == (d["x"], d["y"], d["z"]), fn
         assert info.num_fluid_cubes == len(ref["fluid"]["fluid_cubes"]), fn

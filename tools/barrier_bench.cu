@@ -1,13 +1,13 @@
-// barrier_bench.cu -- what does one "grid-wide sum" cost on a B200?  (tools/gpu_session.sh barrier)
+// barrier_bench.cu -- what does one "grid-wide sum" cost on an H100?  (tools/gpu_session.sh barrier)
 //
 // The persistent PCG solver needs two grid-wide reductions per iteration.  With the fluid working set in L2 the solve is bound by
-// their latency (profiles/r02_s6_pcg_overhead.md: ~8 us per phase with no work at all), so the candidates are timed in isolation:
-//   cg592     cooperative_groups grid.sync() + every block re-reads all partials       (what the solver did in round 1)
-//   flat592   monotonic arrival counter (one atomic per block, acquire spin by thread 0) + every block re-reads all partials
-//   flat148   the same with 148 blocks of 1024 threads
-//   two592    two-level: blocks sharing an SM-sized group of 4 first meet on a group counter, the last of a group arrives globally;
-//             the group's partials are pre-added by that last block, so that 148 instead of 592 partials are re-read
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o barrier_bench barrier_bench.cu     Run: ./barrier_bench
+// their latency, so the candidates are timed in isolation (#SM = 132 on an H100 SXM):
+//   cg4       cooperative_groups grid.sync() + every block re-reads all partials       (what the solver did in round 1)
+//   flat4     monotonic arrival counter (one atomic per block, acquire spin by thread 0) + every block re-reads all partials
+//   flat1     the same with #SM blocks of 1024 threads
+//   two4      two-level: blocks sharing an SM-sized group of 4 first meet on a group counter, the last of a group arrives globally;
+//             the group's partials are pre-added by that last block, so that #SM instead of 4 x #SM partials are re-read
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o barrier_bench barrier_bench.cu     Run: ./barrier_bench
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
@@ -219,17 +219,17 @@ int main() {
     auto reset = [&] { CHECK(cudaMemset(counters, 0, 4096 * sizeof(unsigned))); };
     {
         const int blocks = sms * 4;
-        time_it("cg592", blocks, 256, iters, [&](int n) {
+        time_it("cg4", blocks, 256, iters, [&](int n) {
             void *args[] = {&partials, &n, &out};
             CHECK(cudaLaunchCooperativeKernel((const void *)k_cg<256>, dim3(blocks), dim3(256), args, 0, 0));
         });
-        time_it("flat592", blocks, 256, iters, [&](int n) {
+        time_it("flat4", blocks, 256, iters, [&](int n) {
             reset();
             unsigned *c = counters;
             void *args[] = {&partials, &c, &n, &out};
             CHECK(cudaLaunchCooperativeKernel((const void *)k_flat<256>, dim3(blocks), dim3(256), args, 0, 0));
         });
-        time_it("two592", blocks, 256, iters, [&](int n) {
+        time_it("two4", blocks, 256, iters, [&](int n) {
             reset();
             unsigned *gc = counters + 8, *c = counters;
             void *args[] = {&partials, &gpart, &gc, &c, &n, &out};
@@ -271,11 +271,11 @@ int main() {
     }
     {
         const int blocks = sms;
-        time_it("cg148", blocks, 1024, iters, [&](int n) {
+        time_it("cg1", blocks, 1024, iters, [&](int n) {
             void *args[] = {&partials, &n, &out};
             CHECK(cudaLaunchCooperativeKernel((const void *)k_cg<1024>, dim3(blocks), dim3(1024), args, 0, 0));
         });
-        time_it("flat148", blocks, 1024, iters, [&](int n) {
+        time_it("flat1", blocks, 1024, iters, [&](int n) {
             reset();
             unsigned *c = counters;
             void *args[] = {&partials, &c, &n, &out};

@@ -53,7 +53,7 @@ if want multi2; then        # needs gpurun --gpus 2: the multi-GPU tests, per-st
     SANITIZE_TIMEOUT=400 bash tools/sanitize.sh slab 2>&1 | tee $OUT/session_sanitize_slab.txt | tail -12
 fi
 if want barrier; then       # cost of one grid-wide sum, candidates in isolation (tools/barrier_bench.cu; built here if the binary did not travel)
-    [ -x tools/barrier_bench ] || nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/barrier_bench tools/barrier_bench.cu
+    [ -x tools/barrier_bench ] || nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/barrier_bench tools/barrier_bench.cu
     ./tools/barrier_bench > $OUT/session_barrier.txt 2>&1; cat $OUT/session_barrier.txt
 fi
 if want sanitize; then
@@ -85,7 +85,7 @@ if want blubrun; then
     tail -2 $OUT/session_run.txt
 fi
 if want matchab; then       # warp aggregation of the scatter kernels: peer groups (match.any, default) against adjacent runs; cost of MATCH.ANY itself
-    [ -x tools/match_bench ] || nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/match_bench tools/match_bench.cu
+    [ -x tools/match_bench ] || nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/match_bench tools/match_bench.cu
     ./tools/match_bench > $OUT/session_match_bench.txt 2>&1; cat $OUT/session_match_bench.txt
     BLUB_SCATTER_AGG=adjacent python tools/profile_targets.py stages dam_256 3 56 110 > $OUT/session_timeline_agg_adjacent.txt 2>&1
     echo "== adjacent runs"; grep -E "after|p2g|density_gather|advect|correct|binning|total|Error|error" $OUT/session_timeline_agg_adjacent.txt

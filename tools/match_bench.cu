@@ -1,5 +1,5 @@
-// Cost of match.any.sync (SASS MATCH.ANY) next to SHFL and REDG on sm_100a: the scatter kernels find the lanes that share a dual cell with it.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/match_bench tools/match_bench.cu && ./tools/match_bench
+// Cost of match.any.sync (SASS MATCH.ANY) next to SHFL and REDG on sm_90a: the scatter kernels find the lanes that share a dual cell with it.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/match_bench tools/match_bench.cu && ./tools/match_bench
 // Prints SM cycles per warp-instruction with all warps of a full grid issuing back to back (throughput), for key patterns with 1 .. 32 distinct
 // values per warp, and the same loop with one SHFL.IDX instead.
 #include <cstdio>
@@ -24,9 +24,9 @@ __global__ void k(int distinct, int iters, unsigned *out, long long *cycles) {
 }
 
 int main() {
-    const int blocks = 148 * 4, threads = 256, iters = 4096;
+    const int blocks = 132 * 4, threads = 256, iters = 4096;
     unsigned *out;
-    long long *cyc, h[148 * 4];
+    long long *cyc, h[132 * 4];  // four blocks on each of the 132 SMs of an H100 SXM
     cudaMalloc(&out, blocks * threads * sizeof(unsigned));
     cudaMalloc(&cyc, blocks * sizeof(long long));
     auto run = [&](const char *name, int mode, int distinct) {

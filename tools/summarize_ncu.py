@@ -1,7 +1,7 @@
-"""Turns ncu outputs (brought back in gpurun_out/) into the small text summaries kept under profiles/.
+"""Turns Nsight Compute outputs (CSV launch lists, .ncu-rep reports) into small text summaries for profiles/.
 
-    python tools/summarize_ncu.py launches gpurun_out/launches_step_v1.csv > profiles/r01_v1_launches_step.md
-    python tools/summarize_ncu.py report gpurun_out/pcg_v1.ncu-rep > profiles/r01_v1_pcg_kernels.md
+    python tools/summarize_ncu.py launches launches_step.csv > profiles/launches_step.md
+    python tools/summarize_ncu.py report pcg.ncu-rep > profiles/pcg_kernels.md
 """
 import collections
 import csv
@@ -67,7 +67,7 @@ def report(path):
 
 
 def traffic(path):
-    """dram bytes of the persistent PCG solve kernel -> profiles/pcg_traffic.json (read by bench.py as roofline.traffic)."""
+    """dram bytes of the persistent PCG solve kernel, as JSON."""
     import json
 
     raw = subprocess.run(["ncu", "-i", path, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

@@ -1,6 +1,6 @@
 """Which work unit should the sparse PCG kernel hand out?  For marker volumes of a dam break (here: generated with the CPU oracle,
 tools have no GPU), count for several unit shapes how many units hold fluid, how many sequential passes a persistent grid of
-592 blocks x 8 warps needs per phase, and how full the processed units are.
+BLOCKS blocks x 8 warps needs per phase, and how full the processed units are.
 
     python tools/work_units.py markers.npz        # arrays m<step> of shape [nz, ny, nx], FLUID = 1
 """
@@ -8,8 +8,9 @@ import sys
 
 import numpy as np
 
-SHAPES = [("tile 128x8x4 / block", (128, 8, 4), 592), ("brick 32x8x4 / 2 warps", (32, 8, 4), 592 * 4), ("brick 32x4x4 / warp", (32, 4, 4), 592 * 8),
-          ("brick 64x2x4 / warp", (64, 2, 4), 592 * 8), ("brick 128x1x4 / warp (row)", (128, 1, 4), 592 * 8), ("brick 16x8x4 / warp", (16, 8, 4), 592 * 8)]
+BLOCKS = 132 * 3  # the column solver's grid on an H100 SXM: three resident blocks on each of 132 SMs
+SHAPES = [("tile 128x8x4 / block", (128, 8, 4), BLOCKS), ("brick 32x8x4 / 2 warps", (32, 8, 4), BLOCKS * 4), ("brick 32x4x4 / warp", (32, 4, 4), BLOCKS * 8),
+          ("brick 64x2x4 / warp", (64, 2, 4), BLOCKS * 8), ("brick 128x1x4 / warp (row)", (128, 1, 4), BLOCKS * 8), ("brick 16x8x4 / warp", (16, 8, 4), BLOCKS * 8)]
 
 
 def main(path):

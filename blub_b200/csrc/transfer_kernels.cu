@@ -9,9 +9,13 @@
 //
 //   * P2G SCATTER (default; the form z-slab ranks always use): one thread per particle; the lanes of a warp that share a dual cell -- found
 //     with match.any, adjacent or not -- add their contributions up in groups of four with two shuffle steps, and the lowest lane of a
-//     group adds (sum w*value, sum w) of each face into 64-bit fixed-point accumulators with integer atomics: 10.7 faces per particle instead
-//     of 24 (17.8 with runs of adjacent lanes only), and sums that do not depend on the arrival order of the atomics (deterministic).
-//     A sparse finish pass normalises and puts the accumulators back to zero (no memsets, no dense pass).
+//     group forms (sum w*value, sum w) of each face as 64-bit fixed-point integers: 10.7 faces per particle instead of 24 (17.8 with runs
+//     of adjacent lanes only).  A block walks chunks of 256 consecutive (cell-sorted) particles and adds the faces inside the chunk's
+//     window into a shared-memory tile with 32-bit atomics (low / high words), then flushes each touched tile word with ONE global
+//     64-bit reduction; faces outside the window go to the global volume directly.  ~6 global reductions per particle instead of ~21, and
+//     sums that do not depend on the arrival order of the atomics or on the split between tile and global path (deterministic).
+//     A sparse finish pass normalises and puts the accumulators back to zero (no memsets, no dense pass).  The density scatter is tiled
+//     the same way.
 //   * CELL LISTS (gather form and binning): a counting sort of particle INDICES by primal cell -- count (one integer atomic per particle),
 //     exclusive scan, fill, and a canonicalisation (rank counting) that puts every cell's slice into ascending particle index.  The
 //     lists are therefore a pure function of the particle array: the same input gives the same lists, run after run, whatever
@@ -686,15 +690,92 @@ __device__ __forceinline__ bool warp_group_sum(int key, float (&v)[NV]) {
     return MATCH ? matched_group_sum<NV>(key, v) : segmented_run_sum<NV>(key, v);
 }
 
+// ---- block-private accumulator tiles of the scatters
+// A block walks chunks of PT consecutive particles (warp k of a chunk still owns particles 32k .. 32k + 31, so the warp peer groups and
+// the integers formed per group and face are those of a plain one-thread-per-particle launch).  Particles are re-sorted into x-fastest
+// primal-cell order every few steps, so a chunk covers a short run of x-adjacent cells in one or two rows and its faces fall into a small
+// box: the group heads add the faces that lie inside the chunk's box (its WINDOW) into a shared-memory tile, and after the chunk every
+// non-zero tile word goes out as ONE global 64-bit reduction -- 5.7 global reductions per particle instead of 19-21 on a sorted dam
+// break, 8.8 instead of 25 after the order has decayed (tools/red_stats.py).  Faces outside the window (a far-off particle, a decayed or
+// unsorted order) take the global path directly, decided per face: slower, never wrong.
+//
+// The tile words are 32-bit: a 64-bit shared atomicAdd compiles to a CAS loop on sm_90a, a 32-bit one to a native ATOMS.ADD.  A 64-bit
+// sum is kept as a low word and a high word; the add that wraps the low word carries into the high one, so (hi << 32) | lo is the sum
+// modulo 2^64 whatever the order of arrival -- and the global sums, integer adds modulo 2^64 too, come out bit for bit as without tile.
+struct TileWindow {
+    int ox, oy, oz; // face (x, y, z) of tile entry 0
+    int ex, ey, ez; // extent; ex * ey * ez <= the tile's capacity (ex may be 0: no tile)
+};
+__device__ __forceinline__ void tile_add(uint32_t *lo, uint32_t *hi, long long q) {
+    const uint32_t ql = (uint32_t)q;
+    const uint32_t old = atomicAdd(lo, ql);
+    const uint32_t h = (uint32_t)((unsigned long long)q >> 32) + (old + ql < old ? 1u : 0u);
+    if (h != 0u) atomicAdd(hi, h);
+}
+__device__ __forceinline__ long long tile_word(const uint32_t *lo, const uint32_t *hi) {
+    return (long long)(((unsigned long long)*hi << 32) | *lo);
+}
+// The window of the chunk starting at particle b, from the primal cells of its particles (every thread of the block calls this, `cell`
+// of its own particle, `valid` whether it has one).  It covers the faces [min - 1, max + 1] of those cells in every dimension, which
+// holds every face they reach; a box of more than CAP faces is cut -- z first, then y (neither below 3 faces), then x -- around the
+// cell of the chunk's middle particle, so that one far-off particle does not push the others out.  Ends with __syncthreads().
+template <int CAP>
+__device__ __forceinline__ TileWindow scatter_window(uint32_t b, uint32_t np, bool valid, int3 cell, int (*scratch)[8], TileWindow *shared_win) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int big = 0x3fffffff;
+    const int mnx = __reduce_min_sync(0xffffffffu, valid ? cell.x : big), mxx = __reduce_max_sync(0xffffffffu, valid ? cell.x : -big);
+    const int mny = __reduce_min_sync(0xffffffffu, valid ? cell.y : big), mxy = __reduce_max_sync(0xffffffffu, valid ? cell.y : -big);
+    const int mnz = __reduce_min_sync(0xffffffffu, valid ? cell.z : big), mxz = __reduce_max_sync(0xffffffffu, valid ? cell.z : -big);
+    if (lane == 0) {
+        scratch[warp][0] = mnx; scratch[warp][1] = mny; scratch[warp][2] = mnz;
+        scratch[warp][3] = mxx; scratch[warp][4] = mxy; scratch[warp][5] = mxz;
+    }
+    const uint32_t n = min(np - b, (uint32_t)PT); // b < np
+    if (threadIdx.x == n / 2) { scratch[PT / 32][0] = cell.x; scratch[PT / 32][1] = cell.y; scratch[PT / 32][2] = cell.z; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int lo[3], hi[3], e[3];
+        for (int d = 0; d < 3; ++d) {
+            lo[d] = big; hi[d] = -big;
+            for (int w = 0; w < PT / 32; ++w) { lo[d] = min(lo[d], scratch[w][d]); hi[d] = max(hi[d], scratch[w][3 + d]); }
+            lo[d] -= 1; hi[d] += 1;
+            e[d] = hi[d] - lo[d] + 1;
+        }
+        e[2] = min(e[2], max(3, CAP / (e[0] * e[1])));
+        e[1] = min(e[1], max(3, CAP / (e[0] * e[2])));
+        e[0] = min(e[0], CAP / (e[1] * e[2]));
+        int o[3];
+        for (int d = 0; d < 3; ++d) o[d] = min(max(scratch[PT / 32][d] - e[d] / 2, lo[d]), hi[d] - e[d] + 1);
+        *shared_win = TileWindow{o[0], o[1], o[2], e[0], e[1], e[2]};
+    }
+    __syncthreads();
+    return *shared_win;
+}
+// tile entry of face (x, y, z), or -1 outside the window
+__device__ __forceinline__ int tile_entry(const TileWindow &w, int x, int y, int z) {
+    const int rx = x - w.ox, ry = y - w.oy, rz = z - w.oz;
+    return ((unsigned)rx < (unsigned)w.ex && (unsigned)ry < (unsigned)w.ey && (unsigned)rz < (unsigned)w.ez) ? (rz * w.ey + ry) * w.ex + rx : -1;
+}
+// global cell index of tile entry t
+__device__ __forceinline__ int tile_cell(const GridDim &g, const TileWindow &w, int t) {
+    const int q = t / w.ex;
+    return lin(g, w.ox + (t - q * w.ex), w.oy + q % w.ey, w.oz + q / w.ey);
+}
+
+// P2G tile: per face 3 components x {sum w * value, sum w} x {low, high} words, word planes of P2G_TILE entries
+constexpr int P2G_TILE = 1184;
+constexpr int P2G_TILE_BYTES = 12 * P2G_TILE * 4; // 56,832 B: with the 1 KB the hardware reserves per block, 4 blocks fit into 228 KB
+constexpr int DENSITY_TILE = 2048;                // density tile: {low, high} word planes (16 KB)
+
 template <bool MARK, bool MATCH>
-__device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
+__device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float3 p,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
                                                          const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
-                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker) {
+                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker, const TileWindow &win,
+                                                         uint32_t *__restrict__ tile) {
     const uint32_t np = params->num_particles;
     if ((i & ~31u) >= np) return;  // whole warp beyond the last particle (z-slab ranks launch over their capacity)
     const bool valid = i < np;     // no per-lane early return: every lane of a live warp takes part in the shuffles
-    const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 1.0f);
     if (MARK && valid) marker[cell_of_position(g, p)] = (int8_t)CELL_FLUID; // transfer_build_linkedlist.comp:17-19
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 rows[3] = {valid ? rowx[i] : zero, valid ? rowy[i] : zero, valid ? rowz[i] : zero};
@@ -721,30 +802,68 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
         }
         const bool head = warp_group_sum<MATCH, 16>(valid ? base : -1 - (int)(threadIdx.x & 31), acc);
         if (head && valid) {
+            uint32_t *const t = tile + 4 * c * P2G_TILE; // planes: value low, value high, weight low, weight high
 #pragma unroll
             for (int k = 0; k < 8; ++k)
             {
                 // a contribution whose weight rounds to 0 is left out entirely (value too), so a face with weight 0 also has value 0
                 const long long wq = to_fixed<FIXED_WEIGHT_BITS>(acc[2 * k + 1]);
                 if (wq > 0) {
-                    longlong2 *const f = nw[c] + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz;
                     const long long num = to_fixed<FIXED_VALUE_BITS>(acc[2 * k]);
-                    if (num != 0) fixed_add(&f->x, num);
-                    fixed_add(&f->y, wq);
+                    const int e = tile_entry(win, dx + (k & 1), dy + ((k >> 1) & 1), dz + (k >> 2));
+                    if (e >= 0) {
+                        if (num != 0) tile_add(t + e, t + P2G_TILE + e, num);
+                        tile_add(t + 2 * P2G_TILE + e, t + 3 * P2G_TILE + e, wq);
+                    } else {
+                        longlong2 *const f = nw[c] + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz;
+                        if (num != 0) fixed_add(&f->x, num);
+                        fixed_add(&f->y, wq);
+                    }
                 }
             }
         }
     }
 }
-// 4 resident blocks per SM (64 registers, no spills for sm_90a); a 5 / 6-block bound (48 / 40 registers) spills
+// 4 resident blocks per SM (64 registers, no spills for sm_90a; P2G_TILE_BYTES of dynamic shared memory); a 5 / 6-block bound
+// (48 / 40 registers) spills
 template <bool MARK, bool MATCH>
 __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
                                                          const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
                                                          longlong2 *__restrict__ nwz, int8_t *__restrict__ marker) {
-    // a bounded grid strides over the particles: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
+    extern __shared__ uint32_t tile[]; // [12][P2G_TILE]
+    __shared__ int scratch[PT / 32 + 1][8];
+    __shared__ TileWindow shared_win;
+    longlong2 *const nw[3] = {nwx, nwy, nwz};
+    // a bounded grid strides over the chunks: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
-    for (uint32_t i = blockIdx.x * PT + threadIdx.x; (i & ~31u) < np_; i += gridDim.x * PT) p2g_scatter_kernel_one<MARK, MATCH>(i, g, params, pos, rowx, rowy, rowz, nwx, nwy, nwz, marker);
+    for (uint32_t b = blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
+        const uint32_t i = b + threadIdx.x;
+        const bool valid = i < np_;
+        const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 1.0f);
+        const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
+        const TileWindow win = scatter_window<P2G_TILE>(b, np_, valid, cell, scratch, &shared_win);
+        const int size = win.ex * win.ey * win.ez;
+        for (int t = threadIdx.x; t < size; t += PT)
+#pragma unroll
+            for (int k = 0; k < 12; ++k) tile[k * P2G_TILE + t] = 0u;
+        __syncthreads();
+        p2g_scatter_kernel_one<MARK, MATCH>(i, g, params, p, rowx, rowy, rowz, nwx, nwy, nwz, marker, win, tile);
+        __syncthreads();
+        // flush: one global reduction per non-zero word; the next chunk's window is set up behind a barrier (scatter_window)
+        for (int t = threadIdx.x; t < size; t += PT) {
+            int cell_index = -1;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const uint32_t *const tc = tile + 4 * c * P2G_TILE + t;
+                const long long num = tile_word(tc, tc + P2G_TILE), wq = tile_word(tc + 2 * P2G_TILE, tc + 3 * P2G_TILE);
+                if (num == 0 && wq == 0) continue;
+                if (cell_index < 0) cell_index = tile_cell(g, win, t);
+                if (num != 0) fixed_add(&nw[c][cell_index].x, num);
+                if (wq != 0) fixed_add(&nw[c][cell_index].y, wq);
+            }
+        }
+    }
 }
 
 // Normalisation + global forces + "don't flow into solid" for the scatter form: transfer_gather_velocity.comp:116-127 -- and the
@@ -811,14 +930,13 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
 
 // ------------------------------------------------------------------------------------------------ density projection
 // Scatter counterpart of density_projection_gather_error.comp:41-97: dual cell d = trunc(pos - 0.5), cell centres d + {0,1}^3;
-// warp-aggregated like the P2G scatter.
+// warp-aggregated and tiled like the P2G scatter.
 template <bool MATCH>
-__device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
-                                                             long long *__restrict__ density) {
+__device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float3 p,
+                                                             long long *__restrict__ density, const TileWindow &win, uint32_t *__restrict__ tile) {
     const uint32_t np = params->num_particles;
     if ((i & ~31u) >= np) return; // whole warp beyond the last particle
     const bool valid = i < np;
-    const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
     const int dx = (int)(p.x - 0.5f), dy = (int)(p.y - 0.5f), dz = (int)(p.z - 0.5f);
     const float qx = (float)dx + 0.5f, qy = (float)dy + 0.5f, qz = (float)dz + 0.5f;
     const float wx[2] = {saturatef(1.0f - fabsf(qx - p.x)), saturatef(1.0f - fabsf(qx + 1.0f - p.x))};
@@ -832,15 +950,38 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
     if (head && valid) {
 #pragma unroll
         for (int k = 0; k < 8; ++k)
-            if (acc[k] > 0.0f) fixed_add(density + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz, to_fixed<FIXED_WEIGHT_BITS>(acc[k]));
+            if (acc[k] > 0.0f) {
+                const long long q = to_fixed<FIXED_WEIGHT_BITS>(acc[k]);
+                const int e = tile_entry(win, dx + (k & 1), dy + ((k >> 1) & 1), dz + (k >> 2));
+                if (e >= 0) tile_add(tile + e, tile + DENSITY_TILE + e, q);
+                else fixed_add(density + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz, q);
+            }
     }
 }
 template <bool MATCH>
 __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                              long long *__restrict__ density) {
-    // a bounded grid strides over the particles: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
+    __shared__ uint32_t tile[2 * DENSITY_TILE]; // low words, high words
+    __shared__ int scratch[PT / 32 + 1][8];
+    __shared__ TileWindow shared_win;
+    // a bounded grid strides over the chunks: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
-    for (uint32_t i = blockIdx.x * PT + threadIdx.x; (i & ~31u) < np_; i += gridDim.x * PT) density_scatter_kernel_one<MATCH>(i, g, params, pos, density);
+    for (uint32_t b = blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
+        const uint32_t i = b + threadIdx.x;
+        const bool valid = i < np_;
+        const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
+        const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
+        const TileWindow win = scatter_window<DENSITY_TILE>(b, np_, valid, cell, scratch, &shared_win);
+        const int size = win.ex * win.ey * win.ez;
+        for (int t = threadIdx.x; t < size; t += PT) tile[t] = tile[DENSITY_TILE + t] = 0u;
+        __syncthreads();
+        density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
+        __syncthreads();
+        for (int t = threadIdx.x; t < size; t += PT) { // flush, as in p2g_scatter_kernel
+            const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
+            if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
+        }
+    }
 }
 
 // density_projection_gather_error.comp:99-199
@@ -919,6 +1060,11 @@ void configure_transfer_kernels() {
     BLUB_CUDA_CHECK(cudaFuncSetAttribute(p2g_gather_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GATHER_SMEM_BYTES));
     BLUB_CUDA_CHECK(cudaFuncSetAttribute(p2g_gather_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GATHER_SMEM_BYTES));
     BLUB_CUDA_CHECK(cudaFuncSetAttribute(p2g_gather_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GATHER_SMEM_BYTES));
+    // the P2G scatter tile: the whole shared-memory carveout, so that 4 blocks of P2G_TILE_BYTES are resident per SM
+    for (const auto kernel : {p2g_scatter_kernel<true, true>, p2g_scatter_kernel<true, false>}) {
+        BLUB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, P2G_TILE_BYTES));
+        BLUB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
 }
 
 
@@ -958,7 +1104,7 @@ void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *par
         for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(nw[c], 0, (size_t)g.n * sizeof(longlong2), st));
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? p2g_scatter_kernel<true, true> : p2g_scatter_kernel<true, false>;
-    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker);
+    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, P2G_TILE_BYTES, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker);
 }
 
 void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,

@@ -7,6 +7,8 @@ tests/test_variants_emulated.py feeds positions of the CPU oracle's dam break, r
 
 Schemes: none = one reduction per (particle, face); adjacent4 = runs of adjacent lanes with the same dual cell, cut into groups of four
 (segmented_run_sum); match4 / match8 / matchall = all lanes of the warp with the same dual cell (matched_group_sum), groups of 4 / 8 / any size.
+tiled_global_reductions: what is left of the match4 reductions for the global volumes once a block adds a chunk's faces up in a
+shared-memory tile first (p2g_scatter_kernel / density_scatter_kernel).
 """
 import sys
 
@@ -44,6 +46,69 @@ def reductions_per_particle(p, nx, ny, comps=(0, 1, 2)):
     return {a: 8.0 * b / m for a, b in tot.items()}
 
 
+def chunk_windows(cells, cap):
+    """The tile window of every chunk, as p2g_scatter_kernel / density_scatter_kernel pick it (scatter_window in transfer_kernels.cu).
+    cells: [chunks, ch, 3] primal cells (x, y, z) of the chunk's particles, -1 for slots past the last particle.  The box covers the faces
+    [min - 1, max + 1] of the chunk's cells in every dimension; a box larger than `cap` faces is cut, z first, then y (neither below 3), then x,
+    around the cell of the chunk's middle particle.  Returns (origin, extent), [chunks, 3] each."""
+    valid = cells[:, :, 0] >= 0
+    n = valid.sum(axis=1)
+    big = np.iinfo(np.int64).max
+    mn = np.where(valid[:, :, None], cells, big).min(axis=1)
+    mx = np.where(valid[:, :, None], cells, -1).max(axis=1)
+    anchor = cells[np.arange(len(cells)), n // 2]
+    lo, hi = mn - 1, mx + 1
+    e = hi - lo + 1
+    ex, ey, ez = e[:, 0].copy(), e[:, 1].copy(), e[:, 2].copy()
+    ez = np.minimum(ez, np.maximum(3, cap // (ex * ey)))
+    ey = np.minimum(ey, np.maximum(3, cap // (ex * ez)))
+    ex = np.minimum(ex, cap // (ey * ez))
+    ext = np.stack([ex, ey, ez], axis=1)
+    origin = np.clip(anchor - ext // 2, lo, hi - ext + 1)
+    return origin, ext
+
+
+def tiled_global_reductions(p, nx, ny, ch, cap, comps=(0, 1, 2)):
+    """Global 64-bit reductions per particle of the tiled scatter: chunks of `ch` consecutive particles share a block-private tile of at most
+    `cap` faces (chunk_windows).  A peer-group head (match4) adds a face that lies inside its chunk's window into the tile, any other face
+    straight into the global volume; after the chunk every touched tile entry is flushed by one global reduction per word.  Words per face:
+    2 for the velocity components (sum w * value, sum w), 1 for the density.  Returns (total, of which flushes, of which outside the window)."""
+    nz_max = int(p[:, 2].max()) + 2
+    m = len(p) // 32 * 32
+    nchunk = (m + ch - 1) // ch
+    lo = 0.5 if comps == (3,) else 1.0
+    q = np.maximum(p[:m].astype(np.float32), np.float32(lo))  # simulated particles never reach the upper clamp plane
+    cells = np.full((nchunk * ch, 3), -1, np.int64)
+    cells[:m] = q.astype(np.int64)
+    origin, ext = chunk_windows(cells.reshape(nchunk, ch, 3), cap)
+    chunk = np.arange(m) // ch
+    words = 1 if comps == (3,) else 2
+    outside = flushed = 0
+    idx = np.arange(32)[None, :]
+    for c in comps:
+        off = np.full(3, 0.5, np.float32)
+        if c < 3:
+            off[c] = 1.0
+        d = (q - off).astype(np.int64)
+        k = (d[:, 0] + nx * (d[:, 1] + ny * d[:, 2])).reshape(-1, 32)
+        ks, perm = np.sort(k, axis=1), np.argsort(k, axis=1, kind="stable")
+        st = np.ones_like(ks, bool)
+        st[:, 1:] = ks[:, 1:] != ks[:, :-1]
+        r = idx - np.maximum.accumulate(np.where(st, idx, 0), axis=1)
+        head = np.zeros_like(k, bool)
+        np.put_along_axis(head, perm, (r & 3) == 0, axis=1)
+        h = np.flatnonzero(head.reshape(-1))
+        keys = []
+        for o in range(8):
+            f = d[h] + np.array([o & 1, (o >> 1) & 1, o >> 2])
+            rel = f - origin[chunk[h]]
+            inside = ((rel >= 0) & (rel < ext[chunk[h]])).all(axis=1)
+            outside += int((~inside).sum()) * words
+            keys.append((chunk[h][inside] * nz_max + f[inside, 2]) * ny * nx + f[inside, 1] * nx + f[inside, 0])
+        flushed += len(np.unique(np.concatenate(keys))) * words
+    return (outside + flushed) / m, flushed / m, outside / m
+
+
 def sort_by_primal_cell(p, order, nx, ny):
     """the stable counting sort of the binning stage: x-fastest cell order, ascending previous index inside a cell"""
     ci = p.astype(np.int32)
@@ -56,3 +121,6 @@ if __name__ == "__main__":
     for key in data.files:
         v, d = reductions_per_particle(data[key], nx, ny), reductions_per_particle(data[key], nx, ny, comps=(3,))
         print(key, "P2G", " ".join(f"{a} {b:.2f}" for a, b in v.items()), "| density", " ".join(f"{a} {b:.2f}" for a, b in d.items()))
+        # the kernels' chunk and tile sizes (PT, P2G_TILE, DENSITY_TILE in transfer_kernels.cu)
+        tv, td = tiled_global_reductions(data[key], nx, ny, 256, 1184), tiled_global_reductions(data[key], nx, ny, 256, 2048, comps=(3,))
+        print(key, "tiled global reductions per particle: P2G %.2f (flush %.2f + outside %.2f) | density %.2f (flush %.2f + outside %.2f)" % (tv + td))

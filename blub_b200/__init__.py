@@ -14,6 +14,7 @@ from .fluid import (  # noqa: F401
     lib,
     lib_path,
     scene_info,
+    state_info,
 )
 
-__all__ = ["HybridFluid", "SolverConfig", "BlubError", "DT_120HZ", "lib", "lib_path", "scene_info", "kernel_launch_count"]
+__all__ = ["HybridFluid", "SolverConfig", "BlubError", "DT_120HZ", "lib", "lib_path", "scene_info", "state_info", "kernel_launch_count"]

@@ -11,7 +11,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libblubcore.so")
-SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "c_api.cpp"]
+SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
+           "c_api.cpp"]
 # the mesh voxelizer shares its arithmetic with a host twin and a NumPy restatement: no FMA contraction, so that all three agree bit for bit
 EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"]}
 HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "voxelize_core.hpp", os.path.join("..", "..", "include", "blub_fluid.h")]
@@ -45,7 +46,7 @@ def build(force=False, verbose=False):
             subprocess.check_call(cmd)
             rebuilt = True
     if rebuilt or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart", "-lz"]  # zlib: CRC-32 of the state file
         if verbose:
             print(" ".join(cmd), flush=True)
         subprocess.check_call(cmd)

@@ -136,6 +136,10 @@ class PressureSolver {
     bool tma_available() const { return tma_blocks_ > 0; }
     bool columns_available() const { return column_blocks_ > 0; }
     bool persistent_available() const { return persistent_blocks_ > 0; }
+    // the value of blub_fluid_set_solver_path that selects the flags above (0, 1, 2, 4 or 6); set_path throws std::invalid_argument
+    // on a request that cannot be met and then changes nothing
+    int path() const { return !use_persistent ? 0 : use_tma ? 2 : use_dense ? 4 : use_columns ? 1 : 6; }
+    void set_path(int path);
 
   private:
     void *tma_maps_ = nullptr;       // PcgTmaMaps (tensor maps of r, s0, s1, codes)
@@ -191,6 +195,13 @@ class HybridFluid {
     void invalidate_graphs() { destroy_graphs(); }
     void set_transfer_path(int scatter);
     void marker_written_externally() { fluid_bits_stale_ = true; }
+    // number of whole steps taken (drives the rebinning cadence)
+    uint32_t step_count() const { return step_counter_; }
+    // Checkpoint / restart (state_file.cpp, format in DESIGN.md §8).  save_state synchronises, then writes everything a later step
+    // depends on to `path` atomically; it refuses z-slab ranks and a fluid left inside a step by step_stages (std::invalid_argument).
+    void save_state(const std::string &path);
+    // a new fluid whose next step is bit for bit the step the saved fluid would have taken next (same library build, same GPU model)
+    static std::unique_ptr<HybridFluid> load_state(const std::string &path, int device, cudaStream_t stream);
 
     Quirks quirks;
 
@@ -260,6 +271,7 @@ class HybridFluid {
     };
     GraphRolesAfter graph_roles_after_[2][2][2][2] = {};
     bool capturing_ = false;
+    bool mid_step_ = false; // the last step_stages call did not end at stage 14: the fluid is inside a step and cannot be saved
 
     GridDim grid_;
     int device_;
@@ -296,6 +308,20 @@ class HybridFluid {
     uint32_t step_param_slot_ = 0;
     cudaEvent_t param_events_[64] = {};
 };
+
+// Errors of the state file reader / writer: IoError = the file cannot be opened, written or read (BLUB_ERR_IO); ParseError = it is not a
+// valid state file of this format version (BLUB_ERR_PARSE).
+struct IoError : std::runtime_error {
+    explicit IoError(const std::string &what) : std::runtime_error(what) {}
+};
+struct ParseError : std::runtime_error {
+    explicit ParseError(const std::string &what) : std::runtime_error(what) {}
+};
+struct StateInfo {
+    uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
+};
+// Host only: reads and validates the whole state file (header, every section length and checksum).
+StateInfo read_state_info(const std::string &path);
 
 void voxelize_rigid_solid(void *rgba16f, const uint32_t dim[3], const BlubRigidObject &o, float grid_to_world_scale, const float fluid_world_position[3],
                           double total_time, double delta, int clear_first, cudaStream_t stream, BlubRigidState *state_out);

@@ -12,6 +12,9 @@
 //   --record FPS PREFIX   the controller's "recording with fixed frame length" (simulation_controller.rs:80-82,174-176): the render
 //                  clock advances by 1 / FPS per frame, the simulation runs the steps that belong to the frame (Timer::simulation_frame_loop),
 //                  and instead of a screenshot the particle positions are written to PREFIX00000.f32, PREFIX00001.f32, ...
+//   --save-state FILE  the fluid's complete state after the last step (blub_fluid_save_state); --checkpoint-every N also rewrites FILE every
+//                  N steps at batch boundaries.  --load-state FILE resumes such a file instead of seeding the scene's fluid cubes: the scene
+//                  still provides scale, origin and static objects, and the simulation clock restarts at step_count * dt.
 //   --models DIR   where the scene's static_objects find their OBJ files (the reference reads `models/<model>`,
 //                  src/scene/models.rs:253).  Every step then runs Scene::step's order (src/scene/mod.rs:192-211): animate the
 //                  models at the already advanced simulation time, voxelize their hulls, step the fluid.
@@ -40,16 +43,17 @@ int main(int argc, char **argv) {
     if (argc < 2) {
         std::fprintf(stderr, "usage: blub_run scene.json [--steps N] [--batch 16] [--hz 120] [--device 0] [--no-graph]\n"
                              "                [--stats out.json] [--trace out.json] [--dump particles.f32] [--models DIR] [--record FPS PREFIX]\n"
-                             "                [--solver TOLERANCE MAX_ITERATIONS CHECK_FREQUENCY] [--rebin EVERY_N_STEPS]\n");
+                             "                [--solver TOLERANCE MAX_ITERATIONS CHECK_FREQUENCY] [--rebin EVERY_N_STEPS]\n"
+                             "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE]\n");
         return 2;
     }
     const char *scene = argv[1];
     int steps = 160, batch = 16, device = 0, graph = 1;
     long hz = 120;
-    std::string stats_path, trace_path, dump_path, models_dir = "models", record_prefix;
+    std::string stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
     double record_fps = 0.0;
     float solver_tol = -1.0f;
-    int solver_max = 0, solver_freq = 0, rebin = -1;
+    int solver_max = 0, solver_freq = 0, rebin = -1, checkpoint_every = 0;
     for (int i = 2; i < argc; ++i) {
         auto next = [&](const char *flag) -> const char * {
             if (i + 1 >= argc) { std::fprintf(stderr, "blub_run: %s needs a value\n", flag); std::exit(2); }
@@ -66,6 +70,9 @@ int main(int argc, char **argv) {
         else if (!std::strcmp(argv[i], "--models")) models_dir = next("--models");
         else if (!std::strcmp(argv[i], "--solver")) { solver_tol = (float)std::atof(next("--solver")); solver_max = std::atoi(next("--solver")); solver_freq = std::atoi(next("--solver")); }
         else if (!std::strcmp(argv[i], "--rebin")) rebin = std::atoi(next("--rebin"));
+        else if (!std::strcmp(argv[i], "--save-state")) save_path = next("--save-state");
+        else if (!std::strcmp(argv[i], "--checkpoint-every")) checkpoint_every = std::atoi(next("--checkpoint-every"));
+        else if (!std::strcmp(argv[i], "--load-state")) load_path = next("--load-state");
         else if (!std::strcmp(argv[i], "--record")) { record_fps = std::atof(next("--record")); record_prefix = next("--record"); }
         else { std::fprintf(stderr, "blub_run: unknown option %s\n", argv[i]); return 2; }
     }
@@ -74,12 +81,30 @@ int main(int argc, char **argv) {
     const uint64_t dt_ns = blub_simulation_delta_ns((uint64_t)hz);
     const double dt = (double)blub_duration_as_secs_f32(dt_ns);
     if (!record_prefix.empty() && !(record_fps > 0.0)) { std::fprintf(stderr, "blub_run: bad --record FPS\n"); return 2; }
+    if (!record_prefix.empty() && !load_path.empty()) { std::fprintf(stderr, "blub_run: --load-state cannot resume a --record run\n"); return 2; }
+    if (checkpoint_every < 0 || (checkpoint_every > 0 && save_path.empty())) {
+        std::fprintf(stderr, "blub_run: --checkpoint-every needs a positive N and --save-state FILE\n");
+        return 2;
+    }
 
     BlubSceneInfo info;
     if (blub_scene_info(scene, &info)) die("cannot read scene");
     BlubFluid *fluid = nullptr;
-    if (blub_scene_load(&fluid, scene, device, nullptr)) die("cannot create fluid");
-    blub_fluid_set_graph_replay(fluid, graph);
+    if (load_path.empty()) {
+        if (blub_scene_load(&fluid, scene, device, nullptr)) die("cannot create fluid");
+        blub_fluid_set_graph_replay(fluid, graph);
+    } else { // the file holds every setting of the saved run; only options given on this command line override them
+        BlubStateInfo state;
+        if (blub_state_info(load_path.c_str(), &state)) die("cannot read the state file");
+        if (std::memcmp(state.grid_dimension, info.grid_dimension, sizeof(state.grid_dimension)) != 0) {
+            std::fprintf(stderr, "blub_run: the state file's grid %ux%ux%u is not the scene's %ux%ux%u\n", state.grid_dimension[0], state.grid_dimension[1],
+                         state.grid_dimension[2], info.grid_dimension[0], info.grid_dimension[1], info.grid_dimension[2]);
+            return 1;
+        }
+        if (blub_fluid_load_state(&fluid, load_path.c_str(), device, nullptr)) die("cannot load the state file");
+        if (!graph) blub_fluid_set_graph_replay(fluid, 0);
+        std::printf("resumed %s after step %u\n", load_path.c_str(), blub_fluid_step_count(fluid));
+    }
     if (solver_max > 0) { // the GUI's solver sliders (src/gui/mod.rs:228-250) write the same two SolverConfig structs
         for (int which = 0; which < 2; ++which) {
             BlubSolverConfig *c = blub_fluid_solver_config(fluid, which);
@@ -112,7 +137,8 @@ int main(int argc, char **argv) {
         if (blub_device_malloc(&voxels, cells * 8, device)) die("cannot allocate the voxel volume");
         if (blub_fluid_set_solid_voxels(fluid, voxels)) die("set_solid_voxels failed");
     }
-    uint64_t simulated_ns = 0, rendered_ns = 0; // Timer::total_simulated_time / total_rendered_time
+    // Timer::total_simulated_time / total_rendered_time; a resumed run continues the clock, so that animated solids are where they were
+    uint64_t simulated_ns = (uint64_t)blub_fluid_step_count(fluid) * dt_ns, rendered_ns = 0;
     auto scene_step = [&]() {
         simulated_ns += dt_ns; // advanced BEFORE the step it belongs to (src/timer.rs:122-124)
         const double simulated = (double)blub_duration_as_secs_f32(simulated_ns);
@@ -134,8 +160,17 @@ int main(int argc, char **argv) {
         return n;
     };
 
+    int done = 0, saved_at = -1;
+    auto save_state = [&]() {
+        if (blub_fluid_save_state(fluid, save_path.c_str())) die("cannot save the state");
+        saved_at = done;
+        std::printf("saved the state after step %u to %s\n", blub_fluid_step_count(fluid), save_path.c_str());
+    };
+    auto checkpoint = [&]() { // at batch / frame boundaries only
+        if (checkpoint_every > 0 && done - (saved_at < 0 ? 0 : saved_at) >= checkpoint_every) save_state();
+    };
+
     const auto t0 = std::chrono::steady_clock::now();
-    int done = 0;
     if (!record_prefix.empty()) { // RecordingWithFixedFrameLength: one frame = 1 / FPS on the render clock
         const uint64_t frame_ns = (uint64_t)(1e9 / record_fps); // Duration::from_secs_f64(1.0 / fps), truncated to nanoseconds
         uint64_t clock_ns = 0; // the Timer's own simulation clock; scene_step keeps the same count in simulated_ns
@@ -150,6 +185,7 @@ int main(int argc, char **argv) {
             std::snprintf(name, sizeof(name), "%05d.f32", frame);
             write_particles(record_prefix + name);
             std::printf("frame %d: %u step(s), simulated %.6f s\n", frame, n, (double)blub_duration_as_secs_f32(simulated_ns));
+            checkpoint();
         }
     }
     while (done < steps) { // MAX_FAST_FORWARD_SIMULATION_BATCH_SIZE = 16, then wait for the GPU
@@ -159,9 +195,12 @@ int main(int argc, char **argv) {
         blub_fluid_update_statistics(fluid);
         done += n;
         std::printf("simulation fast forwarding batch finished (progress %d/%d)\n", done, steps);
+        checkpoint();
     }
     const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     std::printf("Fast forward of %.6fs took %.6fs to compute (%.2f steps/s)\n", steps * dt, secs, steps / secs);
+
+    if (!save_path.empty() && saved_at != done) save_state(); // before the extra timed step of --trace
 
     if (!stats_path.empty()) {
         FILE *f = std::fopen(stats_path.c_str(), "w");

@@ -35,6 +35,10 @@ template <class F> int guarded(F &&f) {
         return fail(BLUB_ERR_INVALID_ARGUMENT, e.what());
     } catch (const std::ios_base::failure &e) {
         return fail(BLUB_ERR_IO, e.what());
+    } catch (const blub::IoError &e) {
+        return fail(BLUB_ERR_IO, e.what());
+    } catch (const blub::ParseError &e) {
+        return fail(BLUB_ERR_PARSE, e.what());
     } catch (const std::exception &e) {
         return fail(BLUB_ERR_PARSE, e.what());
     } catch (...) {
@@ -359,6 +363,37 @@ int blub_fluid_synchronize(BlubFluid *fluid) {
     return guarded([&] { fluid->impl->synchronize(); return BLUB_OK; });
 }
 
+int blub_fluid_save_state(BlubFluid *fluid, const char *path) {
+    if (!fluid || !path) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->save_state(path); return BLUB_OK; });
+}
+
+int blub_fluid_load_state(BlubFluid **out, const char *path, int device, void *cuda_stream) {
+    if (!out || !path) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *out = nullptr;
+    return guarded([&] {
+        std::unique_ptr<BlubFluid> f(new BlubFluid());
+        f->impl = blub::HybridFluid::load_state(path, device, static_cast<cudaStream_t>(cuda_stream));
+        *out = f.release();
+        return BLUB_OK;
+    });
+}
+
+int blub_state_info(const char *path, BlubStateInfo *out) {
+    if (!path || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::StateInfo s = blub::read_state_info(path);
+        for (int k = 0; k < 3; ++k) out->grid_dimension[k] = s.grid_dimension[k];
+        out->max_num_particles = s.max_num_particles;
+        out->num_particles = s.num_particles;
+        out->step_count = s.step_count;
+        out->format_version = s.format_version;
+        return BLUB_OK;
+    });
+}
+
+uint32_t blub_fluid_step_count(const BlubFluid *fluid) { return fluid ? fluid->impl->step_count() : 0; }
+
 int blub_scene_info(const char *path, BlubSceneInfo *out) {
     if (!path || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
@@ -509,17 +544,11 @@ int blub_fluid_step_timed(BlubFluid *fluid, double dt, float ms_per_stage[14]) {
 
 int blub_fluid_set_solver_path(BlubFluid *fluid, int persistent) {
     if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
-    blub::PressureSolver &s = fluid->impl->solver();
-    // validate first: a refused request leaves the solver (and the cached step graphs) exactly as they were
-    if (persistent < 0 || persistent > 6 || persistent == 3 || persistent == 5)
-        return fail(BLUB_ERR_INVALID_ARGUMENT, "solver path must be 0 (three kernels), 1 (persistent, default), 2 (TMA-staged), 4 (dense) or 6 (tiles only)");
-    if (persistent == 2 && !s.tma_available()) return fail(BLUB_ERR_INVALID_ARGUMENT, "TMA solver needs nx % 128 == 0 and cooperative launch");
-    s.use_persistent = persistent != 0;
-    s.use_tma = persistent == 2;
-    s.use_dense = persistent == 4;
-    s.use_columns = persistent == 1;
-    fluid->impl->invalidate_graphs();
-    return BLUB_OK;
+    return guarded([&] {
+        fluid->impl->solver().set_path(persistent); // a refused request leaves the solver and the cached step graphs as they were
+        fluid->impl->invalidate_graphs();
+        return BLUB_OK;
+    });
 }
 
 int blub_fluid_set_transfer_path(BlubFluid *fluid, int scatter) {

@@ -89,7 +89,7 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
     }
     configure_transfer_kernels();
     {
-        // Default: the scatter form, faster than the gather on the 256^3 dam break; the gather is bit-reproducible.  BLUB_P2G=gather or
+        // Default: the scatter form, faster than the gather on the 256^3 dam break; both are bit-reproducible.  BLUB_P2G=gather or
         // blub_fluid_set_transfer_path(f, 0) selects the gather.
         const char *tp = std::getenv("BLUB_P2G");
         set_transfer_path(tp && std::string(tp) == "gather" ? 0 : 1);
@@ -407,7 +407,8 @@ void HybridFluid::refresh_fluid_bits() {
     fluid_bits_stale_ = false;
 }
 
-// 0: gather form of P2G (default), 1: scatter form (fixed-point integer reductions into accumulator volumes; what the sharded step uses)
+// 1: scatter form of P2G (default; fixed-point integer reductions into accumulator volumes; what the sharded step uses), 0: gather form over
+// per-step cell lists.  Both are bit-reproducible run to run; they agree with each other to rounding only.
 void HybridFluid::set_transfer_path(int scatter) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     if ((scatter || slab_world_ > 1) && !numw_[0].ptr)
@@ -614,6 +615,7 @@ void HybridFluid::step_stages(double simulation_delta_seconds, int from, int to)
     if (!(dt > 0.0f)) throw std::invalid_argument("simulation delta must be positive");
     upload_step_params(dt);
     for (int s = from; s < to && s < 14; ++s) run_stage(s, dt);
+    mid_step_ = to < 14;
 }
 
 void HybridFluid::step_timed(double simulation_delta_seconds, float ms[14]) {

@@ -1802,6 +1802,17 @@ void PressureSolver::read_work(cudaStream_t stream, uint32_t out[4]) {
     out[3] = (uint32_t)(4 * PCG_TZ);
 }
 
+void PressureSolver::set_path(int path) {
+    // validate first: a refused request leaves the solver exactly as it was
+    if (path < 0 || path > 6 || path == 3 || path == 5)
+        throw std::invalid_argument("solver path must be 0 (three kernels), 1 (persistent, default), 2 (TMA-staged), 4 (dense) or 6 (tiles only)");
+    if (path == 2 && !tma_available()) throw std::invalid_argument("TMA solver needs nx % 128 == 0 and cooperative launch");
+    use_persistent = path != 0;
+    use_tma = path == 2;
+    use_dense = path == 4;
+    use_columns = path == 1;
+}
+
 void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which, const int8_t *marker, const StepParams *dparams,
                            const Quirks &quirks) {
     const GridDim g = grid_;

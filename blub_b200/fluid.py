@@ -91,6 +91,11 @@ class SceneInfo(C.Structure):
                 ("num_static_objects", C.c_uint32)]
 
 
+class StateInfo(C.Structure):
+    _fields_ = [("grid_dimension", C.c_uint32 * 3), ("max_num_particles", C.c_uint32), ("num_particles", C.c_uint32), ("step_count", C.c_uint32),
+                ("format_version", C.c_uint32)]
+
+
 def lib_path() -> str:
     return os.path.join(_HERE, "libblubcore.so")
 
@@ -148,6 +153,10 @@ def lib():
         "blub_fluid_view": (C.c_int, [vp, C.POINTER(FluidView)]),
         "blub_fluid_set_quirks": (C.c_int, [vp, C.POINTER(Quirks)]),
         "blub_fluid_synchronize": (C.c_int, [vp]),
+        "blub_fluid_save_state": (C.c_int, [vp, C.c_char_p]),
+        "blub_fluid_load_state": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
+        "blub_state_info": (C.c_int, [C.c_char_p, C.POINTER(StateInfo)]),
+        "blub_fluid_step_count": (u32, [vp]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -272,6 +281,13 @@ def scene_info(path):
     return info
 
 
+def state_info(path):
+    """Validates a state file written by HybridFluid.save_state (host only) and returns its StateInfo."""
+    info = StateInfo()
+    _check(lib().blub_state_info(os.fsencode(path), C.byref(info)))
+    return info
+
+
 class HybridFluid:
     """HybridFluid::new (hybrid_fluid.rs:92-100)."""
 
@@ -322,6 +338,23 @@ class HybridFluid:
         h = C.c_void_p()
         _check(L.blub_scene_load(C.byref(h), os.fsencode(path), device, cuda_stream))
         return cls(0, 0, 0, 0, _handle=h)
+
+    @classmethod
+    def from_state(cls, path, device=0, cuda_stream=None):
+        """A fluid restored from a file of save_state: its next step is bit for bit the one the saved fluid would have taken.
+        The solid-voxel volume is not part of the state; attach it again with set_solid_voxels."""
+        L = lib()
+        h = C.c_void_p()
+        _check(L.blub_fluid_load_state(C.byref(h), os.fsencode(path), device, cuda_stream))
+        return cls(0, 0, 0, 0, _handle=h)
+
+    def save_state(self, path):
+        """Waits for the enqueued steps, then writes everything a later step depends on to `path` (atomically)."""
+        _check(self.L.blub_fluid_save_state(self.h, os.fsencode(path)))
+
+    @property
+    def step_count(self):
+        return int(self.L.blub_fluid_step_count(self.h))
 
     def close(self):
         if getattr(self, "h", None):

@@ -126,6 +126,27 @@ int blub_fluid_synchronize(BlubFluid *fluid);
 const char *blub_last_error(void);
 const char *blub_version(void);
 
+/* ---- checkpoint / restart (not part of the reference surface; file format: DESIGN.md section 8) ------------------------------ */
+/* Everything a later step depends on (particles in their array order, grid velocities, marker, both pressure warm starts, step
+ * counter, solver configs / paths, transfer path, graph replay, gravity, rebinning settings, quirks, solver statistics), written after
+ * everything enqueued so far has finished (synchronises).  The file is written as `path`.tmp, flushed to disk and renamed over `path`.
+ * Only between whole steps: a fluid whose last blub_fluid_step_stages call did not end at stage 14, and z-slab ranks, are refused with
+ * BLUB_ERR_INVALID_ARGUMENT.  BLUB_ERR_IO: the file cannot be written. */
+int blub_fluid_save_state(BlubFluid *fluid, const char *path);
+/* A new fluid on `device` whose next step is bit for bit the step the saved fluid would have taken next (same library build, same
+ * GPU model).  The file's settings win over the BLUB_* environment variables.  The solid-voxel volume is not part of the state:
+ * attach it again with blub_fluid_set_solid_voxels.  BLUB_ERR_IO: the file cannot be opened or read; BLUB_ERR_PARSE: bad magic, format
+ * version or checksum, truncated file, or a size that disagrees with the header (all sizes are checked before anything is allocated). */
+int blub_fluid_load_state(BlubFluid **out, const char *path, int device, void *cuda_stream);
+/* Host only, no device needed: validates the whole file (magic, version, sizes, checksums) and reports what it holds. */
+typedef struct {
+    uint32_t grid_dimension[3];
+    uint32_t max_num_particles, num_particles, step_count, format_version;
+} BlubStateInfo;
+int blub_state_info(const char *path, BlubStateInfo *out);
+/* number of whole steps this fluid has taken (restored by blub_fluid_load_state) */
+uint32_t blub_fluid_step_count(const BlubFluid *fluid);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their
@@ -274,9 +295,9 @@ int blub_fluid_step_timed(BlubFluid *fluid, double simulation_delta_seconds, flo
  * All paths run the same recurrence; 4 and 6 are bit-identical to each other.  A request that cannot be met returns
  * BLUB_ERR_INVALID_ARGUMENT and changes nothing. */
 int blub_fluid_set_solver_path(BlubFluid *fluid, int persistent);
-/* particle -> grid velocity transfer (transfer_gather_velocity.comp): 1 (default) = warp-aggregated float-atomic scatter into accumulator
- * volumes (faster; sums differ in the last bits from run to run; what z-slab ranks always use), 0 = gather over per-step cell lists
- * (bit-identical output run to run) */
+/* particle -> grid velocity transfer (transfer_gather_velocity.comp): 1 (default) = warp-aggregated scatter into 64-bit fixed-point
+ * accumulator volumes (faster; what z-slab ranks always use), 0 = gather over per-step cell lists.  Both are bit-identical run to run;
+ * they agree with each other to rounding only. */
 int blub_fluid_set_transfer_path(BlubFluid *fluid, int scatter);
 /* blub_fluid_step replays a captured CUDA graph of the step by default; 0 = launch every kernel eagerly instead */
 int blub_fluid_set_graph_replay(BlubFluid *fluid, int enabled);

@@ -11,11 +11,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libblubcore.so")
-SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
+SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
            "c_api.cpp"]
 # the mesh voxelizer shares its arithmetic with a host twin and a NumPy restatement: no FMA contraction, so that all three agree bit for bit
 EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"]}
-HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "voxelize_core.hpp", os.path.join("..", "..", "include", "blub_fluid.h")]
+HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "voxelize_core.hpp", "xoshiro.hpp", os.path.join("..", "..", "include", "blub_fluid.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -217,7 +217,24 @@ class HybridFluid {
     uint32_t max_num_particles() const { return max_num_particles_; }
     void set_particles(uint32_t count, const float *pos4, const float *vx4, const float *vy4, const float *vz4);
 
+    // Sources and drains (flow_kernels.cu): replaces the whole flow set; 0 / 0 clears it.  Throws std::invalid_argument and changes nothing on a
+    // non-finite value, a box that is empty after clamping, overlapping sources, a source overlapping a drain, more than 16 boxes of a kind,
+    // a z-slab rank or a fluid inside a step.  While the set is not empty the particle count lives on the device (num_particles()
+    // synchronises).
+    void set_flow(const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
+    bool has_flow() const { return flow_active_; }
+    const FlowSet &flow_set() const { return flow_; }
+    // cumulative {emitted, drained, refused for capacity} (synchronises)
+    void flow_counters(uint64_t out[3]);
+
   private:
+    bool device_count_mode() const { return slab_world_ > 1 || flow_active_; }
+    void run_flow_prologue();
+    void restore_flow(const FlowSet &set, const uint64_t counters[3]); // state file load
+    FlowSet flow_{};
+    bool flow_active_ = false;
+    FlowScratch flow_scratch_{}; // the drain compaction writes into pos_[1 - cur_] (free at stage 0) and row_alt_ (allocated with the first drain)
+    uint32_t flow_scratch_cells_ = 0; // source cells the scratch has room for
     void upload_step_params(float dt);
     void run_stage(int stage, float dt);
     void refresh_fluid_bits();
@@ -320,6 +337,9 @@ struct ParseError : std::runtime_error {
 struct StateInfo {
     uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
 };
+// A flow set from the public boxes (grid units), clamped like add_fluid_cube; throws std::invalid_argument when it breaks a rule of set_flow
+// that does not depend on the fluid.
+FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
 // Host only: reads and validates the whole state file (header, every section length and checksum).
 StateInfo read_state_info(const std::string &path);
 
@@ -344,6 +364,9 @@ struct SceneStaticObject {
 struct SceneBox {
     float min[3], max[3];
 };
+struct SceneSource {
+    float min[3], max[3], velocity[3];
+};
 struct SceneConfig {
     float gravity[3] = {0, 0, 0};
     float world_position[3] = {0, 0, 0};
@@ -351,6 +374,8 @@ struct SceneConfig {
     uint32_t grid_dimension[3] = {0, 0, 0};
     uint32_t max_num_particles = 0;
     std::vector<SceneBox> fluid_cubes;
+    std::vector<SceneSource> sources; // optional fluid.sources / fluid.drains (world units, m/s)
+    std::vector<SceneBox> drains;
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };

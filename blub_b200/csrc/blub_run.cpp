@@ -160,6 +160,7 @@ int main(int argc, char **argv) {
         return n;
     };
 
+    const bool has_flow = blub_fluid_has_flow(fluid) == 1;
     int done = 0, saved_at = -1;
     auto save_state = [&]() {
         if (blub_fluid_save_state(fluid, save_path.c_str())) die("cannot save the state");
@@ -194,7 +195,10 @@ int main(int argc, char **argv) {
         if (blub_fluid_synchronize(fluid)) die("synchronize failed");
         blub_fluid_update_statistics(fluid);
         done += n;
-        std::printf("simulation fast forwarding batch finished (progress %d/%d)\n", done, steps);
+        if (has_flow) // sources and drains change the particle count as the run goes
+            std::printf("simulation fast forwarding batch finished (progress %d/%d, %u particles)\n", done, steps, blub_fluid_num_particles(fluid));
+        else
+            std::printf("simulation fast forwarding batch finished (progress %d/%d)\n", done, steps);
         checkpoint();
     }
     const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
@@ -213,6 +217,12 @@ int main(int argc, char **argv) {
             std::fprintf(f, ", \"%s\": [", names[which]);
             for (size_t k = 0; k < n; ++k) std::fprintf(f, "%s{\"error\": %.9g, \"iteration_count\": %d}", k ? ", " : "", s[k].error, s[k].iteration_count);
             std::fprintf(f, "]");
+        }
+        if (has_flow) {
+            uint64_t c[3] = {0, 0, 0};
+            if (blub_fluid_flow_counters(fluid, c)) die("cannot read the flow counters");
+            std::fprintf(f, ", \"flow\": {\"emitted\": %llu, \"drained\": %llu, \"refused\": %llu}", (unsigned long long)c[0], (unsigned long long)c[1],
+                         (unsigned long long)c[2]);
         }
         std::fprintf(f, "}\n");
         std::fclose(f);

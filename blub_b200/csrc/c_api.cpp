@@ -394,6 +394,18 @@ int blub_state_info(const char *path, BlubStateInfo *out) {
 
 uint32_t blub_fluid_step_count(const BlubFluid *fluid) { return fluid ? fluid->impl->step_count() : 0; }
 
+int blub_fluid_set_flow(BlubFluid *fluid, const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_flow(sources, num_sources, drains, num_drains); return BLUB_OK; });
+}
+
+int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
+
+int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->flow_counters(out); return BLUB_OK; });
+}
+
 int blub_scene_info(const char *path, BlubSceneInfo *out) {
     if (!path || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {

@@ -70,4 +70,35 @@ void launch_position_change(cudaStream_t st, const GridDim &g, const FluidBits &
 void launch_correct_particles(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos,
                               const int8_t *marker, float *const u[3]);
 
+// exclusive scan of n 32-bit integers in place (the 3-kernel scan of the cell lists); block_sums: exclusive_scan_blocks(n) entries
+int exclusive_scan_blocks(int64_t n);
+void launch_exclusive_scan(cudaStream_t st, uint32_t *data, int64_t n, uint32_t *block_sums);
+
+// ---- sources and drains (flow_kernels.cu, DESIGN.md §8 "Sources and drains") ----
+constexpr int FLOW_MAX_BOXES = 16;
+constexpr uint32_t FLOW_CHUNK = 1024; // particles per block-chunk of the drain compaction
+struct FlowBox {
+    int lo[3], hi[3]; // cells [lo, hi), clamped to [1, dim - 1]
+};
+// Passed by value: a change of the set drops the cached step graphs.
+struct FlowSet {
+    int num_sources, num_drains;
+    FlowBox source[FLOW_MAX_BOXES], drain[FLOW_MAX_BOXES];
+    float velocity[FLOW_MAX_BOXES][3];    // cells/s
+    uint32_t source_base[FLOW_MAX_BOXES + 1]; // exclusive prefix of the source box volumes: index of a box's first cell in the source cell list
+};
+struct FlowScratch {
+    uint32_t *chunk_drained;      // drained particles per FLOW_CHUNK chunk, then their exclusive scan
+    uint32_t *source_count;       // particles per source cell (source_base order, x fastest within a box)
+    uint32_t *emit_offsets;       // particles to emit per source cell, then their exclusive scan (one more entry: the total)
+    uint32_t *scan_sums;          // block sums of both scans
+    uint32_t *scalars;            // [0] first drained index (~0u: none), [1] drained this step, [2] count before the prologue
+    unsigned long long *counters; // cumulative emitted, drained, refused for capacity
+    uint32_t num_chunks, source_cells;
+};
+// Drain, count, emit and set the source velocity (in that order, see DESIGN.md); the particle count lives in params->num_particles.
+// pos_spare / row_spare: arrays of the same capacity the drain compaction writes into before it copies the suffix back.
+void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params, uint32_t capacity, const FlowSet &fs, const FlowScratch &s, float4 *pos,
+                          float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox);
+
 } // namespace blub

@@ -4,11 +4,13 @@
 #include <cstddef>
 #include <cstdlib>
 #include <cstring>
+#include <algorithm>
 
 #include <nvtx3/nvToolsExt.h>
 
 #include "blub_core.hpp"
 #include "fluid_kernels.hpp"
+#include "xoshiro.hpp"
 
 namespace blub {
 
@@ -175,6 +177,12 @@ HybridFluid::~HybridFluid() {
     field_density_.reset();
     if (window_) cudaFree(window_);
     for (int k = 0; k < 3; ++k) cudaFree(row_alt_[k]);
+    cudaFree(flow_scratch_.chunk_drained);
+    cudaFree(flow_scratch_.source_count);
+    cudaFree(flow_scratch_.emit_offsets);
+    cudaFree(flow_scratch_.scan_sums);
+    cudaFree(flow_scratch_.scalars);
+    cudaFree(flow_scratch_.counters);
     cudaFree(mig_counters_);
     if (slab_error_host_) cudaFreeHost(slab_error_host_);
     cudaFree(params_dev_);
@@ -184,43 +192,17 @@ HybridFluid::~HybridFluid() {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Particle seeding, hybrid_fluid.rs:609-678.  The jitter stream is rand 0.8.5 `SmallRng` (xoshiro256++ seeded from a
-// u64 through SplitMix64) drawing cgmath::Vector3<f32> as x, y, z with f32 = (next_u32 >> 8) * 2^-24 and next_u32 = high
-// half of next_u64 -- third-party crates that are not vendored in the reference checkout (Cargo.lock: rand 0.8.5,
-// rand_core 0.6.4, cgmath 0.18.0); restated from their published algorithms.
-namespace {
-struct Xoshiro256pp {
-    uint64_t s[4];
-    static uint64_t rotl(uint64_t x, int k) { return (x << k) | (x >> (64 - k)); }
-    explicit Xoshiro256pp(uint64_t state) {
-        for (int i = 0; i < 4; ++i) {
-            state += 0x9e3779b97f4a7c15ull;
-            uint64_t z = state;
-            z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-            z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-            s[i] = z ^ (z >> 31);
-        }
-    }
-    uint64_t next_u64() {
-        const uint64_t result = rotl(s[0] + s[3], 23) + s[0];
-        const uint64_t t = s[1] << 17;
-        s[2] ^= s[0]; s[3] ^= s[1]; s[1] ^= s[2]; s[0] ^= s[3];
-        s[2] ^= t;
-        s[3] = rotl(s[3], 45);
-        return result;
-    }
-    float next_f32() { return (float)((uint32_t)(next_u64() >> 32) >> 8) * (1.0f / 16777216.0f); }
-};
-
-uint32_t clamp_to_grid(uint32_t dim, float v) { // hybrid_fluid.rs:609-617; Rust `as u32` saturates, NaN -> 0
+// Particle seeding, hybrid_fluid.rs:609-678.  The jitter stream is cgmath::Vector3<f32> drawn as x, y, z from Xoshiro256pp
+// (xoshiro.hpp, shared with the source emission on the device).
+static uint32_t clamp_to_grid(uint32_t dim, float v) { // hybrid_fluid.rs:609-617; Rust `as u32` saturates, NaN -> 0
     uint32_t u = !(v > 0.0f) ? 0u : (v >= 4294967040.0f ? 0xFFFFFFFFu : (uint32_t)v);
     uint32_t m = dim - 1 < u ? dim - 1 : u;
     return m < 1 ? 1 : m;
 }
-} // namespace
 
 bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3]) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (flow_active_) num_particles_ = num_particles(); // sources and drains change the count on the device
     // a slab rank takes GLOBAL grid coordinates: the cube is clamped against the global grid and every rank keeps its part
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny,
                              slab_world_ > 1 ? (uint32_t)(solver_->comm.owned_nz * slab_world_) : (uint32_t)grid_.nz};
@@ -253,6 +235,7 @@ bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3
     BLUB_CUDA_CHECK(cudaMemcpyAsync(pos_[cur_] + num_particles_, fresh.data(), (size_t)num_new * sizeof(float4), cudaMemcpyHostToDevice, stream_));
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // `fresh` is pageable: finish before it dies (queue.write_buffer semantics)
     num_particles_ += num_new;
+    if (flow_active_) set_device_particle_count(num_particles_);
     return truncated;
 }
 
@@ -302,8 +285,8 @@ void HybridFluid::set_device_particle_count(uint32_t n) {
 }
 
 uint32_t HybridFluid::num_particles() const {
-    if (slab_world_ <= 1) return num_particles_;
-    uint32_t n = 0; // authoritative count lives on the device (migration)
+    if (!device_count_mode()) return num_particles_;
+    uint32_t n = 0; // authoritative count lives on the device (migration, sources and drains)
     cudaSetDevice(device_);
     cudaMemcpyAsync(&n, reinterpret_cast<const char *>(params_dev_) + offsetof(StepParams, num_particles), sizeof(uint32_t), cudaMemcpyDeviceToHost, stream_);
     cudaStreamSynchronize(stream_);
@@ -329,7 +312,7 @@ void HybridFluid::set_particles(uint32_t count, const float *pos4, const float *
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
     num_particles_ = count;
-    if (slab_world_ > 1) set_device_particle_count(count);
+    if (device_count_mode()) set_device_particle_count(count);
 }
 
 // windows[k] = rank k's slab window as mapped in THIS process (cudaIpcOpenMemHandle, or a plain peer pointer when all
@@ -381,9 +364,11 @@ void HybridFluid::upload_step_params(float dt) {
     for (int c = 0; c < 3; ++c) h->gravity_dt[c] = gravity_[c] * dt;
     h->tolerance[0] = field_velocity_->config.error_tolerance / dt; // pressure_solver.rs:193-201
     h->tolerance[1] = field_density_->config.error_tolerance / dt;
+    h->step_count = step_counter_;
     h->num_particles = num_particles_;
-    // sharded: the particle count changes on the device (migration) and is the last field: leave it alone
-    const size_t bytes = slab_world_ > 1 ? offsetof(StepParams, num_particles) : sizeof(StepParams);
+    // sharded or with sources / drains: the particle count changes on the device (migration, flow prologue) and is the last field: leave
+    // it alone
+    const size_t bytes = device_count_mode() ? offsetof(StepParams, num_particles) : sizeof(StepParams);
     BLUB_CUDA_CHECK(cudaMemcpyAsync(params_dev_, h, bytes, cudaMemcpyHostToDevice, stream_));
     BLUB_CUDA_CHECK(cudaEventRecord(param_events_[slot], stream_));
 }
@@ -423,10 +408,15 @@ void HybridFluid::run_stage(int stage, float dt) {
     longlong2 *nw[3] = {numw_[0].ptr, numw_[1].ptr, numw_[2].ptr};
     const FluidBits &bits = fluid_bits_;
     const bool shard = slab_world_ > 1 && solver_->comm.world > 1;
-    const uint32_t np = slab_world_ > 1 ? max_num_particles_ : num_particles_; // sharded: the device-side count guards the kernels
+    // sharded or with sources / drains: the device-side count guards the kernels, launches are sized by the capacity
+    const uint32_t np = device_count_mode() ? max_num_particles_ : num_particles_;
     const NvtxScope scope(stage >= 0 && stage < 14 ? kScopeLabels[stage] : "stage");
     switch (stage) {
     case 0: // transfer particle velocity to grid (:806-833)
+        if (flow_active_) {
+            const NvtxScope flow_scope("fluid sources & drains");
+            run_flow_prologue();
+        }
         if (!shard && !use_scatter_) {
             // cell lists -> marker (+ FLUID bits) -> one gather per component; deterministic, no accumulator volumes
             launch_cell_lists(stream_, grid_, params_dev_, np, pos_[cur_], 1.0f, lists_);
@@ -542,7 +532,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
         return;
     }
     GraphSignature sig;
-    sig.num_particles = num_particles_;
+    sig.num_particles = flow_active_ ? 0xFFFFFFFEu : num_particles_; // with sources / drains the launches do not depend on the count
     sig.voxels = voxels_;
     sig.precond_mode = quirks.precond_mode;
     sig.max_it[0] = field_velocity_->config.max_num_iterations; sig.freq[0] = field_velocity_->config.error_check_frequency;
@@ -551,7 +541,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
         destroy_graphs();
         graph_signature_ = sig;
     }
-    const bool binning = binning_step() && num_particles_ > 0;
+    const bool binning = binning_step() && (flow_active_ || num_particles_ > 0);
     // Host-side buffer roles that a captured step bakes in (and changes): the graph is keyed by them.
     struct Roles {
         int cur, row_parity;
@@ -641,6 +631,115 @@ void HybridFluid::solve_only(int which, double simulation_delta_seconds) {
     solver_->solve(stream_, field(which), which, marker_.ptr, params_dev_, quirks);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Sources and drains (flow_kernels.cu).  Not in the reference.
+FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+    if (num_sources > (uint32_t)FLOW_MAX_BOXES || num_drains > (uint32_t)FLOW_MAX_BOXES) throw std::invalid_argument("at most 16 sources and 16 drains");
+    if ((num_sources && !sources) || (num_drains && !drains)) throw std::invalid_argument("NULL box array");
+    FlowSet fs{};
+    auto box_of = [&](const float mn[3], const float mx[3], const char *what) {
+        FlowBox b;
+        for (int k = 0; k < 3; ++k) {
+            if (!std::isfinite(mn[k]) || !std::isfinite(mx[k])) throw std::invalid_argument(std::string(what) + " corner is not finite");
+            b.lo[k] = (int)clamp_to_grid(dim[k], mn[k]);
+            b.hi[k] = (int)clamp_to_grid(dim[k], mx[k]);
+            if (b.hi[k] <= b.lo[k]) throw std::invalid_argument(std::string(what) + " box is empty after clamping to the grid");
+        }
+        return b;
+    };
+    auto overlap = [](const FlowBox &a, const FlowBox &b) {
+        for (int k = 0; k < 3; ++k)
+            if (a.hi[k] <= b.lo[k] || b.hi[k] <= a.lo[k]) return false;
+        return true;
+    };
+    fs.num_sources = (int)num_sources;
+    fs.num_drains = (int)num_drains;
+    for (uint32_t s = 0; s < num_sources; ++s) {
+        fs.source[s] = box_of(sources[s].min_grid, sources[s].max_grid, "source");
+        for (int k = 0; k < 3; ++k) {
+            if (!std::isfinite(sources[s].velocity_grid[k])) throw std::invalid_argument("source velocity is not finite");
+            fs.velocity[s][k] = sources[s].velocity_grid[k];
+        }
+        const FlowBox &b = fs.source[s];
+        fs.source_base[s + 1] = fs.source_base[s] + (uint32_t)((b.hi[0] - b.lo[0]) * (b.hi[1] - b.lo[1]) * (b.hi[2] - b.lo[2]));
+    }
+    for (uint32_t s = num_sources; s < (uint32_t)FLOW_MAX_BOXES; ++s) fs.source_base[s + 1] = fs.source_base[s];
+    for (uint32_t d = 0; d < num_drains; ++d) fs.drain[d] = box_of(drains[d].min_grid, drains[d].max_grid, "drain");
+    for (uint32_t s = 0; s < num_sources; ++s) {
+        for (uint32_t t = s + 1; t < num_sources; ++t)
+            if (overlap(fs.source[s], fs.source[t])) throw std::invalid_argument("two sources overlap");
+        for (uint32_t d = 0; d < num_drains; ++d)
+            if (overlap(fs.source[s], fs.drain[d])) throw std::invalid_argument("a source overlaps a drain");
+    }
+    return fs;
+}
+
+void HybridFluid::set_flow(const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_flow: z-slab ranks have no sources or drains");
+    if (mid_step_) throw std::invalid_argument("set_flow: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    restore_flow(make_flow_set(dim, sources, num_sources, drains, num_drains), nullptr);
+}
+
+// Applies a validated set; counters != nullptr also sets the cumulative counters (state file load).
+void HybridFluid::restore_flow(const FlowSet &fs, const uint64_t counters[3]) {
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    const bool active = fs.num_sources > 0 || fs.num_drains > 0;
+    FlowScratch &s = flow_scratch_;
+    if (active) {
+        if (!s.counters) {
+            s.num_chunks = (max_num_particles_ + FLOW_CHUNK - 1) / FLOW_CHUNK;
+            BLUB_CUDA_CHECK(cudaMalloc(&s.counters, 3 * sizeof(unsigned long long)));
+            BLUB_CUDA_CHECK(cudaMemset(s.counters, 0, 3 * sizeof(unsigned long long)));
+            BLUB_CUDA_CHECK(cudaMalloc(&s.scalars, 4 * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMalloc(&s.chunk_drained, ((size_t)s.num_chunks + 1) * sizeof(uint32_t)));
+        }
+        const uint32_t cells = fs.source_base[FLOW_MAX_BOXES];
+        if (cells > flow_scratch_cells_ || !s.scan_sums) {
+            cudaFree(s.source_count);
+            cudaFree(s.emit_offsets);
+            cudaFree(s.scan_sums);
+            s.source_count = s.emit_offsets = s.scan_sums = nullptr;
+            const uint32_t room = std::max(cells, flow_scratch_cells_);
+            BLUB_CUDA_CHECK(cudaMalloc(&s.source_count, ((size_t)room + 1) * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMalloc(&s.emit_offsets, ((size_t)room + 1) * sizeof(uint32_t)));
+            const int64_t longest = std::max<int64_t>((int64_t)room + 1, (int64_t)s.num_chunks);
+            BLUB_CUDA_CHECK(cudaMalloc(&s.scan_sums, ((size_t)exclusive_scan_blocks(longest) + 1024) * sizeof(uint32_t)));
+            flow_scratch_cells_ = room;
+        }
+        s.source_cells = cells;
+        if (fs.num_drains && !row_alt_[0]) {
+            const size_t pbytes = ((size_t)max_num_particles_ + 64) * sizeof(float4);
+            for (int k = 0; k < 3; ++k) {
+                BLUB_CUDA_CHECK(cudaMalloc(&row_alt_[k], pbytes));
+                BLUB_CUDA_CHECK(cudaMemset(row_alt_[k], 0, pbytes));
+            }
+        }
+    }
+    if (counters) {
+        if (!s.counters) throw std::invalid_argument("flow counters without a flow set");
+        BLUB_CUDA_CHECK(cudaMemcpy(s.counters, counters, 3 * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    }
+    if (active && !flow_active_) set_device_particle_count(num_particles_); // from now on the device owns the count
+    if (!active && flow_active_) num_particles_ = num_particles();          // read it back once
+    flow_ = fs;
+    flow_active_ = active;
+    destroy_graphs();
+}
+
+void HybridFluid::flow_counters(uint64_t out[3]) {
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    out[0] = out[1] = out[2] = 0;
+    if (!flow_scratch_.counters) return;
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(out, flow_scratch_.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+}
+
+void HybridFluid::run_flow_prologue() {
+    launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, voxels_);
+}
+
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream) {
     std::unique_ptr<HybridFluid> f(new HybridFluid(cfg.grid_dimension[0], cfg.grid_dimension[1], cfg.grid_dimension[2], cfg.max_num_particles, device, stream));
     const float scale = cfg.grid_to_world_scale;
@@ -651,6 +750,22 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
     }
     const float g[3] = {cfg.gravity[0] / scale, cfg.gravity[1] / scale, cfg.gravity[2] / scale}; // :139
     f->set_gravity_grid(g);
+    if (!cfg.sources.empty() || !cfg.drains.empty()) { // after the cubes
+        std::vector<BlubFluidSource> src(cfg.sources.size());
+        std::vector<BlubFluidDrain> drn(cfg.drains.size());
+        for (size_t i = 0; i < src.size(); ++i)
+            for (int k = 0; k < 3; ++k) {
+                src[i].min_grid[k] = cfg.sources[i].min[k] / scale;
+                src[i].max_grid[k] = cfg.sources[i].max[k] / scale;
+                src[i].velocity_grid[k] = cfg.sources[i].velocity[k] / scale;
+            }
+        for (size_t i = 0; i < drn.size(); ++i)
+            for (int k = 0; k < 3; ++k) {
+                drn[i].min_grid[k] = cfg.drains[i].min[k] / scale;
+                drn[i].max_grid[k] = cfg.drains[i].max[k] / scale;
+            }
+        f->set_flow(src.data(), (uint32_t)src.size(), drn.data(), (uint32_t)drn.size());
+    }
     return f;
 }
 

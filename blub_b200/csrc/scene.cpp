@@ -170,6 +170,26 @@ SceneConfig parse_scene_file(const std::string &path) {
         vec3(need(c, "max"), "fluid_cubes.max", b.max);
         cfg.fluid_cubes.push_back(b);
     }
+    // sources and drains (not in the reference, whose serde structs ignore unknown keys): world units and m/s, both optional
+    if (const JsonValue *srcs = fluid.get("sources")) {
+        if (srcs->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.sources` is not an array");
+        for (const JsonValue &s : srcs->array) {
+            SceneSource b;
+            vec3(need(s, "min"), "sources.min", b.min);
+            vec3(need(s, "max"), "sources.max", b.max);
+            vec3(need(s, "velocity"), "sources.velocity", b.velocity);
+            cfg.sources.push_back(b);
+        }
+    }
+    if (const JsonValue *drns = fluid.get("drains")) {
+        if (drns->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.drains` is not an array");
+        for (const JsonValue &d : drns->array) {
+            SceneBox b;
+            vec3(need(d, "min"), "drains.min", b.min);
+            vec3(need(d, "max"), "drains.max", b.max);
+            cfg.drains.push_back(b);
+        }
+    }
     if (const JsonValue *objs = root.get("static_objects")) { // #[serde(default)]
         if (objs->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `static_objects` is not an array");
         for (const JsonValue &o : objs->array) { // StaticObjectConfig, src/scene/models.rs:11-19

@@ -20,14 +20,25 @@ namespace {
 static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the state file is little-endian and written as the host lays it out");
 
 constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
-constexpr uint32_t kFormatVersion = 1;
-constexpr uint32_t kNumSections = 13;
+// version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters
+constexpr uint32_t kFormatVersionFlow = 2;
+constexpr uint32_t kNumSections = 14; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
-    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY
+    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW
 };
+
+// Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
+struct FlowSection {
+    uint32_t num_sources, num_drains;
+    int32_t source[16][6]; // lo x, y, z, hi x, y, z
+    float velocity[16][3]; // cells/s
+    int32_t drain[16][6];
+    uint64_t counters[3];  // emitted, drained, refused for capacity
+};
+static_assert(sizeof(FlowSection) == 992 && FLOW_MAX_BOXES == 16, "flow section layout");
 
 struct StateHeader {
     char magic[8];
@@ -61,14 +72,16 @@ struct Section {
     uint64_t length;
 };
 
-// The sections of a file in their order, with the lengths its header implies.
-void expected_sections(const StateHeader &h, Section out[kNumSections]) {
+// The sections of a file in their order, with the lengths its header implies; returns their number.
+uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const Section s[kNumSections] = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
                                      {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
                                      {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
-                                     {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]}};
+                                     {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
+                                     {SEC_FLOW, sizeof(FlowSection)}};
     std::memcpy(out, s, sizeof(s));
+    return h.format_version == kFormatVersionFlow ? 14 : 13;
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -140,9 +153,8 @@ StateHeader read_header(File &f) {
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
-    if (h.format_version != kFormatVersion)
-        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads version " +
-                         std::to_string(kFormatVersion) + ")");
+    if (h.format_version != 1 && h.format_version != kFormatVersionFlow)
+        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads versions 1 and 2)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -156,11 +168,13 @@ StateHeader read_header(File &f) {
         throw ParseError(f.path + ": precond_mode, transfer path or graph replay flag out of range");
     const uint32_t sp = h.solver_path;
     if (sp > 6 || sp == 3 || sp == 5 || (sp == 2 && d[0] % 128)) throw ParseError(f.path + ": solver path out of range");
-    if (h.num_sections != kNumSections) throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, expected 13");
     Section sec[kNumSections];
-    expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec);
+    if (h.num_sections != ns)
+        throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(h.format_version) + " has " +
+                         std::to_string(ns));
     uint64_t total = sizeof(StateHeader);
-    for (const Section &s : sec) total += sizeof(SectionHead) + s.length + 4;
+    for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
     if (size != total)
         throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
@@ -220,15 +234,54 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
     f.write(&crc, 4);
 }
 
+// The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.
+FlowSet flow_set_of(const FlowSection &fl, const StateHeader &h, const std::string &path) {
+    if (fl.num_sources > 16 || fl.num_drains > 16 || fl.num_sources + fl.num_drains == 0)
+        throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
+    std::vector<BlubFluidSource> src(fl.num_sources);
+    std::vector<BlubFluidDrain> drn(fl.num_drains);
+    for (uint32_t b = 0; b < fl.num_sources; ++b)
+        for (int k = 0; k < 3; ++k) {
+            src[b].min_grid[k] = (float)fl.source[b][k];
+            src[b].max_grid[k] = (float)fl.source[b][3 + k];
+            src[b].velocity_grid[k] = fl.velocity[b][k];
+        }
+    for (uint32_t b = 0; b < fl.num_drains; ++b)
+        for (int k = 0; k < 3; ++k) {
+            drn[b].min_grid[k] = (float)fl.drain[b][k];
+            drn[b].max_grid[k] = (float)fl.drain[b][3 + k];
+        }
+    FlowSet fs;
+    try {
+        fs = make_flow_set(h.grid_dimension, src.data(), fl.num_sources, drn.data(), fl.num_drains);
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": section 14: " + e.what());
+    }
+    for (uint32_t b = 0; b < fl.num_sources; ++b)
+        for (int k = 0; k < 3; ++k)
+            if (fs.source[b].lo[k] != fl.source[b][k] || fs.source[b].hi[k] != fl.source[b][3 + k])
+                throw ParseError(path + ": section 14: a source corner lies outside [1, dim - 1]");
+    for (uint32_t b = 0; b < fl.num_drains; ++b)
+        for (int k = 0; k < 3; ++k)
+            if (fs.drain[b].lo[k] != fl.drain[b][k] || fs.drain[b].hi[k] != fl.drain[b][3 + k])
+                throw ParseError(path + ": section 14: a drain corner lies outside [1, dim - 1]");
+    return fs;
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
     File f(path, "rb");
     const StateHeader h = read_header(f);
     Section sec[kNumSections];
-    expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec);
     Staging st(false);
-    for (const Section &s : sec) read_section(f, s, st, [](int, const char *, size_t, uint64_t) {});
+    for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
+    if (ns == 14) {
+        FlowSection fl;
+        read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
+        flow_set_of(fl, h, f.path);
+    }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
     info.max_num_particles = h.max_num_particles;
@@ -246,13 +299,13 @@ void HybridFluid::save_state(const std::string &path) {
     update_statistics(); // every finished solve is in the history now
     StateHeader h{}; // no padding: every byte written is a field or zero
     std::memcpy(h.magic, kMagic, sizeof(kMagic));
-    h.format_version = kFormatVersion;
+    h.format_version = flow_active_ ? kFormatVersionFlow : 1;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
     h.grid_dimension[2] = (uint32_t)grid_.nz;
     h.max_num_particles = max_num_particles_;
-    h.num_particles = num_particles_;
+    h.num_particles = num_particles(); // the device count while sources or drains are set
     h.step_count = step_counter_;
     h.resort_every = internal_resort_every_;
     h.rebin_frequency = dynamic_settings_.particle_rebinning_step_frequency;
@@ -265,7 +318,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = kNumSections;
+    h.num_sections = flow_active_ ? 14 : 13;
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -281,7 +334,7 @@ void HybridFluid::save_state(const std::string &path) {
         Staging st(true);
         File f(tmp, "wb");
         f.write(&h, sizeof(h));
-        const uint64_t np = (uint64_t)num_particles_ * sizeof(float4), n = (uint64_t)grid_.n;
+        const uint64_t np = (uint64_t)h.num_particles * sizeof(float4), n = (uint64_t)grid_.n;
         write_device_section(f, SEC_POSITIONS, pos_[cur_], np, st, stream_);
         for (int c = 0; c < 3; ++c) write_device_section(f, SEC_VELOCITY_X + c, row_[c], np, st, stream_);
         for (int c = 0; c < 3; ++c) write_device_section(f, SEC_GRID_VELOCITY_X + c, u_[c].ptr, 4 * n, st, stream_);
@@ -291,6 +344,25 @@ void HybridFluid::save_state(const std::string &path) {
         write_host_section(f, SEC_SOLVER_SCALARS, scalars, sizeof(scalars));
         write_host_section(f, SEC_STATS_VELOCITY, stats[0].data(), stats[0].size() * sizeof(SolverStatisticSample));
         write_host_section(f, SEC_STATS_DENSITY, stats[1].data(), stats[1].size() * sizeof(SolverStatisticSample));
+        if (flow_active_) {
+            FlowSection fl{};
+            fl.num_sources = (uint32_t)flow_.num_sources;
+            fl.num_drains = (uint32_t)flow_.num_drains;
+            for (int b = 0; b < FLOW_MAX_BOXES; ++b)
+                for (int k = 0; k < 3; ++k) {
+                    if (b < flow_.num_sources) {
+                        fl.source[b][k] = flow_.source[b].lo[k];
+                        fl.source[b][3 + k] = flow_.source[b].hi[k];
+                        fl.velocity[b][k] = flow_.velocity[b][k];
+                    }
+                    if (b < flow_.num_drains) {
+                        fl.drain[b][k] = flow_.drain[b].lo[k];
+                        fl.drain[b][3 + k] = flow_.drain[b].hi[k];
+                    }
+                }
+            flow_counters(fl.counters);
+            write_host_section(f, SEC_FLOW, &fl, sizeof(fl));
+        }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
         f.f = nullptr;
@@ -306,7 +378,7 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     File f(path, "rb");
     const StateHeader h = read_header(f); // every size is checked before anything is allocated
     Section sec[kNumSections];
-    expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec);
     std::unique_ptr<HybridFluid> fluid(
         new HybridFluid(h.grid_dimension[0], h.grid_dimension[1], h.grid_dimension[2], h.max_num_particles, device, stream));
     HybridFluid &x = *fluid;
@@ -347,6 +419,13 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         x.field(which).stats.assign(samples.begin(), samples.end());
     }
     x.fluid_bits_stale_ = true; // rebuilt from the restored marker volume before the next grid pass that reads it
+    if (ns == 14) {
+        FlowSection fl;
+        to_host(sec[13], &fl);
+        const FlowSet fs = flow_set_of(fl, h, f.path);
+        BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
+        x.restore_flow(fs, fl.counters); // the device takes over the restored count
+    }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;
 }

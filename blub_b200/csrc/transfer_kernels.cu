@@ -1028,6 +1028,15 @@ __global__ void __launch_bounds__(PT) binning_permute_kernel(const StepParams *_
 // ------------------------------------------------------------------------------------------------ launchers
 int binning_scan_blocks(const GridDim &g) { return blocks_for(g.n + 1, SCAN_THREADS * SCAN_ITEMS); }
 
+int exclusive_scan_blocks(int64_t n) { return blocks_for(n, SCAN_THREADS * SCAN_ITEMS); }
+
+void launch_exclusive_scan(cudaStream_t st, uint32_t *data, int64_t n, uint32_t *block_sums) {
+    const int nb = exclusive_scan_blocks(n);
+    BLUB_LAUNCH(scan_block_sums_kernel, nb, SCAN_THREADS, 0, st, data, n, block_sums);
+    BLUB_LAUNCH(scan_sums_kernel, 1, 1024, 0, st, block_sums, nb);
+    BLUB_LAUNCH(scan_apply_kernel, nb, SCAN_THREADS, 0, st, data, n, block_sums);
+}
+
 void launch_cell_lists(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float clamp_lo, const CellLists &l) {
     const int64_t n1 = g.n + 1; // cell_start[n] = number of particles
     const int nb = binning_scan_blocks(g);

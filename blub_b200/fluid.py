@@ -96,6 +96,16 @@ class StateInfo(C.Structure):
                 ("format_version", C.c_uint32)]
 
 
+class FluidSource(C.Structure):
+    """BlubFluidSource: a source box in grid cells and its velocity in cells/s."""
+
+    _fields_ = [("min_grid", C.c_float * 3), ("max_grid", C.c_float * 3), ("velocity_grid", C.c_float * 3)]
+
+
+class FluidDrain(C.Structure):
+    _fields_ = [("min_grid", C.c_float * 3), ("max_grid", C.c_float * 3)]
+
+
 def lib_path() -> str:
     return os.path.join(_HERE, "libblubcore.so")
 
@@ -157,6 +167,9 @@ def lib():
         "blub_fluid_load_state": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
         "blub_state_info": (C.c_int, [C.c_char_p, C.POINTER(StateInfo)]),
         "blub_fluid_step_count": (u32, [vp]),
+        "blub_fluid_set_flow": (C.c_int, [vp, C.POINTER(FluidSource), u32, C.POINTER(FluidDrain), u32]),
+        "blub_fluid_flow_counters": (C.c_int, [vp, C.POINTER(C.c_uint64)]),
+        "blub_fluid_has_flow": (C.c_int, [vp]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -479,6 +492,30 @@ class HybridFluid:
         names = {"tma": 2, "dense": 4, "tiles": 6}
         mode = names[persistent] if persistent in names else (int(persistent) if persistent not in (True, False) else (1 if persistent else 0))
         _check(self.L.blub_fluid_set_solver_path(self.h, mode))
+
+    def set_flow(self, sources=(), drains=()):
+        """Replaces the flow set: sources = [(min, max, velocity)], drains = [(min, max)], boxes in grid cells, velocities in cells/s.
+        Empty lists clear it.  Raises BlubError (and changes nothing) on overlaps, more than 16 boxes of a kind, non-finite values, boxes
+        empty after clamping, z-slab ranks and a fluid inside a step."""
+        src = (FluidSource * max(len(sources), 1))()
+        for k, (mn, mx, vel) in enumerate(sources):
+            src[k].min_grid[:], src[k].max_grid[:], src[k].velocity_grid[:] = [float(v) for v in mn], [float(v) for v in mx], [float(v) for v in vel]
+        drn = (FluidDrain * max(len(drains), 1))()
+        for k, (mn, mx) in enumerate(drains):
+            drn[k].min_grid[:], drn[k].max_grid[:] = [float(v) for v in mn], [float(v) for v in mx]
+        _check(self.L.blub_fluid_set_flow(self.h, src, len(sources), drn, len(drains)))
+
+    @property
+    def has_flow(self):
+        """True while the flow set is not empty (the particle count then lives on the device)."""
+        return self.L.blub_fluid_has_flow(self.h) == 1
+
+    @property
+    def flow_counters(self):
+        """Cumulative {"emitted", "drained", "refused"} particle counts of the sources and drains (synchronises)."""
+        out = (C.c_uint64 * 3)()
+        _check(self.L.blub_fluid_flow_counters(self.h, out))
+        return {"emitted": int(out[0]), "drained": int(out[1]), "refused": int(out[2])}
 
     def set_transfer_path(self, scatter):
         """True / "scatter" (default): warp-aggregated atomic scatter; False / "gather": deterministic gather P2G over per-step cell lists."""

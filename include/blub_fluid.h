@@ -147,6 +147,27 @@ int blub_state_info(const char *path, BlubStateInfo *out);
 /* number of whole steps this fluid has taken (restored by blub_fluid_load_state) */
 uint32_t blub_fluid_step_count(const BlubFluid *fluid);
 
+/* ---- sources and drains (not part of the reference surface; rules: DESIGN.md section 8) ---------------------------------------- */
+/* Boxes in grid cells, corners clamped to [1, dim - 1] as blub_fluid_add_cube clamps them (the max corner is exclusive).  At the start of
+ * every step the fluid removes the particles whose cell lies in a drain box (survivors keep their order), tops every source cell that holds
+ * fewer than 4 particles and is neither solid nor a border cell up to 8 (appended after the survivors, up to max_num_particles), and gives
+ * every particle in a source cell the source velocity (cells/s) with C = 0. */
+typedef struct {
+    float min_grid[3], max_grid[3], velocity_grid[3];
+} BlubFluidSource;
+typedef struct {
+    float min_grid[3], max_grid[3];
+} BlubFluidDrain;
+/* Replaces the whole flow set; 0 / 0 clears it.  At most 16 boxes of each kind.  BLUB_ERR_INVALID_ARGUMENT, changing nothing: a non-finite
+ * value, a box empty after clamping, two overlapping sources, a source overlapping a drain, too many boxes, a z-slab rank, or a fluid left
+ * inside a step by blub_fluid_step_stages.  While the set is not empty the particle count lives on the device: blub_fluid_num_particles
+ * then synchronises. */
+int blub_fluid_set_flow(BlubFluid *fluid, const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
+/* Cumulative counts since the fluid was created (or saved): out[0] emitted, out[1] drained, out[2] refused for capacity.  Synchronises. */
+int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]);
+/* 1 when the fluid has a non-empty flow set, 0 when not or when fluid is NULL */
+int blub_fluid_has_flow(const BlubFluid *fluid);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their

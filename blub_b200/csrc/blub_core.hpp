@@ -85,6 +85,7 @@ class PressureField {
 
     PcgScalars *scalars = nullptr; // device
     bool touched = false;          // "timestamp_last_iteration == 0" of :601-603
+    uint8_t *p_tiles = nullptr;    // device, per solver tile: the tile was active in this field's last solve (p may be non-zero there)
 
   private:
     struct Pending {
@@ -115,6 +116,8 @@ class PressureSolver {
     SlabComm comm; // filled by HybridFluid::attach_slab_peers; world == 1 when not sharded
     // {tiles walked by the tile body, quad columns walked by the column body, cells per tile, cells per column} of the last solve (blocking)
     void read_work(cudaStream_t stream, uint32_t out[4]);
+    // The next solve of each field prepares every tile: enqueue after anything outside a step wrote a grid volume.
+    void prepare_dense_next(cudaStream_t stream);
 
   private:
     GridDim grid_;
@@ -126,6 +129,9 @@ class PressureSolver {
     int *num_active_ = nullptr;
     int num_blocks_ = 0;
     int persistent_blocks_ = 0;      // co-resident blocks of the cooperative solver; 0 = not available
+    // device {scratch volumes, pressure of field 0, of field 1}: non-zero = the next solve prepares every tile.  Kept on the device so
+    // that a captured step graph follows them; set by prepare_dense_next and by solves on paths that may write outside the active tiles.
+    int *dense_flags_ = nullptr;
 
   public:
     bool use_persistent = true;      // one cooperative launch per solve (diag2 preconditioner); false = three kernels per iteration
@@ -144,6 +150,7 @@ class PressureSolver {
   private:
     void *tma_maps_ = nullptr;       // PcgTmaMaps (tensor maps of r, s0, s1, codes)
     int tma_blocks_ = 0, column_blocks_ = 0;
+    int code_slots_ = 0;              // column solver: passes per thread whose code words stay in shared memory
     int *tile_cols_ = nullptr;        // column solver: per-tile column counts | exclusive offsets | total
     int *col_list_ = nullptr;         // compacted quad columns (linear index of the quad in its tile's first plane)
     unsigned *barrier_ = nullptr;     // arrival counter of the column solver's grid-wide reductions
@@ -195,6 +202,8 @@ class HybridFluid {
     void invalidate_graphs() { destroy_graphs(); }
     void set_transfer_path(int scatter);
     void marker_written_externally() { fluid_bits_stale_ = true; }
+    // a grid volume was written from outside the step: the next solves prepare every tile
+    void grids_written_externally() { solver_->prepare_dense_next(stream_); }
     // number of whole steps taken (drives the rebinning cadence)
     uint32_t step_count() const { return step_counter_; }
     // Checkpoint / restart (state_file.cpp, format in DESIGN.md §8).  save_state synchronises, then writes everything a later step

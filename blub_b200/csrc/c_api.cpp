@@ -457,6 +457,7 @@ int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t by
         BLUB_CUDA_CHECK(cudaMemcpyAsync(t.ptr, host_src, bytes, cudaMemcpyHostToDevice, fluid->impl->stream()));
         BLUB_CUDA_CHECK(cudaStreamSynchronize(fluid->impl->stream()));
         if (tap == BLUB_TAP_MARKER) fluid->impl->marker_written_externally();
+        fluid->impl->grids_written_externally();
         return BLUB_OK;
     });
 }
@@ -514,6 +515,7 @@ int blub_fluid_time_solve(BlubFluid *fluid, int which, double dt, int repetition
             for (int k = 0; k < repetitions; ++k) {
                 BLUB_CUDA_CHECK(cudaMemcpyAsync(h.solver().residual(), backup, bytes, cudaMemcpyDeviceToDevice, st));
                 BLUB_CUDA_CHECK(cudaMemsetAsync(h.field(which).pressure(), 0, bytes, st));
+                h.grids_written_externally();
                 BLUB_CUDA_CHECK(cudaEventRecord(e0, st));
                 h.solve_only(which, dt);
                 BLUB_CUDA_CHECK(cudaEventRecord(e1, st));

@@ -204,13 +204,33 @@ __device__ __forceinline__ float guarded_div(float num, float den) { // pressure
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// prepare (once per solve, every tile): marker -> codes + per-tile activity; establish the zero invariant:
-// p <- 0 and rhs <- 0 off-fluid (pressure_init.comp:37-43 zeroes p there), s <- 0 everywhere.
+// prepare (once per solve): marker -> codes + per-tile activity; establish the zero invariant:
+// p <- 0 and rhs <- 0 off-fluid (pressure_init.comp:37-43 zeroes p there), s, s1 <- 0 everywhere (s1 may be null).
+// Sparse set-up (dense_flags non-null and both flags of this solve clear): a tile that holds no FLUID cell now, was inactive in the
+// previous solve (tile_active: codes, r, s, s1 are all 0 there) and was not active in this field's previous solve (p_tiles: p is 0
+// there) is left as it is -- it is all zeros already.  The column solver writes only inside active tiles, and the rhs kernels write
+// FLUID cells of the marker the solve is prepared from.
 __global__ void __launch_bounds__(PCG_THREADS) pcg_prepare_kernel(GridDim g, TileMap t, const int8_t *__restrict__ m, uint8_t *__restrict__ codes,
-                                                                  uint8_t *__restrict__ tile_active, int *__restrict__ tile_cols, float *__restrict__ p,
-                                                                  float *__restrict__ r, float *__restrict__ s) {
+                                                                  uint8_t *__restrict__ tile_active, int *__restrict__ tile_cols, uint8_t *__restrict__ p_tiles,
+                                                                  const int *__restrict__ dense_flags, int which, float *__restrict__ p, float *__restrict__ r,
+                                                                  float *__restrict__ s, float *__restrict__ s1) {
     __shared__ int sh_units;
     const TileCtx c = tile_ctx(g, t);
+    const bool sparse = dense_flags && !dense_flags[0] && !dense_flags[1 + which];
+    if (sparse && !tile_active[c.tile] && !p_tiles[c.tile]) { // block-uniform
+        bool fluid = false;
+        if (c.valid) {
+#pragma unroll
+            for (int k = 0; k < PCG_TZ; ++k) {
+                const char4 cc = *reinterpret_cast<const char4 *>(m + c.i + k * g.sz);
+                fluid = fluid || cc.x == CELL_FLUID || cc.y == CELL_FLUID || cc.z == CELL_FLUID || cc.w == CELL_FLUID;
+            }
+        }
+        if (!__syncthreads_or(fluid)) {
+            if (linear_tid() == 0) tile_cols[c.tile] = 0;
+            return;
+        }
+    }
     if (linear_tid() == 0) sh_units = 0;
     __syncthreads();
     int any = 0; // planes of this thread's column whose quad holds a FLUID cell
@@ -248,6 +268,7 @@ __global__ void __launch_bounds__(PCG_THREADS) pcg_prepare_kernel(GridDim g, Til
             }
             *reinterpret_cast<uchar4 *>(codes + i) = out;
             st4(s + i, zero4());
+            if (s1) st4(s1 + i, zero4());
         }
     }
     const int ncols = __syncthreads_count(any > 0); // columns (thread's quad x PCG_TZ planes) that hold a FLUID cell
@@ -260,6 +281,7 @@ __global__ void __launch_bounds__(PCG_THREADS) pcg_prepare_kernel(GridDim g, Til
         const int flag = sh_units == 0 ? 0 : (4 * sh_units >= 3 * PCG_THREADS * PCG_TZ ? 2 : 1);
         tile_active[c.tile] = (uint8_t)flag;
         tile_cols[c.tile] = flag == 1 ? ncols : 0; // the column solver walks sparsely filled tiles column by column
+        p_tiles[c.tile] = (uint8_t)(flag != 0);
     }
 }
 
@@ -547,6 +569,7 @@ struct PcgSolveArgs {
     unsigned *barrier;      // column solver: arrival counter of its grid-wide reductions (0 at the start of a solve)
     const int *col_list;    // column solver: compacted quad columns (4 cells x PCG_TZ planes) of the sparsely filled tiles, see pcg_solve_columns_kernel
     const int *num_cols;
+    int code_slots;         // column solver: passes per thread whose code words stay in shared memory (see pass_codes)
     float *p, *r, *s0, *s1;
     PcgScalars *scal;
     float *partials;        // 3 x gridDim.x
@@ -1137,13 +1160,19 @@ __global__ void __launch_bounds__(PCG_THREADS) pcg_column_fill_kernel(GridDim g,
 }
 
 // One block: compacts the tiles the tile loop walks (all active tiles, or only the dense ones when the columns take the rest) and
-// scans the per-tile column counts.  Deterministic (ascending tile id).
+// scans the per-tile column counts.  Deterministic (ascending tile id).  Runs after the prepare kernel: clears the set-up flags of the
+// solve (dense_flags[0], dense_flags[1 + which]) when it is given them.
 __global__ void __launch_bounds__(1024) pcg_compact_kernel(const uint8_t *__restrict__ tile_active, const int *__restrict__ tile_cols, int tile_lo, int ntiles,
                                                            int dense_only, int *__restrict__ tile_list, int *__restrict__ tile_list_flagged,
-                                                           int *__restrict__ num_active, int *__restrict__ col_offset, int *__restrict__ num_cols) {
+                                                           int *__restrict__ num_active, int *__restrict__ col_offset, int *__restrict__ num_cols,
+                                                           int *__restrict__ dense_flags, int which) {
     __shared__ int sh[1024], shc[1024];
     __shared__ int carry, carry_c;
     if (threadIdx.x == 0) { carry = 0; carry_c = 0; }
+    if (dense_flags && threadIdx.x == 0) {
+        dense_flags[0] = 0;
+        dense_flags[1 + which] = 0;
+    }
     __syncthreads();
     for (int base = tile_lo; base < ntiles; base += 1024) { // [tile_lo, ntiles): the owned tiles of a slab, else all
         const int idx = base + threadIdx.x;
@@ -1193,9 +1222,34 @@ __device__ __forceinline__ TileCtx column_ctx(int i, int sz) {
     return c;
 }
 
+// Code words of a thread's pass (tile or column) number `pass` of a phase.  They do not change during a solve, but the acquire of every
+// grid-wide reduction invalidates L1, so reloading them costs an L2 round trip at the head of every pass, before any operand load can
+// start.  The first phase (init) loads them and keeps the first `slots` passes of each thread in a slot of dynamic shared memory that
+// only this thread uses ([pass][plane][thread]: conflict-free); later phases read them from there.  Passes beyond the slots reload.
+__device__ __forceinline__ void pass_codes(const TileEnv &e, const TileCtx &c, unsigned (&w)[PCG_TZ + 2], unsigned *sh_cw, int slots, int pass, bool fill) {
+    if (pass >= slots) {
+        load_column_codes(e, c, w);
+        return;
+    }
+    unsigned *slot = sh_cw + pass * (PCG_TZ + 2) * PCG_THREADS + linear_tid();
+    if (fill) {
+        load_column_codes(e, c, w);
+#pragma unroll
+        for (int k = 0; k < PCG_TZ + 2; ++k) slot[k * PCG_THREADS] = w[k];
+    } else {
+#pragma unroll
+        for (int k = 0; k < PCG_TZ + 2; ++k) w[k] = slot[k * PCG_THREADS];
+    }
+}
+constexpr int PCG_CODE_SLOT_BYTES = (PCG_TZ + 2) * PCG_THREADS * 4; // 6 KB
+// 8 slots = 48 KB per block, ~150 KB of shared memory per SM at three blocks: the 256^3 dam break ran 4 and 8 slots alike (126.6-126.8
+// steps/s), 12 slots shrink L1 to ~28 KB and ran 112.9 (H100 SXM at 400 W, profiles/h100_pcg_setup.json)
+constexpr int PCG_CODE_SLOTS = 8;
+
 // Three resident blocks per SM (up to 85 registers): for sm_90a, a four-block bound (64 registers) spills the column body to local memory,
 // and on an H100 SXM (700 W limit) the 256^3 dam break runs 100.9 instead of 97.7 steps/s with three blocks (profiles/h100_choices.json).
 __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSolveArgs a) {
+    extern __shared__ unsigned sh_cw[]; // a.code_slots x (PCG_TZ + 2) x PCG_THREADS code words
     __shared__ ReduceScratch sc;
     __shared__ double sh_csum[SLAB_MAX_WORLD];
     __shared__ float sh_cmax[SLAB_MAX_WORLD];
@@ -1233,15 +1287,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSo
 
     // ---- init: r <- b - A p, sigma <- z.r (pressure_init.comp:45-83, pressure_solver.rs:625-649); s stays 0
     float acc = 0.0f;
+    int pass = 0;
     PCG_FOR_EACH_TILE(tile) {
         const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
         unsigned w[PCG_TZ + 2];
-        load_column_codes(e, c, w);
+        pass_codes(e, c, w, sh_cw, a.code_slots, pass++, true);
         init_tile<false>(e, c, w, a.p, a.r, acc);
     }
     PCG_FOR_EACH_COLUMN(c) {
         unsigned w[PCG_TZ + 2];
-        load_column_codes(e, c, w);
+        pass_codes(e, c, w, sh_cw, a.code_slots, pass++, true);
         init_tile<true>(e, c, w, a.p, a.r, acc);
     }
     if (sharded) grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumB, pmax, acc, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
@@ -1254,15 +1309,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSo
         const float *s_in = (it & 1) ? a.s1 : a.s0;
         float *s_out = (it & 1) ? a.s0 : a.s1;
         acc = 0.0f;
+        pass = 0;
         PCG_FOR_EACH_TILE(tile) {
             const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
             unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
             search_tile<false>(e, c, w, a.r, s_in, s_out, beta, acc);
         }
         PCG_FOR_EACH_COLUMN(c) {
             unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
             search_tile<true>(e, c, w, a.r, s_in, s_out, beta, acc);
         }
         if (sharded) grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumA, pmax, acc, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
@@ -1272,15 +1328,16 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSo
         const bool with_err = (a.max_iterations == it) || (it > 0 && it % a.check_frequency == 0); // pressure_solver.rs:676-677
         acc = 0.0f;
         float err = 0.0f;
+        pass = 0;
         PCG_FOR_EACH_TILE(tile) {
             const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
             unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
             update_tile<false>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
         }
         PCG_FOR_EACH_COLUMN(c) {
             unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
             update_tile<true>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
         }
         if (sharded) grid_allreduce<true>(cm_, ++seq, a.barrier, round, psumB, pmax, acc, err, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
@@ -1639,6 +1696,9 @@ PressureField::PressureField(const GridDim &grid, const SolverConfig &cfg, void 
     else pressure_.alloc(grid);
     BLUB_CUDA_CHECK(cudaMalloc(&scalars, sizeof(PcgScalars)));
     BLUB_CUDA_CHECK(cudaMemset(scalars, 0, sizeof(PcgScalars)));
+    const int ntiles = make_tilemap(grid).ntiles;
+    BLUB_CUDA_CHECK(cudaMalloc(&p_tiles, (size_t)ntiles));
+    BLUB_CUDA_CHECK(cudaMemset(p_tiles, 0, (size_t)ntiles));
     BLUB_CUDA_CHECK(cudaMallocHost(&pinned_, sizeof(float) * 2 * NUM_PRESSURE_ERROR_BUFFER));
     ring_.resize(NUM_PRESSURE_ERROR_BUFFER);
     for (int k = 0; k < NUM_PRESSURE_ERROR_BUFFER; ++k) {
@@ -1653,6 +1713,7 @@ PressureField::~PressureField() {
     for (auto &p : ring_) cudaEventDestroy(p.event);
     if (pinned_) cudaFreeHost(pinned_);
     if (scalars) cudaFree(scalars);
+    if (p_tiles) cudaFree(p_tiles);
     pressure_.release();
 }
 
@@ -1740,6 +1801,8 @@ PressureSolver::PressureSolver(const GridDim &grid, void *external_residual) : g
     BLUB_CUDA_CHECK(cudaMemset(tile_active_, 0, (size_t)num_blocks_));
     BLUB_CUDA_CHECK(cudaMalloc(&tile_list_, sizeof(int) * (2 * (size_t)num_blocks_ + 1))); // ids | count | ids with the dense flag
     num_active_ = tile_list_ + num_blocks_;
+    BLUB_CUDA_CHECK(cudaMalloc(&dense_flags_, 3 * sizeof(int)));
+    BLUB_CUDA_CHECK(cudaMemset(dense_flags_, 1, 3 * sizeof(int))); // the first solve of each field prepares every tile
     // persistent cooperative solver: as many blocks as can be co-resident
     int dev = 0, coop = 0, sms = 0, per_sm = 0;
     BLUB_CUDA_CHECK(cudaGetDevice(&dev));
@@ -1775,6 +1838,14 @@ PressureSolver::PressureSolver(const GridDim &grid, void *external_residual) : g
         BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, pcg_solve_columns_kernel, PCG_THREADS, 0));
         column_blocks_ = sms * per;
         if (column_blocks_ > 2048) column_blocks_ = 2048;
+        // as many code slots as leave the number of resident blocks (and with it the grouping of the partial sums) unchanged
+        for (code_slots_ = PCG_CODE_SLOTS; code_slots_ > 0; --code_slots_) {
+            const int bytes = code_slots_ * PCG_CODE_SLOT_BYTES;
+            int per_slots = 0;
+            BLUB_CUDA_CHECK(cudaFuncSetAttribute(pcg_solve_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+            BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_slots, pcg_solve_columns_kernel, PCG_THREADS, bytes));
+            if (per_slots == per) break;
+        }
     }
     use_columns = column_blocks_ > 0 && !(env && std::string(env) == "tiles");
 }
@@ -1787,8 +1858,11 @@ PressureSolver::~PressureSolver() {
     if (tile_cols_) cudaFree(tile_cols_);
     if (col_list_) cudaFree(col_list_);
     if (barrier_) cudaFree(barrier_);
+    if (dense_flags_) cudaFree(dense_flags_);
     delete static_cast<PcgTmaMaps *>(tma_maps_);
 }
+
+void PressureSolver::prepare_dense_next(cudaStream_t stream) { BLUB_CUDA_CHECK(cudaMemsetAsync(dense_flags_, 1, 3 * sizeof(int), stream)); }
 
 void PressureSolver::read_work(cudaStream_t stream, uint32_t out[4]) {
     const TileMap t = make_tilemap(grid_);
@@ -1828,34 +1902,44 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
 
     field.touched = true; // the volume is zero-initialised at allocation (pressure_solver.rs:601-603)
 
+    if (comm.world > 1 && !(mode == 0 && persistent_blocks_ > 0 && use_persistent))
+        throw std::invalid_argument("the z-slab sharded solve needs the persistent solver with precond_mode 0");
+    const bool persistent = mode == 0 && persistent_blocks_ > 0 && use_persistent;
+    // Set-up sized by the fluid: only the tiles that hold FLUID now or were active in the previous solve (p: this field's previous
+    // solve) are prepared.  Kept to the single-GPU column solver, whose kernels write inside the active tiles only; everything else,
+    // the first solve and any solve after a write from outside the step prepare every tile, and so does the solve after them.
+    // The choice is made on the device (dense_flags_), so that a captured step graph follows writes from outside the step.
+    const bool columns = persistent && use_columns && column_blocks_ > 0 && !use_tma && !use_dense;
+    int *const flags = columns && comm.world == 1 ? dense_flags_ : nullptr;
+
     BLUB_LAUNCH(pcg_reset_scalars_kernel, 1, 1, 0, stream, scal, barrier_);
     int *const scratch_cols = tile_cols_ ? tile_cols_ : num_active_; // (no cooperative launch: the counts are not used)
-    BLUB_LAUNCH(pcg_prepare_kernel, grid, block, 0, stream, g, t, marker, codes_.ptr, tile_active_, scratch_cols, p, r, s);
+    // the persistent solvers ping-pong s between search_ and aux_: both zero off the fluid
+    BLUB_LAUNCH(pcg_prepare_kernel, grid, block, 0, stream, g, t, marker, codes_.ptr, tile_active_, scratch_cols, field.p_tiles, flags, which, p, r, s,
+                persistent ? aux_.ptr : nullptr);
+    if (!flags) prepare_dense_next(stream);
     if (mode != 0) { // the stored preconditioner vectors must obey the zero invariant as well
         BLUB_CUDA_CHECK(cudaMemsetAsync(aux_.ptr, 0, (size_t)g.n * sizeof(float), stream));
         BLUB_CUDA_CHECK(cudaMemsetAsync(aux_temp_.ptr, 0, (size_t)g.n * sizeof(float), stream));
     }
-    if (comm.world > 1 && !(mode == 0 && persistent_blocks_ > 0 && use_persistent))
-        throw std::invalid_argument("the z-slab sharded solve needs the persistent solver with precond_mode 0");
-    if (mode == 0 && persistent_blocks_ > 0 && use_persistent) {
-        // one cooperative launch for the whole solve; s ping-pongs between search_ and aux_ (both zero off the active tiles)
-        BLUB_CUDA_CHECK(cudaMemsetAsync(aux_.ptr, 0, (size_t)g.n * sizeof(float), stream));
+    if (persistent) {
+        // one cooperative launch for the whole solve
         const int ghost_tiles = (comm.halo / PCG_TZ) * t.tiles_x * t.tiles_y; // ghost planes are whole tiles (SLAB_HALO == PCG_TZ)
-        const bool columns = use_columns && column_blocks_ > 0 && !use_tma && !use_dense;
         int *col_offset = tile_cols_ + t.ntiles, *num_cols = tile_cols_ + 2 * t.ntiles;
         BLUB_LAUNCH(pcg_compact_kernel, 1, 1024, 0, stream, tile_active_, tile_cols_, ghost_tiles, t.ntiles - ghost_tiles, columns ? 1 : 0, tile_list_, num_active_ + 1,
-                    num_active_, col_offset, num_cols);
+                    num_active_, col_offset, num_cols, flags, which);
         PcgSolveArgs args;
         args.g = g; args.t = t; args.codes = st; args.tile_list = tile_list_; args.tile_list_flagged = num_active_ + 1; args.num_active = num_active_;
         args.p = p; args.r = r; args.s0 = s; args.s1 = aux_.ptr; args.scal = scal; args.partials = partials_;
         args.params = dparams; args.which = which; args.max_iterations = max_it; args.check_frequency = freq;
         args.comm = comm;
-        args.col_list = col_list_; args.num_cols = num_cols; args.barrier = barrier_;
+        args.col_list = col_list_; args.num_cols = num_cols; args.barrier = barrier_; args.code_slots = code_slots_;
         if (columns) { // dense tiles by the tile body, everything else column by column
             BLUB_LAUNCH(pcg_column_fill_kernel, grid, block, 0, stream, g, t, st, ta, col_offset, ghost_tiles, t.ntiles - ghost_tiles, col_list_);
             int nblocks = column_blocks_;
             void *kargs[] = {&args};
-            BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)pcg_solve_columns_kernel, dim3(nblocks), t.block(), kargs, 0, stream));
+            BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)pcg_solve_columns_kernel, dim3(nblocks), t.block(), kargs,
+                                                        (size_t)code_slots_ * PCG_CODE_SLOT_BYTES, stream));
             g_kernel_launches.fetch_add(1, std::memory_order_relaxed);
             return;
         }

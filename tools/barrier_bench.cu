@@ -5,6 +5,8 @@
 //   cg4       cooperative_groups grid.sync() + every block re-reads all partials       (what the solver did in round 1)
 //   flat4     monotonic arrival counter (one atomic per block, acquire spin by thread 0) + every block re-reads all partials
 //   flat1     the same with #SM blocks of 1024 threads
+//   last3/4   one reader: the block that takes the last ticket adds the partials and publishes the total; the others poll that word
+//   flat3     flat4 on the column solver's grid of 3 x #SM blocks
 //   two4      two-level: blocks sharing an SM-sized group of 4 first meet on a group counter, the last of a group arrives globally;
 //             the group's partials are pre-added by that last block, so that #SM instead of 4 x #SM partials are re-read
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o barrier_bench barrier_bench.cu     Run: ./barrier_bench
@@ -96,6 +98,50 @@ __global__ void __launch_bounds__(THREADS) k_flat(float *partials, unsigned *cou
         }
         __syncthreads();
         carry = all_sum<THREADS>(partials + (it & 1) * gridDim.x, gridDim.x, shd);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *out = carry;
+}
+
+// one reader: the block that takes the last ticket adds all partials and publishes {round, total} with a release store; the others poll
+// that word only (the column solver's grid_reduce)
+struct LastResult {
+    unsigned round;
+    float pad;
+    double tot;
+};
+__device__ __forceinline__ void st_release(unsigned *p, unsigned v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS) k_last(float *partials, unsigned *counter, int iters, double *out) {
+    __shared__ float sh[THREADS / 32];
+    __shared__ double shd[THREADS / 32];
+    __shared__ int last;
+    __shared__ double result;
+    LastResult *res = reinterpret_cast<LastResult *>(counter + 32);
+    double carry = 0.0;
+    for (int it = 0; it < iters; ++it) {
+        const unsigned round = (unsigned)it + 1u;
+        const float bs = block_sum<THREADS>((float)(threadIdx.x & 3) + (float)carry * 1e-30f, sh);
+        if (threadIdx.x == 0) {
+            partials[(it & 1) * gridDim.x + blockIdx.x] = bs;
+            __threadfence();
+            last = atomicAdd(counter, 1u) == round * gridDim.x - 1u;
+            __threadfence();
+        }
+        __syncthreads();
+        if (last) {
+            const double t = all_sum<THREADS>(partials + (it & 1) * gridDim.x, gridDim.x, shd);
+            if (threadIdx.x == 0) {
+                result = t;
+                __stcg(&res->tot, t);
+                st_release(&res->round, round);
+            }
+        } else if (threadIdx.x == 0) {
+            while (ld_acquire(&res->round) != round) {}
+            result = __ldcg(&res->tot);
+        }
+        __syncthreads();
+        carry = result;
+        __syncthreads();
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) *out = carry;
 }
@@ -217,17 +263,26 @@ int main() {
     CHECK(cudaMalloc(&out, sizeof(double)));
     const int iters = 2000;
     auto reset = [&] { CHECK(cudaMemset(counters, 0, 4096 * sizeof(unsigned))); };
+    for (int per_sm = 3; per_sm <= 4; ++per_sm) { // three blocks per SM: the column solver's grid
+        const int blocks = sms * per_sm;
+        time_it(per_sm == 3 ? "flat3" : "flat4", blocks, 256, iters, [&](int n) {
+            reset();
+            unsigned *c = counters;
+            void *args[] = {&partials, &c, &n, &out};
+            CHECK(cudaLaunchCooperativeKernel((const void *)k_flat<256>, dim3(blocks), dim3(256), args, 0, 0));
+        });
+        time_it(per_sm == 3 ? "last3" : "last4", blocks, 256, iters, [&](int n) {
+            reset();
+            unsigned *c = counters;
+            void *args[] = {&partials, &c, &n, &out};
+            CHECK(cudaLaunchCooperativeKernel((const void *)k_last<256>, dim3(blocks), dim3(256), args, 0, 0));
+        });
+    }
     {
         const int blocks = sms * 4;
         time_it("cg4", blocks, 256, iters, [&](int n) {
             void *args[] = {&partials, &n, &out};
             CHECK(cudaLaunchCooperativeKernel((const void *)k_cg<256>, dim3(blocks), dim3(256), args, 0, 0));
-        });
-        time_it("flat4", blocks, 256, iters, [&](int n) {
-            reset();
-            unsigned *c = counters;
-            void *args[] = {&partials, &c, &n, &out};
-            CHECK(cudaLaunchCooperativeKernel((const void *)k_flat<256>, dim3(blocks), dim3(256), args, 0, 0));
         });
         time_it("two4", blocks, 256, iters, [&](int n) {
             reset();

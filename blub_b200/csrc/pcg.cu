@@ -1838,16 +1838,25 @@ PressureSolver::PressureSolver(const GridDim &grid, void *external_residual) : g
         BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, pcg_solve_columns_kernel, PCG_THREADS, 0));
         column_blocks_ = sms * per;
         if (column_blocks_ > 2048) column_blocks_ = 2048;
-        // as many code slots as leave the number of resident blocks (and with it the grouping of the partial sums) unchanged
-        for (code_slots_ = PCG_CODE_SLOTS; code_slots_ > 0; --code_slots_) {
+        // as many code slots as leave the number of resident blocks (and with it the grouping of the partial sums) unchanged.  The
+        // attribute is the largest size any solver asks for, so that solvers with different slot counts can live in one process.
+        // BLUB_PCG_CODE_SLOTS=N (0..8, test hook) starts the search at N: the grid and every sum stay the same, passes beyond N reload.
+        int max_slots = PCG_CODE_SLOTS;
+        const char *slots_env = std::getenv("BLUB_PCG_CODE_SLOTS");
+        if (slots_env && slots_env[0] >= '0' && slots_env[0] <= '0' + PCG_CODE_SLOTS && slots_env[1] == '\0') max_slots = slots_env[0] - '0';
+        BLUB_CUDA_CHECK(cudaFuncSetAttribute(pcg_solve_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PCG_CODE_SLOTS * PCG_CODE_SLOT_BYTES));
+        for (code_slots_ = max_slots; code_slots_ > 0; --code_slots_) {
             const int bytes = code_slots_ * PCG_CODE_SLOT_BYTES;
             int per_slots = 0;
-            BLUB_CUDA_CHECK(cudaFuncSetAttribute(pcg_solve_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
             BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_slots, pcg_solve_columns_kernel, PCG_THREADS, bytes));
             if (per_slots == per) break;
         }
     }
     use_columns = column_blocks_ > 0 && !(env && std::string(env) == "tiles");
+    // BLUB_PCG_SETUP=dense (test hook): the column solver prepares every tile on every solve, as the other paths do -- the comparator
+    // of the set-up sized by the fluid, with the same arithmetic
+    const char *setup_env = std::getenv("BLUB_PCG_SETUP");
+    dense_setup_ = setup_env && std::string(setup_env) == "dense";
 }
 
 PressureSolver::~PressureSolver() {
@@ -1910,7 +1919,7 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
     // the first solve and any solve after a write from outside the step prepare every tile, and so does the solve after them.
     // The choice is made on the device (dense_flags_), so that a captured step graph follows writes from outside the step.
     const bool columns = persistent && use_columns && column_blocks_ > 0 && !use_tma && !use_dense;
-    int *const flags = columns && comm.world == 1 ? dense_flags_ : nullptr;
+    int *const flags = columns && comm.world == 1 && !dense_setup_ ? dense_flags_ : nullptr;
 
     BLUB_LAUNCH(pcg_reset_scalars_kernel, 1, 1, 0, stream, scal, barrier_);
     int *const scratch_cols = tile_cols_ ? tile_cols_ : num_active_; // (no cooperative launch: the counts are not used)

@@ -171,8 +171,8 @@ class HybridFluid {
     ~HybridFluid();
     HybridFluid(const HybridFluid &) = delete;
 
-    // returns true when the cube was truncated to max_num_particles (hybrid_fluid.rs:627-633)
-    bool add_fluid_cube(const float min_grid[3], const float max_grid[3]);
+    // returns true when the cube was truncated to max_num_particles (hybrid_fluid.rs:627-633); the new particles carry `tag`
+    bool add_fluid_cube(const float min_grid[3], const float max_grid[3], uint32_t tag = 0);
     void set_gravity_grid(const float g[3]) { gravity_[0] = g[0]; gravity_[1] = g[1]; gravity_[2] = g[2]; }
     uint32_t num_particles() const;
     uint32_t num_active_particles() const { return num_particles(); }
@@ -230,14 +230,21 @@ class HybridFluid {
     // Sources and drains (flow_kernels.cu): replaces the whole flow set; 0 / 0 clears it.  Throws std::invalid_argument and changes nothing on a
     // non-finite value, a box that is empty after clamping, overlapping sources, a source overlapping a drain, more than 16 boxes of a kind,
     // a z-slab rank or a fluid inside a step.  While the set is not empty the particle count lives on the device (num_particles()
-    // synchronises).
-    void set_flow(const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
+    // synchronises).  source_tags: the tag of each source's emitted particles (nullptr = all 0).
+    void set_flow(const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
     bool has_flow() const { return flow_active_; }
     const FlowSet &flow_set() const { return flow_; }
     // cumulative {emitted, drained, refused for capacity} (synchronises)
     void flow_counters(uint64_t out[3]);
 
+    // Particle tags (flow_kernels.cu): the raw bits of the fourth word of every position.  paint_tags is stream-ordered and throws
+    // std::invalid_argument (changing nothing) under the rules of set_flow for one box; tag_census synchronises and throws on num_tags of 0 or
+    // above TAG_CENSUS_MAX or first + num_tags above 2^32.
+    void paint_tags(const float min_grid[3], const float max_grid[3], uint32_t tag);
+    void tag_census(uint32_t first, uint32_t num_tags, BlubTagCensus *out);
+
   private:
+    BlubTagCensus *census_dev_ = nullptr; // TAG_CENSUS_MAX records, allocated with the first census
     bool device_count_mode() const { return slab_world_ > 1 || flow_active_; }
     void run_flow_prologue();
     void restore_flow(const FlowSet &set, const uint64_t counters[3]); // state file load
@@ -266,7 +273,7 @@ class HybridFluid {
     MigrateOut slab_migrate_targets();
     void slab_migrate_finish();
     void set_device_particle_count(uint32_t n);
-    bool add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3]);
+    bool add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3], uint32_t tag);
     uint32_t seeded_global_ = 0;
     float4 *row_alt_[3] = {nullptr, nullptr, nullptr}; // spare velocity rows: migration compacts out of place
     unsigned int *mig_counters_ = nullptr;
@@ -347,9 +354,13 @@ struct ParseError : std::runtime_error {
 struct StateInfo {
     uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
 };
+// A box in grid units clamped like add_fluid_cube (corners in [1, dim - 1], max exclusive); throws std::invalid_argument on a non-finite corner
+// or a box that is empty after clamping (`what` names it in the message).
+FlowBox clamp_box(const uint32_t dim[3], const float min_grid[3], const float max_grid[3], const char *what);
 // A flow set from the public boxes (grid units), clamped like add_fluid_cube; throws std::invalid_argument when it breaks a rule of set_flow
-// that does not depend on the fluid.
-FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains);
+// that does not depend on the fluid.  source_tags may be nullptr (all 0).
+FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
+                      uint32_t num_drains);
 // Host only: reads and validates the whole state file (header, every section length and checksum).
 StateInfo read_state_info(const std::string &path);
 
@@ -373,9 +384,11 @@ struct SceneStaticObject {
 };
 struct SceneBox {
     float min[3], max[3];
+    uint32_t tag = 0; // optional "tag" of a fluid cube (drains have none)
 };
 struct SceneSource {
     float min[3], max[3], velocity[3];
+    uint32_t tag = 0;
 };
 struct SceneConfig {
     float gravity[3] = {0, 0, 0};

@@ -7,7 +7,8 @@
 //   --stats FILE   solver statistics history as JSON (the GUI's residual / iteration plots, src/gui/mod.rs:177-210)
 //   --trace FILE   one step as a Chrome trace with the reference's profiler scope labels (src/gui/mod.rs:487-491,
 //                  hybrid_fluid.rs:780-973)
-//   --dump FILE    particle positions (float32 x,y,z,pad) for an external viewer -- the renderer hand-off
+//   --dump FILE    particle positions (float32 x,y,z,pad) for an external viewer -- the renderer hand-off; pad holds the particle's tag bits
+//                  (read it as uint32)
 //                  (hybrid_fluid.rs:351-369) without wgpu
 //   --record FPS PREFIX   the controller's "recording with fixed frame length" (simulation_controller.rs:80-82,174-176): the render
 //                  clock advances by 1 / FPS per frame, the simulation runs the steps that belong to the frame (Timer::simulation_frame_loop),

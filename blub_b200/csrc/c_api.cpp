@@ -277,10 +277,12 @@ int blub_enable_peer_access(int device, int peer) {
     });
 }
 
-int blub_fluid_add_cube(BlubFluid *fluid, const float min_grid[3], const float max_grid[3]) {
+int blub_fluid_add_cube_tagged(BlubFluid *fluid, const float min_grid[3], const float max_grid[3], uint32_t tag) {
     if (!fluid || !min_grid || !max_grid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
-    return guarded([&] { return fluid->impl->add_fluid_cube(min_grid, max_grid) ? BLUB_WARN_TRUNCATED : BLUB_OK; });
+    return guarded([&] { return fluid->impl->add_fluid_cube(min_grid, max_grid, tag) ? BLUB_WARN_TRUNCATED : BLUB_OK; });
 }
+
+int blub_fluid_add_cube(BlubFluid *fluid, const float min_grid[3], const float max_grid[3]) { return blub_fluid_add_cube_tagged(fluid, min_grid, max_grid, 0); }
 
 int blub_fluid_set_gravity_grid(BlubFluid *fluid, const float g[3]) {
     if (!fluid || !g) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
@@ -394,9 +396,24 @@ int blub_state_info(const char *path, BlubStateInfo *out) {
 
 uint32_t blub_fluid_step_count(const BlubFluid *fluid) { return fluid ? fluid->impl->step_count() : 0; }
 
-int blub_fluid_set_flow(BlubFluid *fluid, const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+int blub_fluid_set_flow_tagged(BlubFluid *fluid, const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources,
+                               const BlubFluidDrain *drains, uint32_t num_drains) {
     if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
-    return guarded([&] { fluid->impl->set_flow(sources, num_sources, drains, num_drains); return BLUB_OK; });
+    return guarded([&] { fluid->impl->set_flow(sources, source_tags, num_sources, drains, num_drains); return BLUB_OK; });
+}
+
+int blub_fluid_set_flow(BlubFluid *fluid, const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+    return blub_fluid_set_flow_tagged(fluid, sources, nullptr, num_sources, drains, num_drains);
+}
+
+int blub_fluid_paint_tags(BlubFluid *fluid, const float min_grid[3], const float max_grid[3], uint32_t tag) {
+    if (!fluid || !min_grid || !max_grid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->paint_tags(min_grid, max_grid, tag); return BLUB_OK; });
+}
+
+int blub_fluid_tag_census(BlubFluid *fluid, uint32_t first_tag, uint32_t num_tags, BlubTagCensus *out) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->tag_census(first_tag, num_tags, out); return BLUB_OK; });
 }
 
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }

@@ -10,8 +10,14 @@
 //   3. sources: flow_need_kernel turns the counts into the number of particles each source cell gets, an exclusive scan orders them by
 //      (source, cell x fastest, slot), and flow_emit_kernel appends them after the survivors up to the capacity and sets the new count and
 //      the cumulative counters.
-// The jitter of an emitted particle is a function of (step, cell, slot): Xoshiro256pp seeded with step << 32 | cell, 8 slots x 3 draws.
+// The jitter of an emitted particle is a function of (step, cell, slot): Xoshiro256pp seeded with step << 32 | cell, 8 slots x 3 draws; it carries
+// the tag of its source.
+//
+// Particle tags share the drains' cell rule and live here too: paint_tags_kernel sets the tag of the particles whose cell lies in a box, and
+// tag_census_kernel adds up count, positions, velocities and cell bounds per tag.  A tag is the raw bits of the fourth word of a position:
+// every path copies it, none puts it through float arithmetic.
 #include <algorithm>
+#include <climits>
 
 #include "fluid_kernels.hpp"
 #include "xoshiro.hpp"
@@ -168,7 +174,7 @@ __global__ void __launch_bounds__(PT) flow_emit_kernel(GridDim g, StepParams *__
             const uint32_t e = off + slot - count; // this cell's slots count..7 in order
             if (slot < count || e >= emitted) continue;
             const uint32_t i = survivors + e;
-            pos[i] = make_float4(p[0], p[1], p[2], 0.0f);
+            pos[i] = make_float4(p[0], p[1], p[2], __uint_as_float(fs.tag[k])); // the source's tag, as bits
             rx[i] = make_float4(0.0f, 0.0f, 0.0f, fs.velocity[k][0]);
             ry[i] = make_float4(0.0f, 0.0f, 0.0f, fs.velocity[k][1]);
             rz[i] = make_float4(0.0f, 0.0f, 0.0f, fs.velocity[k][2]);
@@ -179,6 +185,90 @@ __global__ void __launch_bounds__(PT) flow_emit_kernel(GridDim g, StepParams *__
         s.counters[0] += emitted;
         s.counters[1] += s.scalars[1];
         s.counters[2] += total - emitted;
+    }
+}
+
+// ---- particle tags ----
+__device__ __forceinline__ uint32_t live_count(const StepParams *params, uint32_t n_host) { return params ? params->num_particles : n_host; }
+
+__global__ void __launch_bounds__(PT) paint_tags_kernel(GridDim g, const StepParams *__restrict__ params, uint32_t n_host, FlowBox box, uint32_t tag,
+                                                        float4 *__restrict__ pos) {
+    const uint32_t n = live_count(params, n_host);
+    for (uint32_t i = blockIdx.x * PT + threadIdx.x; i < n; i += gridDim.x * PT)
+        if (in_box(box, flow_cell(g, pos[i]))) pos[i].w = __uint_as_float(tag); // only the fourth word is stored
+}
+
+// 2^16 fixed point: the product with a power of two is exact, __float2ll_rn rounds it to nearest even; integer sums do not depend on the order
+__device__ __forceinline__ unsigned long long census_fixed(float v) {
+    return (unsigned long long)__float2ll_rn(v * (float)(1 << BLUB_TAG_CENSUS_FRAC_BITS));
+}
+
+// Per tag in [first, first + num_tags): count, sums of positions and velocities (v_c = row c .w) and the cell bounds.  Each block adds up its
+// particles in a private shared-memory table, a warp whose 32 particles share one tag with one table update; then the block flushes its
+// non-empty entries with one global atomic per field.
+__global__ void __launch_bounds__(PT) tag_census_kernel(GridDim g, const StepParams *__restrict__ params, uint32_t n_host, uint32_t first, uint32_t num_tags,
+                                                        const float4 *__restrict__ pos, const float4 *__restrict__ rx, const float4 *__restrict__ ry,
+                                                        const float4 *__restrict__ rz, BlubTagCensus *__restrict__ out) {
+    __shared__ unsigned long long sum[6][TAG_CENSUS_MAX]; // position x, y, z, velocity x, y, z
+    __shared__ int lo[3][TAG_CENSUS_MAX], hi[3][TAG_CENSUS_MAX];
+    __shared__ uint32_t count[TAG_CENSUS_MAX];
+    for (uint32_t t = threadIdx.x; t < num_tags; t += PT) {
+        count[t] = 0u;
+        for (int k = 0; k < 6; ++k) sum[k][t] = 0ull;
+        for (int k = 0; k < 3; ++k) {
+            lo[k][t] = INT_MAX;
+            hi[k][t] = INT_MIN;
+        }
+    }
+    __syncthreads();
+    const uint32_t n = live_count(params, n_host);
+    const int lane = threadIdx.x & 31;
+    // whole warps walk the loop, as in flow_count_kernel
+    for (uint32_t i = blockIdx.x * PT + threadIdx.x; (i & ~31u) < n; i += gridDim.x * PT) {
+        const bool live = i < n;
+        const float4 p = live ? pos[i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        const uint32_t key = live ? __float_as_uint(p.w) - first : NONE; // tags below `first` wrap to large keys
+        const bool in = key < num_tags;
+        if (!__any_sync(0xffffffffu, in)) continue;
+        const float4 vx = in ? rx[i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f), vy = in ? ry[i] : vx, vz = in ? rz[i] : vx;
+        const int3 c = flow_cell(g, p);
+        unsigned long long q[6] = {census_fixed(p.x), census_fixed(p.y), census_fixed(p.z), census_fixed(vx.w), census_fixed(vy.w), census_fixed(vz.w)};
+        int cmin[3] = {c.x, c.y, c.z}, cmax[3] = {c.x, c.y, c.z};
+        uint32_t particles = 1u;
+        if (__all_sync(0xffffffffu, key == __shfl_sync(0xffffffffu, key, 0))) { // the whole warp has one tag in range
+            particles = 32u;
+#pragma unroll
+            for (int k = 0; k < 6; ++k)
+                for (int o = 16; o > 0; o >>= 1) q[k] += __shfl_xor_sync(0xffffffffu, q[k], o);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                cmin[k] = __reduce_min_sync(0xffffffffu, cmin[k]);
+                cmax[k] = __reduce_max_sync(0xffffffffu, cmax[k]);
+            }
+            if (lane != 0) continue;
+        } else if (!in) {
+            continue;
+        }
+        atomicAdd(count + key, particles);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) atomicAdd(&sum[k][key], q[k]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            atomicMin(&lo[k][key], cmin[k]);
+            atomicMax(&hi[k][key], cmax[k]);
+        }
+    }
+    __syncthreads();
+    for (uint32_t t = threadIdx.x; t < num_tags; t += PT) {
+        if (count[t] == 0u) continue;
+        BlubTagCensus &o = out[t];
+        atomicAdd(reinterpret_cast<unsigned long long *>(&o.count), (unsigned long long)count[t]);
+        for (int k = 0; k < 3; ++k) {
+            atomicAdd(reinterpret_cast<unsigned long long *>(&o.position_sum_fx[k]), sum[k][t]);
+            atomicAdd(reinterpret_cast<unsigned long long *>(&o.velocity_sum_fx[k]), sum[3 + k][t]);
+            atomicMin(&o.cell_min[k], lo[k][t]);
+            atomicMax(&o.cell_max[k], hi[k][t]);
+        }
     }
 }
 
@@ -208,6 +298,20 @@ void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params,
     } else {
         BLUB_LAUNCH(flow_emit_kernel, 1, PT, 0, st, g, params, capacity, fs, pos, row[0], row[1], row[2], s); // count and counters only
     }
+}
+
+void launch_paint_tags(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t n_host, uint32_t np_upper, const FlowBox &box, uint32_t tag,
+                       float4 *pos) {
+    if (np_upper == 0) return;
+    BLUB_LAUNCH(paint_tags_kernel, std::min(blocks_for(np_upper, PT), device_sm_count() * 16), PT, 0, st, g, params, n_host, box, tag, pos);
+}
+
+void launch_tag_census(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t n_host, uint32_t np_upper, uint32_t first, uint32_t num_tags,
+                       const float4 *pos, float4 *const row[3], BlubTagCensus *out) {
+    if (np_upper == 0) return;
+    // 8 blocks of 256 threads and 19 KB per SM: every block flushes at most num_tags entries
+    BLUB_LAUNCH(tag_census_kernel, std::min(blocks_for(np_upper, PT), device_sm_count() * 8), PT, 0, st, g, params, n_host, first, num_tags, pos, row[0],
+                row[1], row[2], out);
 }
 
 } // namespace blub

@@ -1,5 +1,6 @@
 // fluid_kernels.hpp -- launchers of the non-PCG kernels (fluid_kernels.cu, transfer_kernels.cu).  All enqueue-only on `st`.
 #pragma once
+#include "../../include/blub_fluid.h"
 #include "common.cuh"
 
 namespace blub {
@@ -85,6 +86,7 @@ struct FlowSet {
     int num_sources, num_drains;
     FlowBox source[FLOW_MAX_BOXES], drain[FLOW_MAX_BOXES];
     float velocity[FLOW_MAX_BOXES][3];    // cells/s
+    uint32_t tag[FLOW_MAX_BOXES];         // the particle tag every emitted particle of a source carries
     uint32_t source_base[FLOW_MAX_BOXES + 1]; // exclusive prefix of the source box volumes: index of a box's first cell in the source cell list
 };
 struct FlowScratch {
@@ -100,5 +102,14 @@ struct FlowScratch {
 // pos_spare / row_spare: arrays of the same capacity the drain compaction writes into before it copies the suffix back.
 void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params, uint32_t capacity, const FlowSet &fs, const FlowScratch &s, float4 *pos,
                           float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox);
+
+// ---- particle tags (flow_kernels.cu, DESIGN.md §8 "Particle tags"): the raw bits of the fourth word of every position ----
+constexpr uint32_t TAG_CENSUS_MAX = 256; // tags per census: the block-private table
+// The particle count: params->num_particles when `params` is not null (device-count mode), else `n_host`.  np_upper sizes the launch.
+void launch_paint_tags(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t n_host, uint32_t np_upper, const FlowBox &box, uint32_t tag,
+                       float4 *pos);
+// out: num_tags device records, count / sums zero and bounds at INT32_MAX / INT32_MIN on entry
+void launch_tag_census(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t n_host, uint32_t np_upper, uint32_t first, uint32_t num_tags,
+                       const float4 *pos, float4 *const row[3], BlubTagCensus *out);
 
 } // namespace blub

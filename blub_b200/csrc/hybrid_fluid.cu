@@ -132,6 +132,7 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
         field_density_.reset(new PressureField(grid_, cfg));
     }
     BLUB_CUDA_CHECK(cudaMalloc(&params_dev_, sizeof(StepParams)));
+    BLUB_CUDA_CHECK(cudaMemset(params_dev_, 0, sizeof(StepParams))); // a device count of 0 until particles arrive
     BLUB_CUDA_CHECK(cudaMallocHost(&params_host_, sizeof(StepParams) * 64));
     for (int k = 0; k < 64; ++k) BLUB_CUDA_CHECK(cudaEventCreateWithFlags(&param_events_[k], cudaEventDisableTiming));
     BLUB_CUDA_CHECK(cudaDeviceSynchronize());
@@ -183,6 +184,7 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.scan_sums);
     cudaFree(flow_scratch_.scalars);
     cudaFree(flow_scratch_.counters);
+    cudaFree(census_dev_);
     cudaFree(mig_counters_);
     if (slab_error_host_) cudaFreeHost(slab_error_host_);
     cudaFree(params_dev_);
@@ -200,7 +202,13 @@ static uint32_t clamp_to_grid(uint32_t dim, float v) { // hybrid_fluid.rs:609-61
     return m < 1 ? 1 : m;
 }
 
-bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3]) {
+static float tag_bits(uint32_t tag) { // the tag as the raw bits of the fourth position word
+    float w;
+    std::memcpy(&w, &tag, sizeof(w));
+    return w;
+}
+
+bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3], uint32_t tag) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     if (flow_active_) num_particles_ = num_particles(); // sources and drains change the count on the device
     // a slab rank takes GLOBAL grid coordinates: the cube is clamped against the global grid and every rank keeps its part
@@ -217,7 +225,7 @@ bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3
         num_new = max_num_particles_ - num_particles_;
         truncated = true;
     }
-    if (slab_world_ > 1) return add_fluid_cube_slab(mn, ext);
+    if (slab_world_ > 1) return add_fluid_cube_slab(mn, ext, tag);
     if (num_new == 0) return truncated;
     Xoshiro256pp rng((uint64_t)(num_particles_ + num_new)); // :637
     std::vector<float4> fresh(num_new);
@@ -230,7 +238,7 @@ bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3
             const float r = rng.next_f32();
             p[k] = cell[k] + (strat[k] * 0.5f + r * 0.5f); // stratified jitter, :664-665
         }
-        fresh[i] = make_float4(p[0], p[1], p[2], 0.0f);
+        fresh[i] = make_float4(p[0], p[1], p[2], tag_bits(tag));
     }
     BLUB_CUDA_CHECK(cudaMemcpyAsync(pos_[cur_] + num_particles_, fresh.data(), (size_t)num_new * sizeof(float4), cudaMemcpyHostToDevice, stream_));
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // `fresh` is pageable: finish before it dies (queue.write_buffer semantics)
@@ -242,7 +250,7 @@ bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3
 // Slab rank: the same particle stream as the single-GPU seeding (same RNG draws in the same order -- the seed is the GLOBAL
 // particle count, hybrid_fluid.rs:637), of which this rank keeps the particles whose cell lies in its planes, re-based to
 // local z.  `seeded_global_` mirrors the reference's running num_particles for the seed of the next cube.
-bool HybridFluid::add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3]) {
+bool HybridFluid::add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3], uint32_t tag) {
     const uint32_t num_new = ext[0] * ext[1] * ext[2] * PARTICLES_PER_GRID_CELL;
     if (num_new == 0) return false;
     const int zs = solver_->comm.owned_nz;
@@ -260,7 +268,7 @@ bool HybridFluid::add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3
             const float r = rng.next_f32();
             p[k] = cell[k] + (strat[k] * 0.5f + r * 0.5f);
         }
-        if (cz >= z0 && cz < z1) fresh.push_back(make_float4(p[0], p[1], p[2] - (float)z0 + (float)SLAB_HALO, 0.0f));
+        if (cz >= z0 && cz < z1) fresh.push_back(make_float4(p[0], p[1], p[2] - (float)z0 + (float)SLAB_HALO, tag_bits(tag)));
     }
     seeded_global_ += num_new;
     bool truncated = false;
@@ -633,20 +641,22 @@ void HybridFluid::solve_only(int which, double simulation_delta_seconds) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // Sources and drains (flow_kernels.cu).  Not in the reference.
-FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+FlowBox clamp_box(const uint32_t dim[3], const float mn[3], const float mx[3], const char *what) {
+    FlowBox b;
+    for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(mn[k]) || !std::isfinite(mx[k])) throw std::invalid_argument(std::string(what) + " corner is not finite");
+        b.lo[k] = (int)clamp_to_grid(dim[k], mn[k]);
+        b.hi[k] = (int)clamp_to_grid(dim[k], mx[k]);
+        if (b.hi[k] <= b.lo[k]) throw std::invalid_argument(std::string(what) + " box is empty after clamping to the grid");
+    }
+    return b;
+}
+
+FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
+                      uint32_t num_drains) {
     if (num_sources > (uint32_t)FLOW_MAX_BOXES || num_drains > (uint32_t)FLOW_MAX_BOXES) throw std::invalid_argument("at most 16 sources and 16 drains");
     if ((num_sources && !sources) || (num_drains && !drains)) throw std::invalid_argument("NULL box array");
     FlowSet fs{};
-    auto box_of = [&](const float mn[3], const float mx[3], const char *what) {
-        FlowBox b;
-        for (int k = 0; k < 3; ++k) {
-            if (!std::isfinite(mn[k]) || !std::isfinite(mx[k])) throw std::invalid_argument(std::string(what) + " corner is not finite");
-            b.lo[k] = (int)clamp_to_grid(dim[k], mn[k]);
-            b.hi[k] = (int)clamp_to_grid(dim[k], mx[k]);
-            if (b.hi[k] <= b.lo[k]) throw std::invalid_argument(std::string(what) + " box is empty after clamping to the grid");
-        }
-        return b;
-    };
     auto overlap = [](const FlowBox &a, const FlowBox &b) {
         for (int k = 0; k < 3; ++k)
             if (a.hi[k] <= b.lo[k] || b.hi[k] <= a.lo[k]) return false;
@@ -655,7 +665,8 @@ FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uin
     fs.num_sources = (int)num_sources;
     fs.num_drains = (int)num_drains;
     for (uint32_t s = 0; s < num_sources; ++s) {
-        fs.source[s] = box_of(sources[s].min_grid, sources[s].max_grid, "source");
+        fs.source[s] = clamp_box(dim, sources[s].min_grid, sources[s].max_grid, "source");
+        fs.tag[s] = source_tags ? source_tags[s] : 0u;
         for (int k = 0; k < 3; ++k) {
             if (!std::isfinite(sources[s].velocity_grid[k])) throw std::invalid_argument("source velocity is not finite");
             fs.velocity[s][k] = sources[s].velocity_grid[k];
@@ -664,7 +675,7 @@ FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uin
         fs.source_base[s + 1] = fs.source_base[s] + (uint32_t)((b.hi[0] - b.lo[0]) * (b.hi[1] - b.lo[1]) * (b.hi[2] - b.lo[2]));
     }
     for (uint32_t s = num_sources; s < (uint32_t)FLOW_MAX_BOXES; ++s) fs.source_base[s + 1] = fs.source_base[s];
-    for (uint32_t d = 0; d < num_drains; ++d) fs.drain[d] = box_of(drains[d].min_grid, drains[d].max_grid, "drain");
+    for (uint32_t d = 0; d < num_drains; ++d) fs.drain[d] = clamp_box(dim, drains[d].min_grid, drains[d].max_grid, "drain");
     for (uint32_t s = 0; s < num_sources; ++s) {
         for (uint32_t t = s + 1; t < num_sources; ++t)
             if (overlap(fs.source[s], fs.source[t])) throw std::invalid_argument("two sources overlap");
@@ -674,11 +685,12 @@ FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, uin
     return fs;
 }
 
-void HybridFluid::set_flow(const BlubFluidSource *sources, uint32_t num_sources, const BlubFluidDrain *drains, uint32_t num_drains) {
+void HybridFluid::set_flow(const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
+                           uint32_t num_drains) {
     if (slab_world_ > 1) throw std::invalid_argument("set_flow: z-slab ranks have no sources or drains");
     if (mid_step_) throw std::invalid_argument("set_flow: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
-    restore_flow(make_flow_set(dim, sources, num_sources, drains, num_drains), nullptr);
+    restore_flow(make_flow_set(dim, sources, source_tags, num_sources, drains, num_drains), nullptr);
 }
 
 // Applies a validated set; counters != nullptr also sets the cumulative counters (state file load).
@@ -740,31 +752,69 @@ void HybridFluid::run_flow_prologue() {
     launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, voxels_);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Particle tags (flow_kernels.cu).  Not in the reference.  In device-count mode the kernels read the count from StepParams (a step or
+// set_device_particle_count wrote it); otherwise the host count is passed, since StepParams may not have been uploaded yet.
+void HybridFluid::paint_tags(const float min_grid[3], const float max_grid[3], uint32_t tag) {
+    if (slab_world_ > 1) throw std::invalid_argument("paint_tags: z-slab ranks cannot paint");
+    if (mid_step_) throw std::invalid_argument("paint_tags: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    const FlowBox box = clamp_box(dim, min_grid, max_grid, "paint");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const bool dev = device_count_mode();
+    launch_paint_tags(stream_, grid_, dev ? params_dev_ : nullptr, num_particles_, dev ? max_num_particles_ : num_particles_, box, tag, pos_[cur_]);
+}
+
+void HybridFluid::tag_census(uint32_t first, uint32_t num_tags, BlubTagCensus *out) {
+    if (num_tags == 0 || num_tags > TAG_CENSUS_MAX) throw std::invalid_argument("tag_census: num_tags must be 1 .. 256");
+    if ((uint64_t)first + num_tags > (1ull << 32)) throw std::invalid_argument("tag_census: first_tag + num_tags exceeds 2^32");
+    if (!out) throw std::invalid_argument("tag_census: NULL output");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (!census_dev_) BLUB_CUDA_CHECK(cudaMalloc(&census_dev_, TAG_CENSUS_MAX * sizeof(BlubTagCensus)));
+    for (uint32_t t = 0; t < num_tags; ++t) {
+        out[t] = BlubTagCensus{};
+        for (int k = 0; k < 3; ++k) {
+            out[t].cell_min[k] = INT32_MAX;
+            out[t].cell_max[k] = INT32_MIN;
+        }
+    }
+    const size_t bytes = (size_t)num_tags * sizeof(BlubTagCensus);
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(census_dev_, out, bytes, cudaMemcpyHostToDevice, stream_));
+    const bool dev = device_count_mode();
+    launch_tag_census(stream_, grid_, dev ? params_dev_ : nullptr, num_particles_, dev ? max_num_particles_ : num_particles_, first, num_tags, pos_[cur_],
+                      row_, census_dev_);
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(out, census_dev_, bytes, cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+}
+
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream) {
     std::unique_ptr<HybridFluid> f(new HybridFluid(cfg.grid_dimension[0], cfg.grid_dimension[1], cfg.grid_dimension[2], cfg.max_num_particles, device, stream));
     const float scale = cfg.grid_to_world_scale;
     for (const SceneBox &b : cfg.fluid_cubes) { // src/scene/mod.rs:132-138
         const float mn[3] = {b.min[0] / scale, b.min[1] / scale, b.min[2] / scale};
         const float mx[3] = {b.max[0] / scale, b.max[1] / scale, b.max[2] / scale};
-        f->add_fluid_cube(mn, mx);
+        f->add_fluid_cube(mn, mx, b.tag);
     }
     const float g[3] = {cfg.gravity[0] / scale, cfg.gravity[1] / scale, cfg.gravity[2] / scale}; // :139
     f->set_gravity_grid(g);
     if (!cfg.sources.empty() || !cfg.drains.empty()) { // after the cubes
         std::vector<BlubFluidSource> src(cfg.sources.size());
         std::vector<BlubFluidDrain> drn(cfg.drains.size());
-        for (size_t i = 0; i < src.size(); ++i)
+        std::vector<uint32_t> tags(cfg.sources.size());
+        for (size_t i = 0; i < src.size(); ++i) {
+            tags[i] = cfg.sources[i].tag;
             for (int k = 0; k < 3; ++k) {
                 src[i].min_grid[k] = cfg.sources[i].min[k] / scale;
                 src[i].max_grid[k] = cfg.sources[i].max[k] / scale;
                 src[i].velocity_grid[k] = cfg.sources[i].velocity[k] / scale;
             }
+        }
         for (size_t i = 0; i < drn.size(); ++i)
             for (int k = 0; k < 3; ++k) {
                 drn[i].min_grid[k] = cfg.drains[i].min[k] / scale;
                 drn[i].max_grid[k] = cfg.drains[i].max[k] / scale;
             }
-        f->set_flow(src.data(), (uint32_t)src.size(), drn.data(), (uint32_t)drn.size());
+        f->set_flow(src.data(), tags.data(), (uint32_t)src.size(), drn.data(), (uint32_t)drn.size());
     }
     return f;
 }

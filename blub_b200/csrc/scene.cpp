@@ -137,6 +137,11 @@ void vec3(const JsonValue &obj, const char *what, float out[3]) {
     out[1] = num_f32(need(obj, "y"), what);
     out[2] = num_f32(need(obj, "z"), what);
 }
+// optional particle tag of a fluid cube or a source (not in the reference, whose serde structs ignore unknown keys): an integer in [0, 2^32)
+uint32_t tag_of(const JsonValue &obj, const char *what) {
+    const JsonValue *v = obj.get("tag");
+    return v ? num_u32(*v, what) : 0u;
+}
 
 } // namespace
 
@@ -168,6 +173,7 @@ SceneConfig parse_scene_file(const std::string &path) {
         SceneBox b;
         vec3(need(c, "min"), "fluid_cubes.min", b.min);
         vec3(need(c, "max"), "fluid_cubes.max", b.max);
+        b.tag = tag_of(c, "fluid_cubes.tag");
         cfg.fluid_cubes.push_back(b);
     }
     // sources and drains (not in the reference, whose serde structs ignore unknown keys): world units and m/s, both optional
@@ -178,6 +184,7 @@ SceneConfig parse_scene_file(const std::string &path) {
             vec3(need(s, "min"), "sources.min", b.min);
             vec3(need(s, "max"), "sources.max", b.max);
             vec3(need(s, "velocity"), "sources.velocity", b.velocity);
+            b.tag = tag_of(s, "sources.tag");
             cfg.sources.push_back(b);
         }
     }

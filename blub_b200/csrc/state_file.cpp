@@ -20,8 +20,10 @@ namespace {
 static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the state file is little-endian and written as the host lays it out");
 
 constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
-// version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters
-constexpr uint32_t kFormatVersionFlow = 2;
+// version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters; version 4:
+// section 14 followed by the sources' particle tags (written only when one of them is not 0).  Version 3 is not a format: no build writes
+// it and readers refuse it.
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4;
 constexpr uint32_t kNumSections = 14; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
@@ -39,6 +41,12 @@ struct FlowSection {
     uint64_t counters[3];  // emitted, drained, refused for capacity
 };
 static_assert(sizeof(FlowSection) == 992 && FLOW_MAX_BOXES == 16, "flow section layout");
+// Section 14 of version 4
+struct FlowSectionTagged {
+    FlowSection flow;
+    uint32_t source_tags[16]; // unused slots zero
+};
+static_assert(sizeof(FlowSectionTagged) == 1056, "tagged flow section layout");
 
 struct StateHeader {
     char magic[8];
@@ -79,9 +87,9 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
                                      {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
                                      {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
-                                     {SEC_FLOW, sizeof(FlowSection)}};
+                                     {SEC_FLOW, h.format_version == kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)}};
     std::memcpy(out, s, sizeof(s));
-    return h.format_version == kFormatVersionFlow ? 14 : 13;
+    return h.format_version >= kFormatVersionFlow ? 14 : 13;
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -153,8 +161,8 @@ StateHeader read_header(File &f) {
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
-    if (h.format_version != 1 && h.format_version != kFormatVersionFlow)
-        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads versions 1 and 2)");
+    if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags)
+        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads versions 1, 2 and 4)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -234,8 +242,9 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
     f.write(&crc, 4);
 }
 
-// The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.
-FlowSet flow_set_of(const FlowSection &fl, const StateHeader &h, const std::string &path) {
+// The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.  tags: the sources'
+// particle tags (version 4), or nullptr.
+FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHeader &h, const std::string &path) {
     if (fl.num_sources > 16 || fl.num_drains > 16 || fl.num_sources + fl.num_drains == 0)
         throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
     std::vector<BlubFluidSource> src(fl.num_sources);
@@ -253,7 +262,7 @@ FlowSet flow_set_of(const FlowSection &fl, const StateHeader &h, const std::stri
         }
     FlowSet fs;
     try {
-        fs = make_flow_set(h.grid_dimension, src.data(), fl.num_sources, drn.data(), fl.num_drains);
+        fs = make_flow_set(h.grid_dimension, src.data(), tags, fl.num_sources, drn.data(), fl.num_drains);
     } catch (const std::invalid_argument &e) {
         throw ParseError(path + ": section 14: " + e.what());
     }
@@ -278,9 +287,9 @@ StateInfo read_state_info(const std::string &path) {
     Staging st(false);
     for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
     if (ns == 14) {
-        FlowSection fl;
+        FlowSectionTagged fl{};
         read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
-        flow_set_of(fl, h, f.path);
+        flow_set_of(fl.flow, fl.source_tags, h, f.path);
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -299,7 +308,9 @@ void HybridFluid::save_state(const std::string &path) {
     update_statistics(); // every finished solve is in the history now
     StateHeader h{}; // no padding: every byte written is a field or zero
     std::memcpy(h.magic, kMagic, sizeof(kMagic));
-    h.format_version = flow_active_ ? kFormatVersionFlow : 1;
+    bool source_tags = false;
+    for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
+    h.format_version = !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -345,12 +356,14 @@ void HybridFluid::save_state(const std::string &path) {
         write_host_section(f, SEC_STATS_VELOCITY, stats[0].data(), stats[0].size() * sizeof(SolverStatisticSample));
         write_host_section(f, SEC_STATS_DENSITY, stats[1].data(), stats[1].size() * sizeof(SolverStatisticSample));
         if (flow_active_) {
-            FlowSection fl{};
+            FlowSectionTagged tagged{};
+            FlowSection &fl = tagged.flow;
             fl.num_sources = (uint32_t)flow_.num_sources;
             fl.num_drains = (uint32_t)flow_.num_drains;
             for (int b = 0; b < FLOW_MAX_BOXES; ++b)
                 for (int k = 0; k < 3; ++k) {
                     if (b < flow_.num_sources) {
+                        tagged.source_tags[b] = flow_.tag[b];
                         fl.source[b][k] = flow_.source[b].lo[k];
                         fl.source[b][3 + k] = flow_.source[b].hi[k];
                         fl.velocity[b][k] = flow_.velocity[b][k];
@@ -361,7 +374,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &fl, sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags ? sizeof(tagged) : sizeof(fl));
         }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
@@ -420,11 +433,11 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     }
     x.fluid_bits_stale_ = true; // rebuilt from the restored marker volume before the next grid pass that reads it
     if (ns == 14) {
-        FlowSection fl;
+        FlowSectionTagged fl{};
         to_host(sec[13], &fl);
-        const FlowSet fs = flow_set_of(fl, h, f.path);
+        const FlowSet fs = flow_set_of(fl.flow, fl.source_tags, h, f.path);
         BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
-        x.restore_flow(fs, fl.counters); // the device takes over the restored count
+        x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

@@ -1009,12 +1009,11 @@ __global__ void __launch_bounds__(PT) density_rhs_kernel(GridDim g, const StepPa
 // ------------------------------------------------------------------------------------------------ binning
 // particle_binning_rewrite_particles.comp: the cell lists ARE the sorted order -- dst[j] = src[order[j]] (x-fastest cell order,
 // ascending previous index inside a cell: deterministic; the reference's atomic ranks are not, and its inclusive - index
-// addressing loses a particle, SURVEY B2).
+// addressing loses a particle, SURVEY B2).  The whole float4 moves: its fourth word is the particle's tag (raw bits, never arithmetic).
 __device__ __forceinline__ void binning_permute_kernel_one(uint32_t j, const StepParams *__restrict__ params, const uint32_t *__restrict__ order,
                                                              const float4 *__restrict__ src, float4 *__restrict__ dst) {
     if (j >= params->num_particles) return;
-    const float4 p = src[order[j]];
-    dst[j] = make_float4(p.x, p.y, p.z, 0.0f);
+    dst[j] = src[order[j]];
 }
 __global__ void __launch_bounds__(PT) binning_permute_kernel(const StepParams *__restrict__ params, const uint32_t *__restrict__ order,
                                                              const float4 *__restrict__ src, float4 *__restrict__ dst) {

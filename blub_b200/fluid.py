@@ -26,6 +26,8 @@ TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, 
 
 BLUB_OK = 0
 BLUB_WARN_TRUNCATED = 100
+TAG_CENSUS_FRAC_BITS = 16  # BLUB_TAG_CENSUS_FRAC_BITS: census sums are sums of rint(value * 2^16)
+TAG_CENSUS_MAX = 256       # tags per census
 
 
 class BlubError(RuntimeError):
@@ -106,6 +108,13 @@ class FluidDrain(C.Structure):
     _fields_ = [("min_grid", C.c_float * 3), ("max_grid", C.c_float * 3)]
 
 
+class TagCensus(C.Structure):
+    """BlubTagCensus: what the particles of one tag add up to (sums in 2^16 fixed point)."""
+
+    _fields_ = [("count", C.c_uint64), ("position_sum_fx", C.c_int64 * 3), ("velocity_sum_fx", C.c_int64 * 3), ("cell_min", C.c_int32 * 3),
+                ("cell_max", C.c_int32 * 3)]
+
+
 def lib_path() -> str:
     return os.path.join(_HERE, "libblubcore.so")
 
@@ -151,6 +160,7 @@ def lib():
         "blub_ipc_close": (C.c_int, [vp]),
         "blub_enable_peer_access": (C.c_int, [C.c_int, C.c_int]),
         "blub_fluid_add_cube": (C.c_int, [vp, f3, f3]),
+        "blub_fluid_add_cube_tagged": (C.c_int, [vp, f3, f3, u32]),
         "blub_fluid_set_gravity_grid": (C.c_int, [vp, f3]),
         "blub_fluid_num_particles": (u32, [vp]),
         "blub_fluid_grid_dimension": (None, [vp, C.POINTER(u32)]),
@@ -170,6 +180,9 @@ def lib():
         "blub_fluid_set_flow": (C.c_int, [vp, C.POINTER(FluidSource), u32, C.POINTER(FluidDrain), u32]),
         "blub_fluid_flow_counters": (C.c_int, [vp, C.POINTER(C.c_uint64)]),
         "blub_fluid_has_flow": (C.c_int, [vp]),
+        "blub_fluid_set_flow_tagged": (C.c_int, [vp, C.POINTER(FluidSource), C.POINTER(u32), u32, C.POINTER(FluidDrain), u32]),
+        "blub_fluid_paint_tags": (C.c_int, [vp, f3, f3, u32]),
+        "blub_fluid_tag_census": (C.c_int, [vp, u32, u32, C.POINTER(TagCensus)]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -381,8 +394,9 @@ class HybridFluid:
             pass
 
     # -- reference surface --------------------------------------------------------------------
-    def add_fluid_cube(self, min_grid, max_grid):
-        rc = _check(self.L.blub_fluid_add_cube(self.h, _f3(min_grid), _f3(max_grid)), allow=(BLUB_OK, BLUB_WARN_TRUNCATED))
+    def add_fluid_cube(self, min_grid, max_grid, tag=0):
+        """hybrid_fluid.rs:620-678; every new particle carries the particle tag `tag` (uint32).  True when truncated to max_num_particles."""
+        rc = _check(self.L.blub_fluid_add_cube_tagged(self.h, _f3(min_grid), _f3(max_grid), int(tag)), allow=(BLUB_OK, BLUB_WARN_TRUNCATED))
         return rc == BLUB_WARN_TRUNCATED
 
     def set_gravity_grid(self, g):
@@ -494,16 +508,45 @@ class HybridFluid:
         _check(self.L.blub_fluid_set_solver_path(self.h, mode))
 
     def set_flow(self, sources=(), drains=()):
-        """Replaces the flow set: sources = [(min, max, velocity)], drains = [(min, max)], boxes in grid cells, velocities in cells/s.
-        Empty lists clear it.  Raises BlubError (and changes nothing) on overlaps, more than 16 boxes of a kind, non-finite values, boxes
-        empty after clamping, z-slab ranks and a fluid inside a step."""
+        """Replaces the flow set: sources = [(min, max, velocity[, tag])], drains = [(min, max)], boxes in grid cells, velocities in cells/s;
+        the particles a source emits carry its tag (default 0).  Empty lists clear it.  Raises BlubError (and changes nothing) on overlaps, more
+        than 16 boxes of a kind, non-finite values, boxes empty after clamping, z-slab ranks and a fluid inside a step."""
         src = (FluidSource * max(len(sources), 1))()
-        for k, (mn, mx, vel) in enumerate(sources):
+        tags = (C.c_uint32 * max(len(sources), 1))()
+        for k, (mn, mx, vel, *tag) in enumerate(sources):
             src[k].min_grid[:], src[k].max_grid[:], src[k].velocity_grid[:] = [float(v) for v in mn], [float(v) for v in mx], [float(v) for v in vel]
+            tags[k] = int(tag[0]) if tag else 0
         drn = (FluidDrain * max(len(drains), 1))()
         for k, (mn, mx) in enumerate(drains):
             drn[k].min_grid[:], drn[k].max_grid[:] = [float(v) for v in mn], [float(v) for v in mx]
-        _check(self.L.blub_fluid_set_flow(self.h, src, len(sources), drn, len(drains)))
+        _check(self.L.blub_fluid_set_flow_tagged(self.h, src, tags, len(sources), drn, len(drains)))
+
+    # -- particle tags ------------------------------------------------------------------------
+    def paint_tags(self, min_grid, max_grid, tag):
+        """Tags every particle whose cell lies in the box (corners clamped as add_fluid_cube clamps them, max exclusive).  Enqueued on the
+        fluid's stream, no synchronisation."""
+        _check(self.L.blub_fluid_paint_tags(self.h, _f3(min_grid), _f3(max_grid), int(tag)))
+
+    def particle_tags(self):
+        """The tag of every particle in array order: a uint32 view of the fourth column of the positions."""
+        return self.download_particles(TAP_POS)[:, 3].view(np.uint32)
+
+    def tag_census(self, first=0, count=TAG_CENSUS_MAX):
+        """Census of tags first .. first + count - 1 (count <= 256): the raw fields of BlubTagCensus as arrays ("count", "position_sum_fx",
+        "velocity_sum_fx", "cell_min", "cell_max"), plus "centroid" and "mean_velocity" (float64, NaN for an empty tag).  Synchronises."""
+        count = int(count)
+        out = (TagCensus * max(count, 1))()
+        _check(self.L.blub_fluid_tag_census(self.h, int(first), count, out))
+        recs = out[:count]
+        res = {"count": np.array([r.count for r in recs], dtype=np.uint64)}
+        for name, dt in (("position_sum_fx", np.int64), ("velocity_sum_fx", np.int64), ("cell_min", np.int32), ("cell_max", np.int32)):
+            res[name] = np.array([list(getattr(r, name)) for r in recs], dtype=dt).reshape(-1, 3)
+        scale = float(1 << TAG_CENSUS_FRAC_BITS)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            n = res["count"].astype(np.float64)[:, None]
+            res["centroid"] = res["position_sum_fx"].astype(np.float64) / scale / n
+            res["mean_velocity"] = res["velocity_sum_fx"].astype(np.float64) / scale / n
+        return res
 
     @property
     def has_flow(self):

@@ -69,7 +69,7 @@ typedef struct {
 
 /* The ten read-only resources of HybridFluid::bind_group_renderer (hybrid_fluid.rs:351-369,700-713). */
 typedef struct {
-    const void *particles_position_ll;            /* num_particles x {float3 pos, uint32 unused}  */
+    const void *particles_position_ll;            /* num_particles x {float3 pos, uint32 tag} (see "particle tags") */
     const void *particles_velocity_x;             /* num_particles x float4 (C column xyz, v_x)   */
     const void *particles_velocity_y;
     const void *particles_velocity_z;
@@ -167,6 +167,36 @@ int blub_fluid_set_flow(BlubFluid *fluid, const BlubFluidSource *sources, uint32
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]);
 /* 1 when the fluid has a non-empty flow set, 0 when not or when fluid is NULL */
 int blub_fluid_has_flow(const BlubFluid *fluid);
+
+/* ---- particle tags (not part of the reference surface; rules: DESIGN.md section 8) ---------------------------------------------
+ * The fourth word of every particle position is its tag: a uint32 stored as raw bits, which no step reads and every path copies (binning,
+ * re-sort, drain compaction, z-slab migration, checkpoints).  A fluid whose tags are all 0 computes exactly what it computed before tags
+ * existed.  Tags are set by blub_fluid_add_cube_tagged (the new particles), by the sources of blub_fluid_set_flow_tagged (every particle they
+ * emit), by blub_fluid_paint_tags, and directly through the fourth word of blub_fluid_set_particles / blub_fluid_upload(BLUB_TAP_PARTICLE_POS).
+ * Non-zero bits written there are kept by the binning (before tags existed it zeroed the word). */
+/* blub_fluid_add_cube with every new particle tagged `tag` (blub_fluid_add_cube is tag 0) */
+int blub_fluid_add_cube_tagged(BlubFluid *fluid, const float min_grid[3], const float max_grid[3], uint32_t tag);
+/* blub_fluid_set_flow with a tag per source (NULL = all 0; blub_fluid_set_flow passes NULL): the particles a source emits carry its tag,
+ * particles already in a source cell keep theirs */
+int blub_fluid_set_flow_tagged(BlubFluid *fluid, const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources,
+                               const BlubFluidDrain *drains, uint32_t num_drains);
+/* Tags every particle whose cell (the drains' cell rule) lies in the box, corners clamped as blub_fluid_add_cube clamps them (max exclusive).
+ * Stream-ordered, never synchronises; works on the device-resident count while a flow set is active.  BLUB_ERR_INVALID_ARGUMENT, changing
+ * nothing: a non-finite corner, a box empty after clamping, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_paint_tags(BlubFluid *fluid, const float min_grid[3], const float max_grid[3], uint32_t tag);
+/* What the particles of one tag add up to.  Sums are 2^16 fixed point: every particle contributes rint(value * 65536) (round to nearest
+ * even; the product is exact), added as int64, so they are exact and independent of the particle order.  They stay exact for positions below
+ * 2^10 cells, |v| <= 2^20 cells/s and at most 2^26 particles per tag.  Cells by the drains' rule; count == 0: cell_min = INT32_MAX,
+ * cell_max = INT32_MIN. */
+#define BLUB_TAG_CENSUS_FRAC_BITS 16
+typedef struct {
+    uint64_t count;
+    int64_t position_sum_fx[3], velocity_sum_fx[3]; /* velocity component c = .w of velocity row c */
+    int32_t cell_min[3], cell_max[3];
+} BlubTagCensus;
+/* out[k] = census of tag first_tag + k for k < num_tags; particles with other tags are skipped.  On a z-slab rank: this rank's particles.
+ * Synchronises.  BLUB_ERR_INVALID_ARGUMENT: num_tags of 0 or above 256, or first_tag + num_tags above 2^32. */
+int blub_fluid_tag_census(BlubFluid *fluid, uint32_t first_tag, uint32_t num_tags, BlubTagCensus *out);
 
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
@@ -289,7 +319,7 @@ enum {
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes);
-/* replace the particle set (positions xyz_, three velocity rows); rows may be NULL (zero) */
+/* replace the particle set (positions xyz + the tag bits in the fourth word, three velocity rows); rows may be NULL (zero) */
 int blub_fluid_set_particles(BlubFluid *fluid, uint32_t count, const float *pos4, const float *vx4, const float *vy4,
                              const float *vz4);
 /* run stages [from, to) of the 14-stage list of one step (same numbering as oracle/blub_oracle.c:orc_step_stages) */

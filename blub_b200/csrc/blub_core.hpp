@@ -243,7 +243,20 @@ class HybridFluid {
     void paint_tags(const float min_grid[3], const float max_grid[3], uint32_t tag);
     void tag_census(uint32_t first, uint32_t num_tags, BlubTagCensus *out);
 
+    // Solid load probes (load_kernels.cu): replaces the whole set (0 clears it), resets the history and drops the step graphs.  Throws
+    // std::invalid_argument and changes nothing on more than LOAD_PROBES_MAX probes, a non-finite corner or pivot, a box empty after clamping,
+    // a z-slab rank or a fluid inside a step.  While the set is not empty, stage 2 of every step records one BlubSolidLoad per probe.
+    void set_load_probes(const BlubLoadProbe *probes, uint32_t num_probes);
+    uint32_t num_load_probes() const { return num_load_probes_; }
+    // the newest min(capacity, recorded, LOAD_HISTORY_LENGTH) records of `probe`, oldest first; returns their number (synchronises)
+    uint32_t load_history(uint32_t probe, BlubSolidLoad *out, uint32_t capacity);
+
   private:
+    LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
+    BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
+    uint32_t num_load_probes_ = 0, load_max_cells_ = 0;
+    std::deque<uint32_t> load_steps_; // step numbers of the records in the ring, oldest first (at most LOAD_HISTORY_LENGTH)
+    void note_load_record(uint32_t step);
     BlubTagCensus *census_dev_ = nullptr; // TAG_CENSUS_MAX records, allocated with the first census
     bool device_count_mode() const { return slab_world_ > 1 || flow_active_; }
     void run_flow_prologue();
@@ -357,6 +370,9 @@ struct StateInfo {
 // A box in grid units clamped like add_fluid_cube (corners in [1, dim - 1], max exclusive); throws std::invalid_argument on a non-finite corner
 // or a box that is empty after clamping (`what` names it in the message).
 FlowBox clamp_box(const uint32_t dim[3], const float min_grid[3], const float max_grid[3], const char *what);
+// A load probe in grid units: corners converted as clamp_box converts them but clamped to [0, dim] (max exclusive); throws
+// std::invalid_argument on a non-finite corner or pivot or a box that is empty after clamping.
+LoadProbeBox clamp_load_probe(const uint32_t dim[3], const BlubLoadProbe &probe);
 // A flow set from the public boxes (grid units), clamped like add_fluid_cube; throws std::invalid_argument when it breaks a rule of set_flow
 // that does not depend on the fluid.  source_tags may be nullptr (all 0).
 FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
@@ -390,6 +406,10 @@ struct SceneSource {
     float min[3], max[3], velocity[3];
     uint32_t tag = 0;
 };
+struct SceneLoadProbe {
+    float min[3], max[3], pivot[3];
+    bool has_pivot = false; // without one the pivot is the box centre
+};
 struct SceneConfig {
     float gravity[3] = {0, 0, 0};
     float world_position[3] = {0, 0, 0};
@@ -399,10 +419,13 @@ struct SceneConfig {
     std::vector<SceneBox> fluid_cubes;
     std::vector<SceneSource> sources; // optional fluid.sources / fluid.drains (world units, m/s)
     std::vector<SceneBox> drains;
+    std::vector<SceneLoadProbe> load_probes; // optional fluid.load_probes (world units)
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };
 SceneConfig parse_scene_file(const std::string &path);
+// the scene's load probes in grid cells: corners and pivot / grid_to_world_scale, pivot (min + max) / 2 when the scene gives none
+std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
 // Scene::create_fluid_from_config, src/scene/mod.rs:109-144
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream);
 

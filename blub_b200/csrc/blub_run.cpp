@@ -16,6 +16,10 @@
 //   --save-state FILE  the fluid's complete state after the last step (blub_fluid_save_state); --checkpoint-every N also rewrites FILE every
 //                  N steps at batch boundaries.  --load-state FILE resumes such a file instead of seeding the scene's fluid cubes: the scene
 //                  still provides scale, origin and static objects, and the simulation clock restarts at step_count * dt.
+//   --loads FILE   the history of the scene's solid load probes (fluid.load_probes) as JSON: the probes in grid cells and one record per
+//                  step and probe, force in cells^4/s^2 and torque in cells^5/s^2 per unit density.  The device ring holds the newest 1024
+//                  steps; the runner reads it at every batch or frame boundary, so a long run loses nothing.  With --load-state the scene's
+//                  probes are set again (a state file holds none).
 //   --models DIR   where the scene's static_objects find their OBJ files (the reference reads `models/<model>`,
 //                  src/scene/models.rs:253).  Every step then runs Scene::step's order (src/scene/mod.rs:192-211): animate the
 //                  models at the already advanced simulation time, voxelize their hulls, step the fluid.
@@ -45,13 +49,13 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "usage: blub_run scene.json [--steps N] [--batch 16] [--hz 120] [--device 0] [--no-graph]\n"
                              "                [--stats out.json] [--trace out.json] [--dump particles.f32] [--models DIR] [--record FPS PREFIX]\n"
                              "                [--solver TOLERANCE MAX_ITERATIONS CHECK_FREQUENCY] [--rebin EVERY_N_STEPS]\n"
-                             "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE]\n");
+                             "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE] [--loads out.json]\n");
         return 2;
     }
     const char *scene = argv[1];
     int steps = 160, batch = 16, device = 0, graph = 1;
     long hz = 120;
-    std::string stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
+    std::string loads_path, stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
     double record_fps = 0.0;
     float solver_tol = -1.0f;
     int solver_max = 0, solver_freq = 0, rebin = -1, checkpoint_every = 0;
@@ -66,6 +70,7 @@ int main(int argc, char **argv) {
         else if (!std::strcmp(argv[i], "--device")) device = std::atoi(next("--device"));
         else if (!std::strcmp(argv[i], "--no-graph")) graph = 0;
         else if (!std::strcmp(argv[i], "--stats")) stats_path = next("--stats");
+        else if (!std::strcmp(argv[i], "--loads")) loads_path = next("--loads");
         else if (!std::strcmp(argv[i], "--trace")) trace_path = next("--trace");
         else if (!std::strcmp(argv[i], "--dump")) dump_path = next("--dump");
         else if (!std::strcmp(argv[i], "--models")) models_dir = next("--models");
@@ -83,6 +88,10 @@ int main(int argc, char **argv) {
     const double dt = (double)blub_duration_as_secs_f32(dt_ns);
     if (!record_prefix.empty() && !(record_fps > 0.0)) { std::fprintf(stderr, "blub_run: bad --record FPS\n"); return 2; }
     if (!record_prefix.empty() && !load_path.empty()) { std::fprintf(stderr, "blub_run: --load-state cannot resume a --record run\n"); return 2; }
+    if (!loads_path.empty() && batch > BLUB_LOAD_HISTORY_LENGTH) {
+        std::fprintf(stderr, "blub_run: --loads reads the load history at batch boundaries: --batch must not exceed %d\n", BLUB_LOAD_HISTORY_LENGTH);
+        return 2;
+    }
     if (checkpoint_every < 0 || (checkpoint_every > 0 && save_path.empty())) {
         std::fprintf(stderr, "blub_run: --checkpoint-every needs a positive N and --save-state FILE\n");
         return 2;
@@ -115,6 +124,10 @@ int main(int argc, char **argv) {
         }
     }
     if (rebin >= 0) *blub_fluid_rebinning_frequency(fluid) = (uint32_t)rebin;
+    BlubLoadProbe probes[BLUB_LOAD_PROBES_MAX];
+    uint32_t num_probes = 0;
+    if (blub_scene_load_probes(scene, probes, BLUB_LOAD_PROBES_MAX, &num_probes)) die("cannot read the scene's load probes");
+    if (!load_path.empty() && num_probes && blub_fluid_set_load_probes(fluid, probes, num_probes)) die("cannot set the load probes");
     std::printf("scene %s: grid %ux%ux%u, %u particles (max %u), %u static object(s), dt %.9f s\n", scene, info.grid_dimension[0],
                 info.grid_dimension[1], info.grid_dimension[2], blub_fluid_num_particles(fluid), info.max_num_particles, info.num_static_objects, dt);
 
@@ -161,6 +174,19 @@ int main(int argc, char **argv) {
         return n;
     };
 
+    // every record of every probe, collected at batch / frame boundaries (the ring holds the newest BLUB_LOAD_HISTORY_LENGTH steps)
+    std::vector<std::vector<BlubSolidLoad>> loads(num_probes);
+    std::vector<BlubSolidLoad> ring(BLUB_LOAD_HISTORY_LENGTH);
+    auto collect_loads = [&]() {
+        if (loads_path.empty()) return;
+        for (uint32_t p = 0; p < num_probes; ++p) {
+            uint32_t n = 0;
+            if (blub_fluid_load_history(fluid, p, ring.data(), BLUB_LOAD_HISTORY_LENGTH, &n)) die("cannot read the load history");
+            for (uint32_t k = 0; k < n; ++k)
+                if (loads[p].empty() || ring[k].step > loads[p].back().step) loads[p].push_back(ring[k]);
+        }
+    };
+
     const bool has_flow = blub_fluid_has_flow(fluid) == 1;
     int done = 0, saved_at = -1;
     auto save_state = [&]() {
@@ -186,6 +212,7 @@ int main(int argc, char **argv) {
             char name[32];
             std::snprintf(name, sizeof(name), "%05d.f32", frame);
             write_particles(record_prefix + name);
+            collect_loads();
             std::printf("frame %d: %u step(s), simulated %.6f s\n", frame, n, (double)blub_duration_as_secs_f32(simulated_ns));
             checkpoint();
         }
@@ -196,6 +223,7 @@ int main(int argc, char **argv) {
         if (blub_fluid_synchronize(fluid)) die("synchronize failed");
         blub_fluid_update_statistics(fluid);
         done += n;
+        collect_loads();
         if (has_flow) // sources and drains change the particle count as the run goes
             std::printf("simulation fast forwarding batch finished (progress %d/%d, %u particles)\n", done, steps, blub_fluid_num_particles(fluid));
         else
@@ -226,6 +254,28 @@ int main(int argc, char **argv) {
                          (unsigned long long)c[2]);
         }
         std::fprintf(f, "}\n");
+        std::fclose(f);
+    }
+    if (!loads_path.empty()) {
+        FILE *f = std::fopen(loads_path.c_str(), "w");
+        if (!f) { std::perror("blub_run: --loads"); return 1; }
+        const double fs = (double)(1 << BLUB_LOAD_FORCE_FRAC_BITS), ts = (double)(1 << BLUB_LOAD_TORQUE_FRAC_BITS);
+        std::fprintf(f, "{\"grid_to_world_scale\": %.9g, \"dt\": %.9g, \"force_units\": \"cells^4/s^2 per unit density\", "
+                        "\"torque_units\": \"cells^5/s^2 per unit density\", \"probes\": [",
+                     info.grid_to_world_scale, dt);
+        for (uint32_t p = 0; p < num_probes; ++p) {
+            const BlubLoadProbe &q = probes[p];
+            std::fprintf(f, "%s\n {\"min\": [%.9g, %.9g, %.9g], \"max\": [%.9g, %.9g, %.9g], \"pivot\": [%.9g, %.9g, %.9g], \"records\": [", p ? "," : "",
+                         q.min_grid[0], q.min_grid[1], q.min_grid[2], q.max_grid[0], q.max_grid[1], q.max_grid[2], q.pivot_grid[0], q.pivot_grid[1], q.pivot_grid[2]);
+            for (size_t k = 0; k < loads[p].size(); ++k) {
+                const BlubSolidLoad &r = loads[p][k];
+                std::fprintf(f, "%s\n  {\"step\": %u, \"wetted_faces\": %u, \"force\": [%.17g, %.17g, %.17g], \"torque\": [%.17g, %.17g, %.17g]}", k ? "," : "",
+                             r.step, r.wetted_faces, r.force_fx[0] / fs, r.force_fx[1] / fs, r.force_fx[2] / fs, r.torque_fx[0] / ts, r.torque_fx[1] / ts,
+                             r.torque_fx[2] / ts);
+            }
+            std::fprintf(f, "]}");
+        }
+        std::fprintf(f, "\n]}\n");
         std::fclose(f);
     }
     if (!trace_path.empty()) { // "Write Chrometrace" (src/gui/mod.rs:487-491): one eagerly launched, event-timed step

@@ -416,6 +416,29 @@ int blub_fluid_tag_census(BlubFluid *fluid, uint32_t first_tag, uint32_t num_tag
     return guarded([&] { fluid->impl->tag_census(first_tag, num_tags, out); return BLUB_OK; });
 }
 
+int blub_fluid_set_load_probes(BlubFluid *fluid, const BlubLoadProbe *probes, uint32_t num_probes) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_load_probes(probes, num_probes); return BLUB_OK; });
+}
+
+int blub_fluid_load_history(BlubFluid *fluid, uint32_t probe, BlubSolidLoad *out, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *count = 0;
+    return guarded([&] { *count = fluid->impl->load_history(probe, out, capacity); return BLUB_OK; });
+}
+
+int blub_load_probe_cells(const uint32_t dim[3], const BlubLoadProbe *probe, uint32_t lo[3], uint32_t hi[3]) {
+    if (!dim || !probe || !lo || !hi) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::LoadProbeBox b = blub::clamp_load_probe(dim, *probe);
+        for (int k = 0; k < 3; ++k) {
+            lo[k] = (uint32_t)b.lo[k];
+            hi[k] = (uint32_t)b.hi[k];
+        }
+        return BLUB_OK;
+    });
+}
+
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
 
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {
@@ -436,6 +459,16 @@ int blub_scene_info(const char *path, BlubSceneInfo *out) {
         out->grid_to_world_scale = c.grid_to_world_scale;
         out->num_fluid_cubes = (uint32_t)c.fluid_cubes.size();
         out->num_static_objects = c.num_static_objects;
+        return BLUB_OK;
+    });
+}
+
+int blub_scene_load_probes(const char *path, BlubLoadProbe *out, uint32_t capacity, uint32_t *count) {
+    if (!path || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const std::vector<BlubLoadProbe> probes = blub::scene_load_probes_grid(blub::parse_scene_file(path));
+        for (size_t k = 0; k < probes.size() && k < capacity; ++k) out[k] = probes[k];
+        *count = (uint32_t)probes.size();
         return BLUB_OK;
     });
 }

@@ -112,4 +112,17 @@ void launch_paint_tags(cudaStream_t st, const GridDim &g, const StepParams *para
 void launch_tag_census(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t n_host, uint32_t np_upper, uint32_t first, uint32_t num_tags,
                        const float4 *pos, float4 *const row[3], BlubTagCensus *out);
 
+// ---- solid load probes (load_kernels.cu, DESIGN.md §8 "Solid load probes") ----
+constexpr int LOAD_PROBES_MAX = BLUB_LOAD_PROBES_MAX;
+constexpr uint32_t LOAD_HISTORY_LENGTH = BLUB_LOAD_HISTORY_LENGTH;
+struct LoadProbeBox {
+    int lo[3], hi[3]; // cells [lo, hi), clamped to [0, dim]
+    float pivot[3];   // grid cells
+};
+// One record per probe into ring[probe * LOAD_HISTORY_LENGTH + params->step_count % LOAD_HISTORY_LENGTH]: the slot is zeroed, then every
+// wetted face of the probe's box adds its fixed-point force and torque.  probes: num_probes device boxes; max_cells: cells of the largest box
+// (sizes the launch).  marker / p_vel: the volumes the velocity solve used.
+void launch_solid_loads(cudaStream_t st, const GridDim &g, const StepParams *params, int num_probes, uint32_t max_cells, const LoadProbeBox *probes,
+                        const int8_t *marker, const float *p_vel, BlubSolidLoad *ring);
+
 } // namespace blub

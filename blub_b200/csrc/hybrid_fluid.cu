@@ -185,6 +185,8 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.scalars);
     cudaFree(flow_scratch_.counters);
     cudaFree(census_dev_);
+    cudaFree(load_probes_dev_);
+    cudaFree(load_ring_);
     cudaFree(mig_counters_);
     if (slab_error_host_) cudaFreeHost(slab_error_host_);
     cudaFree(params_dev_);
@@ -451,6 +453,11 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 2: // primary pressure solver (:843-852)
         solver_->solve(stream_, *field_velocity_, 0, marker_.ptr, params_dev_, quirks);
         if (!capturing_) field_velocity_->enqueue_error_buffer_read(stream_, dt); // the scalars live until this field's next solve
+        if (num_load_probes_ > 0) { // the marker and pressure this solve used: stage 6 rewrites the marker
+            launch_solid_loads(stream_, grid_, params_dev_, (int)num_load_probes_, load_max_cells_, load_probes_dev_, marker_.ptr, field_velocity_->pressure(),
+                               load_ring_);
+            if (!capturing_) note_load_record(step_counter_);
+        }
         break;
     case 3: // particle binning every n-th step, including step 0 (:854-894)
         if (binning_step()) {
@@ -603,6 +610,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
     }
     slab_exchange_index_ = before.exchange_index + after.exchanges;
     step_counter_ = before.step_counter + 1;
+    if (num_load_probes_ > 0) note_load_record(before.step_counter);
     field_velocity_->enqueue_error_buffer_read(stream_, dt);
     field_density_->enqueue_error_buffer_read(stream_, dt);
 }
@@ -787,6 +795,79 @@ void HybridFluid::tag_census(uint32_t first, uint32_t num_tags, BlubTagCensus *o
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Solid load probes (load_kernels.cu).  Not in the reference.  The records stay on the device; the host only keeps the step numbers it
+// recorded, so that a step never synchronises and load_history knows which ring slots hold what.
+static int clamp_to_closed_grid(uint32_t dim, float v) { // clamp_to_grid's conversion, clamped to [0, dim]: the border cells are walls
+    const uint32_t u = !(v > 0.0f) ? 0u : (v >= 4294967040.0f ? 0xFFFFFFFFu : (uint32_t)v);
+    return (int)(u < dim ? u : dim);
+}
+
+LoadProbeBox clamp_load_probe(const uint32_t dim[3], const BlubLoadProbe &probe) {
+    LoadProbeBox b;
+    for (int k = 0; k < 3; ++k) {
+        if (!std::isfinite(probe.min_grid[k]) || !std::isfinite(probe.max_grid[k])) throw std::invalid_argument("load probe corner is not finite");
+        if (!std::isfinite(probe.pivot_grid[k])) throw std::invalid_argument("load probe pivot is not finite");
+        b.lo[k] = clamp_to_closed_grid(dim[k], probe.min_grid[k]);
+        b.hi[k] = clamp_to_closed_grid(dim[k], probe.max_grid[k]);
+        if (b.hi[k] <= b.lo[k]) throw std::invalid_argument("load probe box is empty after clamping to the grid");
+        b.pivot[k] = probe.pivot_grid[k];
+    }
+    return b;
+}
+
+void HybridFluid::set_load_probes(const BlubLoadProbe *probes, uint32_t num_probes) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_load_probes: z-slab ranks have no load probes");
+    if (mid_step_) throw std::invalid_argument("set_load_probes: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    if (num_probes > (uint32_t)LOAD_PROBES_MAX) throw std::invalid_argument("set_load_probes: at most 16 probes");
+    if (num_probes && !probes) throw std::invalid_argument("set_load_probes: NULL probe array");
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    LoadProbeBox boxes[LOAD_PROBES_MAX];
+    uint32_t max_cells = 0;
+    for (uint32_t p = 0; p < num_probes; ++p) {
+        boxes[p] = clamp_load_probe(dim, probes[p]);
+        const LoadProbeBox &b = boxes[p];
+        max_cells = std::max(max_cells, (uint32_t)(b.hi[0] - b.lo[0]) * (uint32_t)(b.hi[1] - b.lo[1]) * (uint32_t)(b.hi[2] - b.lo[2]));
+    }
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // no step in flight reads the old boxes or writes the ring
+    if (num_probes > 0) {
+        const size_t ring_bytes = (size_t)LOAD_PROBES_MAX * LOAD_HISTORY_LENGTH * sizeof(BlubSolidLoad);
+        if (!load_ring_) {
+            BLUB_CUDA_CHECK(cudaMalloc(&load_probes_dev_, LOAD_PROBES_MAX * sizeof(LoadProbeBox)));
+            BLUB_CUDA_CHECK(cudaMalloc(&load_ring_, ring_bytes));
+        }
+        BLUB_CUDA_CHECK(cudaMemcpy(load_probes_dev_, boxes, num_probes * sizeof(LoadProbeBox), cudaMemcpyHostToDevice));
+        BLUB_CUDA_CHECK(cudaMemset(load_ring_, 0, ring_bytes));
+    }
+    num_load_probes_ = num_probes;
+    load_max_cells_ = max_cells;
+    load_steps_.clear();
+    destroy_graphs();
+}
+
+void HybridFluid::note_load_record(uint32_t step) {
+    if (!load_steps_.empty() && load_steps_.back() == step) return; // the same step again (a repeated step_stages): the same slot
+    load_steps_.push_back(step);
+    // a slot holds the newest of the steps that map to it
+    while (load_steps_.size() > LOAD_HISTORY_LENGTH || (uint64_t)load_steps_.front() + LOAD_HISTORY_LENGTH <= step) load_steps_.pop_front();
+}
+
+uint32_t HybridFluid::load_history(uint32_t probe, BlubSolidLoad *out, uint32_t capacity) {
+    if (probe >= num_load_probes_) throw std::invalid_argument("load_history: no such load probe");
+    if (capacity && !out) throw std::invalid_argument("load_history: NULL output");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    std::vector<BlubSolidLoad> ring(LOAD_HISTORY_LENGTH);
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(ring.data(), load_ring_ + (size_t)probe * LOAD_HISTORY_LENGTH, LOAD_HISTORY_LENGTH * sizeof(BlubSolidLoad),
+                                    cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    // the recorded steps increase and lie within LOAD_HISTORY_LENGTH of each other: they fill distinct slots
+    const uint32_t n = std::min<uint32_t>(capacity, (uint32_t)load_steps_.size());
+    const size_t first = load_steps_.size() - n;
+    for (uint32_t k = 0; k < n; ++k) out[k] = ring[load_steps_[first + k] % LOAD_HISTORY_LENGTH];
+    return n;
+}
+
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream) {
     std::unique_ptr<HybridFluid> f(new HybridFluid(cfg.grid_dimension[0], cfg.grid_dimension[1], cfg.grid_dimension[2], cfg.max_num_particles, device, stream));
     const float scale = cfg.grid_to_world_scale;
@@ -816,7 +897,25 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
             }
         f->set_flow(src.data(), tags.data(), (uint32_t)src.size(), drn.data(), (uint32_t)drn.size());
     }
+    if (!cfg.load_probes.empty()) {
+        const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);
+        f->set_load_probes(probes.data(), (uint32_t)probes.size());
+    }
     return f;
+}
+
+std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg) {
+    const float scale = cfg.grid_to_world_scale;
+    std::vector<BlubLoadProbe> out(cfg.load_probes.size());
+    for (size_t i = 0; i < out.size(); ++i) {
+        const SceneLoadProbe &p = cfg.load_probes[i];
+        for (int k = 0; k < 3; ++k) {
+            out[i].min_grid[k] = p.min[k] / scale;
+            out[i].max_grid[k] = p.max[k] / scale;
+            out[i].pivot_grid[k] = p.has_pivot ? p.pivot[k] / scale : 0.5f * (out[i].min_grid[k] + out[i].max_grid[k]);
+        }
+    }
+    return out;
 }
 
 } // namespace blub

@@ -197,6 +197,25 @@ SceneConfig parse_scene_file(const std::string &path) {
             cfg.drains.push_back(b);
         }
     }
+    // solid load probes (not in the reference): world units, the pivot optional
+    if (const JsonValue *probes = fluid.get("load_probes")) {
+        if (probes->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.load_probes` is not an array");
+        if (probes->array.size() > (size_t)BLUB_LOAD_PROBES_MAX) throw std::runtime_error("scene JSON: `fluid.load_probes` holds more than 16 probes");
+        for (const JsonValue &p : probes->array) {
+            if (p.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.load_probes` entry is not an object");
+            SceneLoadProbe b;
+            vec3(need(p, "min"), "load_probes.min", b.min);
+            vec3(need(p, "max"), "load_probes.max", b.max);
+            if (const JsonValue *pivot = p.get("pivot")) {
+                vec3(*pivot, "load_probes.pivot", b.pivot);
+                b.has_pivot = true;
+            }
+            for (int k = 0; k < 3; ++k)
+                if (!std::isfinite(b.min[k]) || !std::isfinite(b.max[k]) || (b.has_pivot && !std::isfinite(b.pivot[k])))
+                    throw std::runtime_error("scene JSON: a `fluid.load_probes` value is out of the float range");
+            cfg.load_probes.push_back(b);
+        }
+    }
     if (const JsonValue *objs = root.get("static_objects")) { // #[serde(default)]
         if (objs->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `static_objects` is not an array");
         for (const JsonValue &o : objs->array) { // StaticObjectConfig, src/scene/models.rs:11-19

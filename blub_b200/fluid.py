@@ -28,6 +28,10 @@ BLUB_OK = 0
 BLUB_WARN_TRUNCATED = 100
 TAG_CENSUS_FRAC_BITS = 16  # BLUB_TAG_CENSUS_FRAC_BITS: census sums are sums of rint(value * 2^16)
 TAG_CENSUS_MAX = 256       # tags per census
+LOAD_PROBES_MAX = 16            # BLUB_LOAD_PROBES_MAX
+LOAD_HISTORY_LENGTH = 1024      # BLUB_LOAD_HISTORY_LENGTH: records per probe in the device ring
+LOAD_FORCE_FRAC_BITS = 16       # BLUB_LOAD_FORCE_FRAC_BITS: force sums are sums of rint(q * 2^16)
+LOAD_TORQUE_FRAC_BITS = 8       # BLUB_LOAD_TORQUE_FRAC_BITS: torque sums are sums of rint(r_b * q * 2^8)
 
 
 class BlubError(RuntimeError):
@@ -115,6 +119,18 @@ class TagCensus(C.Structure):
                 ("cell_max", C.c_int32 * 3)]
 
 
+class LoadProbe(C.Structure):
+    """BlubLoadProbe: a box of cells and a pivot, in grid cells."""
+
+    _fields_ = [("min_grid", C.c_float * 3), ("max_grid", C.c_float * 3), ("pivot_grid", C.c_float * 3)]
+
+
+class SolidLoad(C.Structure):
+    """BlubSolidLoad: one step's pressure force (2^16 fixed point) and torque (2^8) on the solids of a probe box."""
+
+    _fields_ = [("step", C.c_uint32), ("wetted_faces", C.c_uint32), ("force_fx", C.c_int64 * 3), ("torque_fx", C.c_int64 * 3)]
+
+
 def lib_path() -> str:
     return os.path.join(_HERE, "libblubcore.so")
 
@@ -183,6 +199,10 @@ def lib():
         "blub_fluid_set_flow_tagged": (C.c_int, [vp, C.POINTER(FluidSource), C.POINTER(u32), u32, C.POINTER(FluidDrain), u32]),
         "blub_fluid_paint_tags": (C.c_int, [vp, f3, f3, u32]),
         "blub_fluid_tag_census": (C.c_int, [vp, u32, u32, C.POINTER(TagCensus)]),
+        "blub_fluid_set_load_probes": (C.c_int, [vp, C.POINTER(LoadProbe), u32]),
+        "blub_fluid_load_history": (C.c_int, [vp, u32, C.POINTER(SolidLoad), u32, C.POINTER(u32)]),
+        "blub_load_probe_cells": (C.c_int, [C.POINTER(u32), C.POINTER(LoadProbe), C.POINTER(u32), C.POINTER(u32)]),
+        "blub_scene_load_probes": (C.c_int, [C.c_char_p, C.POINTER(LoadProbe), u32, C.POINTER(u32)]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -305,6 +325,31 @@ def scene_info(path):
     info = SceneInfo()
     _check(lib().blub_scene_info(os.fsencode(path), C.byref(info)))
     return info
+
+
+def _load_probes(probes):
+    """[(min, max[, pivot])] in grid cells -> a BlubLoadProbe array; the pivot defaults to the box centre (min + max) / 2 in float32."""
+    arr = (LoadProbe * max(len(probes), 1))()
+    for k, (mn, mx, *pivot) in enumerate(probes):
+        mn, mx = np.asarray(mn, dtype=np.float32), np.asarray(mx, dtype=np.float32)
+        pv = np.asarray(pivot[0], dtype=np.float32) if pivot and pivot[0] is not None else (mn + mx) * np.float32(0.5)
+        arr[k].min_grid[:], arr[k].max_grid[:], arr[k].pivot_grid[:] = [float(v) for v in mn], [float(v) for v in mx], [float(v) for v in pv]
+    return arr
+
+
+def load_probe_cells(dims, probe):
+    """The cells [lo, hi) a load probe (min, max[, pivot]) holds on a grid of `dims` cells (host only)."""
+    lo, hi = (C.c_uint32 * 3)(), (C.c_uint32 * 3)()
+    _check(lib().blub_load_probe_cells((C.c_uint32 * 3)(*[int(d) for d in dims]), _load_probes([probe]), lo, hi))
+    return tuple(lo), tuple(hi)
+
+
+def scene_load_probes(path):
+    """The scene's fluid.load_probes in grid cells: [(min, max, pivot)] (host only)."""
+    count = C.c_uint32(0)
+    arr = (LoadProbe * LOAD_PROBES_MAX)()
+    _check(lib().blub_scene_load_probes(os.fsencode(path), arr, LOAD_PROBES_MAX, C.byref(count)))
+    return [(tuple(p.min_grid), tuple(p.max_grid), tuple(p.pivot_grid)) for p in arr[:count.value]]
 
 
 def state_info(path):
@@ -546,6 +591,28 @@ class HybridFluid:
             n = res["count"].astype(np.float64)[:, None]
             res["centroid"] = res["position_sum_fx"].astype(np.float64) / scale / n
             res["mean_velocity"] = res["velocity_sum_fx"].astype(np.float64) / scale / n
+        return res
+
+    # -- solid load probes --------------------------------------------------------------------
+    def set_load_probes(self, probes=()):
+        """Replaces the load probe set: probes = [(min, max[, pivot])] in grid cells (at most 16; pivot default: the box centre).  Resets the
+        history.  An empty list clears the set.  Raises BlubError (and changes nothing) on too many probes, non-finite values, boxes empty
+        after clamping to [0, dim], z-slab ranks and a fluid inside a step."""
+        _check(self.L.blub_fluid_set_load_probes(self.h, _load_probes(probes), len(probes)))
+
+    def load_history(self, probe, capacity=LOAD_HISTORY_LENGTH):
+        """The newest records of one probe, oldest first: the raw fields of BlubSolidLoad as arrays ("step", "wetted_faces", "force_fx",
+        "torque_fx") plus float64 "force" (cells^4/s^2 per unit density) and "torque" (cells^5/s^2).  Synchronises."""
+        capacity = int(capacity)
+        out = (SolidLoad * max(capacity, 1))()
+        count = C.c_uint32(0)
+        _check(self.L.blub_fluid_load_history(self.h, int(probe), out, capacity, C.byref(count)))
+        recs = out[:count.value]
+        res = {"step": np.array([r.step for r in recs], dtype=np.uint32), "wetted_faces": np.array([r.wetted_faces for r in recs], dtype=np.uint32),
+               "force_fx": np.array([list(r.force_fx) for r in recs], dtype=np.int64).reshape(-1, 3),
+               "torque_fx": np.array([list(r.torque_fx) for r in recs], dtype=np.int64).reshape(-1, 3)}
+        res["force"] = res["force_fx"].astype(np.float64) / float(1 << LOAD_FORCE_FRAC_BITS)
+        res["torque"] = res["torque_fx"].astype(np.float64) / float(1 << LOAD_TORQUE_FRAC_BITS)
         return res
 
     @property

@@ -198,6 +198,41 @@ typedef struct {
  * Synchronises.  BLUB_ERR_INVALID_ARGUMENT: num_tags of 0 or above 256, or first_tag + num_tags above 2^32. */
 int blub_fluid_tag_census(BlubFluid *fluid, uint32_t first_tag, uint32_t num_tags, BlubTagCensus *out);
 
+/* ---- solid load probes (not part of the reference surface; rules: DESIGN.md section 8) -----------------------------------------
+ * A probe is a box of cells plus a pivot, in grid cells.  The corners are converted as blub_fluid_add_cube converts them but clamped to
+ * [0, dim] (the border cells, the tank walls, can be held); the max corner is exclusive.  While a fluid has probes, every step adds up on the
+ * GPU, right after the velocity solve, the projection pressure on every wetted face of each probe: a face between a SOLID cell inside the box
+ * and a FLUID neighbour (which may lie outside it).  q = -p_vel[fluid cell] * inv_dt (float32) is pressure / density (the velocity solve's
+ * volume, BLUB_TAP_PRESSURE_VELOCITY, holds -p dt / density); the face force is q
+ * along the face axis, from the fluid cell into the solid one, and the torque is (face centre - pivot) x force.  Every face contributes
+ * rint(q * 2^16) to the force sums and rint((r_b * q) * 2^8) to the torque sums, added as int64: the records are exact and independent of the
+ * launch order.  They are exact while |q| < 2^22, |r| < 2^11 and a probe has at most 2^21 wetted faces.
+ * Units: force per unit fluid density in cells^4/s^2 (newtons = value * density * s^4, s = grid_to_world_scale in m per cell); torque
+ * in cells^5/s^2 (times density * s^5).  Only the pressure of the velocity projection is measured: no density-correction pressure, no shear.
+ * Probes are not part of the saved state: a loaded fluid has none. */
+#define BLUB_LOAD_PROBES_MAX 16
+#define BLUB_LOAD_HISTORY_LENGTH 1024 /* records per probe in the device ring: slot = step % 1024 */
+#define BLUB_LOAD_FORCE_FRAC_BITS 16
+#define BLUB_LOAD_TORQUE_FRAC_BITS 8
+typedef struct {
+    float min_grid[3], max_grid[3], pivot_grid[3];
+} BlubLoadProbe;
+typedef struct {
+    uint32_t step;         /* blub_fluid_step_count before the step that wrote the record */
+    uint32_t wetted_faces;
+    int64_t force_fx[3];   /* force * 2^16 */
+    int64_t torque_fx[3];  /* torque * 2^8 */
+} BlubSolidLoad;
+/* Replaces the whole probe set (0 clears it), resets the history and drops the cached step graphs.  Every step then records one
+ * BlubSolidLoad per probe on the device without synchronising.  BLUB_ERR_INVALID_ARGUMENT, changing nothing: more than 16 probes, a
+ * non-finite corner or pivot, a box empty after clamping, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_load_probes(BlubFluid *fluid, const BlubLoadProbe *probes, uint32_t num_probes);
+/* The newest min(capacity, recorded, 1024) records of probe `probe`, oldest first; *count receives their number.  Synchronises; works
+ * inside a step as well (after stage 2 the record of the current step is there).  BLUB_ERR_INVALID_ARGUMENT: a probe index outside the set. */
+int blub_fluid_load_history(BlubFluid *fluid, uint32_t probe, BlubSolidLoad *out, uint32_t capacity, uint32_t *count);
+/* Host only: the cells [lo, hi) a probe holds on a grid of `dim` cells.  BLUB_ERR_INVALID_ARGUMENT: a non-finite value or an empty box. */
+int blub_load_probe_cells(const uint32_t dim[3], const BlubLoadProbe *probe, uint32_t lo[3], uint32_t hi[3]);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their
@@ -214,6 +249,9 @@ typedef struct {
     uint32_t num_static_objects;
 } BlubSceneInfo;
 int blub_scene_info(const char *scene_json_path, BlubSceneInfo *out);
+/* The scene's optional fluid.load_probes in grid cells (world / grid_to_world_scale; a missing pivot is the box centre).  Writes at most
+ * `capacity` probes and sets *count to the number the scene holds.  blub_scene_load sets them on the fluid it creates. */
+int blub_scene_load_probes(const char *scene_json_path, BlubLoadProbe *out, uint32_t capacity, uint32_t *count);
 
 /* ---- analytic rigid solids (stand-in for the mesh voxelizer, src/scene/voxelization.rs:118-157) ---------------------------
  * One oriented box or sphere with the reference's rigid animation (StaticObjectConfig / RigidAnimation, src/scene/models.rs:11-46,

@@ -271,6 +271,10 @@ class HybridFluid {
     bool binning_step() const;
     uint32_t internal_resort_every_ = 8; // see binning_step(); single GPU and z-slab ranks alike
     void destroy_graphs();
+    // brick schedule of the density and P2G scatters, rebuilt at every re-sort (single GPU, unless BLUB_SCATTER_SCHEDULE=off: then valid == nullptr).  It is
+    // not state: a fluid that is loaded, or whose particles are replaced or added to, runs the 256-particle chunks until its next re-sort.
+    ScatterSchedule sched_{};
+    void invalidate_schedule();
 
     // ---- z-slab sharding of the whole step (slab.cu) ----
     struct SlabHaloItem {

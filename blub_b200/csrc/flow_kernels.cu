@@ -119,9 +119,11 @@ __global__ void __launch_bounds__(PT) flow_compact_kernel(GridDim g, FlowSet fs,
 
 __global__ void __launch_bounds__(PT) flow_copy_back_kernel(FlowScratch s, float4 *__restrict__ pos, float4 *__restrict__ rx, float4 *__restrict__ ry,
                                                             float4 *__restrict__ rz, const float4 *__restrict__ pos2, const float4 *__restrict__ rx2,
-                                                            const float4 *__restrict__ ry2, const float4 *__restrict__ rz2) {
+                                                            const float4 *__restrict__ ry2, const float4 *__restrict__ rz2, uint32_t *schedule_valid) {
     const uint32_t first = s.scalars[0];
     if (first == NONE) return;
+    // the survivors moved to lower indices: the scatter schedule no longer describes the order (it stays correct, but its windows miss)
+    if (schedule_valid != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *schedule_valid = 0u;
     const uint32_t m = s.scalars[2] - s.scalars[1];
     for (uint32_t i = first + blockIdx.x * PT + threadIdx.x; i < m; i += gridDim.x * PT) {
         pos[i] = pos2[i];
@@ -275,7 +277,7 @@ __global__ void __launch_bounds__(PT) tag_census_kernel(GridDim g, const StepPar
 } // namespace
 
 void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params, uint32_t capacity, const FlowSet &fs, const FlowScratch &s, float4 *pos,
-                          float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox) {
+                          float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox, uint32_t *schedule_valid) {
     const int particle_blocks = std::min(blocks_for(capacity, PT), device_sm_count() * 16); // bounded grid-stride loops over the device count
     BLUB_CUDA_CHECK(cudaMemsetAsync(s.scalars, 0xFF, sizeof(uint32_t), st));
     BLUB_CUDA_CHECK(cudaMemsetAsync(s.scalars + 1, 0, sizeof(uint32_t), st));
@@ -287,7 +289,7 @@ void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params,
         BLUB_LAUNCH(flow_compact_kernel, std::max(std::min((int)s.num_chunks, device_sm_count() * 8), 1), PT, 0, st, g, fs, pos, row[0], row[1], row[2],
                     pos_spare, row_spare[0], row_spare[1], row_spare[2], s);
         BLUB_LAUNCH(flow_copy_back_kernel, std::max(particle_blocks, 1), PT, 0, st, s, pos, row[0], row[1], row[2], pos_spare, row_spare[0], row_spare[1],
-                    row_spare[2]);
+                    row_spare[2], schedule_valid);
     }
     if (s.source_cells) {
         const int cell_blocks = std::min(blocks_for(s.source_cells, PT), device_sm_count() * 8);

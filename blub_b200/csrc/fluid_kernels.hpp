@@ -35,24 +35,46 @@ struct CellLists {
     CrowdedCells crowd;
 };
 
+// Brick schedule of the density and P2G scatters (transfer_kernels.cu, DESIGN.md §3.2): built from the cell lists at every re-sort; work
+// items of aligned particle warps grouped by the cell brick they were sorted into.  It never changes a result, only how many faces go through a
+// block's tile.  Kept on the device, so that a captured step graph follows a rebuild or an invalidation.
+struct ScatterSchedule {
+    uint32_t *valid;       // device word, non-zero: the schedule describes the particle order (cleared by anything else that re-indexes)
+    uint32_t *brick_warps; // nbricks + 1: warps per brick, then their exclusive scan (entry nbricks: the warps it covers)
+    uint32_t *brick_items; // nbricks + 1: work items per brick, then their exclusive scan (entry nbricks: the number of items)
+    uint32_t *item_start;  // per item: its first entry of `warps`
+    uint32_t *item_brick;  // per item: its brick
+    int4 *item_box;        // per item: (lo, -), (hi, -) -- the primal cells its particles were in at the last density scatter (lo > hi: none)
+    uint32_t *warps;       // warp ids (warp w = particles 32w .. 32w + 31), by brick, ascending within a brick
+    int nbricks;
+};
+bool scatter_schedule_enabled(); // false under BLUB_SCATTER_SCHEDULE=off
+int scatter_schedule_bricks(const GridDim &g);
+uint32_t scatter_schedule_max_items(const GridDim &g, uint32_t max_warps);
+// after launch_binning: builds the schedule from the cell_start of that binning and sets `valid`
+void launch_scatter_schedule(cudaStream_t st, const GridDim &g, const CellLists &l, const ScatterSchedule &s);
+
 void configure_transfer_kernels(); // once per device, before the first launch (dynamic shared memory opt-in)
 // clamp_lo: 1.0 velocity transfer, 0.5 density transfer, 0.0 binning (see transfer_position)
 void launch_cell_lists(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float clamp_lo, const CellLists &l);
 void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits);
 void launch_p2g_gather(cudaStream_t st, const GridDim &g, const StepParams *params, const CellLists &l, const float4 *pos, float4 *const row[3],
                        const int8_t *marker, float *const u[3]);
-// scatter form of P2G / density in two halves, for callers that exchange halos in between (z-slab sharding)
+// scatter form of P2G / density in two halves, for callers that exchange halos in between (z-slab sharding).  sched: the brick schedule, or
+// one with valid == nullptr (z-slab ranks, BLUB_SCATTER_SCHEDULE=off): 256-particle chunks only.
 void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float4 *const row[3],
-                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators);
+                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators, const ScatterSchedule &sched);
 // particle_words: wpr * ny * nz words, 1 bit per cell "a particle marked this cell" (before the boundary rule); the finish pass visits and
 // re-zeroes the accumulators of the one-cell dilation of those cells only
 void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,
                        const uint2 *vox, const FluidBits &bits, uint32_t *particle_words);
-// density: 64-bit fixed-point accumulator volume (FIXED_WEIGHT_BITS, common.cuh)
-void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density);
+// density: 64-bit fixed-point accumulator volume (FIXED_WEIGHT_BITS, common.cuh).  sched: the brick schedule, or one with valid == nullptr
+// (z-slab ranks, BLUB_SCATTER_SCHEDULE=off): 256-particle chunks only.
+void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density,
+                            const ScatterSchedule &sched);
 void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs);
 void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos,
-                        const int8_t *marker, long long *density, float *rhs);
+                        const int8_t *marker, long long *density, float *rhs, const ScatterSchedule &sched);
 void launch_boundary_marker(cudaStream_t st, const GridDim &g, int8_t *marker, const uint2 *vox, const FluidBits &bits, uint32_t *particle_words = nullptr);
 void launch_fluid_bits(cudaStream_t st, const GridDim &g, const int8_t *marker, const FluidBits &bits);
 int binning_scan_blocks(const GridDim &g);
@@ -100,8 +122,9 @@ struct FlowScratch {
 };
 // Drain, count, emit and set the source velocity (in that order, see DESIGN.md); the particle count lives in params->num_particles.
 // pos_spare / row_spare: arrays of the same capacity the drain compaction writes into before it copies the suffix back.
+// schedule_valid: the scatter schedule's flag (or nullptr), cleared when the drains remove particles
 void launch_flow_prologue(cudaStream_t st, const GridDim &g, StepParams *params, uint32_t capacity, const FlowSet &fs, const FlowScratch &s, float4 *pos,
-                          float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox);
+                          float4 *pos_spare, float4 *const row[3], float4 *const row_spare[3], const uint2 *vox, uint32_t *schedule_valid);
 
 // ---- particle tags (flow_kernels.cu, DESIGN.md §8 "Particle tags"): the raw bits of the fourth word of every position ----
 constexpr uint32_t TAG_CENSUS_MAX = 256; // tags per census: the block-private table

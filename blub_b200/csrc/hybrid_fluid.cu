@@ -90,6 +90,18 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
         BLUB_CUDA_CHECK(cudaMalloc(&lists_.crowd.sums, max_crowded * 18 * sizeof(float2)));
     }
     configure_transfer_kernels();
+    if (slab_world_ == 1 && scatter_schedule_enabled()) { // z-slab ranks re-index their particles in every step's migration
+        const uint32_t max_warps = max_num_particles / 32 + 1, max_items = scatter_schedule_max_items(grid_, max_warps);
+        sched_.nbricks = scatter_schedule_bricks(grid_);
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.valid, sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMemset(sched_.valid, 0, sizeof(uint32_t))); // no schedule before the first re-sort
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.brick_warps, ((size_t)sched_.nbricks + 1) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.brick_items, ((size_t)sched_.nbricks + 1) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.item_start, (size_t)max_items * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.item_brick, (size_t)max_items * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.item_box, 2 * (size_t)max_items * sizeof(int4)));
+        BLUB_CUDA_CHECK(cudaMalloc(&sched_.warps, (size_t)max_warps * sizeof(uint32_t)));
+    }
     {
         // Default: the scatter form, faster than the gather on the 256^3 dam break; both are bit-reproducible.  BLUB_P2G=gather or
         // blub_fluid_set_transfer_path(f, 0) selects the gather.
@@ -172,6 +184,13 @@ HybridFluid::~HybridFluid() {
     cudaFree(lists_.crowd.cells);
     cudaFree(lists_.crowd.slot_of_cell);
     cudaFree(lists_.crowd.sums);
+    cudaFree(sched_.valid);
+    cudaFree(sched_.brick_warps);
+    cudaFree(sched_.brick_items);
+    cudaFree(sched_.item_start);
+    cudaFree(sched_.item_brick);
+    cudaFree(sched_.item_box);
+    cudaFree(sched_.warps);
     if (solver_ && solver_->comm.seq) cudaFree(solver_->comm.seq);
     solver_.reset();
     field_velocity_.reset();
@@ -243,6 +262,7 @@ bool HybridFluid::add_fluid_cube(const float min_grid[3], const float max_grid[3
         fresh[i] = make_float4(p[0], p[1], p[2], tag_bits(tag));
     }
     BLUB_CUDA_CHECK(cudaMemcpyAsync(pos_[cur_] + num_particles_, fresh.data(), (size_t)num_new * sizeof(float4), cudaMemcpyHostToDevice, stream_));
+    invalidate_schedule();
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // `fresh` is pageable: finish before it dies (queue.write_buffer semantics)
     num_particles_ += num_new;
     if (flow_active_) set_device_particle_count(num_particles_);
@@ -288,6 +308,10 @@ bool HybridFluid::add_fluid_cube_slab(const uint32_t mn[3], const uint32_t ext[3
     return truncated;
 }
 
+void HybridFluid::invalidate_schedule() {
+    if (sched_.valid) BLUB_CUDA_CHECK(cudaMemsetAsync(sched_.valid, 0, sizeof(uint32_t), stream_));
+}
+
 void HybridFluid::set_device_particle_count(uint32_t n) {
     BLUB_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<char *>(params_dev_) + offsetof(StepParams, num_particles), &n, sizeof(uint32_t),
                                     cudaMemcpyHostToDevice, stream_));
@@ -320,6 +344,7 @@ void HybridFluid::set_particles(uint32_t count, const float *pos4, const float *
         if (rows[c]) BLUB_CUDA_CHECK(cudaMemcpyAsync(row_[c], rows[c], bytes, cudaMemcpyHostToDevice, stream_));
         else BLUB_CUDA_CHECK(cudaMemsetAsync(row_[c], 0, bytes, stream_));
     }
+    invalidate_schedule();
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
     num_particles_ = count;
     if (device_count_mode()) set_device_particle_count(count);
@@ -435,11 +460,11 @@ void HybridFluid::run_stage(int stage, float dt) {
             if (np > 0) launch_p2g_gather(stream_, grid_, params_dev_, lists_, pos_[cur_], row_, marker_.ptr, u);
             else for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(u[c], 0, (size_t)grid_.n * sizeof(float), stream_));
         } else if (!shard) {
-            launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, false);
+            launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, false, sched_);
             launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, voxels_, bits, particle_words_);
             fluid_bits_stale_ = false;
         } else {
-            launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, true);
+            launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, true, sched_);
             const SlabHaloItem items[4] = {{nw[0], sizeof(longlong2), 0}, {nw[1], sizeof(longlong2), 0}, {nw[2], sizeof(longlong2), 0}, {marker_.ptr, 1, 1}};
             slab_halo_exchange(items, 4); // X1
             launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, voxels_, bits, particle_words_);
@@ -462,7 +487,10 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 3: // particle binning every n-th step, including step 0 (:854-894)
         if (binning_step()) {
             launch_binning(stream_, grid_, params_dev_, np, pos_[cur_], pos_[1 - cur_], lists_);
-            if (np > 0) cur_ = 1 - cur_; // ping-pong instead of the reference's full-buffer copy-back (:884-892)
+            if (np > 0) {
+                cur_ = 1 - cur_; // ping-pong instead of the reference's full-buffer copy-back (:884-892)
+                if (sched_.valid) launch_scatter_schedule(stream_, grid_, lists_, sched_);
+            }
         }
         break;
     case 4: // make velocity grid divergence free (:901-904)
@@ -496,9 +524,9 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 9: // density projection: compute density error (:928-932)
         if (!shard) {
-            launch_density_rhs(stream_, grid_, params_dev_, np, pos_[cur_], marker_.ptr, density_.ptr, solver_->residual());
+            launch_density_rhs(stream_, grid_, params_dev_, np, pos_[cur_], marker_.ptr, density_.ptr, solver_->residual(), sched_);
         } else {
-            launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr);
+            launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr, sched_);
             const SlabHaloItem items[1] = {{density_.ptr, sizeof(long long), 0}};
             slab_halo_exchange(items, 1); // X4
             launch_density_finish(stream_, grid_, params_dev_, marker_.ptr, density_.ptr, solver_->residual());
@@ -757,7 +785,7 @@ void HybridFluid::flow_counters(uint64_t out[3]) {
 }
 
 void HybridFluid::run_flow_prologue() {
-    launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, voxels_);
+    launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, voxels_, sched_.valid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -767,6 +767,137 @@ constexpr int P2G_TILE = 1184;
 constexpr int P2G_TILE_BYTES = 12 * P2G_TILE * 4; // 56,832 B: with the 1 KB the hardware reserves per block, 4 blocks fit into 228 KB
 constexpr int DENSITY_TILE = 2048;                // density tile: {low, high} word planes (16 KB)
 
+// ---- brick schedule of the density and P2G scatters (built at every re-sort, DESIGN.md §3.2)
+// After a re-sort the particles are in x-fastest cell order, so a chunk of 256 consecutive particles covers one short run of a cell row and
+// every cell row is flushed once by each of the chunks of the 3 x 3 cell rows around it.  The schedule groups the aligned warps (particles
+// 32w .. 32w + 31) by the BRICK of SCHED_BX x SCHED_BY x SCHED_BZ cells that holds the cell of their first particle, and cuts each brick's
+// warps (ascending) into work items of at most SCHED_K warps.  A block runs a work item's warps through one tile -- its window set from
+// where the item's particles are at the time of the scatter (item_window) -- and flushes it once.  A
+// warp still holds the particles it holds in a plain launch, so every peer group and every integer it forms is the same, and the sums come
+// out bit for bit the same whatever warps share a tile: the schedule only decides how much goes the tile way.  Coverage is all that
+// correctness rests on: the items hold warps [0, brick_warps[nbricks]) once each, the 256-particle chunks take the rest.
+constexpr int SCHED_BX = 28, SCHED_BY = 4, SCHED_BZ = 4; // cells per brick
+constexpr int P2G_MIN_ITEM_WAVES = 8;                     // P2G walks the work items only when they fill this many waves of 4 blocks per SM
+constexpr uint32_t SCHED_K = 64;                         // warps per work item at most: a long tail and too few items for a small fluid cost more
+// the cells of a brick (+-1) and room for warps that start near its high x edge and reach over it
+static_assert((SCHED_BX + 4) * (SCHED_BY + 2) * (SCHED_BZ + 2) <= DENSITY_TILE, "a brick's window fits the density tile");
+
+__device__ __forceinline__ uint32_t warps_before(uint32_t particle) { return (particle >> 5) + ((particle & 31u) != 0u ? 1u : 0u); }
+__device__ __forceinline__ int3 brick_origin(const GridDim &g, int b) {
+    const int nbx = (g.nx + SCHED_BX - 1) / SCHED_BX, nby = (g.ny + SCHED_BY - 1) / SCHED_BY;
+    return make_int3(b % nbx * SCHED_BX, b / nbx % nby * SCHED_BY, b / nbx / nby * SCHED_BZ);
+}
+// The warps whose first particle lies in the x-run [x0, x0 + SCHED_BX) of row (y, z): [warps_before(start of the run), warps_before(its end)).
+// Over all runs of all bricks these ranges cover [0, warps_before(np)) once each.
+__device__ __forceinline__ uint2 run_warps(const GridDim &g, const uint32_t *__restrict__ cell_start, int x0, int y, int z) {
+    const int c0 = lin(g, x0, y, z);
+    return make_uint2(warps_before(cell_start[c0]), warps_before(cell_start[c0 + min(SCHED_BX, g.nx - x0)]));
+}
+// one thread per brick: its warp and work item counts (the entries at nbricks, the totals after the scans, are set to 0 here)
+__global__ void __launch_bounds__(PT) schedule_count_kernel(GridDim g, const uint32_t *__restrict__ cell_start, ScatterSchedule s) {
+    const int b = blockIdx.x * PT + threadIdx.x;
+    if (b == 0) s.brick_warps[s.nbricks] = s.brick_items[s.nbricks] = 0u;
+    if (b >= s.nbricks) return;
+    const int3 o = brick_origin(g, b);
+    uint32_t warps = 0;
+    for (int z = o.z; z < min(o.z + SCHED_BZ, g.nz); ++z)
+        for (int y = o.y; y < min(o.y + SCHED_BY, g.ny); ++y) {
+            const uint2 r = run_warps(g, cell_start, o.x, y, z);
+            warps += r.y - r.x;
+        }
+    s.brick_warps[b] = warps;
+    s.brick_items[b] = (warps + SCHED_K - 1) / SCHED_K;
+}
+// one warp per brick (after the scans): its warps in ascending order, and the first warp and the brick of each of its work items
+__global__ void __launch_bounds__(PT) schedule_fill_kernel(GridDim g, const uint32_t *__restrict__ cell_start, ScatterSchedule s) {
+    const int b = (blockIdx.x * PT + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= s.nbricks) return; // warp-uniform
+    const int3 o = brick_origin(g, b);
+    const uint32_t first = s.brick_warps[b], item0 = s.brick_items[b], nitems = s.brick_items[b + 1] - item0;
+    for (uint32_t k = lane; k < nitems; k += 32) {
+        s.item_start[item0 + k] = first + k * SCHED_K;
+        s.item_brick[item0 + k] = (uint32_t)b;
+        s.item_box[2 * (item0 + k)] = make_int4(1, 1, 1, 0); // empty until the density scatter has seen the item
+        s.item_box[2 * (item0 + k) + 1] = make_int4(0, 0, 0, 0);
+    }
+    uint32_t out = first;
+    for (int z = o.z; z < min(o.z + SCHED_BZ, g.nz); ++z)
+        for (int y = o.y; y < min(o.y + SCHED_BY, g.ny); ++y) {
+            const uint2 r = run_warps(g, cell_start, o.x, y, z);
+            for (uint32_t w = r.x + lane; w < r.y; w += 32) s.warps[out + (w - r.x)] = w;
+            out += r.y - r.x;
+        }
+}
+// The work items of the schedule (none while it is invalid or absent); `tail` = the first particle it does not cover
+__device__ __forceinline__ uint32_t schedule_items(const ScatterSchedule &s, uint32_t &tail) {
+    tail = 0u;
+    if (s.valid == nullptr || *s.valid == 0u) return 0u;
+    tail = 32u * s.brick_warps[s.nbricks];
+    return s.brick_items[s.nbricks];
+}
+// The tile window of work item `it` from the box of its particles' primal cells, [lo, hi] (lo > hi: none of them is left, no tile): the
+// faces [lo - 1, hi + 1] in every dimension; a box of more than CAP entries is cut -- z first, then y (neither below the brick's rows + 2),
+// then x -- around the middle of the item's brick.
+template <int CAP>
+__device__ __forceinline__ TileWindow box_window(const GridDim &g, const ScatterSchedule &s, uint32_t it, int4 lo_cell, int4 hi_cell) {
+    if (lo_cell.x > hi_cell.x || lo_cell.y > hi_cell.y || lo_cell.z > hi_cell.z) return TileWindow{0, 0, 0, 0, 0, 0};
+    const int lo[3] = {lo_cell.x - 1, lo_cell.y - 1, lo_cell.z - 1}, hi[3] = {hi_cell.x + 1, hi_cell.y + 1, hi_cell.z + 1};
+    int e[3] = {hi[0] - lo[0] + 1, hi[1] - lo[1] + 1, hi[2] - lo[2] + 1};
+    e[2] = min(e[2], max(SCHED_BZ + 2, CAP / (e[0] * e[1])));
+    e[1] = min(e[1], max(SCHED_BY + 2, CAP / (e[0] * e[2])));
+    e[0] = min(e[0], CAP / (e[1] * e[2]));
+    const int3 b = brick_origin(g, (int)s.item_brick[it]);
+    const int mid[3] = {b.x + SCHED_BX / 2, b.y + SCHED_BY / 2, b.z + SCHED_BZ / 2};
+    int o[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) o[d] = min(max(mid[d] - e[d] / 2, lo[d]), hi[d] - e[d] + 1);
+    return TileWindow{o[0], o[1], o[2], e[0], e[1], e[2]};
+}
+// The window of work item `it` (its warps are s.warps[w0 .. w1)) for the density scatter, from the primal cells its particles are in NOW:
+// particles drift away from the brick they were sorted into, and a window fixed at the re-sort loses them within a few steps.  The box of
+// those cells is also kept in s.item_box: the next step's P2G scatter takes its window from it (the density correction in between moves
+// particles by a fraction of a cell; a face that leaves the window takes the global path).  Every thread of the block calls this; it ends
+// with __syncthreads().
+template <int CAP>
+__device__ __forceinline__ TileWindow item_window(const GridDim &g, const ScatterSchedule &s, uint32_t it, uint32_t w0, uint32_t w1, uint32_t np,
+                                                  const float4 *__restrict__ pos, float clamp_lo, int (*scratch)[8], TileWindow *shared_win) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int big = 0x3fffffff;
+    int mn[3] = {big, big, big}, mx[3] = {-big, -big, -big};
+    for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
+        const uint32_t i = 32u * s.warps[k] + lane;
+        if (i < np) {
+            const float3 p = transfer_position(g, pos[i], clamp_lo);
+            const int c[3] = {min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1)};
+#pragma unroll
+            for (int d = 0; d < 3; ++d) { mn[d] = min(mn[d], c[d]); mx[d] = max(mx[d], c[d]); }
+        }
+    }
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        mn[d] = __reduce_min_sync(0xffffffffu, mn[d]);
+        mx[d] = __reduce_max_sync(0xffffffffu, mx[d]);
+    }
+    if (lane == 0)
+#pragma unroll
+        for (int d = 0; d < 3; ++d) { scratch[warp][d] = mn[d]; scratch[warp][3 + d] = mx[d]; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int lo[3], hi[3];
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            lo[d] = big; hi[d] = -big;
+            for (int w = 0; w < PT / 32; ++w) { lo[d] = min(lo[d], scratch[w][d]); hi[d] = max(hi[d], scratch[w][3 + d]); }
+        }
+        const int4 l = make_int4(lo[0], lo[1], lo[2], 0), h = make_int4(hi[0], hi[1], hi[2], 0);
+        s.item_box[2 * it] = l;
+        s.item_box[2 * it + 1] = h;
+        *shared_win = box_window<CAP>(g, s, it, l, h);
+    }
+    __syncthreads();
+    return *shared_win;
+}
+
 template <bool MARK, bool MATCH>
 __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float3 p,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
@@ -830,14 +961,52 @@ template <bool MARK, bool MATCH>
 __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                          const float4 *__restrict__ rowx, const float4 *__restrict__ rowy,
                                                          const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
-                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker) {
+                                                         longlong2 *__restrict__ nwz, int8_t *__restrict__ marker, ScatterSchedule sched,
+                                                         uint32_t min_items) {
     extern __shared__ uint32_t tile[]; // [12][P2G_TILE]
     __shared__ int scratch[PT / 32 + 1][8];
     __shared__ TileWindow shared_win;
     longlong2 *const nw[3] = {nwx, nwy, nwz};
-    // a bounded grid strides over the chunks: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
-    for (uint32_t b = blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
+    // the work items of the brick schedule, their windows from the cell boxes the last density scatter left (item_window): one zeroing and
+    // one flush per item, its warps 8 at a time.  Fewer than min_items items (a small fluid) would leave SMs idle at 4 blocks per SM while
+    // each block walks up to 8 rounds of warps: the chunks then take every particle.
+    uint32_t tail;
+    uint32_t items = schedule_items(sched, tail);
+    if (items < min_items) items = tail = 0u;
+    for (uint32_t it = blockIdx.x; it < items; it += gridDim.x) { // block-uniform
+        if (threadIdx.x == 0) shared_win = box_window<P2G_TILE>(g, sched, it, sched.item_box[2 * it], sched.item_box[2 * it + 1]);
+        __syncthreads();
+        const TileWindow win = shared_win;
+        const int size = win.ex * win.ey * win.ez;
+        for (int t = threadIdx.x; t < size; t += PT)
+#pragma unroll
+            for (int k = 0; k < 12; ++k) tile[k * P2G_TILE + t] = 0u;
+        __syncthreads();
+        const uint32_t w0 = sched.item_start[it], w1 = it + 1 < items ? sched.item_start[it + 1] : tail / 32u;
+        for (uint32_t k = w0 + (threadIdx.x >> 5); k < w1; k += PT / 32) { // warp-uniform
+            const uint32_t i = 32u * sched.warps[k] + (threadIdx.x & 31);
+            const float3 p = transfer_position(g, i < np_ ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 1.0f);
+            p2g_scatter_kernel_one<MARK, MATCH>(i, g, params, p, rowx, rowy, rowz, nwx, nwy, nwz, marker, win, tile);
+        }
+        __syncthreads();
+        for (int t = threadIdx.x; t < size; t += PT) {
+            int cell_index = -1;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const uint32_t *const tc = tile + 4 * c * P2G_TILE + t;
+                const long long num = tile_word(tc, tc + P2G_TILE), wq = tile_word(tc + 2 * P2G_TILE, tc + 3 * P2G_TILE);
+                if (num == 0 && wq == 0) continue;
+                if (cell_index < 0) cell_index = tile_cell(g, win, t);
+                if (num != 0) fixed_add(&nw[c][cell_index].x, num);
+                if (wq != 0) fixed_add(&nw[c][cell_index].y, wq);
+            }
+        }
+        __syncthreads(); // the tile and shared_win are read to the end before the next item
+    }
+    // chunks of PT particles from the first one the schedule does not cover (all of them without schedule); a bounded grid strides over
+    // them: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
+    for (uint32_t b = tail + blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
         const uint32_t i = b + threadIdx.x;
         const bool valid = i < np_;
         const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 1.0f);
@@ -960,13 +1129,36 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
 }
 template <bool MATCH>
 __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
-                                                             long long *__restrict__ density) {
+                                                             long long *__restrict__ density, ScatterSchedule sched) {
     __shared__ uint32_t tile[2 * DENSITY_TILE]; // low words, high words
     __shared__ int scratch[PT / 32 + 1][8];
     __shared__ TileWindow shared_win;
-    // a bounded grid strides over the chunks: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
     const uint32_t np_ = params->num_particles;
-    for (uint32_t b = blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // the work items of the brick schedule: one window, one zeroing and one flush per item, its warps 8 at a time
+    uint32_t tail;
+    const uint32_t items = schedule_items(sched, tail);
+    for (uint32_t it = blockIdx.x; it < items; it += gridDim.x) { // block-uniform
+        const uint32_t w0 = sched.item_start[it], w1 = it + 1 < items ? sched.item_start[it + 1] : tail / 32u;
+        const TileWindow win = item_window<DENSITY_TILE>(g, sched, it, w0, w1, np_, pos, 0.5f, scratch, &shared_win);
+        const int size = win.ex * win.ey * win.ez;
+        for (int t = threadIdx.x; t < size; t += PT) tile[t] = tile[DENSITY_TILE + t] = 0u;
+        __syncthreads();
+        for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
+            const uint32_t i = 32u * sched.warps[k] + lane;
+            const float3 p = transfer_position(g, i < np_ ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
+            density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
+        }
+        __syncthreads();
+        for (int t = threadIdx.x; t < size; t += PT) { // flush, as in p2g_scatter_kernel
+            const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
+            if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
+        }
+        // the next item's window is set up behind a barrier (item_window); the first chunk's too (scatter_window)
+    }
+    // chunks of PT particles from the first one the schedule does not cover (all of them without schedule); a bounded grid strides over
+    // them: launch cost does not grow with the CAPACITY a z-slab rank sizes its launches by
+    for (uint32_t b = tail + blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
         const uint32_t i = b + threadIdx.x;
         const bool valid = i < np_;
         const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
@@ -977,7 +1169,7 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
         __syncthreads();
         density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
         __syncthreads();
-        for (int t = threadIdx.x; t < size; t += PT) { // flush, as in p2g_scatter_kernel
+        for (int t = threadIdx.x; t < size; t += PT) {
             const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
             if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
         }
@@ -1102,8 +1294,32 @@ static bool scatter_groups_by_match() {
     return by_match;
 }
 
+// Whether re-sorts build the brick schedule of the scatters: BLUB_SCATTER_SCHEDULE=off (read once) keeps both on the 256-particle
+// chunks, the reference the schedule is tested against.
+bool scatter_schedule_enabled() {
+    static const bool on = [] {
+        const char *e = std::getenv("BLUB_SCATTER_SCHEDULE");
+        return !(e && std::strcmp(e, "off") == 0);
+    }();
+    return on;
+}
+
+int scatter_schedule_bricks(const GridDim &g) {
+    return ((g.nx + SCHED_BX - 1) / SCHED_BX) * ((g.ny + SCHED_BY - 1) / SCHED_BY) * ((g.nz + SCHED_BZ - 1) / SCHED_BZ);
+}
+uint32_t scatter_schedule_max_items(const GridDim &g, uint32_t max_warps) { return (uint32_t)scatter_schedule_bricks(g) + max_warps / SCHED_K + 1; }
+
+void launch_scatter_schedule(cudaStream_t st, const GridDim &g, const CellLists &l, const ScatterSchedule &s) {
+    const int nb = s.nbricks;
+    BLUB_LAUNCH(schedule_count_kernel, blocks_for(nb, PT), PT, 0, st, g, l.cell_start, s);
+    launch_exclusive_scan(st, s.brick_warps, (int64_t)nb + 1, l.block_sums);
+    launch_exclusive_scan(st, s.brick_items, (int64_t)nb + 1, l.block_sums);
+    BLUB_LAUNCH(schedule_fill_kernel, blocks_for((int64_t)nb * 32, PT), PT, 0, st, g, l.cell_start, s);
+    BLUB_CUDA_CHECK(cudaMemsetAsync(s.valid, 1, sizeof(uint32_t), st)); // non-zero: valid
+}
+
 void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float4 *const row[3],
-                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators) {
+                        longlong2 *const nw[3], int8_t *marker, bool clear_accumulators, const ScatterSchedule &sched) {
     // transfer_clear.comp: marker <- AIR.  The (num, weight) volumes (they replace the linked-list head volume) are all zero here on one GPU:
     // they are allocated zeroed and launch_p2g_finish puts back to zero what the scatter touched.  A z-slab rank also receives partial sums
     // from its neighbours in the overlap planes, some of them from particles whose cells it never sees: it clears the volumes the plain way.
@@ -1112,7 +1328,8 @@ void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *par
         for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(nw[c], 0, (size_t)g.n * sizeof(longlong2), st));
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? p2g_scatter_kernel<true, true> : p2g_scatter_kernel<true, false>;
-    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, P2G_TILE_BYTES, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker);
+    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, P2G_TILE_BYTES, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker, sched,
+                (uint32_t)(P2G_MIN_ITEM_WAVES * 4 * device_sm_count()));
 }
 
 void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,
@@ -1122,11 +1339,12 @@ void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *para
                 nw[1], nw[2]);
 }
 
-void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density) {
+void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density,
+                            const ScatterSchedule &sched) {
     BLUB_CUDA_CHECK(cudaMemsetAsync(density, 0, (size_t)g.n * sizeof(long long), st));
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? density_scatter_kernel<true> : density_scatter_kernel<false>;
-    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, density);
+    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, density, sched);
 }
 
 void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs) {
@@ -1134,8 +1352,8 @@ void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *
 }
 
 void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos,
-                        const int8_t *marker, long long *density, float *rhs) {
-    launch_density_scatter(st, g, params, np_upper, pos, density);
+                        const int8_t *marker, long long *density, float *rhs, const ScatterSchedule &sched) {
+    launch_density_scatter(st, g, params, np_upper, pos, density, sched);
     launch_density_finish(st, g, params, marker, density, rhs);
 }
 

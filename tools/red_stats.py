@@ -8,7 +8,8 @@ tests/test_variants_emulated.py feeds positions of the CPU oracle's dam break, r
 Schemes: none = one reduction per (particle, face); adjacent4 = runs of adjacent lanes with the same dual cell, cut into groups of four
 (segmented_run_sum); match4 / match8 / matchall = all lanes of the warp with the same dual cell (matched_group_sum), groups of 4 / 8 / any size.
 tiled_global_reductions: what is left of the match4 reductions for the global volumes once a block adds a chunk's faces up in a
-shared-memory tile first (p2g_scatter_kernel / density_scatter_kernel).
+shared-memory tile first (p2g_scatter_kernel / density_scatter_kernel); scheduled_global_reductions: the same for the density scatter's
+brick schedule (work items of warps grouped by the cell brick they were sorted into).
 """
 import sys
 
@@ -73,7 +74,6 @@ def tiled_global_reductions(p, nx, ny, ch, cap, comps=(0, 1, 2)):
     `cap` faces (chunk_windows).  A peer-group head (match4) adds a face that lies inside its chunk's window into the tile, any other face
     straight into the global volume; after the chunk every touched tile entry is flushed by one global reduction per word.  Words per face:
     2 for the velocity components (sum w * value, sum w), 1 for the density.  Returns (total, of which flushes, of which outside the window)."""
-    nz_max = int(p[:, 2].max()) + 2
     m = len(p) // 32 * 32
     nchunk = (m + ch - 1) // ch
     lo = 0.5 if comps == (3,) else 1.0
@@ -81,7 +81,93 @@ def tiled_global_reductions(p, nx, ny, ch, cap, comps=(0, 1, 2)):
     cells = np.full((nchunk * ch, 3), -1, np.int64)
     cells[:m] = q.astype(np.int64)
     origin, ext = chunk_windows(cells.reshape(nchunk, ch, 3), cap)
-    chunk = np.arange(m) // ch
+    return _unit_global_reductions(p, q, nx, ny, np.arange(m) // ch, origin, ext, comps)
+
+
+# Brick schedule of the scatters (launch_scatter_schedule in transfer_kernels.cu): bricks of BRICK cells, work items of at most
+# SCHED_K warps.
+BRICK, SCHED_K = (28, 4, 4), 64
+
+
+def brick_schedule(cell_start, dims, brick=BRICK, k=SCHED_K):
+    """Restatement of the schedule build from the cell lists of a re-sort (cell_start: [n + 1], the particles of cell c are the sorted
+    indices cell_start[c] .. cell_start[c + 1]).  A warp w (particles 32w .. 32w + 31) belongs to the brick of its first particle's cell;
+    brick b = (bz * nby + by) * nbx + bx lists its warps in ascending order, cut into work items of at most k.  Returns the device arrays:
+    brick_warps and brick_items ([nbricks + 1], exclusive scans of the per-brick counts), item_start, item_brick, warps."""
+    nx, ny, nz = dims
+    bx, by, bz = brick
+    nbx, nby, nbz = -(-nx // bx), -(-ny // by), -(-nz // bz)
+    cs = (np.asarray(cell_start, np.int64) + 31) // 32  # warps whose first particle lies before each cell boundary
+    counts, items, item_start, item_brick, warps = [], [], [], [], []
+    for b in range(nbx * nby * nbz):
+        x0, y0, z0 = b % nbx * bx, b // nbx % nby * by, b // nbx // nby * bz
+        ws = []
+        for z in range(z0, min(z0 + bz, nz)):
+            for y in range(y0, min(y0 + by, ny)):
+                c0 = (z * ny + y) * nx + x0
+                ws.extend(range(cs[c0], cs[c0 + min(bx, nx - x0)]))
+        counts.append(len(ws))
+        items.append(-(-len(ws) // k))
+        item_start.extend(len(warps) + j for j in range(0, len(ws), k))
+        item_brick.extend([b] * items[-1])
+        warps.extend(ws)
+    scan = lambda a: np.concatenate([[0], np.cumsum(a)]).astype(np.int64)
+    return scan(counts), scan(items), np.array(item_start, np.int64), np.array(item_brick, np.int64), np.array(warps, np.int64)
+
+
+def item_windows(cells, item_brick, dims, cap, brick=BRICK):
+    """The tile window of every work item as density_scatter_kernel picks it (item_window): cells [items, L, 3] the primal cells of the item's
+    particles NOW (-1 past its last particle).  The faces [min - 1, max + 1] of those cells, cut z first, then y (neither below the brick's
+    rows + 2), then x, around the middle of the item's brick."""
+    nx, ny, nz = dims
+    bx, by, bz = brick
+    nbx, nby = -(-nx // bx), -(-ny // by)
+    valid = cells[:, :, 0] >= 0
+    big = np.iinfo(np.int64).max // 4
+    lo = np.where(valid[:, :, None], cells, big).min(axis=1) - 1
+    hi = np.where(valid[:, :, None], cells, -big).max(axis=1) + 1
+    e = hi - lo + 1
+    ex, ey, ez = e[:, 0].copy(), e[:, 1].copy(), e[:, 2].copy()
+    ez = np.minimum(ez, np.maximum(bz + 2, cap // (ex * ey)))
+    ey = np.minimum(ey, np.maximum(by + 2, cap // (ex * ez)))
+    ex = np.minimum(ex, cap // (ey * ez))
+    ext = np.stack([ex, ey, ez], axis=1)
+    b = np.asarray(item_brick)
+    mid = np.stack([b % nbx * bx + bx // 2, b // nbx % nby * by + by // 2, b // nbx // nby * bz + bz // 2], axis=1)
+    origin = np.minimum(np.maximum(mid - ext // 2, lo), hi - ext + 1)
+    return origin, ext
+
+
+def scheduled_global_reductions(p, sort_p, nx, ny, nz, cap=2048, comps=(3,)):
+    """tiled_global_reductions of the scheduled density scatter: p [n, 3] the positions scattered, sort_p the positions of the same array at
+    its last re-sort (sort_by_primal_cell order then).  The work items of brick_schedule share a tile; their windows come from p."""
+    m = len(p) // 32 * 32
+    cells = sort_p.astype(np.int64)
+    lin = cells[:, 0] + nx * (cells[:, 1] + ny * cells[:, 2])
+    assert (np.diff(lin) >= 0).all(), "sort_p must be in primal-cell order"
+    cell_start = np.searchsorted(lin, np.arange(nx * ny * nz + 1), side="left")
+    _, _, item_start, item_brick, warps = brick_schedule(cell_start, (nx, ny, nz))
+    item_of_warp = np.repeat(np.arange(len(item_start)), np.diff(np.append(item_start, len(warps))))
+    unit = np.empty(len(warps), np.int64)
+    unit[warps] = item_of_warp
+    unit = unit[np.arange(m) // 32]
+    lo = 0.5 if comps == (3,) else 1.0
+    q = np.maximum(p[:m].astype(np.float32), np.float32(lo))
+    c = q.astype(np.int64)
+    order = np.argsort(unit, kind="stable")
+    counts = np.bincount(unit, minlength=len(item_start))
+    pad = np.full((len(item_start), max(int(counts.max()), 1), 3), -1, np.int64)
+    slot = np.arange(m) - np.repeat(np.concatenate([[0], np.cumsum(counts)[:-1]]), counts)
+    pad[unit[order], slot] = c[order]
+    origin, ext = item_windows(pad, item_brick, (nx, ny, nz), cap)
+    return _unit_global_reductions(p, q, nx, ny, unit, origin, ext, comps)
+
+
+def _unit_global_reductions(p, q, nx, ny, unit, origin, ext, comps):
+    """unit[i]: the tile (chunk or work item) of particle i; origin / ext: the windows of the units"""
+    nz_max = int(p[:, 2].max()) + 2
+    m = len(q)
+    chunk = unit
     words = 1 if comps == (3,) else 2
     outside = flushed = 0
     idx = np.arange(32)[None, :]

@@ -121,6 +121,40 @@ struct SlabComm {
     unsigned int *seq = nullptr;  // device counter of all-reduce rounds done so far (identical on every rank)
 };
 
+// One mailbox round: round `seq` uses slot seq & 1.  Rank k stores {value bits, seq} as ONE 64-bit word per value, two values, into
+// entry k of every rank's mailbox (P2P store over NVLink), then polls entry j of its OWN mailbox for every rank j until it carries `seq`.
+// Two slots suffice: a rank can only be one round ahead of the slowest one, because finishing round n needs everybody's n-th message.
+// The PCG all-reduces (pcg.cu) and the stream-ordered slab barrier (slab.cu) share the slots and the round counter SlabComm::seq.
+constexpr long long MAILBOX_SPIN_LIMIT = 40LL * 1000 * 1000; // ~10 s: a dead peer ends the round with an error instead of hanging the GPU
+__device__ __forceinline__ unsigned long long *mailbox_entry(unsigned long long *mailbox, unsigned seq, int rank) {
+    return mailbox + (int)(seq & 1u) * 2 * SLAB_MAX_WORLD + 2 * rank;
+}
+// The system-scope fence first publishes everything this GPU wrote before (what other blocks wrote: as far as the caller has ordered it
+// before this thread, by a grid barrier or an arrival counter).
+__device__ __forceinline__ void mailbox_post(unsigned long long *entry, unsigned seq, unsigned v0, unsigned v1) {
+    __threadfence_system();
+    volatile unsigned long long *dst = entry;
+    dst[0] = ((unsigned long long)seq << 32) | (unsigned long long)v0;
+    dst[1] = ((unsigned long long)seq << 32) | (unsigned long long)v1;
+}
+// Spins until both words of `entry` carry `seq`, at most spin_limit times, and at least once but no longer once the block's dead flag is
+// set; sets the flag when the words never came.  v0 / v1: the words last read.  The system-scope fence after it is the acquire of what the
+// peers wrote before their posts.
+__device__ __forceinline__ void mailbox_poll(const unsigned long long *entry, unsigned seq, long long spin_limit, int *dead, unsigned long long &v0,
+                                             unsigned long long &v1) {
+    const volatile unsigned long long *src = entry;
+    long long spins = 0;
+    bool ok = false;
+    while (!*dead || spins == 0) {
+        v0 = src[0];
+        v1 = src[1];
+        if ((unsigned)(v0 >> 32) == seq && (unsigned)(v1 >> 32) == seq) { ok = true; break; }
+        if (++spins > spin_limit) break;
+    }
+    if (!ok) *dead = 1;
+    __threadfence_system();
+}
+
 // A particle on its way to the neighbouring slab: 64 B.
 struct MigrantRecord {
     float4 pos, rx, ry, rz;

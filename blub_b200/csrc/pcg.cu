@@ -7,7 +7,7 @@
 // ~85 B/cell/iteration).  Here a solve is
 //     prepare  (once): marker -> 1-byte codes (diag, fluid) + tile activity; p, r, s <- 0 off-fluid ("zero invariant": the
 //              7-point stencil, the dot products and the maxima then need no masks at all)
-//     solve    ONE persistent cooperative kernel (pcg_solve_persistent_kernel): per iteration
+//     solve    ONE persistent cooperative kernel (pcg_solve_columns_kernel by default): per iteration
 //                 phase A  s' = z + beta s fused with s'.A s'   (pressure_update_search.comp + pressure_apply_coeff.comp)
 //                 phase B  p += a s', r -= a A s', z.r, max|r|  (pressure_update_pressure_and_residual.comp + both
 //                          preconditioner passes + the BETA / MAX_ERROR reductions)
@@ -16,9 +16,12 @@
 //              (the reference zeroes its indirect-dispatch arguments instead, pressure_reduce.comp:89-92), per-thread
 //              skipping of fluid-free quads in sparsely filled tiles, and -- for z-slab sharded fluids -- the halo
 //              exchange and the scalar all-reduce INSIDE the kernel (P2P stores, mailboxes).
-// Alternatives kept and tested: a three-kernel-per-iteration path (dot / update / search with last-block-done reductions;
-// used for precond_mode 1 and when cooperative launch is unavailable) and two TMA-staged forms of the persistent kernel
-// (tensor-map box loads into shared memory; bit-compatible, measured slower -- see DESIGN.md 3.1).
+// The three persistent kernels run one solve loop (pcg_solve) and differ only in their walker -- how a phase deals its work: the
+// column solver's dense tiles plus a list of fluid columns, the tile kernel's active tiles (pcg_solve_persistent_kernel, solver paths 4
+// and 6), or tensor-map boxes staged in shared memory (pcg_solve_tma_kernel, path 2; bit-compatible, measured slower -- see DESIGN.md
+// 3.1) -- and in their reducer: an arrival counter (grid_reduce / grid_allreduce), or cooperative_groups grid barriers.
+// Also kept and tested: a three-kernel-per-iteration path (dot / update / search with last-block-done reductions; used for
+// precond_mode 1 and when cooperative launch is unavailable).
 //
 // Layout: four cells per thread along x (128-bit loads) marching 4 z-planes with the z-neighbours kept in registers and
 // the x-neighbours exchanged by warp shuffles; fp32 vectors, 1-byte cell codes, padded arrays (common.cuh); tiles without
@@ -28,6 +31,7 @@
 #include <cudaTypedefs.h>  // PFN_cuTensorMapEncodeTiled
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "blub_core.hpp"
 
@@ -578,39 +582,19 @@ struct PcgSolveArgs {
     SlabComm comm;          // world == 1: single GPU
 };
 
-// ---- cross-GPU all-reduce through peer-mapped mailboxes (z-slab sharding) ---------------------------------------
-// Round `seq` uses slot seq & 1.  Rank k stores {value bits, seq} as ONE 64-bit word into entry k of every rank's
-// mailbox (P2P store over NVLink), then every block of every rank spins on its OWN mailbox until all `world` entries
-// carry `seq` and adds them in rank order: identical result on every rank and in every block, no second barrier.
-// Two slots suffice: a rank can only be one round ahead of the slowest one, because finishing round n needs
-// everybody's n-th message.  The system-scope fences around it also publish / acquire the ghost planes pushed before.
-constexpr long long COMM_SPIN_LIMIT = 40LL * 1000 * 1000; // ~10 s: a dead peer ends the solve instead of hanging the GPU
-__device__ __forceinline__ void comm_allreduce(const SlabComm &c, unsigned seq, double &sum, float &mx, double *sh_sum, float *sh_max,
-                                               int *sh_dead) {
+// ---- cross-GPU all-reduce through peer-mapped mailboxes (z-slab sharding, protocol in common.cuh) ----------------
+// Every block of every rank polls its OWN mailbox until all `world` entries carry `seq` and adds them in rank order: identical
+// result on every rank and in every block, no second barrier.  The system-scope fences of the post and the poll also publish /
+// acquire the ghost planes pushed before.
+__device__ __forceinline__ void mailbox_gather(const SlabComm &c, unsigned seq, double &sum, float &mx, double *sh_sum, float *sh_max, int *sh_dead) {
     const int tid = linear_tid();
-    const int slot = (int)(seq & 1u) * 2 * SLAB_MAX_WORLD;
-    if (blockIdx.x == 0 && tid < c.world) {
-        __threadfence_system(); // everything this GPU wrote before (all blocks: ordered by the preceding grid barrier)
-        volatile unsigned long long *dst = c.mailbox[tid] + slot + 2 * c.rank;
-        dst[0] = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint((float)sum);
-        dst[1] = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint(mx);
-    }
     if (tid < c.world) {
-        volatile unsigned long long *src = c.mailbox[c.rank] + slot + 2 * tid;
-        unsigned long long v0 = 0, v1 = 0;
-        long long spins = 0;
-        bool ok = false;
-        while (!*sh_dead || spins == 0) {
-            v0 = src[0];
-            v1 = src[1];
-            if ((unsigned)(v0 >> 32) == seq && (unsigned)(v1 >> 32) == seq) { ok = true; break; }
-            if (++spins > COMM_SPIN_LIMIT) break;
-        }
-        if (!ok) *sh_dead = 1;
+        unsigned long long v0, v1;
+        // the fence ending the poll is the acquire, by the threads that saw the flags (the block follows through the barrier below): it
+        // orders the block's later loads of the ghost planes after the peers' pushes and drops stale L1 lines of this SM
+        mailbox_poll(mailbox_entry(c.mailbox[c.rank], seq, tid), seq, MAILBOX_SPIN_LIMIT, sh_dead, v0, v1);
         sh_sum[tid] = (double)__uint_as_float((unsigned)v0);
         sh_max[tid] = __uint_as_float((unsigned)v1);
-        __threadfence_system(); // acquire, by the threads that saw the flags (the block follows through the barrier below): orders the
-                                // block's later loads of the ghost planes after the peers' pushes and drops stale L1 lines of this SM
     }
     __syncthreads();
     double t = 0.0;
@@ -619,18 +603,18 @@ __device__ __forceinline__ void comm_allreduce(const SlabComm &c, unsigned seq, 
         t += sh_sum[k];
         m = fmaxf(m, sh_max[k]);
     }
-    __syncthreads();
+    __syncthreads(); // the mailbox copies are reused by the next round
     sum = t;
     mx = m;
 }
-
-// First thing a sharded solve does: one empty all-reduce round.  A rank that has entered its solver kernel has finished its
-// prepare kernel (stream order), which zeroes r and p off-fluid in ALL its planes -- ghost planes included -- with read-modify-
-// write; without the round a fast neighbour's first ghost-plane push could land in the middle of that and be lost.
-__device__ __forceinline__ void slab_start_handshake(const SlabComm &c, unsigned &seq, double *sh_sum, float *sh_max, int *sh_dead) {
-    double none = 0.0;
-    float nomax = 0.0f;
-    comm_allreduce(c, ++seq, none, nomax, sh_sum, sh_max, sh_dead);
+// Block 0 posts this rank's values; everything this GPU wrote before is ordered before the post by the preceding grid barrier (all
+// blocks) and the post's system-scope fence.
+__device__ __forceinline__ void comm_allreduce(const SlabComm &c, unsigned seq, double &sum, float &mx, double *sh_sum, float *sh_max,
+                                               int *sh_dead) {
+    const int tid = linear_tid();
+    if (blockIdx.x == 0 && tid < c.world)
+        mailbox_post(mailbox_entry(c.mailbox[tid], seq, c.rank), seq, __float_as_uint((float)sum), __float_as_uint(mx));
+    mailbox_gather(c, seq, sum, mx, sh_sum, sh_max, sh_dead);
 }
 
 // NOTE: r, s, p are written by other blocks between grid barriers: no __restrict__/read-only (LDG.NC) path for them.
@@ -828,102 +812,74 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
     }
 }
 
-// Tiles are dealt round robin: all blocks sweep the volume as one front, so the z-neighbour planes of a layer of tiles are still
-// in L2 when the next layer needs them.  (Grouping sparse tiles into equal-"work" slots was tried and is slower: a tile pass
-// costs a chain of dependent memory latencies whatever its fill.)  The id of the next tile is fetched one pass ahead.
-#define PCG_FOR_EACH_TILE(tile)                                                                                                      \
-    for (int li_ = blockIdx.x, tile = li_ < nact ? a.tile_list_flagged[li_] : 0, next_ = 0; li_ < nact; li_ += gridDim.x, tile = next_) \
-        if ((next_ = li_ + (int)gridDim.x < nact ? a.tile_list_flagged[li_ + gridDim.x] : 0), true)
-
-template <bool SKIP>
-__global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(PcgSolveArgs a) {
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
-    __shared__ float sh[PCG_THREADS / 32];
-    __shared__ double shd;
-    __shared__ float shf;
-    __shared__ double sh_csum[SLAB_MAX_WORLD];
-    __shared__ float sh_cmax[SLAB_MAX_WORLD];
-    __shared__ int sh_dead;
-    const TileMap t = a.t;
-    const SlabComm &cm_ = a.comm;
-    const bool sharded = cm_.world > 1;
-    const int nact = *a.num_active;
-    float *psumA = a.partials, *psumB = a.partials + gridDim.x, *pmax = a.partials + 2 * gridDim.x;
+// Formed from the kernel parameters where a phase needs it, not kept in the walkers: values derived from parameters are re-read from the
+// constant bank instead of holding registers through the whole solve (a TileEnv member made the TMA kernel spill three times as much).
+__device__ __forceinline__ TileEnv make_tile_env(const PcgSolveArgs &a) {
+    const SlabComm &cm = a.comm;
     TileEnv e;
     e.g = a.g;
     e.codes = a.codes;
-    e.sharded = sharded;
-    // slab geometry: tiles tz_first..tz_last are owned; the planes just outside are ghost planes fed by the neighbours
-    e.tz_first = cm_.halo / PCG_TZ;
-    e.tz_last = t.tiles_z - 1 - cm_.halo / PCG_TZ;
-    e.push = cm_.owned_nz * a.g.sz; // index distance between an owned boundary plane and its image in the neighbour
-    e.peer_r_lo = cm_.peer_r[0];
-    e.peer_r_hi = cm_.peer_r[1];
-    unsigned seq = 0;
-    if (linear_tid() == 0) sh_dead = 0;
-    if (sharded) seq = *cm_.seq;
+    e.sharded = cm.world > 1;
+    // slab geometry: tile layers tz_first..tz_last are owned; the planes just outside are ghost planes fed by the neighbours
+    e.tz_first = cm.halo / PCG_TZ;
+    e.tz_last = a.t.tiles_z - 1 - cm.halo / PCG_TZ;
+    e.push = cm.owned_nz * a.g.sz; // index distance between an owned boundary plane and its image in the neighbour
+    e.peer_r_lo = cm.peer_r[0];
+    e.peer_r_hi = cm.peer_r[1];
+    return e;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The solve, written once for the three persistent kernels.  A kernel hands it
+//   a walker:  init(acc), search(it, beta, acc) = phase A, update(it, alpha, acc, err) = phase B -- the kernel's share of the work of a
+//              phase -- and each_tile(f), which calls f(c) for every tile (and column) of that share;
+//   a reducer: the grid-wide sums, on z-slab ranks followed by or fused with the all-rank round: open(psum) and close(psum) are empty
+//              rounds, sum(psum, acc, tot) a sum, sum_max(psum, pmax, acc, err, tot, gmax) a sum and a maximum.
+// Partial buffers (gridDim.x floats each): init on 1, phase A on 0, phase B on 1 + 2 for the maximum (a fast block never overwrites
+// what a slow one still reads), the empty rounds of a sharded solve on 0.
+struct SlabRounds {
+    const SlabComm &c;
+    unsigned seq; // all-reduce rounds done so far
+    double *sh_sum;
+    float *sh_max;
+    int *sh_dead; // set when a peer did not answer (or a TMA transaction was lost): the solve ends with done = -1
+};
+
+template <class Walker, class Reducer>
+__device__ __forceinline__ void pcg_solve(const PcgSolveArgs &a, Walker &wk, Reducer &rd) {
+    SlabRounds &sr = rd.sr;
+    const bool sharded = sr.c.world > 1;
+    // partial buffers, formed where they are used: three pointers kept across the loop cost registers the phases need
+    auto partials = [&](int k) { return a.partials + k * gridDim.x; };
+    if (linear_tid() == 0) *sr.sh_dead = 0;
+    if (sharded) sr.seq = *sr.c.seq;
     __syncthreads();
-    if (sharded) slab_start_handshake(cm_, seq, sh_csum, sh_cmax, &sh_dead);
+    // First thing a sharded solve does: one empty round.  A rank that has entered its solver kernel has finished its prepare kernel
+    // (stream order), which zeroes r and p off-fluid in ALL its planes -- ghost planes included -- with read-modify-write; without the
+    // round a fast neighbour's first ghost-plane push could land in the middle of that and be lost.
+    if (sharded) rd.open(partials(0));
 
     // ---- init: r <- b - A p, sigma <- z.r (pressure_init.comp:45-83, pressure_solver.rs:625-649); s stays 0
     float acc = 0.0f;
-    PCG_FOR_EACH_TILE(tile) {
-        const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-        unsigned w[PCG_TZ + 2];
-        load_column_codes(e, c, w);
-        if (SKIP && warp_has_no_fluid(w)) continue;
-        if (!SKIP || (tile & TILE_DENSE_BIT)) init_tile<false>(e, c, w, a.p, a.r, acc);
-        else init_tile<true>(e, c, w, a.p, a.r, acc);
-    }
-    double tot = grid_sum(grid, psumB, acc, sh, &shd);
-    float gmax = 0.0f;
-    if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
+    wk.init(acc);
+    double tot;
+    rd.sum(partials(1), acc, tot);
     float sigma = (float)tot;
-    float alpha = 0.0f, beta = 0.0f, max_error = 0.0f;
+    float alpha = 0.0f, beta = 0.0f, max_error = 0.0f, gmax;
     int num_iterations = 0;
 
     for (int it = 0;; ++it) {
-        const float *s_in = (it & 1) ? a.s1 : a.s0;
-        float *s_out = (it & 1) ? a.s0 : a.s1;
         acc = 0.0f;
-        PCG_FOR_EACH_TILE(tile) {
-            const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-            unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
-            if (SKIP && warp_has_no_fluid(w)) continue;
-            if (!SKIP || (tile & TILE_DENSE_BIT)) search_tile<false>(e, c, w, a.r, s_in, s_out, beta, acc);
-            else search_tile<true>(e, c, w, a.r, s_in, s_out, beta, acc);
-        }
-        tot = grid_sum(grid, psumA, acc, sh, &shd);
-        if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
+        wk.search(it, beta, acc);
+        rd.sum(partials(0), acc, tot);
         alpha = guarded_div(sigma, (float)tot); // RESULTMODE_ALPHA, pressure_reduce.comp:73-75
 
-        const bool with_err = (a.max_iterations == it) || (it > 0 && it % a.check_frequency == 0); // pressure_solver.rs:676-677
         acc = 0.0f;
         float err = 0.0f;
-        PCG_FOR_EACH_TILE(tile) {
-            const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-            unsigned w[PCG_TZ + 2];
-            load_column_codes(e, c, w);
-            if (SKIP && warp_has_no_fluid(w)) continue;
-            if (!SKIP || (tile & TILE_DENSE_BIT)) update_tile<false>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
-            else update_tile<true>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
-        }
-        {
-            const float bm = block_max(err, sh);
-            if (linear_tid() == 0) pmax[blockIdx.x] = bm;
-        }
-        tot = grid_sum(grid, psumB, acc, sh, &shd); // the barrier inside also publishes pmax
-        {
-            const float em = final_max(pmax, gridDim.x, sh);
-            if (linear_tid() == 0) shf = em;
-            __syncthreads();
-            gmax = shf;
-            __syncthreads();
-        }
-        if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
+        wk.update(it, alpha, acc, err);
+        rd.sum_max(partials(1), partials(2), acc, err, tot, gmax);
         const float zr = (float)tot;
+        const bool with_err = (a.max_iterations == it) || (it > 0 && it % a.check_frequency == 0); // pressure_solver.rs:676-677
         if (with_err) {
             const float tol = a.params->tolerance[a.which];
             if (a.max_iterations == it || gmax < tol) { // pressure_reduce.comp:82-94: statistics + stop everything
@@ -936,23 +892,20 @@ __global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(Pc
         sigma = zr;
     }
     if (sharded) {
-        // hand the boundary planes of the solution to the neighbours (warm start of their next init, pressure gradient
-        // across the slab face), then one more round so that nobody leaves before its ghost planes are complete
-        float *const peer_p_lo = cm_.peer_p[a.which][0], *const peer_p_hi = cm_.peer_p[a.which][1];
-        for (int li = blockIdx.x; li < nact; li += gridDim.x) {
-            const TileCtx c = tile_ctx_id(e.g, t, a.tile_list[li]);
-            if (!c.valid) continue;
+        // hand the boundary planes of the solution to the neighbours (warm start of their next init, pressure gradient across the slab
+        // face), then one more round so that nobody leaves before its ghost planes are complete
+        float *const peer_p_lo = sr.c.peer_p[a.which][0], *const peer_p_hi = sr.c.peer_p[a.which][1];
+        const TileEnv e = make_tile_env(a);
+        wk.each_tile([&](const TileCtx &c) {
+            if (!c.valid) return;
             if (c.tz == e.tz_first && peer_p_lo) st4(peer_p_lo + c.i + e.push, ld4(a.p + c.i));
             if (c.tz == e.tz_last && peer_p_hi) {
                 const int i = c.i + (PCG_TZ - 1) * e.g.sz;
                 st4(peer_p_hi + i - e.push, ld4(a.p + i));
             }
-        }
-        grid.sync();
-        double dummy = 0.0;
-        float dmax = 0.0f;
-        comm_allreduce(cm_, ++seq, dummy, dmax, sh_csum, sh_cmax, &sh_dead);
-        if (blockIdx.x == 0 && linear_tid() == 0) *cm_.seq = seq;
+        });
+        rd.close(partials(0));
+        if (blockIdx.x == 0 && linear_tid() == 0) *sr.c.seq = sr.seq;
     }
     if (blockIdx.x == 0 && linear_tid() == 0) {
         a.scal->alpha = alpha;
@@ -960,10 +913,117 @@ __global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(Pc
         a.scal->sigma = sigma;
         a.scal->max_error = max_error;
         a.scal->num_iterations = num_iterations;
-        a.scal->done = sh_dead ? -1 : 1;
+        a.scal->done = *sr.sh_dead ? -1 : 1;
     }
 }
-#undef PCG_FOR_EACH_TILE
+
+// Reducer of the tile and TMA kernels: cooperative_groups grid barrier, every block re-reads the partials (block_sum / final_sum /
+// final_max); on z-slab ranks a mailbox round after it.
+struct SyncReduce {
+    SlabRounds sr;
+    cooperative_groups::grid_group grid;
+    float *sh;
+    double *shd;
+    float *shf;
+    __device__ __forceinline__ void open(float *) {
+        double none = 0.0;
+        float nomax = 0.0f;
+        comm_allreduce(sr.c, ++sr.seq, none, nomax, sr.sh_sum, sr.sh_max, sr.sh_dead);
+    }
+    __device__ __forceinline__ void close(float *psum) {
+        grid.sync(); // every block's pushes before block 0 posts
+        open(psum);
+    }
+    __device__ __forceinline__ void sum(float *psum, float acc, double &tot) {
+        tot = grid_sum(grid, psum, acc, sh, shd);
+        float nomax = 0.0f;
+        if (sr.c.world > 1) comm_allreduce(sr.c, ++sr.seq, tot, nomax, sr.sh_sum, sr.sh_max, sr.sh_dead);
+    }
+    __device__ __forceinline__ void sum_max(float *psum, float *pmax, float acc, float err, double &tot, float &gmax) {
+        {
+            const float bm = block_max(err, sh);
+            if (linear_tid() == 0) pmax[blockIdx.x] = bm;
+        }
+        tot = grid_sum(grid, psum, acc, sh, shd); // the barrier inside also publishes pmax
+        {
+            const float em = final_max(pmax, gridDim.x, sh);
+            if (linear_tid() == 0) *shf = em;
+            __syncthreads();
+            gmax = *shf;
+            __syncthreads();
+        }
+        if (sr.c.world > 1) comm_allreduce(sr.c, ++sr.seq, tot, gmax, sr.sh_sum, sr.sh_max, sr.sh_dead);
+    }
+};
+
+// Tiles are dealt round robin: all blocks sweep the volume as one front, so the z-neighbour planes of a layer of tiles are still
+// in L2 when the next layer needs them.  (Grouping sparse tiles into equal-"work" slots was tried and is slower: a tile pass
+// costs a chain of dependent memory latencies whatever its fill.)  The id of the next tile is fetched one pass ahead.
+#define PCG_FOR_EACH_TILE(tile)                                                                                                      \
+    for (int li_ = blockIdx.x, tile = li_ < nact ? a.tile_list_flagged[li_] : 0, next_ = 0; li_ < nact; li_ += gridDim.x, tile = next_) \
+        if ((next_ = li_ + (int)gridDim.x < nact ? a.tile_list_flagged[li_ + gridDim.x] : 0), true)
+
+// Phases of the register-marching kernels (tile and column solver): Walk::passes(fill, body) calls body(c, w, sparse) for every pass of
+// the thread -- a tile or a column with its code words w; sparse: std::true_type for the sparse body -- and fill is set in the first
+// phase of a solve.
+template <class Walk>
+struct MarchWalker : Walk {
+    __device__ __forceinline__ void init(float &acc) const {
+        const TileEnv e = make_tile_env(this->a);
+        this->passes(true, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
+            init_tile<decltype(sparse)::value>(e, c, w, this->a.p, this->a.r, acc);
+        });
+    }
+    __device__ __forceinline__ void search(int it, float beta, float &acc) const {
+        const float *s_in = (it & 1) ? this->a.s1 : this->a.s0;
+        float *s_out = (it & 1) ? this->a.s0 : this->a.s1;
+        const TileEnv e = make_tile_env(this->a);
+        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
+            search_tile<decltype(sparse)::value>(e, c, w, this->a.r, s_in, s_out, beta, acc);
+        });
+    }
+    __device__ __forceinline__ void update(int it, float alpha, float &acc, float &err) const {
+        const float *s = (it & 1) ? this->a.s0 : this->a.s1;
+        const TileEnv e = make_tile_env(this->a);
+        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
+            update_tile<decltype(sparse)::value>(e, c, w, s, this->a.p, this->a.r, alpha, acc, err);
+        });
+    }
+};
+
+// Work of the tile kernel: the active tiles; SKIP: sparse bodies in tiles that are not flagged dense, and warps without fluid skipped
+template <bool SKIP>
+struct TileWalk {
+    const PcgSolveArgs &a;
+    int nact;
+    template <class F> __device__ __forceinline__ void each_tile(F f) const {
+        PCG_FOR_EACH_TILE(tile) f(tile_ctx_id(a.g, a.t, tile & (TILE_DENSE_BIT - 1)));
+    }
+    template <class Body> __device__ __forceinline__ void passes(bool, Body body) const {
+        const TileEnv e = make_tile_env(a);
+        PCG_FOR_EACH_TILE(tile) {
+            const TileCtx c = tile_ctx_id(e.g, a.t, tile & (TILE_DENSE_BIT - 1));
+            unsigned w[PCG_TZ + 2];
+            load_column_codes(e, c, w);
+            if (SKIP && warp_has_no_fluid(w)) continue;
+            if (!SKIP || (tile & TILE_DENSE_BIT)) body(c, w, std::false_type{});
+            else body(c, w, std::true_type{});
+        }
+    }
+};
+
+template <bool SKIP>
+__global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(PcgSolveArgs a) {
+    __shared__ float sh[PCG_THREADS / 32];
+    __shared__ double shd;
+    __shared__ float shf;
+    __shared__ double sh_csum[SLAB_MAX_WORLD];
+    __shared__ float sh_cmax[SLAB_MAX_WORLD];
+    __shared__ int sh_dead;
+    MarchWalker<TileWalk<SKIP>> wk{{a, *a.num_active}};
+    SyncReduce rd{{a.comm, 0u, sh_csum, sh_cmax, &sh_dead}, cooperative_groups::this_grid(), sh, &shd, &shf};
+    pcg_solve(a, wk, rd);
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Grid-wide reduction of the column solver.  With the fluid working set in L2 the solve is bound by the latency of these two
@@ -983,9 +1043,12 @@ struct ReduceScratch {
     float sh[2 * (PCG_THREADS / 32)];
     double shd[PCG_THREADS / 32];
 };
-template <bool WITH_MAX>
-__device__ __forceinline__ void grid_reduce(unsigned *counter, unsigned &round, float *psum, float *pmax, float acc, float err, ReduceScratch &sc, double &tot,
-                                            float &gmax) {
+// First half of both forms: the block's sum (and maximum) formed in one shared-memory pass, published by thread 0 into psum / pmax
+// [blockIdx.x], which then arrives on the counter for round `round` (counted here).  TICKET = false: release, then wait with acquire until
+// everybody of the round has arrived.  TICKET = true: nobody waits; returns true (block-uniform) in the block that arrived last.
+template <bool WITH_MAX, bool TICKET>
+__device__ __forceinline__ bool publish_and_arrive(unsigned *counter, unsigned &round, float *psum, float *pmax, float acc, float err, ReduceScratch &sc,
+                                                   int *sh_last) {
     constexpr int NW = PCG_THREADS / 32;
     const int tid = linear_tid(), lane = tid & 31, w = tid >> 5;
     acc = warp_sum(acc);
@@ -1005,11 +1068,25 @@ __device__ __forceinline__ void grid_reduce(unsigned *counter, unsigned &round, 
         }
         psum[blockIdx.x] = bs;
         if (WITH_MAX) pmax[blockIdx.x] = bm;
-        red_release_u32(counter, 1u);
-        const unsigned target = round * gridDim.x;
-        while (ld_acquire_u32(counter) < target) {}
+        if (TICKET) {
+            __threadfence(); // release: the partials (and this block's pushes into the neighbours' ghost planes) before the ticket
+            const unsigned ticket = atomicAdd(counter, 1u);
+            *sh_last = ticket == round * gridDim.x - 1u ? 1 : 0;
+            __threadfence(); // acquire (matters in the last block): everybody else's partials are visible from here on
+        } else {
+            red_release_u32(counter, 1u);
+            const unsigned target = round * gridDim.x;
+            while (ld_acquire_u32(counter) < target) {}
+        }
     }
     __syncthreads();
+    return TICKET && *sh_last;
+}
+// Every thread: the partials of all blocks added in the same fixed order in fp64 (and their maximum).
+template <bool WITH_MAX>
+__device__ __forceinline__ void read_partials(const float *psum, const float *pmax, ReduceScratch &sc, double &tot, float &gmax) {
+    constexpr int NW = PCG_THREADS / 32;
+    const int tid = linear_tid(), lane = tid & 31, w = tid >> 5;
     double a = 0.0;
     float m = 0.0f;
     for (int k = tid; k < (int)gridDim.x; k += PCG_THREADS) {
@@ -1030,9 +1107,15 @@ __device__ __forceinline__ void grid_reduce(unsigned *counter, unsigned &round, 
         t += sc.shd[k];
         if (WITH_MAX) mm = fmaxf(mm, sc.sh[k]);
     }
-    __syncthreads(); // the scratch is reused by the next reduction
     tot = t;
     gmax = mm;
+}
+template <bool WITH_MAX>
+__device__ __forceinline__ void grid_reduce(unsigned *counter, unsigned &round, float *psum, float *pmax, float acc, float err, ReduceScratch &sc, double &tot,
+                                            float &gmax) {
+    publish_and_arrive<WITH_MAX, false>(counter, round, psum, pmax, acc, err, sc, nullptr);
+    read_partials<WITH_MAX>(psum, pmax, sc, tot, gmax);
+    __syncthreads(); // the scratch is reused by the next reduction
 }
 
 // The same reduction on a z-slab rank, fused with the cross-GPU all-reduce: the block that arrives LAST on the local counter (atomicAdd returns
@@ -1044,87 +1127,39 @@ __device__ __forceinline__ void grid_reduce(unsigned *counter, unsigned &round, 
 template <bool WITH_MAX>
 __device__ __forceinline__ void grid_allreduce(const SlabComm &c, unsigned seq, unsigned *counter, unsigned &round, float *psum, float *pmax, float acc, float err,
                                                ReduceScratch &sc, double *sh_sum, float *sh_max, int *sh_dead, int *sh_last, double &tot, float &gmax) {
-    constexpr int NW = PCG_THREADS / 32;
-    const int tid = linear_tid(), lane = tid & 31, w = tid >> 5;
-    acc = warp_sum(acc);
-    if (WITH_MAX) err = warp_max(err);
-    if (lane == 0) {
-        sc.sh[w] = acc;
-        if (WITH_MAX) sc.sh[NW + w] = err;
+    if (publish_and_arrive<WITH_MAX, true>(counter, round, psum, pmax, acc, err, sc, sh_last)) { // this block adds the GPU's partials and posts
+        double t;
+        float mm;
+        read_partials<WITH_MAX>(psum, pmax, sc, t, mm);
+        // the post's system-scope fence covers everything this GPU wrote before, cumulatively through the ticket
+        if (linear_tid() < c.world) mailbox_post(mailbox_entry(c.mailbox[linear_tid()], seq, c.rank), seq, __float_as_uint((float)t), __float_as_uint(mm));
     }
-    __syncthreads();
-    round += 1u;
-    if (tid == 0) {
-        float bs = 0.0f, bm = 0.0f;
-#pragma unroll
-        for (int k = 0; k < NW; ++k) {
-            bs += sc.sh[k];
-            if (WITH_MAX) bm = fmaxf(bm, sc.sh[NW + k]);
-        }
-        psum[blockIdx.x] = bs;
-        if (WITH_MAX) pmax[blockIdx.x] = bm;
-        __threadfence(); // release: the partials (and this block's pushes into the neighbours' ghost planes) before the ticket
-        const unsigned ticket = atomicAdd(counter, 1u);
-        *sh_last = ticket == round * gridDim.x - 1u ? 1 : 0;
-        __threadfence(); // acquire (matters in the last block): everybody else's partials are visible from here on
-    }
-    __syncthreads();
-    const int slot = (int)(seq & 1u) * 2 * SLAB_MAX_WORLD;
-    if (*sh_last) { // block-uniform: this block adds the GPU's partials in fixed order and publishes the total
-        double a = 0.0;
-        float m = 0.0f;
-        for (int k = tid; k < (int)gridDim.x; k += PCG_THREADS) {
-            a += (double)__ldcg(psum + k);
-            if (WITH_MAX) m = fmaxf(m, __ldcg(pmax + k));
-        }
-        a = warp_sum(a);
-        if (WITH_MAX) m = warp_max(m);
-        if (lane == 0) {
-            sc.shd[w] = a;
-            if (WITH_MAX) sc.sh[w] = m;
-        }
-        __syncthreads();
-        if (tid < c.world) {
-            double t = 0.0;
-            float mm = 0.0f;
-#pragma unroll
-            for (int k = 0; k < NW; ++k) {
-                t += sc.shd[k];
-                if (WITH_MAX) mm = fmaxf(mm, sc.sh[k]);
-            }
-            __threadfence_system(); // everything this GPU wrote before, cumulatively through the ticket
-            volatile unsigned long long *dst = c.mailbox[tid] + slot + 2 * c.rank;
-            dst[0] = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint((float)t);
-            dst[1] = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint(mm);
-        }
-    }
-    if (tid < c.world) {
-        volatile unsigned long long *src = c.mailbox[c.rank] + slot + 2 * tid;
-        unsigned long long v0 = 0, v1 = 0;
-        long long spins = 0;
-        bool ok = false;
-        while (!*sh_dead || spins == 0) {
-            v0 = src[0];
-            v1 = src[1];
-            if ((unsigned)(v0 >> 32) == seq && (unsigned)(v1 >> 32) == seq) { ok = true; break; }
-            if (++spins > COMM_SPIN_LIMIT) break;
-        }
-        if (!ok) *sh_dead = 1;
-        sh_sum[tid] = (double)__uint_as_float((unsigned)v0);
-        sh_max[tid] = __uint_as_float((unsigned)v1);
-        __threadfence_system(); // acquire: later loads of the ghost planes come after the peers' pushes; drops stale L1 lines of this SM
-    }
-    __syncthreads();
-    double t = 0.0;
-    float m = 0.0f;
-    for (int k = 0; k < c.world; ++k) {
-        t += sh_sum[k];
-        m = fmaxf(m, sh_max[k]);
-    }
-    __syncthreads(); // the scratch and the mailbox copies are reused by the next round
-    tot = t;
-    gmax = m;
+    mailbox_gather(c, seq, tot, gmax, sh_sum, sh_max, sh_dead);
 }
+
+// Reducer of the column solver: grid_reduce on one GPU, grid_allreduce on z-slab ranks.
+struct CounterReduce {
+    SlabRounds sr;
+    unsigned *counter;
+    unsigned round; // counter rounds done by this solve (the counter is 0 at its start)
+    ReduceScratch &sc;
+    int *sh_last;
+    template <bool WITH_MAX> __device__ __forceinline__ void reduce(float *psum, float *pmax, float acc, float err, double &tot, float &gmax) {
+        if (sr.c.world > 1) grid_allreduce<WITH_MAX>(sr.c, ++sr.seq, counter, round, psum, pmax, acc, err, sc, sr.sh_sum, sr.sh_max, sr.sh_dead, sh_last, tot, gmax);
+        else grid_reduce<WITH_MAX>(counter, round, psum, pmax, acc, err, sc, tot, gmax);
+    }
+    __device__ __forceinline__ void open(float *psum) {
+        double none;
+        float nomax;
+        reduce<false>(psum, nullptr, 0.0f, 0.0f, none, nomax);
+    }
+    __device__ __forceinline__ void close(float *psum) { open(psum); } // the counter's release orders the pushes before the post
+    __device__ __forceinline__ void sum(float *psum, float acc, double &tot) {
+        float nomax;
+        reduce<false>(psum, nullptr, acc, 0.0f, tot, nomax);
+    }
+    __device__ __forceinline__ void sum_max(float *psum, float *pmax, float acc, float err, double &tot, float &gmax) { reduce<true>(psum, pmax, acc, err, tot, gmax); }
+};
 
 // ---------------------------------------------------------------------------------------------------------------
 // Column solver (default on one GPU): the persistent solver with a work list that follows the fluid.
@@ -1202,9 +1237,6 @@ __global__ void __launch_bounds__(1024) pcg_compact_kernel(const uint8_t *__rest
     if (threadIdx.x == 0) { *num_active = carry; *num_cols = carry_c; }
 }
 
-#define PCG_FOR_EACH_TILE(tile)                                                                                                      \
-    for (int li_ = blockIdx.x, tile = li_ < nact ? a.tile_list_flagged[li_] : 0, next_ = 0; li_ < nact; li_ += gridDim.x, tile = next_) \
-        if ((next_ = li_ + (int)gridDim.x < nact ? a.tile_list_flagged[li_ + gridDim.x] : 0), true)
 // 32 consecutive list entries per warp and pass; the index of the next pass is fetched one pass ahead.  All 32 lanes stay in the loop
 // (the bodies shuffle): lanes beyond the end of the list carry valid = false.
 #define PCG_FOR_EACH_COLUMN(c)                                                                                                            \
@@ -1246,6 +1278,34 @@ constexpr int PCG_CODE_SLOT_BYTES = (PCG_TZ + 2) * PCG_THREADS * 4; // 6 KB
 // steps/s), 12 slots shrink L1 to ~28 KB and ran 112.9 (H100 SXM at 400 W, profiles/h100_pcg_setup.json)
 constexpr int PCG_CODE_SLOTS = 8;
 
+// Work of the column solver: the dense tiles by the tile body, then the column list by the sparse body, code words of the first passes
+// kept in shared memory (pass_codes)
+struct ColumnWalk {
+    const PcgSolveArgs &a;
+    int nact, ncols;
+    int lane, col_stride, warp_first, sz;
+    unsigned *sh_cw;
+    template <class F> __device__ __forceinline__ void each_tile(F f) const {
+        PCG_FOR_EACH_TILE(tile) f(tile_ctx_id(a.g, a.t, tile & (TILE_DENSE_BIT - 1)));
+        PCG_FOR_EACH_COLUMN(c) f(c);
+    }
+    template <class Body> __device__ __forceinline__ void passes(bool fill, Body body) const {
+        const TileEnv e = make_tile_env(a);
+        int pass = 0;
+        PCG_FOR_EACH_TILE(tile) {
+            const TileCtx c = tile_ctx_id(e.g, a.t, tile & (TILE_DENSE_BIT - 1));
+            unsigned w[PCG_TZ + 2];
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, fill);
+            body(c, w, std::false_type{});
+        }
+        PCG_FOR_EACH_COLUMN(c) {
+            unsigned w[PCG_TZ + 2];
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, fill);
+            body(c, w, std::true_type{});
+        }
+    }
+};
+
 // Three resident blocks per SM (up to 85 registers): for sm_90a, a four-block bound (64 registers) spills the column body to local memory,
 // and on an H100 SXM (700 W limit) the 256^3 dam break runs 100.9 instead of 97.7 steps/s with three blocks (profiles/h100_choices.json).
 __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSolveArgs a) {
@@ -1254,143 +1314,14 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSo
     __shared__ double sh_csum[SLAB_MAX_WORLD];
     __shared__ float sh_cmax[SLAB_MAX_WORLD];
     __shared__ int sh_dead, sh_last;
-    const TileMap t = a.t;
-    const SlabComm &cm_ = a.comm;
-    const bool sharded = cm_.world > 1;
-    const int nact = *a.num_active, ncols = *a.num_cols;
-    const int lane = linear_tid() & 31;
     // Tiles are dealt to the blocks from block 0 upwards, columns to the warps from the LAST warp of the last block downwards: when there are
     // fewer dense tiles than blocks (or a remainder), the blocks without a tile take the columns first and a phase is one pass, not two.
     const int col_stride = gridDim.x * PCG_THREADS;
     const int warp_first = col_stride - 32 - (blockIdx.x * (PCG_THREADS / 32) + (linear_tid() >> 5)) * 32;
-    float *psumA = a.partials, *psumB = a.partials + gridDim.x, *pmax = a.partials + 2 * gridDim.x;
-    TileEnv e;
-    e.g = a.g;
-    e.codes = a.codes;
-    e.sharded = sharded;
-    // slab geometry: tile layers tz_first..tz_last are owned; the planes just outside are ghost planes fed by the neighbours
-    e.tz_first = cm_.halo / PCG_TZ;
-    e.tz_last = t.tiles_z - 1 - cm_.halo / PCG_TZ;
-    e.push = cm_.owned_nz * a.g.sz; // index distance between an owned boundary plane and its image in the neighbour
-    e.peer_r_lo = cm_.peer_r[0];
-    e.peer_r_hi = cm_.peer_r[1];
-    const int sz = a.g.sz;
-    unsigned seq = 0;
-    if (linear_tid() == 0) sh_dead = 0;
-    if (sharded) seq = *cm_.seq;
-    __syncthreads();
-    unsigned round = 0;
-    double tot = 0.0;
-    float gmax = 0.0f;
-    // start handshake: one empty round (a rank inside its solver has finished its prepare kernel; see the tile kernel)
-    if (sharded) grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumA, pmax, 0.0f, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
-
-    // ---- init: r <- b - A p, sigma <- z.r (pressure_init.comp:45-83, pressure_solver.rs:625-649); s stays 0
-    float acc = 0.0f;
-    int pass = 0;
-    PCG_FOR_EACH_TILE(tile) {
-        const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-        unsigned w[PCG_TZ + 2];
-        pass_codes(e, c, w, sh_cw, a.code_slots, pass++, true);
-        init_tile<false>(e, c, w, a.p, a.r, acc);
-    }
-    PCG_FOR_EACH_COLUMN(c) {
-        unsigned w[PCG_TZ + 2];
-        pass_codes(e, c, w, sh_cw, a.code_slots, pass++, true);
-        init_tile<true>(e, c, w, a.p, a.r, acc);
-    }
-    if (sharded) grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumB, pmax, acc, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
-    else grid_reduce<false>(a.barrier, round, psumB, pmax, acc, 0.0f, sc, tot, gmax);
-    float sigma = (float)tot;
-    float alpha = 0.0f, beta = 0.0f, max_error = 0.0f;
-    int num_iterations = 0;
-
-    for (int it = 0;; ++it) {
-        const float *s_in = (it & 1) ? a.s1 : a.s0;
-        float *s_out = (it & 1) ? a.s0 : a.s1;
-        acc = 0.0f;
-        pass = 0;
-        PCG_FOR_EACH_TILE(tile) {
-            const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-            unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
-            search_tile<false>(e, c, w, a.r, s_in, s_out, beta, acc);
-        }
-        PCG_FOR_EACH_COLUMN(c) {
-            unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
-            search_tile<true>(e, c, w, a.r, s_in, s_out, beta, acc);
-        }
-        if (sharded) grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumA, pmax, acc, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
-        else grid_reduce<false>(a.barrier, round, psumA, pmax, acc, 0.0f, sc, tot, gmax);
-        alpha = guarded_div(sigma, (float)tot); // RESULTMODE_ALPHA, pressure_reduce.comp:73-75
-
-        const bool with_err = (a.max_iterations == it) || (it > 0 && it % a.check_frequency == 0); // pressure_solver.rs:676-677
-        acc = 0.0f;
-        float err = 0.0f;
-        pass = 0;
-        PCG_FOR_EACH_TILE(tile) {
-            const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-            unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
-            update_tile<false>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
-        }
-        PCG_FOR_EACH_COLUMN(c) {
-            unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, false);
-            update_tile<true>(e, c, w, s_out, a.p, a.r, alpha, acc, err);
-        }
-        if (sharded) grid_allreduce<true>(cm_, ++seq, a.barrier, round, psumB, pmax, acc, err, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, tot, gmax);
-        else grid_reduce<true>(a.barrier, round, psumB, pmax, acc, err, sc, tot, gmax);
-        const float zr = (float)tot;
-        if (with_err) {
-            const float tol = a.params->tolerance[a.which];
-            if (a.max_iterations == it || gmax < tol) { // pressure_reduce.comp:82-94: statistics + stop everything
-                max_error = gmax;
-                num_iterations = it;
-                break;
-            }
-        }
-        beta = guarded_div(zr, sigma); // RESULTMODE_BETA, pressure_reduce.comp:77-80
-        sigma = zr;
-    }
-    if (sharded) {
-        // hand the boundary planes of the solution to the neighbours (warm start of their next init, pressure gradient across the slab
-        // face), then one more round so that nobody leaves before its ghost planes are complete
-        float *const peer_p_lo = cm_.peer_p[a.which][0], *const peer_p_hi = cm_.peer_p[a.which][1];
-        PCG_FOR_EACH_TILE(tile) {
-            const TileCtx c = tile_ctx_id(e.g, t, tile & (TILE_DENSE_BIT - 1));
-            if (!c.valid) continue;
-            if (c.tz == e.tz_first && peer_p_lo) st4(peer_p_lo + c.i + e.push, ld4(a.p + c.i));
-            if (c.tz == e.tz_last && peer_p_hi) {
-                const int i = c.i + (PCG_TZ - 1) * e.g.sz;
-                st4(peer_p_hi + i - e.push, ld4(a.p + i));
-            }
-        }
-        PCG_FOR_EACH_COLUMN(c) {
-            if (!c.valid) continue;
-            if (c.tz == e.tz_first && peer_p_lo) st4(peer_p_lo + c.i + e.push, ld4(a.p + c.i));
-            if (c.tz == e.tz_last && peer_p_hi) {
-                const int i = c.i + (PCG_TZ - 1) * e.g.sz;
-                st4(peer_p_hi + i - e.push, ld4(a.p + i));
-            }
-        }
-        double dummy = 0.0;
-        float dmax = 0.0f;
-        grid_allreduce<false>(cm_, ++seq, a.barrier, round, psumA, pmax, 0.0f, 0.0f, sc, sh_csum, sh_cmax, &sh_dead, &sh_last, dummy, dmax);
-        if (blockIdx.x == 0 && linear_tid() == 0) *cm_.seq = seq;
-    }
-    if (blockIdx.x == 0 && linear_tid() == 0) {
-        a.scal->alpha = alpha;
-        a.scal->beta = beta;
-        a.scal->sigma = sigma;
-        a.scal->max_error = max_error;
-        a.scal->num_iterations = num_iterations;
-        a.scal->done = sh_dead ? -1 : 1;
-    }
+    MarchWalker<ColumnWalk> wk{{a, *a.num_active, *a.num_cols, linear_tid() & 31, col_stride, warp_first, a.g.sz, sh_cw}};
+    CounterReduce rd{{a.comm, 0u, sh_csum, sh_cmax, &sh_dead}, a.barrier, 0u, sc, &sh_last};
+    pcg_solve(a, wk, rd);
 }
-#undef PCG_FOR_EACH_COLUMN
-#undef PCG_FOR_EACH_TILE
 
 // ---------------------------------------------------------------------------------------------------------------
 // TMA-tiled variant of the persistent solver (grids whose x extent is a multiple of 128 cells).
@@ -1446,93 +1377,42 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity, int *s
     }
 }
 
-__global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __grid_constant__ PcgSolveArgs a, const __grid_constant__ PcgTmaMaps maps) {
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    float *const shR = reinterpret_cast<float *>(smem_raw);
-    float *const shS = reinterpret_cast<float *>(smem_raw + TMA_F32_BYTES);
-    uint8_t *const shC = smem_raw + 2 * TMA_F32_BYTES;
-    __shared__ uint64_t bar;
-    __shared__ float sh[PCG_THREADS / 32];
-    __shared__ double shd;
-    __shared__ float shf;
-    __shared__ double sh_csum[SLAB_MAX_WORLD];
-    __shared__ float sh_cmax[SLAB_MAX_WORLD];
-    __shared__ int sh_dead;
-    const GridDim g = a.g;
-    const TileMap t = a.t;
-    const SlabComm &cm_ = a.comm;
-    const bool sharded = cm_.world > 1;
-    const int nact = *a.num_active;
-    const uint8_t *__restrict__ codes = a.codes;
-    float *psumA = a.partials, *psumB = a.partials + gridDim.x, *pmax = a.partials + 2 * gridDim.x;
-    const int tz_first = cm_.halo / PCG_TZ, tz_last = t.tiles_z - 1 - cm_.halo / PCG_TZ;
-    const int push = cm_.owned_nz * g.sz;
-    float *const peer_r_lo = cm_.peer_r[0], *const peer_r_hi = cm_.peer_r[1];
-    const int tid = linear_tid(), lx = threadIdx.x, ly = threadIdx.y;
-    unsigned seq = 0, parity = 0;
-    if (tid == 0) {
-        sh_dead = 0;
-        mbar_init(&bar, 1);
-        fence_proxy_async(); // make the initialised barrier visible to the async (TMA) proxy
+// Work of the TMA kernel: the active tiles, operands staged in shared memory by tensor-map box loads.  Every phase ends with
+// fence_proxy_async_global(): its generic-proxy stores of r, s and p come before the async-proxy (TMA) reads after the grid barrier.
+struct TmaWalk {
+    const PcgSolveArgs &a;
+    const PcgTmaMaps &maps;
+    int nact;
+    float *shR, *shS;
+    uint8_t *shC;
+    uint64_t *bar;
+    int *sh_dead;
+    unsigned parity; // of the mbarrier phase the next box load completes
+    template <class F> __device__ __forceinline__ void each_tile(F f) const {
+        for (int li = blockIdx.x; li < nact; li += gridDim.x) f(tile_ctx_id(a.g, a.t, a.tile_list[li]));
     }
-    if (sharded) seq = *cm_.seq;
-    __syncthreads();
-    if (sharded) slab_start_handshake(cm_, seq, sh_csum, sh_cmax, &sh_dead);
-
-    // ---- init: r <- b - A p, sigma <- z.r (as in the register-marching kernel: runs once, plain loads)
-    float acc = 0.0f;
-    for (int li = blockIdx.x; li < nact; li += gridDim.x) {
-        const TileCtx c = tile_ctx_id(g, t, a.tile_list[li]);
-        int i = c.i;
-        float4 pm = zero4(), p0 = zero4(), pp = zero4();
-        if (c.valid) { pm = ld4(a.p + i - g.sz); p0 = ld4(a.p + i); }
-#pragma unroll
-        for (int k = 0; k < PCG_TZ; ++k, i += g.sz) {
-            float left, right;
-            x_neighbours(a.p, i, p0, c, left, right);
-            if (c.valid) {
-                pp = ld4(a.p + i + g.sz);
-                const uchar4 code = ldcode(codes + i);
-                const float4 ym = ld4(a.p + i - g.sy), yp = ld4(a.p + i + g.sy);
-                float4 r4 = ld4(a.r + i);
-                const float4 Ap = stencil_quad(code, p0, left, right, ym, yp, pm, pp);
-                r4.x -= code.x ? Ap.x : 0.0f;
-                r4.y -= code.y ? Ap.y : 0.0f;
-                r4.z -= code.z ? Ap.z : 0.0f;
-                r4.w -= code.w ? Ap.w : 0.0f;
-                st4(a.r + i, r4);
-                if (sharded) {
-                    if (k == 0 && c.tz == tz_first && peer_r_lo) st4(peer_r_lo + i + push, r4);
-                    if (k == PCG_TZ - 1 && c.tz == tz_last && peer_r_hi) st4(peer_r_hi + i - push, r4);
-                }
-                acc += (precond_diag2(r4.x, code.x) * r4.x + precond_diag2(r4.y, code.y) * r4.y) +
-                       (precond_diag2(r4.z, code.z) * r4.z + precond_diag2(r4.w, code.w) * r4.w);
-            }
-            pm = p0;
-            p0 = pp;
-        }
+    // init as in the register-marching kernels (runs once, plain loads)
+    __device__ __forceinline__ void init(float &acc) const {
+        const TileEnv e = make_tile_env(a);
+        each_tile([&](const TileCtx &c) {
+            unsigned w[PCG_TZ + 2];
+            load_column_codes(e, c, w);
+            init_tile<false>(e, c, w, a.p, a.r, acc);
+        });
+        fence_proxy_async_global();
     }
-    fence_proxy_async_global();
-    double tot = grid_sum(grid, psumB, acc, sh, &shd);
-    float gmax = 0.0f;
-    if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
-    float sigma = (float)tot;
-    float alpha = 0.0f, beta = 0.0f, max_error = 0.0f;
-    int num_iterations = 0;
-
-    // offsets of this thread's quad inside a box: row (ly + 1), columns 4 + 4 lx .. 7 + 4 lx
-    const int qoff = (ly + 1) * TMA_BX + 4 + 4 * lx;
-    const int coff = (ly + 1) * TMA_CX + 16 + 4 * lx;
-    constexpr int PLANE = TMA_BX * TMA_BY, CPLANE = TMA_CX * TMA_BY;
-
-    for (int it = 0;; ++it) {
+    // phase A: boxes of r, s, codes -> smem; s' once per box cell; s'.A s' from smem
+    __device__ __forceinline__ void search(int it, float beta, float &acc) {
+        const TileEnv e = make_tile_env(a);
+        const GridDim &g = e.g;
+        const TileMap &t = a.t;
         const CUtensorMap *map_in = (it & 1) ? &maps.s1 : &maps.s0;
-        const CUtensorMap *map_out = (it & 1) ? &maps.s0 : &maps.s1;
         float *s_out = (it & 1) ? a.s0 : a.s1;
-        // ---- phase A: boxes of r, s, codes -> smem; s' once per box cell; s'.A s' from smem
-        acc = 0.0f;
+        const int tid = linear_tid(), lx = threadIdx.x, ly = threadIdx.y;
+        // offsets of this thread's quad inside a box: row (ly + 1), columns 4 + 4 lx .. 7 + 4 lx
+        const int qoff = (ly + 1) * TMA_BX + 4 + 4 * lx;
+        const int coff = (ly + 1) * TMA_CX + 16 + 4 * lx;
+        constexpr int PLANE = TMA_BX * TMA_BY, CPLANE = TMA_CX * TMA_BY;
         for (int li = blockIdx.x; li < nact; li += gridDim.x) {
             const TileCtx c = tile_ctx_id(g, t, a.tile_list[li]);
             const int tile = c.tile, tx = tile % t.tiles_x, rest = tile / t.tiles_x, ty = rest % t.tiles_y, tz = rest / t.tiles_y;
@@ -1541,12 +1421,12 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
             if (tid == 0) {
                 fence_proxy_async_global();
                 fence_proxy_async(); // generic-proxy reads of the boxes above happen-before the async writes below
-                mbar_arrive_expect_tx(&bar, 2 * TMA_F32_BYTES + TMA_U8_BYTES);
-                tma_load_3d(shR, &maps.r, x0 - 4, y0 - 1, z0 - 1, &bar);
-                tma_load_3d(shS, map_in, x0 - 4, y0 - 1, z0 - 1, &bar);
-                tma_load_3d(shC, &maps.codes, x0 - 16, y0 - 1, z0 - 1, &bar);
+                mbar_arrive_expect_tx(bar, 2 * TMA_F32_BYTES + TMA_U8_BYTES);
+                tma_load_3d(shR, &maps.r, x0 - 4, y0 - 1, z0 - 1, bar);
+                tma_load_3d(shS, map_in, x0 - 4, y0 - 1, z0 - 1, bar);
+                tma_load_3d(shC, &maps.codes, x0 - 16, y0 - 1, z0 - 1, bar);
             }
-            mbar_wait(&bar, parity, &sh_dead);
+            mbar_wait(bar, parity, sh_dead);
             parity ^= 1u;
             // s' = z + beta s for the whole box, in place over s (60 rows x 34 quads)
             for (int qd = tid; qd < TMA_BY * TMA_BZ * (TMA_BX / 4); qd += PCG_THREADS) {
@@ -1562,7 +1442,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
             }
             __syncthreads();
             int i = c.i;
-            if (sharded && c.tz == tz_first) st4(s_out + i - g.sz, *reinterpret_cast<const float4 *>(shS + qoff));
+            if (e.sharded && c.tz == e.tz_first) st4(s_out + i - g.sz, *reinterpret_cast<const float4 *>(shS + qoff));
 #pragma unroll
             for (int k = 0; k < PCG_TZ; ++k, i += g.sz) {
                 const float *S = shS + (k + 1) * PLANE + qoff;
@@ -1573,18 +1453,21 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
                 const float4 As = stencil_quad(code, c0, S[-1], S[4], ym, yp, zm, zp);
                 acc += (c0.x * As.x + c0.y * As.y) + (c0.z * As.z + c0.w * As.w);
                 st4(s_out + i, c0);
-                if (sharded && k == PCG_TZ - 1 && c.tz == tz_last) st4(s_out + i + g.sz, zp);
+                if (e.sharded && k == PCG_TZ - 1 && c.tz == e.tz_last) st4(s_out + i + g.sz, zp);
             }
         }
         fence_proxy_async_global();
-        tot = grid_sum(grid, psumA, acc, sh, &shd);
-        if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
-        alpha = guarded_div(sigma, (float)tot);
-
-        // ---- phase B: box of s' -> smem (p, r, codes: plain loads issued before the wait); update; z.r, max|r|
-        const bool with_err = (a.max_iterations == it) || (it > 0 && it % a.check_frequency == 0);
-        acc = 0.0f;
-        float err = 0.0f;
+    }
+    // phase B: box of s' -> smem (p, r, codes: plain loads issued before the wait); update; z.r, max|r|
+    __device__ __forceinline__ void update(int it, float alpha, float &acc, float &err) {
+        const TileEnv e = make_tile_env(a);
+        const GridDim &g = e.g;
+        const TileMap &t = a.t;
+        const CUtensorMap *map_out = (it & 1) ? &maps.s0 : &maps.s1;
+        const uint8_t *__restrict__ codes = e.codes;
+        const int tid = linear_tid(), lx = threadIdx.x, ly = threadIdx.y;
+        const int qoff = (ly + 1) * TMA_BX + 4 + 4 * lx;
+        constexpr int PLANE = TMA_BX * TMA_BY;
         for (int li = blockIdx.x; li < nact; li += gridDim.x) {
             const TileCtx c = tile_ctx_id(g, t, a.tile_list[li]);
             const int tile = c.tile, tx = tile % t.tiles_x, rest = tile / t.tiles_x, ty = rest % t.tiles_y, tz = rest / t.tiles_y;
@@ -1592,8 +1475,8 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
             if (tid == 0) {
                 fence_proxy_async_global();
                 fence_proxy_async();
-                mbar_arrive_expect_tx(&bar, TMA_F32_BYTES);
-                tma_load_3d(shS, map_out, tx * 128 - 4, ty * 8 - 1, tz * PCG_TZ - 1, &bar);
+                mbar_arrive_expect_tx(bar, TMA_F32_BYTES);
+                tma_load_3d(shS, map_out, tx * 128 - 4, ty * 8 - 1, tz * PCG_TZ - 1, bar);
             }
             float4 p4[PCG_TZ], r4[PCG_TZ];
             uchar4 code[PCG_TZ];
@@ -1603,7 +1486,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
                 r4[k] = ld4(a.r + c.i + k * g.sz);
                 code[k] = ldcode(codes + c.i + k * g.sz);
             }
-            mbar_wait(&bar, parity, &sh_dead);
+            mbar_wait(bar, parity, sh_dead);
             parity ^= 1u;
             int i = c.i;
 #pragma unroll
@@ -1621,9 +1504,9 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
                 rq.w -= alpha * (code[k].w ? As.w : 0.0f);
                 st4(a.p + i, pq);
                 st4(a.r + i, rq);
-                if (sharded) {
-                    if (k == 0 && c.tz == tz_first && peer_r_lo) st4(peer_r_lo + i + push, rq);
-                    if (k == PCG_TZ - 1 && c.tz == tz_last && peer_r_hi) st4(peer_r_hi + i - push, rq);
+                if (e.sharded) {
+                    if (k == 0 && c.tz == e.tz_first && e.peer_r_lo) st4(e.peer_r_lo + i + e.push, rq);
+                    if (k == PCG_TZ - 1 && c.tz == e.tz_last && e.peer_r_hi) st4(e.peer_r_hi + i - e.push, rq);
                 }
                 acc += (precond_diag2(rq.x, code[k].x) * rq.x + precond_diag2(rq.y, code[k].y) * rq.y) +
                        (precond_diag2(rq.z, code[k].z) * rq.z + precond_diag2(rq.w, code[k].w) * rq.w);
@@ -1631,56 +1514,29 @@ __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __g
             }
         }
         fence_proxy_async_global();
-        {
-            const float bm = block_max(err, sh);
-            if (tid == 0) pmax[blockIdx.x] = bm;
-        }
-        tot = grid_sum(grid, psumB, acc, sh, &shd);
-        {
-            const float e = final_max(pmax, gridDim.x, sh);
-            if (tid == 0) shf = e;
-            __syncthreads();
-            gmax = shf;
-            __syncthreads();
-        }
-        if (sharded) comm_allreduce(cm_, ++seq, tot, gmax, sh_csum, sh_cmax, &sh_dead);
-        const float zr = (float)tot;
-        if (with_err) {
-            const float tol = a.params->tolerance[a.which];
-            if (a.max_iterations == it || gmax < tol) {
-                max_error = gmax;
-                num_iterations = it;
-                break;
-            }
-        }
-        beta = guarded_div(zr, sigma);
-        sigma = zr;
     }
-    if (sharded) {
-        float *const peer_p_lo = cm_.peer_p[a.which][0], *const peer_p_hi = cm_.peer_p[a.which][1];
-        for (int li = blockIdx.x; li < nact; li += gridDim.x) {
-            const TileCtx c = tile_ctx_id(g, t, a.tile_list[li]);
-            if (c.tz == tz_first && peer_p_lo) st4(peer_p_lo + c.i + push, ld4(a.p + c.i));
-            if (c.tz == tz_last && peer_p_hi) {
-                const int i = c.i + (PCG_TZ - 1) * g.sz;
-                st4(peer_p_hi + i - push, ld4(a.p + i));
-            }
-        }
-        grid.sync();
-        double dummy = 0.0;
-        float dmax = 0.0f;
-        comm_allreduce(cm_, ++seq, dummy, dmax, sh_csum, sh_cmax, &sh_dead);
-        if (blockIdx.x == 0 && tid == 0) *cm_.seq = seq;
+};
+
+__global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_tma_kernel(const __grid_constant__ PcgSolveArgs a, const __grid_constant__ PcgTmaMaps maps) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    __shared__ uint64_t bar;
+    __shared__ float sh[PCG_THREADS / 32];
+    __shared__ double shd;
+    __shared__ float shf;
+    __shared__ double sh_csum[SLAB_MAX_WORLD];
+    __shared__ float sh_cmax[SLAB_MAX_WORLD];
+    __shared__ int sh_dead;
+    if (linear_tid() == 0) {
+        mbar_init(&bar, 1);
+        fence_proxy_async(); // make the initialised barrier visible to the async (TMA) proxy (the solve's first block barrier follows)
     }
-    if (blockIdx.x == 0 && tid == 0) {
-        a.scal->alpha = alpha;
-        a.scal->beta = beta;
-        a.scal->sigma = sigma;
-        a.scal->max_error = max_error;
-        a.scal->num_iterations = num_iterations;
-        a.scal->done = sh_dead ? -1 : 1;
-    }
+    TmaWalk wk{a, maps, *a.num_active, reinterpret_cast<float *>(smem_raw), reinterpret_cast<float *>(smem_raw + TMA_F32_BYTES),
+               smem_raw + 2 * TMA_F32_BYTES, &bar, &sh_dead, 0u};
+    SyncReduce rd{{a.comm, 0u, sh_csum, sh_cmax, &sh_dead}, cooperative_groups::this_grid(), sh, &shd, &shf};
+    pcg_solve(a, wk, rd);
 }
+#undef PCG_FOR_EACH_COLUMN
+#undef PCG_FOR_EACH_TILE
 
 __global__ void pcg_reset_scalars_kernel(PcgScalars *scal, unsigned *barrier) {
     if (barrier) *barrier = 0u;
@@ -1943,25 +1799,27 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
         args.params = dparams; args.which = which; args.max_iterations = max_it; args.check_frequency = freq;
         args.comm = comm;
         args.col_list = col_list_; args.num_cols = num_cols; args.barrier = barrier_; args.code_slots = code_slots_;
+        void *args_only[] = {&args}, *args_and_maps[] = {&args, tma_maps_};
+        void **kargs = args_only;
+        const void *kernel;
+        int nblocks;
+        size_t smem;
         if (columns) { // dense tiles by the tile body, everything else column by column
             BLUB_LAUNCH(pcg_column_fill_kernel, grid, block, 0, stream, g, t, st, ta, col_offset, ghost_tiles, t.ntiles - ghost_tiles, col_list_);
-            int nblocks = column_blocks_;
-            void *kargs[] = {&args};
-            BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)pcg_solve_columns_kernel, dim3(nblocks), t.block(), kargs,
-                                                        (size_t)code_slots_ * PCG_CODE_SLOT_BYTES, stream));
-            g_kernel_launches.fetch_add(1, std::memory_order_relaxed);
-            return;
+            kernel = (const void *)pcg_solve_columns_kernel;
+            nblocks = column_blocks_;
+            smem = (size_t)code_slots_ * PCG_CODE_SLOT_BYTES;
+        } else if (use_tma && tma_blocks_ > 0) {
+            kernel = (const void *)pcg_solve_tma_kernel;
+            kargs = args_and_maps;
+            nblocks = tma_blocks_ < t.ntiles ? tma_blocks_ : t.ntiles;
+            smem = TMA_SMEM_BYTES;
+        } else {
+            kernel = use_dense ? (const void *)pcg_solve_persistent_kernel<false> : (const void *)pcg_solve_persistent_kernel<true>;
+            nblocks = persistent_blocks_ < t.ntiles ? persistent_blocks_ : t.ntiles;
+            smem = 0;
         }
-        if (use_tma && tma_blocks_ > 0) {
-            int nblocks = tma_blocks_ < t.ntiles ? tma_blocks_ : t.ntiles;
-            void *kargs[] = {&args, tma_maps_};
-            BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)pcg_solve_tma_kernel, dim3(nblocks), t.block(), kargs, TMA_SMEM_BYTES, stream));
-            g_kernel_launches.fetch_add(1, std::memory_order_relaxed);
-            return;
-        }
-        int nblocks = persistent_blocks_ < t.ntiles ? persistent_blocks_ : t.ntiles;
-        void *kargs[] = {&args};
-        BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel(use_dense ? (const void *)pcg_solve_persistent_kernel<false> : (const void *)pcg_solve_persistent_kernel<true>, dim3(nblocks), t.block(), kargs, 0, stream));
+        BLUB_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(nblocks), t.block(), kargs, smem, stream));
         g_kernel_launches.fetch_add(1, std::memory_order_relaxed);
         return;
     }

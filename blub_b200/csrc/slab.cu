@@ -23,27 +23,17 @@
 namespace blub {
 namespace {
 
-constexpr long long BARRIER_SPIN_LIMIT = 40LL * 1000 * 1000;
-
-// one mailbox round (same protocol and the same round counter as comm_allreduce in pcg.cu): stream-ordered barrier
+// one empty mailbox round (common.cuh): stream-ordered barrier; a peer that never answers sets the error flag, and the round still counts
 __global__ void slab_barrier_kernel(SlabComm c, int *error_flag) {
     __shared__ int dead;
     const int tid = threadIdx.x;
     if (tid == 0) dead = 0;
     __syncthreads();
     const unsigned seq = *c.seq + 1u;
-    const int slot = (int)(seq & 1u) * 2 * SLAB_MAX_WORLD;
     if (tid < c.world) {
-        __threadfence_system();
-        volatile unsigned long long *dst = c.mailbox[tid] + slot + 2 * c.rank;
-        dst[0] = (unsigned long long)seq << 32;
-        dst[1] = (unsigned long long)seq << 32;
-        volatile unsigned long long *src = c.mailbox[c.rank] + slot + 2 * tid;
-        long long spins = 0;
-        while ((unsigned)(src[0] >> 32) != seq || (unsigned)(src[1] >> 32) != seq) {
-            if (++spins > BARRIER_SPIN_LIMIT) { dead = 1; break; }
-        }
-        __threadfence_system();
+        mailbox_post(mailbox_entry(c.mailbox[tid], seq, c.rank), seq, 0u, 0u);
+        unsigned long long v0, v1;
+        mailbox_poll(mailbox_entry(c.mailbox[c.rank], seq, tid), seq, MAILBOX_SPIN_LIMIT, &dead, v0, v1);
     }
     __syncthreads();
     if (tid == 0) {

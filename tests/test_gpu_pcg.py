@@ -1,5 +1,7 @@
 """GPU parity of the pressure solve alone: every PCG path of the CUDA library (through the C ABI) against the CPU oracle on the same
 markers and right-hand sides.  Collected first among the GPU tests (tests/conftest.py): cheap, local, and everything else builds on it."""
+import hashlib
+
 import numpy as np
 import pytest
 
@@ -204,3 +206,74 @@ def test_column_solver_is_deterministic_and_handles_mixed_fill():
     assert res[0][2] == res[1][2] and np.array_equal(res[0][0], res[1][0]) and np.array_equal(res[0][1], res[1][1])
     grid_close(orc.grid(O.ARR_P_VEL), res[0][0], "pressure", rel=2e-3, abs_=1e-4)
     assert (res[0][0][m != O.FLUID] == 0).all()
+
+
+# ---- every path pinned bit for bit ---------------------------------------------------------------------------------------------------
+def mixed_fill_system():
+    """Dense block (tile body), thin sheet and spray (column list) on a grid with nx % 128 == 0, so that the TMA solver runs too."""
+    nx, ny, nz = 256, 32, 24
+    rng = np.random.default_rng(23)
+    m = np.full((nz, ny, nx), O.AIR, dtype=np.int8)
+    m[2:20, 2:26, 4:140] = O.FLUID
+    m[4:8, 10:12, 140:250] = O.FLUID
+    m[rng.random((nz, ny, nx)) < 0.01] = O.FLUID
+    m[rng.random((nz, ny, nx)) < 0.01] = O.SOLID
+    m[0], m[-1], m[:, 0], m[:, -1], m[:, :, 0], m[:, :, -1] = 0, 0, 0, 0, 0, 0
+    b = rng.uniform(-1, 1, (nz, ny, nx)).astype(np.float32)
+    return m, b
+
+
+def solve_digests(path, precond, tol, max_it, freq):
+    """SHA-256 of p and r after two solves of the same system (the second warm-starts from the first), with both solves' statistics."""
+    m, b = mixed_fill_system()
+    nz, ny, nx = m.shape
+    gpu = blub_b200.HybridFluid(nx, ny, nz, 8)
+    gpu.set_solver_path(path)
+    gpu.set_quirks(precond_mode=precond)
+    gpu.set_solver_config(0, tol, max_it, freq)
+    gpu.upload_grid(F.TAP_MARKER, m)
+    h, stats = hashlib.sha256(), []
+    for _ in range(2):
+        gpu.upload_grid(F.TAP_RESIDUAL, b)
+        gpu.solve_only(0, DT)
+        e, it = gpu.last_solve(0)
+        stats.append((np.float32(e).view(np.uint32).item(), it))
+    h.update(np.ascontiguousarray(gpu.download_grid(F.TAP_P_VEL)).tobytes())
+    h.update(np.ascontiguousarray(gpu.download_grid(F.TAP_RESIDUAL)).tobytes())
+    return h.hexdigest()[:32], stats
+
+
+# solver path, precond_mode
+DIGEST_PATHS = [(1, 0), (6, 0), (4, 0), (2, 0), (0, 0), (0, 1)]
+DIGEST_SCHEDULES = {"fixed": (0.0, 20, 4), "converging": (2e-3, 128, 4)}
+# Recorded with the build of commit bcf7894 on an H100 80GB HBM3 (132 SMs, 700 W power limit).  The persistent solvers launch as many
+# blocks as fit on the GPU, and that number sets the grouping of their partial sums, so the digests hold for this SM count only.
+DIGESTS_132_SMS = {
+    (1, 0, "converging"): ("6df751a3414bcc0a1ffdc4d4244dc5b7", [(1045782498, 16), (1044237610, 4)]),
+    (1, 0, "fixed"): ("908a50a6a9f52fe7ce427c27b748f858", [(1034478723, 20), (1017826933, 20)]),
+    (6, 0, "converging"): ("6eecdc111733ce03e99153441c2bdffe", [(1045782497, 16), (1044237429, 4)]),
+    (6, 0, "fixed"): ("91be633f35a0d156be3cde17e0188edc", [(1034478717, 20), (1017834031, 20)]),
+    (4, 0, "converging"): ("6eecdc111733ce03e99153441c2bdffe", [(1045782497, 16), (1044237429, 4)]),
+    (4, 0, "fixed"): ("91be633f35a0d156be3cde17e0188edc", [(1034478717, 20), (1017834031, 20)]),
+    (2, 0, "converging"): ("41d987bfe0f6ef3c05650cd07786bfe6", [(1045782494, 16), (1044237318, 4)]),
+    (2, 0, "fixed"): ("0c144d58310804512da86055135fe2b4", [(1034478716, 20), (1017835322, 20)]),
+    (0, 0, "converging"): ("9f7ff2941d366b2bb728d17328e82e70", [(1045782502, 16), (1044237736, 4)]),
+    (0, 0, "fixed"): ("bea6e61e5d31c7bf0d6329d4ef52fe56", [(1034478716, 20), (1017802166, 20)]),
+    (0, 1, "converging"): ("4f097f157a968d33b1b4f8a82943b8a1", [(1068887294, 128), (1068887308, 128)]),
+    (0, 1, "fixed"): ("2cfc3874634fdb1984b1a2de06b6cd3d", [(1068886330, 20), (1068887304, 20)]),
+}
+
+
+@pytest.mark.parametrize("schedule", sorted(DIGEST_SCHEDULES))
+@pytest.mark.parametrize("path,precond", DIGEST_PATHS)
+def test_solver_paths_are_pinned_bit_for_bit(path, precond, schedule):
+    """Every solver path's p, r and statistics against digests recorded from an earlier build: a change to the shared solve loop, the
+    reductions or a path's walk of its work that moves one bit on any path fails here."""
+    import torch
+
+    if torch.cuda.get_device_properties(0).multi_processor_count != 132:
+        pytest.skip("digests recorded with 132 SMs")
+    digest, stats = solve_digests(path, precond, *DIGEST_SCHEDULES[schedule])
+    if schedule == "converging" and precond == 0:  # stops early (the literal two-pass preconditioner of precond_mode 1 runs to the end)
+        assert 0 < stats[0][1] < 128 and stats[0][1] % 4 == 0, stats
+    assert (digest, stats) == DIGESTS_132_SMS[(path, precond, schedule)]

@@ -251,7 +251,26 @@ class HybridFluid {
     // the newest min(capacity, recorded, LOAD_HISTORY_LENGTH) records of `probe`, oldest first; returns their number (synchronises)
     uint32_t load_history(uint32_t probe, BlubSolidLoad *out, uint32_t capacity);
 
+    // Floating bodies (body_kernels.cu): replaces the whole set (0 clears it), resets the history and drops the step graphs.  Throws
+    // std::invalid_argument and changes nothing when make_body_set refuses the set, on a z-slab rank or a fluid inside a step.  While the set is
+    // not empty, stage 0 builds the composite solid volume and stage 2 moves the bodies and records one BlubBodyRecord each.
+    void set_bodies(const BlubBody *bodies, uint32_t num_bodies);
+    uint32_t num_bodies() const { return num_bodies_; }
+    // the current bodies, at most `capacity` of them (synchronises)
+    uint32_t bodies(BlubBody *out, uint32_t capacity);
+    // the newest min(capacity, recorded, BODY_HISTORY_LENGTH) records of `body`, oldest first; returns their number (synchronises)
+    uint32_t body_history(uint32_t body, BlubBodyRecord *out, uint32_t capacity);
+    // the solid volume the step reads: the composite one while there are bodies, else the borrowed one (may be nullptr)
+    const uint2 *solid_volume() const { return num_bodies_ ? composite_ : voxels_; }
+
   private:
+    BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
+    unsigned long long *body_sums_ = nullptr; // composite volume, allocated with the first non-empty set
+    BlubBodyRecord *body_ring_ = nullptr;
+    uint2 *composite_ = nullptr;
+    uint32_t num_bodies_ = 0, body_cube_ = 0;
+    std::deque<uint32_t> body_steps_; // step numbers of the records in the body ring, oldest first
+    void restore_bodies(const std::vector<BlubBody> &bodies); // a validated set (set_bodies, state file load)
     LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
     BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
     uint32_t num_load_probes_ = 0, load_max_cells_ = 0;
@@ -377,6 +396,12 @@ FlowBox clamp_box(const uint32_t dim[3], const float min_grid[3], const float ma
 // A load probe in grid units: corners converted as clamp_box converts them but clamped to [0, dim] (max exclusive); throws
 // std::invalid_argument on a non-finite corner or pivot or a box that is empty after clamping.
 LoadProbeBox clamp_load_probe(const uint32_t dim[3], const BlubLoadProbe &probe);
+// A body set checked against the rules of set_bodies on a grid of `dim` cells; throws std::invalid_argument when it breaks one.  set_bodies
+// (loaded == false) normalises the quaternions; a state file's bodies (loaded == true) are kept bit for bit and their bounding boxes may
+// leave [1, dim - 1] by the rounding of the integrator's clamp (1e-3 cells).
+std::vector<BlubBody> make_body_set(const uint32_t dim[3], const BlubBody *bodies, uint32_t num_bodies, bool loaded);
+// cgmath's Quaternion::from(Euler<Deg>) as (w, x, y, z) (solids.cu)
+void quat_from_euler_deg_wxyz(const float deg[3], float q[4]);
 // A flow set from the public boxes (grid units), clamped like add_fluid_cube; throws std::invalid_argument when it breaks a rule of set_flow
 // that does not depend on the fluid.  source_tags may be nullptr (all 0).
 FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
@@ -414,6 +439,11 @@ struct SceneLoadProbe {
     float min[3], max[3], pivot[3];
     bool has_pivot = false; // without one the pivot is the box centre
 };
+struct SceneBody {
+    int32_t shape = 0;            // "box" 0, "sphere" 1
+    float position[3], half_extent[3], rotation_angles_deg[3] = {0, 0, 0}, relative_density = 1.0f;
+    float velocity[3] = {0, 0, 0}, angular_velocity[3] = {0, 0, 0}; // m/s, rad/s
+};
 struct SceneConfig {
     float gravity[3] = {0, 0, 0};
     float world_position[3] = {0, 0, 0};
@@ -424,12 +454,16 @@ struct SceneConfig {
     std::vector<SceneSource> sources; // optional fluid.sources / fluid.drains (world units, m/s)
     std::vector<SceneBox> drains;
     std::vector<SceneLoadProbe> load_probes; // optional fluid.load_probes (world units)
+    std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };
 SceneConfig parse_scene_file(const std::string &path);
 // the scene's load probes in grid cells: corners and pivot / grid_to_world_scale, pivot (min + max) / 2 when the scene gives none
 std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
+// the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a
+// quaternion (quat_from_euler_deg_wxyz), the angular velocity unchanged
+std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg);
 // Scene::create_fluid_from_config, src/scene/mod.rs:109-144
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream);
 

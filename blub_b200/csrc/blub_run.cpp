@@ -20,6 +20,8 @@
 //                  step and probe, force in cells^4/s^2 and torque in cells^5/s^2 per unit density.  The device ring holds the newest 1024
 //                  steps; the runner reads it at every batch or frame boundary, so a long run loses nothing.  With --load-state the scene's
 //                  probes are set again (a state file holds none).
+//   --bodies FILE  the trajectory of every floating body (fluid.bodies, or the bodies of a --load-state file) as JSON: one record per step
+//                  and body with its load (as --loads) and its pose after the step, read from the device ring at every batch or frame boundary.
 //   --models DIR   where the scene's static_objects find their OBJ files (the reference reads `models/<model>`,
 //                  src/scene/models.rs:253).  Every step then runs Scene::step's order (src/scene/mod.rs:192-211): animate the
 //                  models at the already advanced simulation time, voxelize their hulls, step the fluid.
@@ -49,13 +51,14 @@ int main(int argc, char **argv) {
         std::fprintf(stderr, "usage: blub_run scene.json [--steps N] [--batch 16] [--hz 120] [--device 0] [--no-graph]\n"
                              "                [--stats out.json] [--trace out.json] [--dump particles.f32] [--models DIR] [--record FPS PREFIX]\n"
                              "                [--solver TOLERANCE MAX_ITERATIONS CHECK_FREQUENCY] [--rebin EVERY_N_STEPS]\n"
-                             "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE] [--loads out.json]\n");
+                             "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE] [--loads out.json]\n"
+                             "                [--bodies out.json]\n");
         return 2;
     }
     const char *scene = argv[1];
     int steps = 160, batch = 16, device = 0, graph = 1;
     long hz = 120;
-    std::string loads_path, stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
+    std::string bodies_path, loads_path, stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
     double record_fps = 0.0;
     float solver_tol = -1.0f;
     int solver_max = 0, solver_freq = 0, rebin = -1, checkpoint_every = 0;
@@ -71,6 +74,7 @@ int main(int argc, char **argv) {
         else if (!std::strcmp(argv[i], "--no-graph")) graph = 0;
         else if (!std::strcmp(argv[i], "--stats")) stats_path = next("--stats");
         else if (!std::strcmp(argv[i], "--loads")) loads_path = next("--loads");
+        else if (!std::strcmp(argv[i], "--bodies")) bodies_path = next("--bodies");
         else if (!std::strcmp(argv[i], "--trace")) trace_path = next("--trace");
         else if (!std::strcmp(argv[i], "--dump")) dump_path = next("--dump");
         else if (!std::strcmp(argv[i], "--models")) models_dir = next("--models");
@@ -90,6 +94,10 @@ int main(int argc, char **argv) {
     if (!record_prefix.empty() && !load_path.empty()) { std::fprintf(stderr, "blub_run: --load-state cannot resume a --record run\n"); return 2; }
     if (!loads_path.empty() && batch > BLUB_LOAD_HISTORY_LENGTH) {
         std::fprintf(stderr, "blub_run: --loads reads the load history at batch boundaries: --batch must not exceed %d\n", BLUB_LOAD_HISTORY_LENGTH);
+        return 2;
+    }
+    if (!bodies_path.empty() && batch > BLUB_BODY_HISTORY_LENGTH) {
+        std::fprintf(stderr, "blub_run: --bodies reads the body history at batch boundaries: --batch must not exceed %d\n", BLUB_BODY_HISTORY_LENGTH);
         return 2;
     }
     if (checkpoint_every < 0 || (checkpoint_every > 0 && save_path.empty())) {
@@ -187,6 +195,22 @@ int main(int argc, char **argv) {
         }
     };
 
+    // every record of every body, collected the same way (a state file's bodies are the fluid's own: nothing to set again)
+    BlubBody bodies[BLUB_BODIES_MAX];
+    uint32_t num_bodies = 0;
+    if (blub_fluid_bodies(fluid, bodies, BLUB_BODIES_MAX, &num_bodies)) die("cannot read the bodies");
+    std::vector<std::vector<BlubBodyRecord>> trajectories(num_bodies);
+    std::vector<BlubBodyRecord> body_ring(BLUB_BODY_HISTORY_LENGTH);
+    auto collect_bodies = [&]() {
+        if (bodies_path.empty()) return;
+        for (uint32_t b = 0; b < num_bodies; ++b) {
+            uint32_t n = 0;
+            if (blub_fluid_body_history(fluid, b, body_ring.data(), BLUB_BODY_HISTORY_LENGTH, &n)) die("cannot read the body history");
+            for (uint32_t k = 0; k < n; ++k)
+                if (trajectories[b].empty() || body_ring[k].step > trajectories[b].back().step) trajectories[b].push_back(body_ring[k]);
+        }
+    };
+
     const bool has_flow = blub_fluid_has_flow(fluid) == 1;
     int done = 0, saved_at = -1;
     auto save_state = [&]() {
@@ -213,6 +237,7 @@ int main(int argc, char **argv) {
             std::snprintf(name, sizeof(name), "%05d.f32", frame);
             write_particles(record_prefix + name);
             collect_loads();
+            collect_bodies();
             std::printf("frame %d: %u step(s), simulated %.6f s\n", frame, n, (double)blub_duration_as_secs_f32(simulated_ns));
             checkpoint();
         }
@@ -224,6 +249,7 @@ int main(int argc, char **argv) {
         blub_fluid_update_statistics(fluid);
         done += n;
         collect_loads();
+        collect_bodies();
         if (has_flow) // sources and drains change the particle count as the run goes
             std::printf("simulation fast forwarding batch finished (progress %d/%d, %u particles)\n", done, steps, blub_fluid_num_particles(fluid));
         else
@@ -272,6 +298,32 @@ int main(int argc, char **argv) {
                 std::fprintf(f, "%s\n  {\"step\": %u, \"wetted_faces\": %u, \"force\": [%.17g, %.17g, %.17g], \"torque\": [%.17g, %.17g, %.17g]}", k ? "," : "",
                              r.step, r.wetted_faces, r.force_fx[0] / fs, r.force_fx[1] / fs, r.force_fx[2] / fs, r.torque_fx[0] / ts, r.torque_fx[1] / ts,
                              r.torque_fx[2] / ts);
+            }
+            std::fprintf(f, "]}");
+        }
+        std::fprintf(f, "\n]}\n");
+        std::fclose(f);
+    }
+    if (!bodies_path.empty()) {
+        FILE *f = std::fopen(bodies_path.c_str(), "w");
+        if (!f) { std::perror("blub_run: --bodies"); return 1; }
+        const double fs = (double)(1 << BLUB_LOAD_FORCE_FRAC_BITS), ts = (double)(1 << BLUB_LOAD_TORQUE_FRAC_BITS);
+        std::fprintf(f, "{\"grid_to_world_scale\": %.9g, \"dt\": %.9g, \"units\": \"cells, cells/s, rad/s; force cells^4/s^2 and torque cells^5/s^2 per unit density\", "
+                        "\"bodies\": [",
+                     info.grid_to_world_scale, dt);
+        for (uint32_t b = 0; b < num_bodies; ++b) {
+            const BlubBody &o = bodies[b];
+            std::fprintf(f, "%s\n {\"shape\": \"%s\", \"half_extent\": [%.9g, %.9g, %.9g], \"relative_density\": %.9g, \"records\": [", b ? "," : "",
+                         o.shape == 1 ? "sphere" : "box", o.half_extent[0], o.half_extent[1], o.half_extent[2], o.relative_density);
+            for (size_t k = 0; k < trajectories[b].size(); ++k) {
+                const BlubBodyRecord &r = trajectories[b][k];
+                std::fprintf(f,
+                             "%s\n  {\"step\": %u, \"wetted_faces\": %u, \"force\": [%.17g, %.17g, %.17g], \"torque\": [%.17g, %.17g, %.17g], "
+                             "\"centre\": [%.9g, %.9g, %.9g], \"rotation\": [%.9g, %.9g, %.9g, %.9g], \"velocity\": [%.9g, %.9g, %.9g], "
+                             "\"angular_velocity\": [%.9g, %.9g, %.9g]}",
+                             k ? "," : "", r.step, r.wetted_faces, r.force_fx[0] / fs, r.force_fx[1] / fs, r.force_fx[2] / fs, r.torque_fx[0] / ts,
+                             r.torque_fx[1] / ts, r.torque_fx[2] / ts, r.centre[0], r.centre[1], r.centre[2], r.rotation[0], r.rotation[1], r.rotation[2],
+                             r.rotation[3], r.velocity[0], r.velocity[1], r.velocity[2], r.angular_velocity[0], r.angular_velocity[1], r.angular_velocity[2]);
             }
             std::fprintf(f, "]}");
         }

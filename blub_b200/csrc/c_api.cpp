@@ -66,6 +66,7 @@ Tap tap_of(BlubFluid *f, int tap) {
     case BLUB_TAP_PRESSURE_VELOCITY: return {h.field(0).pressure(), n * 4};
     case BLUB_TAP_PRESSURE_DENSITY: return {h.field(1).pressure(), n * 4};
     case BLUB_TAP_RESIDUAL: return {h.solver().residual(), n * 4};
+    case BLUB_TAP_SOLID_VOXELS: return {const_cast<uint2 *>(h.solid_volume()), n * 8};
     default: return {nullptr, 0};
     }
 }
@@ -439,6 +440,23 @@ int blub_load_probe_cells(const uint32_t dim[3], const BlubLoadProbe *probe, uin
     });
 }
 
+int blub_fluid_set_bodies(BlubFluid *fluid, const BlubBody *bodies, uint32_t num_bodies) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_bodies(bodies, num_bodies); return BLUB_OK; });
+}
+
+int blub_fluid_body_history(BlubFluid *fluid, uint32_t body, BlubBodyRecord *out, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *count = 0;
+    return guarded([&] { *count = fluid->impl->body_history(body, out, capacity); return BLUB_OK; });
+}
+
+int blub_fluid_bodies(BlubFluid *fluid, BlubBody *out, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *count = 0;
+    return guarded([&] { *count = fluid->impl->bodies(out, capacity); return BLUB_OK; });
+}
+
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
 
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {
@@ -473,6 +491,16 @@ int blub_scene_load_probes(const char *path, BlubLoadProbe *out, uint32_t capaci
     });
 }
 
+int blub_scene_bodies(const char *path, BlubBody *out, uint32_t capacity, uint32_t *count) {
+    if (!path || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const std::vector<BlubBody> bodies = blub::scene_bodies_grid(blub::parse_scene_file(path));
+        for (size_t k = 0; k < bodies.size() && k < capacity; ++k) out[k] = bodies[k];
+        *count = (uint32_t)bodies.size();
+        return BLUB_OK;
+    });
+}
+
 int blub_scene_load(BlubFluid **out, const char *path, int device, void *cuda_stream) {
     if (!out || !path) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     *out = nullptr;
@@ -500,6 +528,7 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
 
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes) {
     if (!fluid || !host_src) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    if (tap == BLUB_TAP_SOLID_VOXELS) return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume tap is download only");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");

@@ -89,6 +89,7 @@ struct StepParams {
     float gravity_dt[3]; // GravityGridSpace * Time.SimulationDelta (transfer_gather_velocity.comp:121)
     float tolerance[2];  // error_tolerance / dt per field (pressure_solver.rs:193-201)
     float inv_dt;
+    float gravity[3];       // GravityGridSpace itself (the floating bodies' integrator)
     uint32_t step_count;    // whole steps taken before this one (seeds the source emission)
     uint32_t num_particles; // last: left alone by the upload when the count lives on the device
 };

@@ -148,4 +148,19 @@ struct LoadProbeBox {
 void launch_solid_loads(cudaStream_t st, const GridDim &g, const StepParams *params, int num_probes, uint32_t max_cells, const LoadProbeBox *probes,
                         const int8_t *marker, const float *p_vel, BlubSolidLoad *ring);
 
+// ---- floating bodies (body_kernels.cu, DESIGN.md §8 "Floating bodies") ----
+constexpr int BODIES_MAX = BLUB_BODIES_MAX;
+constexpr uint32_t BODY_HISTORY_LENGTH = BLUB_BODY_HISTORY_LENGTH;
+// The cells a launch walks around each body: a cube of `cube` cells per side from floor(c - e), sized at set time from the largest bounding
+// sphere, so that a captured graph stays valid while the bodies move and turn.
+uint32_t body_cube_side(const BlubBody &b);
+// Stage 0: the composite solid volume (n cells of RGBA16F) = the borrowed volume (or zero when vox == nullptr), then every body written over it.
+void launch_body_composite(cudaStream_t st, const GridDim &g, const uint2 *vox, uint2 *composite, int num_bodies, uint32_t cube, const BlubBody *bodies);
+// End of stage 2: every body's wetted-face sums into sums[8 * body] (zero on entry), then the integrator: it reads and re-zeroes the sums,
+// moves every body and writes its record into ring[body * BODY_HISTORY_LENGTH + params->step_count % BODY_HISTORY_LENGTH].
+void launch_body_step(cudaStream_t st, const GridDim &g, const StepParams *params, int num_bodies, uint32_t cube, BlubBody *bodies, const int8_t *marker,
+                      const float *p_vel, unsigned long long *sums, BlubBodyRecord *ring);
+// Host twins of the device rules the setter checks a body against: the half extents of its grid-axis bounding box at its pose.
+void body_bounding_extents(const BlubBody &b, float e[3]);
+
 } // namespace blub

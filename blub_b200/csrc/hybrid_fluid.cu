@@ -27,6 +27,13 @@ struct NvtxScope {
     explicit NvtxScope(const char *name) { nvtxRangePushA(name); }
     ~NvtxScope() { nvtxRangePop(); }
 };
+// The step numbers of the records in a device ring of `length` slots (slot = step % length), oldest first: the probes' and the bodies' rings.
+void note_record(std::deque<uint32_t> &steps, uint32_t step, uint32_t length) {
+    if (!steps.empty() && steps.back() == step) return; // the same step again (a repeated step_stages): the same slot
+    steps.push_back(step);
+    // a slot holds the newest of the steps that map to it
+    while (steps.size() > length || (uint64_t)steps.front() + length <= step) steps.pop_front();
+}
 } // namespace
 
 HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num_particles, int device, cudaStream_t stream, int slab_rank,
@@ -206,6 +213,10 @@ HybridFluid::~HybridFluid() {
     cudaFree(census_dev_);
     cudaFree(load_probes_dev_);
     cudaFree(load_ring_);
+    cudaFree(bodies_dev_);
+    cudaFree(body_sums_);
+    cudaFree(body_ring_);
+    cudaFree(composite_);
     cudaFree(mig_counters_);
     if (slab_error_host_) cudaFreeHost(slab_error_host_);
     cudaFree(params_dev_);
@@ -396,7 +407,10 @@ void HybridFluid::upload_step_params(float dt) {
     BLUB_CUDA_CHECK(cudaEventSynchronize(param_events_[slot]));
     h->dt = dt;
     h->inv_dt = 1.0f / dt;
-    for (int c = 0; c < 3; ++c) h->gravity_dt[c] = gravity_[c] * dt;
+    for (int c = 0; c < 3; ++c) {
+        h->gravity_dt[c] = gravity_[c] * dt;
+        h->gravity[c] = gravity_[c];
+    }
     h->tolerance[0] = field_velocity_->config.error_tolerance / dt; // pressure_solver.rs:193-201
     h->tolerance[1] = field_density_->config.error_tolerance / dt;
     h->step_count = step_counter_;
@@ -446,8 +460,13 @@ void HybridFluid::run_stage(int stage, float dt) {
     // sharded or with sources / drains: the device-side count guards the kernels, launches are sized by the capacity
     const uint32_t np = device_count_mode() ? max_num_particles_ : num_particles_;
     const NvtxScope scope(stage >= 0 && stage < 14 ? kScopeLabels[stage] : "stage");
+    const uint2 *vox = solid_volume();
     switch (stage) {
     case 0: // transfer particle velocity to grid (:806-833)
+        if (num_bodies_ > 0) { // before the flow prologue: sources do not emit into bodies
+            const NvtxScope body_scope("floating bodies: composite solid volume");
+            launch_body_composite(stream_, grid_, voxels_, composite_, (int)num_bodies_, body_cube_, bodies_dev_);
+        }
         if (flow_active_) {
             const NvtxScope flow_scope("fluid sources & drains");
             run_flow_prologue();
@@ -455,25 +474,25 @@ void HybridFluid::run_stage(int stage, float dt) {
         if (!shard && !use_scatter_) {
             // cell lists -> marker (+ FLUID bits) -> one gather per component; deterministic, no accumulator volumes
             launch_cell_lists(stream_, grid_, params_dev_, np, pos_[cur_], 1.0f, lists_);
-            launch_marker_from_lists(stream_, grid_, lists_, marker_.ptr, voxels_, bits);
+            launch_marker_from_lists(stream_, grid_, lists_, marker_.ptr, vox, bits);
             fluid_bits_stale_ = false;
             if (np > 0) launch_p2g_gather(stream_, grid_, params_dev_, lists_, pos_[cur_], row_, marker_.ptr, u);
             else for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(u[c], 0, (size_t)grid_.n * sizeof(float), stream_));
         } else if (!shard) {
             launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, false, sched_);
-            launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, voxels_, bits, particle_words_);
+            launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, vox, bits, particle_words_);
             fluid_bits_stale_ = false;
         } else {
             launch_p2g_scatter(stream_, grid_, params_dev_, np, pos_[cur_], row_, nw, marker_.ptr, true, sched_);
             const SlabHaloItem items[4] = {{nw[0], sizeof(longlong2), 0}, {nw[1], sizeof(longlong2), 0}, {nw[2], sizeof(longlong2), 0}, {marker_.ptr, 1, 1}};
             slab_halo_exchange(items, 4); // X1
-            launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, voxels_, bits, particle_words_);
+            launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, vox, bits, particle_words_);
             fluid_bits_stale_ = false;
         }
         break;
     case 1: // compute divergence -> PCG residual (:835-840)
         refresh_fluid_bits();
-        launch_divergence_compute(stream_, grid_, bits, marker_.ptr, u, voxels_, solver_->residual());
+        launch_divergence_compute(stream_, grid_, bits, marker_.ptr, u, vox, solver_->residual());
         break;
     case 2: // primary pressure solver (:843-852)
         solver_->solve(stream_, *field_velocity_, 0, marker_.ptr, params_dev_, quirks);
@@ -482,6 +501,11 @@ void HybridFluid::run_stage(int stage, float dt) {
             launch_solid_loads(stream_, grid_, params_dev_, (int)num_load_probes_, load_max_cells_, load_probes_dev_, marker_.ptr, field_velocity_->pressure(),
                                load_ring_);
             if (!capturing_) note_load_record(step_counter_);
+        }
+        if (num_bodies_ > 0) { // after the probes: the integrator moves the bodies the probes saw
+            launch_body_step(stream_, grid_, params_dev_, (int)num_bodies_, body_cube_, bodies_dev_, marker_.ptr, field_velocity_->pressure(), body_sums_,
+                             body_ring_);
+            if (!capturing_) note_record(body_steps_, step_counter_, BODY_HISTORY_LENGTH);
         }
         break;
     case 3: // particle binning every n-th step, including step 0 (:854-894)
@@ -495,7 +519,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 4: // make velocity grid divergence free (:901-904)
         refresh_fluid_bits();
-        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), voxels_, u);
+        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, u);
         break;
     case 5: // extrapolate velocity grid (:906-909)
         refresh_fluid_bits();
@@ -510,16 +534,16 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 7: // advect particles (:917-921)
         if (!shard) {
-            launch_advect(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, voxels_, marker_.ptr);
+            launch_advect(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, vox, marker_.ptr);
         } else {
-            launch_advect_migrate(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, voxels_, marker_.ptr, slab_migrate_targets());
+            launch_advect_migrate(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, vox, marker_.ptr, slab_migrate_targets());
             slab_migrate_finish();
             const SlabHaloItem items[1] = {{marker_.ptr, 1, 1}};
             slab_halo_exchange(items, 1); // X3
         }
         break;
     case 8: // density projection: set boundary marker (:923-927)
-        launch_boundary_marker(stream_, grid_, marker_.ptr, voxels_, bits);
+        launch_boundary_marker(stream_, grid_, marker_.ptr, vox, bits);
         fluid_bits_stale_ = false;
         break;
     case 9: // density projection: compute density error (:928-932)
@@ -639,6 +663,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
     slab_exchange_index_ = before.exchange_index + after.exchanges;
     step_counter_ = before.step_counter + 1;
     if (num_load_probes_ > 0) note_load_record(before.step_counter);
+    if (num_bodies_ > 0) note_record(body_steps_, before.step_counter, BODY_HISTORY_LENGTH);
     field_velocity_->enqueue_error_buffer_read(stream_, dt);
     field_density_->enqueue_error_buffer_read(stream_, dt);
 }
@@ -785,7 +810,7 @@ void HybridFluid::flow_counters(uint64_t out[3]) {
 }
 
 void HybridFluid::run_flow_prologue() {
-    launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, voxels_, sched_.valid);
+    launch_flow_prologue(stream_, grid_, params_dev_, max_num_particles_, flow_, flow_scratch_, pos_[cur_], pos_[1 - cur_], row_, row_alt_, solid_volume(), sched_.valid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -874,12 +899,7 @@ void HybridFluid::set_load_probes(const BlubLoadProbe *probes, uint32_t num_prob
     destroy_graphs();
 }
 
-void HybridFluid::note_load_record(uint32_t step) {
-    if (!load_steps_.empty() && load_steps_.back() == step) return; // the same step again (a repeated step_stages): the same slot
-    load_steps_.push_back(step);
-    // a slot holds the newest of the steps that map to it
-    while (load_steps_.size() > LOAD_HISTORY_LENGTH || (uint64_t)load_steps_.front() + LOAD_HISTORY_LENGTH <= step) load_steps_.pop_front();
-}
+void HybridFluid::note_load_record(uint32_t step) { note_record(load_steps_, step, LOAD_HISTORY_LENGTH); }
 
 uint32_t HybridFluid::load_history(uint32_t probe, BlubSolidLoad *out, uint32_t capacity) {
     if (probe >= num_load_probes_) throw std::invalid_argument("load_history: no such load probe");
@@ -893,6 +913,93 @@ uint32_t HybridFluid::load_history(uint32_t probe, BlubSolidLoad *out, uint32_t 
     const uint32_t n = std::min<uint32_t>(capacity, (uint32_t)load_steps_.size());
     const size_t first = load_steps_.size() - n;
     for (uint32_t k = 0; k < n; ++k) out[k] = ring[load_steps_[first + k] % LOAD_HISTORY_LENGTH];
+    return n;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Floating bodies (body_kernels.cu).  Not in the reference.  The poses live on the device and move inside the step; the host keeps only the
+// step numbers it recorded, as it does for the probes.
+std::vector<BlubBody> make_body_set(const uint32_t dim[3], const BlubBody *bodies, uint32_t num_bodies, bool loaded) {
+    if (num_bodies > (uint32_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
+    if (num_bodies && !bodies) throw std::invalid_argument("set_bodies: NULL body array");
+    std::vector<BlubBody> out(bodies, bodies + num_bodies);
+    for (BlubBody &b : out) {
+        bool finite = std::isfinite(b.relative_density);
+        for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(b.rotation[k]);
+        for (int k = 0; k < 3; ++k)
+            finite = finite && std::isfinite(b.half_extent[k]) && std::isfinite(b.centre[k]) && std::isfinite(b.velocity[k]) && std::isfinite(b.angular_velocity[k]);
+        if (!finite) throw std::invalid_argument("set_bodies: a body value is not finite");
+        if (b.shape != 0 && b.shape != 1) throw std::invalid_argument("set_bodies: shape must be 0 (box) or 1 (sphere)");
+        for (int k = 0; k < (b.shape == 1 ? 1 : 3); ++k)
+            if (!(b.half_extent[k] >= 1.0f)) throw std::invalid_argument("set_bodies: a half extent or radius is below 1 cell");
+        if (!(b.relative_density > 0.0f)) throw std::invalid_argument("set_bodies: relative_density must be > 0");
+        const float *q = b.rotation;
+        const double norm = std::sqrt((double)q[0] * q[0] + (double)q[1] * q[1] + (double)q[2] * q[2] + (double)q[3] * q[3]);
+        if (!(std::fabs(norm - 1.0) <= 1e-3)) throw std::invalid_argument("set_bodies: the rotation quaternion is not of unit norm (within 1e-3)");
+        if (!loaded)
+            for (int k = 0; k < 4; ++k) b.rotation[k] = (float)(q[k] / norm);
+        float e[3];
+        body_bounding_extents(b, e);
+        const float slack = loaded ? 1e-3f : 0.0f;
+        for (int k = 0; k < 3; ++k)
+            if (b.centre[k] - e[k] < 1.0f - slack || b.centre[k] + e[k] > (float)dim[k] - 1.0f + slack)
+                throw std::invalid_argument("set_bodies: a body's bounding box leaves [1, dim - 1]");
+    }
+    return out;
+}
+
+void HybridFluid::set_bodies(const BlubBody *bodies, uint32_t num_bodies) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_bodies: z-slab ranks have no floating bodies");
+    if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    restore_bodies(make_body_set(dim, bodies, num_bodies, false));
+}
+
+void HybridFluid::restore_bodies(const std::vector<BlubBody> &set) {
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // no step in flight reads the old bodies or writes the ring
+    uint32_t cube = 0;
+    for (const BlubBody &b : set) cube = std::max(cube, body_cube_side(b));
+    if (!set.empty()) {
+        const size_t ring_bytes = (size_t)BODIES_MAX * BODY_HISTORY_LENGTH * sizeof(BlubBodyRecord);
+        if (!bodies_dev_) {
+            BLUB_CUDA_CHECK(cudaMalloc(&bodies_dev_, BODIES_MAX * sizeof(BlubBody)));
+            BLUB_CUDA_CHECK(cudaMalloc(&body_sums_, BODIES_MAX * 8 * sizeof(unsigned long long)));
+            BLUB_CUDA_CHECK(cudaMalloc(&body_ring_, ring_bytes));
+            BLUB_CUDA_CHECK(cudaMalloc(&composite_, (size_t)grid_.n * sizeof(uint2)));
+            BLUB_CUDA_CHECK(cudaMemset(composite_, 0, (size_t)grid_.n * sizeof(uint2)));
+        }
+        BLUB_CUDA_CHECK(cudaMemcpy(bodies_dev_, set.data(), set.size() * sizeof(BlubBody), cudaMemcpyHostToDevice));
+        BLUB_CUDA_CHECK(cudaMemset(body_sums_, 0, BODIES_MAX * 8 * sizeof(unsigned long long)));
+        BLUB_CUDA_CHECK(cudaMemset(body_ring_, 0, ring_bytes));
+    }
+    num_bodies_ = (uint32_t)set.size();
+    body_cube_ = cube;
+    body_steps_.clear();
+    destroy_graphs();
+}
+
+uint32_t HybridFluid::bodies(BlubBody *out, uint32_t capacity) {
+    if (capacity && !out) throw std::invalid_argument("bodies: NULL output");
+    const uint32_t n = std::min(capacity, num_bodies_);
+    if (n == 0) return num_bodies_;
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(out, bodies_dev_, n * sizeof(BlubBody), cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    return num_bodies_;
+}
+
+uint32_t HybridFluid::body_history(uint32_t body, BlubBodyRecord *out, uint32_t capacity) {
+    if (body >= num_bodies_) throw std::invalid_argument("body_history: no such body");
+    if (capacity && !out) throw std::invalid_argument("body_history: NULL output");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    std::vector<BlubBodyRecord> ring(BODY_HISTORY_LENGTH);
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(ring.data(), body_ring_ + (size_t)body * BODY_HISTORY_LENGTH, BODY_HISTORY_LENGTH * sizeof(BlubBodyRecord),
+                                    cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    const uint32_t n = std::min<uint32_t>(capacity, (uint32_t)body_steps_.size());
+    const size_t first = body_steps_.size() - n;
+    for (uint32_t k = 0; k < n; ++k) out[k] = ring[body_steps_[first + k] % BODY_HISTORY_LENGTH];
     return n;
 }
 
@@ -929,7 +1036,30 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);
         f->set_load_probes(probes.data(), (uint32_t)probes.size());
     }
+    if (!cfg.bodies.empty()) {
+        const std::vector<BlubBody> bodies = scene_bodies_grid(cfg);
+        f->set_bodies(bodies.data(), (uint32_t)bodies.size());
+    }
     return f;
+}
+
+std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg) {
+    const float scale = cfg.grid_to_world_scale;
+    std::vector<BlubBody> out(cfg.bodies.size());
+    for (size_t i = 0; i < out.size(); ++i) {
+        const SceneBody &s = cfg.bodies[i];
+        BlubBody &b = out[i];
+        b.shape = s.shape;
+        b.relative_density = s.relative_density;
+        for (int k = 0; k < 3; ++k) { // as the static objects are placed (models.rs:196-216)
+            b.centre[k] = (s.position[k] - cfg.world_position[k]) / scale;
+            b.half_extent[k] = s.half_extent[k] / scale;
+            b.velocity[k] = s.velocity[k] / scale;
+            b.angular_velocity[k] = s.angular_velocity[k];
+        }
+        quat_from_euler_deg_wxyz(s.rotation_angles_deg, b.rotation);
+    }
+    return out;
 }
 
 std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg) {

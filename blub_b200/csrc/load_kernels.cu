@@ -8,20 +8,15 @@
 #include <algorithm>
 
 #include "fluid_kernels.hpp"
+#include "solid_faces.cuh"
 
 namespace blub {
 
 namespace {
 
 constexpr int PT = 256;
-constexpr int LOAD_FIELDS = 7; // force x, y, z, torque x, y, z, wetted faces
 
 inline int blocks_for(int64_t n, int per_block) { return (int)((n + per_block - 1) / per_block); }
-
-__device__ __forceinline__ long long force_fixed(float q) { return __float2ll_rn(__fmul_rn(q, (float)(1 << BLUB_LOAD_FORCE_FRAC_BITS))); }
-__device__ __forceinline__ long long torque_fixed(float r, float q) {
-    return __float2ll_rn(__fmul_rn(__fmul_rn(r, q), (float)(1 << BLUB_LOAD_TORQUE_FRAC_BITS)));
-}
 
 // The step's slot of every probe: step number set, sums zero.  Runs in front of solid_load_kernel.
 __global__ void load_slot_clear_kernel(const StepParams *__restrict__ params, int num_probes, BlubSolidLoad *__restrict__ ring) {
@@ -34,8 +29,8 @@ __global__ void load_slot_clear_kernel(const StepParams *__restrict__ params, in
     for (int k = 0; k < 3; ++k) r.force_fx[k] = r.torque_fx[k] = 0;
 }
 
-// blockIdx.y = probe; the blocks of x stride over the probe box's cells, x fastest.  Each thread adds up its faces in registers, the warp
-// reduces with shuffles, and the block adds its warps up in shared memory and issues one global atomic per non-zero field.
+// blockIdx.y = probe; the blocks of x stride over the probe box's cells, x fastest.  Each thread adds up its faces in registers
+// (add_wetted_faces), the block reduces them (block_load_sum) and issues one global atomic per non-zero field.
 __global__ void __launch_bounds__(PT) solid_load_kernel(GridDim g, const StepParams *__restrict__ params, const LoadProbeBox *__restrict__ probes,
                                                         const int8_t *__restrict__ marker, const float *__restrict__ p_vel, BlubSolidLoad *__restrict__ ring) {
     __shared__ unsigned long long part[PT / 32][LOAD_FIELDS];
@@ -47,8 +42,6 @@ __global__ void __launch_bounds__(PT) solid_load_kernel(GridDim g, const StepPar
     const uint32_t quads = ex * ey * (uint32_t)(b.hi[2] - b.lo[2]);
     if (blockIdx.x * PT >= quads) return; // the whole block: the grid is sized for the largest box
     const float inv_dt = params->inv_dt;
-    const int dim[3] = {g.nx, g.ny, g.nz};
-    const int64_t stride[3] = {1, g.sy, g.sz};
     long long acc[6] = {0, 0, 0, 0, 0, 0};
     unsigned long long faces = 0;
     for (uint32_t i = blockIdx.x * PT + threadIdx.x; i < quads; i += gridDim.x * PT) {
@@ -62,53 +55,10 @@ __global__ void __launch_bounds__(PT) solid_load_kernel(GridDim g, const StepPar
         for (int j = 0; j < 4; ++j) {
             if (!((solid >> (8 * j)) & 1u) || x0 + j < b.lo[0] || x0 + j >= b.hi[0]) continue;
             const int c[3] = {x0 + j, y, z};
-            const int64_t s = s0 + j;
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-#pragma unroll
-                for (int d = -1; d <= 1; d += 2) {
-                    const int n = c[a] + d;
-                    if (n < 0 || n >= dim[a]) continue;
-                    const int64_t f = s + d * stride[a];
-                    if (marker[f] != CELL_FLUID) continue;
-                    // the solver's volume holds -p dt / density (divergence_remove: u_face -= p_cell - p_next): q = p / density
-                    const float q = -__fmul_rn(p_vel[f], inv_dt);
-                    // face centre: the mean of the two cell centres; r = centre - pivot
-                    float r[3];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const float centre = k == a ? (float)(d > 0 ? n : c[a]) : (float)c[k] + 0.5f;
-                        r[k] = __fsub_rn(centre, b.pivot[k]);
-                    }
-                    // force -d * q along a; torque components b1 = a + 1, b2 = a + 2 (mod 3): tau_b1 = r_b2 * F_a, tau_b2 = -r_b1 * F_a
-                    const int b1 = a == 2 ? 0 : a + 1, b2 = a == 0 ? 2 : a - 1;
-                    const long long fq = force_fixed(q), t1 = torque_fixed(r[b2], q), t2 = torque_fixed(r[b1], q);
-                    if (d > 0) {
-                        acc[a] -= fq;
-                        acc[3 + b1] -= t1;
-                        acc[3 + b2] += t2;
-                    } else {
-                        acc[a] += fq;
-                        acc[3 + b1] += t1;
-                        acc[3 + b2] -= t2;
-                    }
-                    faces += 1ull;
-                }
-            }
+            faces += add_wetted_faces(g, marker, p_vel, inv_dt, c, s0 + j, b.pivot, acc);
         }
     }
-    unsigned long long v[LOAD_FIELDS] = {(unsigned long long)acc[0], (unsigned long long)acc[1], (unsigned long long)acc[2], (unsigned long long)acc[3],
-                                         (unsigned long long)acc[4], (unsigned long long)acc[5], faces};
-#pragma unroll
-    for (int k = 0; k < LOAD_FIELDS; ++k)
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o); // two's complement: signed sums come out right
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0)
-        for (int k = 0; k < LOAD_FIELDS; ++k) part[warp][k] = v[k];
-    __syncthreads();
-    if (threadIdx.x >= LOAD_FIELDS) return;
-    unsigned long long sum = 0;
-    for (int w = 0; w < PT / 32; ++w) sum += part[w][threadIdx.x];
+    const unsigned long long sum = block_load_sum<PT>(acc, faces, part);
     if (sum == 0) return;
     BlubSolidLoad &rec = ring[(size_t)blockIdx.y * LOAD_HISTORY_LENGTH + params->step_count % LOAD_HISTORY_LENGTH];
     if (threadIdx.x < 3) atomicAdd(reinterpret_cast<unsigned long long *>(&rec.force_fx[threadIdx.x]), sum);

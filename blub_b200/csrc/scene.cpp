@@ -216,6 +216,33 @@ SceneConfig parse_scene_file(const std::string &path) {
             cfg.load_probes.push_back(b);
         }
     }
+    // floating bodies (not in the reference): world units, m/s and rad/s; checked here against the rules of set_bodies
+    if (const JsonValue *bodies = fluid.get("bodies")) {
+        if (bodies->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.bodies` is not an array");
+        for (const JsonValue &o : bodies->array) {
+            if (o.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.bodies` entry is not an object");
+            SceneBody b;
+            const JsonValue &shape = need(o, "shape");
+            if (shape.kind != JsonValue::String || (shape.string != "box" && shape.string != "sphere"))
+                throw std::runtime_error("scene JSON: `bodies.shape` must be \"box\" or \"sphere\"");
+            b.shape = shape.string == "sphere" ? 1 : 0;
+            vec3(need(o, "position"), "bodies.position", b.position);
+            const JsonValue &ext = need(o, "half_extent"); // a sphere's radius: a number, or {x, y, z} with the radius in x
+            if (ext.kind == JsonValue::Number) b.half_extent[0] = b.half_extent[1] = b.half_extent[2] = num_f32(ext, "bodies.half_extent");
+            else vec3(ext, "bodies.half_extent", b.half_extent);
+            b.relative_density = num_f32(need(o, "relative_density"), "bodies.relative_density");
+            if (const JsonValue *v = o.get("rotation_angles_deg")) vec3(*v, "bodies.rotation_angles_deg", b.rotation_angles_deg);
+            if (const JsonValue *v = o.get("velocity")) vec3(*v, "bodies.velocity", b.velocity);
+            if (const JsonValue *v = o.get("angular_velocity")) vec3(*v, "bodies.angular_velocity", b.angular_velocity);
+            cfg.bodies.push_back(b);
+        }
+        try {
+            const std::vector<BlubBody> grid = scene_bodies_grid(cfg);
+            make_body_set(cfg.grid_dimension, grid.data(), (uint32_t)grid.size(), false);
+        } catch (const std::invalid_argument &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.bodies`: ") + e.what());
+        }
+    }
     if (const JsonValue *objs = root.get("static_objects")) { // #[serde(default)]
         if (objs->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `static_objects` is not an array");
         for (const JsonValue &o : objs->array) { // StaticObjectConfig, src/scene/models.rs:11-19

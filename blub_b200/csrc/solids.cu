@@ -94,6 +94,14 @@ __global__ void __launch_bounds__(256) voxelize_box_kernel(uint2 *__restrict__ v
 
 } // namespace
 
+void quat_from_euler_deg_wxyz(const float deg[3], float q[4]) {
+    const Quat r = quat_from_euler_deg(deg);
+    q[0] = r.s;
+    q[1] = r.x;
+    q[2] = r.y;
+    q[3] = r.z;
+}
+
 // StaticMeshData::to_gpu (src/scene/models.rs:186-224) evaluated on the host: where the object is, how it is rotated and how it moves,
 // in voxel space.  Shared by the analytic solids below and the mesh voxelizer (mesh_voxelizer.cu).
 void rigid_state_at(const BlubRigidObject &o, float grid_to_world_scale, const float fluid_world_position[3], double total_time, double delta,

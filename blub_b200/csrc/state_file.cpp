@@ -22,14 +22,15 @@ static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the state file is litt
 constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters; version 4:
 // section 14 followed by the sources' particle tags (written only when one of them is not 0).  Version 3 is not a format: no build writes
-// it and readers refuse it.
-constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4;
-constexpr uint32_t kNumSections = 14; // at most
+// it and readers refuse it.  Version 8: a fluid with floating bodies; the version-4 layout (section 14 may describe an empty flow set) plus
+// section 15, the bodies.  Versions 3, 5, 6 and 7 are not formats either.
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8;
+constexpr uint32_t kNumSections = 15; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
-    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW
+    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -47,6 +48,12 @@ struct FlowSectionTagged {
     uint32_t source_tags[16]; // unused slots zero
 };
 static_assert(sizeof(FlowSectionTagged) == 1056, "tagged flow section layout");
+// Section 15 (version 8): the bodies, unused slots zero
+struct BodySection {
+    uint32_t num_bodies;
+    BlubBody body[16];
+};
+static_assert(sizeof(BodySection) == 1156 && BODIES_MAX == 16, "body section layout");
 
 struct StateHeader {
     char magic[8];
@@ -87,9 +94,10 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
                                      {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
                                      {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
-                                     {SEC_FLOW, h.format_version == kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)}};
+                                     {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
+                                     {SEC_BODIES, sizeof(BodySection)}};
     std::memcpy(out, s, sizeof(s));
-    return h.format_version >= kFormatVersionFlow ? 14 : 13;
+    return h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -161,8 +169,10 @@ StateHeader read_header(File &f) {
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
-    if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags)
-        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads versions 1, 2 and 4)");
+    if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
+        h.format_version != kFormatVersionBodies)
+        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
+                         " is not supported (this library reads versions 1, 2, 4 and 8)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -243,9 +253,9 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
 }
 
 // The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.  tags: the sources'
-// particle tags (version 4), or nullptr.
+// particle tags (version 4), or nullptr.  Version 8 may describe an empty set.
 FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHeader &h, const std::string &path) {
-    if (fl.num_sources > 16 || fl.num_drains > 16 || fl.num_sources + fl.num_drains == 0)
+    if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version != kFormatVersionBodies))
         throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
     std::vector<BlubFluidSource> src(fl.num_sources);
     std::vector<BlubFluidDrain> drn(fl.num_drains);
@@ -277,6 +287,16 @@ FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHead
     return fs;
 }
 
+// The bodies of section 15, checked with the rules of set_bodies; the poses are kept bit for bit.
+std::vector<BlubBody> body_set_of(const BodySection &bs, const StateHeader &h, const std::string &path) {
+    if (bs.num_bodies > 16) throw ParseError(path + ": section 15 holds more than 16 bodies");
+    try {
+        return make_body_set(h.grid_dimension, bs.body, bs.num_bodies, true);
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": section 15: " + e.what());
+    }
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
@@ -286,10 +306,15 @@ StateInfo read_state_info(const std::string &path) {
     const uint32_t ns = expected_sections(h, sec);
     Staging st(false);
     for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
-    if (ns == 14) {
+    if (ns >= 14) {
         FlowSectionTagged fl{};
         read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
         flow_set_of(fl.flow, fl.source_tags, h, f.path);
+    }
+    if (ns == 15) {
+        BodySection bs{};
+        read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
+        body_set_of(bs, h, f.path);
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -310,7 +335,8 @@ void HybridFluid::save_state(const std::string &path) {
     std::memcpy(h.magic, kMagic, sizeof(kMagic));
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
-    h.format_version = !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool with_bodies = num_bodies_ > 0;
+    h.format_version = with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -329,7 +355,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = flow_active_ ? 14 : 13;
+    h.num_sections = with_bodies ? 15 : flow_active_ ? 14 : 13;
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -355,7 +381,7 @@ void HybridFluid::save_state(const std::string &path) {
         write_host_section(f, SEC_SOLVER_SCALARS, scalars, sizeof(scalars));
         write_host_section(f, SEC_STATS_VELOCITY, stats[0].data(), stats[0].size() * sizeof(SolverStatisticSample));
         write_host_section(f, SEC_STATS_DENSITY, stats[1].data(), stats[1].size() * sizeof(SolverStatisticSample));
-        if (flow_active_) {
+        if (flow_active_ || with_bodies) {
             FlowSectionTagged tagged{};
             FlowSection &fl = tagged.flow;
             fl.num_sources = (uint32_t)flow_.num_sources;
@@ -374,7 +400,12 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies ? sizeof(tagged) : sizeof(fl));
+        }
+        if (with_bodies) {
+            BodySection bs{};
+            bs.num_bodies = bodies(bs.body, BODIES_MAX);
+            write_host_section(f, SEC_BODIES, &bs, sizeof(bs));
         }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
@@ -432,12 +463,17 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         x.field(which).stats.assign(samples.begin(), samples.end());
     }
     x.fluid_bits_stale_ = true; // rebuilt from the restored marker volume before the next grid pass that reads it
-    if (ns == 14) {
+    if (ns >= 14) {
         FlowSectionTagged fl{};
         to_host(sec[13], &fl);
         const FlowSet fs = flow_set_of(fl.flow, fl.source_tags, h, f.path);
         BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
-        x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
+        if (fs.num_sources + fs.num_drains > 0) x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
+    }
+    if (ns == 15) { // the history ring is not state: a loaded fluid starts with an empty one
+        BodySection bs{};
+        to_host(sec[14], &bs);
+        x.restore_bodies(body_set_of(bs, h, f.path));
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

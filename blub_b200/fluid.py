@@ -22,7 +22,7 @@ STAGES = [
     "transfer_clear", "advect", "set_boundary_marker", "density_gather_error", "solve_density",
     "position_change", "extrapolate2", "correct_particles",
 ]
-TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, TAP_P_DEN, TAP_RESIDUAL = range(11)
+TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, TAP_P_DEN, TAP_RESIDUAL, TAP_SOLID_VOXELS = range(12)
 
 BLUB_OK = 0
 BLUB_WARN_TRUNCATED = 100
@@ -32,6 +32,8 @@ LOAD_PROBES_MAX = 16            # BLUB_LOAD_PROBES_MAX
 LOAD_HISTORY_LENGTH = 1024      # BLUB_LOAD_HISTORY_LENGTH: records per probe in the device ring
 LOAD_FORCE_FRAC_BITS = 16       # BLUB_LOAD_FORCE_FRAC_BITS: force sums are sums of rint(q * 2^16)
 LOAD_TORQUE_FRAC_BITS = 8       # BLUB_LOAD_TORQUE_FRAC_BITS: torque sums are sums of rint(r_b * q * 2^8)
+BODIES_MAX = 16                 # BLUB_BODIES_MAX
+BODY_HISTORY_LENGTH = 1024      # BLUB_BODY_HISTORY_LENGTH: records per body in the device ring
 
 
 class BlubError(RuntimeError):
@@ -131,6 +133,40 @@ class SolidLoad(C.Structure):
     _fields_ = [("step", C.c_uint32), ("wetted_faces", C.c_uint32), ("force_fx", C.c_int64 * 3), ("torque_fx", C.c_int64 * 3)]
 
 
+class Body(C.Structure):
+    """BlubBody: a floating box (shape 0, half extents) or sphere (shape 1, radius half_extent[0]) in grid cells, cells/s and rad/s."""
+
+    _fields_ = [("shape", C.c_int32), ("half_extent", C.c_float * 3), ("relative_density", C.c_float), ("centre", C.c_float * 3),
+                ("rotation", C.c_float * 4), ("velocity", C.c_float * 3), ("angular_velocity", C.c_float * 3)]
+
+    @classmethod
+    def from_dict(cls, d):
+        b = cls()
+        shape = d.get("shape", "box")
+        b.shape = {"box": 0, "sphere": 1}.get(shape, shape) if isinstance(shape, str) else int(shape)
+        ext = d["half_extent"]
+        b.half_extent[:] = [float(ext)] * 3 if np.ndim(ext) == 0 else [float(v) for v in ext]
+        b.relative_density = float(d["relative_density"])
+        b.centre[:] = [float(v) for v in d["centre"]]
+        b.rotation[:] = [float(v) for v in d.get("rotation", (1.0, 0.0, 0.0, 0.0))]
+        b.velocity[:] = [float(v) for v in d.get("velocity", (0.0, 0.0, 0.0))]
+        b.angular_velocity[:] = [float(v) for v in d.get("angular_velocity", (0.0, 0.0, 0.0))]
+        return b
+
+    def to_dict(self):
+        return {"shape": "sphere" if self.shape == 1 else "box", "half_extent": tuple(self.half_extent), "relative_density": self.relative_density,
+                "centre": tuple(self.centre), "rotation": tuple(self.rotation), "velocity": tuple(self.velocity),
+                "angular_velocity": tuple(self.angular_velocity)}
+
+
+class BodyRecord(C.Structure):
+    """BlubBodyRecord: one step's load on a body (BlubSolidLoad's fixed point) and its pose after the step."""
+
+    _fields_ = [("step", C.c_uint32), ("wetted_faces", C.c_uint32), ("force_fx", C.c_int64 * 3), ("torque_fx", C.c_int64 * 3),
+                ("centre", C.c_float * 3), ("rotation", C.c_float * 4), ("velocity", C.c_float * 3), ("angular_velocity", C.c_float * 3),
+                ("reserved", C.c_uint32)]
+
+
 def lib_path() -> str:
     return os.path.join(_HERE, "libblubcore.so")
 
@@ -203,6 +239,10 @@ def lib():
         "blub_fluid_load_history": (C.c_int, [vp, u32, C.POINTER(SolidLoad), u32, C.POINTER(u32)]),
         "blub_load_probe_cells": (C.c_int, [C.POINTER(u32), C.POINTER(LoadProbe), C.POINTER(u32), C.POINTER(u32)]),
         "blub_scene_load_probes": (C.c_int, [C.c_char_p, C.POINTER(LoadProbe), u32, C.POINTER(u32)]),
+        "blub_fluid_set_bodies": (C.c_int, [vp, C.POINTER(Body), u32]),
+        "blub_fluid_body_history": (C.c_int, [vp, u32, C.POINTER(BodyRecord), u32, C.POINTER(u32)]),
+        "blub_fluid_bodies": (C.c_int, [vp, C.POINTER(Body), u32, C.POINTER(u32)]),
+        "blub_scene_bodies": (C.c_int, [C.c_char_p, C.POINTER(Body), u32, C.POINTER(u32)]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -350,6 +390,14 @@ def scene_load_probes(path):
     arr = (LoadProbe * LOAD_PROBES_MAX)()
     _check(lib().blub_scene_load_probes(os.fsencode(path), arr, LOAD_PROBES_MAX, C.byref(count)))
     return [(tuple(p.min_grid), tuple(p.max_grid), tuple(p.pivot_grid)) for p in arr[:count.value]]
+
+
+def scene_bodies(path):
+    """The scene's fluid.bodies in grid cells, cells/s and rad/s, as dicts (see Body.to_dict; host only)."""
+    count = C.c_uint32(0)
+    arr = (Body * BODIES_MAX)()
+    _check(lib().blub_scene_bodies(os.fsencode(path), arr, BODIES_MAX, C.byref(count)))
+    return [b.to_dict() for b in arr[:min(count.value, BODIES_MAX)]]
 
 
 def state_info(path):
@@ -614,6 +662,48 @@ class HybridFluid:
         res["force"] = res["force_fx"].astype(np.float64) / float(1 << LOAD_FORCE_FRAC_BITS)
         res["torque"] = res["torque_fx"].astype(np.float64) / float(1 << LOAD_TORQUE_FRAC_BITS)
         return res
+
+    # -- floating bodies ----------------------------------------------------------------------
+    def set_bodies(self, bodies=()):
+        """Replaces the floating bodies: dicts {"shape": "box" | "sphere", "half_extent": (hx, hy, hz) or a radius, "relative_density",
+        "centre", "rotation" (w, x, y, z; default identity), "velocity", "angular_velocity"} in grid cells, cells/s and rad/s (at most 16).
+        Resets the history; an empty list clears the set.  Raises BlubError (and changes nothing) on a body that breaks a rule of
+        blub_fluid_set_bodies, z-slab ranks and a fluid inside a step."""
+        arr = (Body * max(len(bodies), 1))()
+        for k, b in enumerate(bodies):
+            arr[k] = b if isinstance(b, Body) else Body.from_dict(b)
+        _check(self.L.blub_fluid_set_bodies(self.h, arr, len(bodies)))
+
+    def bodies(self):
+        """The current bodies as dicts (the pose the next step writes).  Synchronises."""
+        arr = (Body * BODIES_MAX)()
+        count = C.c_uint32(0)
+        _check(self.L.blub_fluid_bodies(self.h, arr, BODIES_MAX, C.byref(count)))
+        return [b.to_dict() for b in arr[:count.value]]
+
+    def body_history(self, body, capacity=BODY_HISTORY_LENGTH):
+        """The newest records of one body, oldest first: "step", "wetted_faces", "force_fx", "torque_fx" as recorded, float64 "force"
+        (cells^4/s^2 per unit density) and "torque" (cells^5/s^2), and float32 "centre", "rotation", "velocity", "angular_velocity" after
+        the step.  Synchronises."""
+        capacity = int(capacity)
+        out = (BodyRecord * max(capacity, 1))()
+        count = C.c_uint32(0)
+        _check(self.L.blub_fluid_body_history(self.h, int(body), out, capacity, C.byref(count)))
+        recs = out[:count.value]
+        res = {"step": np.array([r.step for r in recs], dtype=np.uint32), "wetted_faces": np.array([r.wetted_faces for r in recs], dtype=np.uint32)}
+        for name in ("force_fx", "torque_fx"):
+            res[name] = np.array([list(getattr(r, name)) for r in recs], dtype=np.int64).reshape(-1, 3)
+        for name, width in (("centre", 3), ("rotation", 4), ("velocity", 3), ("angular_velocity", 3)):
+            res[name] = np.array([list(getattr(r, name)) for r in recs], dtype=np.float32).reshape(-1, width)
+        res["force"] = res["force_fx"].astype(np.float64) / float(1 << LOAD_FORCE_FRAC_BITS)
+        res["torque"] = res["torque_fx"].astype(np.float64) / float(1 << LOAD_TORQUE_FRAC_BITS)
+        return res
+
+    def download_solid_voxels(self):
+        """The solid volume the step reads (BLUB_TAP_SOLID_VOXELS) as float16 [nz, ny, nx, 4]."""
+        out = np.empty((self.nz, self.ny, self.nx, 4), dtype=np.float16)
+        _check(self.L.blub_fluid_download(self.h, TAP_SOLID_VOXELS, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
 
     @property
     def has_flow(self):

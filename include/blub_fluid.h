@@ -233,6 +233,57 @@ int blub_fluid_load_history(BlubFluid *fluid, uint32_t probe, BlubSolidLoad *out
 /* Host only: the cells [lo, hi) a probe holds on a grid of `dim` cells.  BLUB_ERR_INVALID_ARGUMENT: a non-finite value or an empty box. */
 int blub_load_probe_cells(const uint32_t dim[3], const BlubLoadProbe *probe, uint32_t lo[3], uint32_t hi[3]);
 
+/* ---- floating bodies (not part of the reference surface; rules: DESIGN.md section 8) -------------------------------------------
+ * A body is an oriented box (half extents) or a sphere (radius = half_extent[0]) in grid cells whose pose lives on the device and which the
+ * fluid's pressure moves.  While a fluid has bodies it owns a composite solid volume: every step first copies the borrowed volume into it
+ * (or zeroes it), then writes every body over it in index order (a later body wins where they overlap): a cell whose centre lies inside a
+ * body gets w = 1 and xyz = v + w x (cell centre - c), the rigid velocity.  Every later stage reads that volume; the borrowed one is never
+ * written.  After the velocity solve each body's pressure force and torque about its centre are summed exactly with the face rule of the
+ * load probes (wetted faces of the SOLID cells it covers; a solid overlapping a body is not told apart from it), and one thread per body
+ * integrates semi-implicit Euler in float32: v += dt (g + F / m), w += dt R (I_b^-1 (R^T tau)) (no gyroscopic term), c += dt v,
+ * q = normalize(q + dt/2 (0, w) q), with m = relative_density * V (V the analytic volume) per unit fluid density.  The tank walls clamp the
+ * pose: a bounding box leaving [1, dim - 1] is shifted back and the outward velocity component zeroed (a clamp, not a collision model);
+ * bodies do not collide with each other.  The new pose is what the next step writes.  The coupling is explicit: it was measured stable for
+ * relative densities 0.5 and 0.75 (a floating box) and 2 (a sinking one); lighter bodies were not measured.  Bodies are state: a fluid with
+ * bodies saves format version 8. */
+#define BLUB_BODIES_MAX 16
+#define BLUB_BODY_HISTORY_LENGTH 1024 /* records per body in the device ring: slot = step % 1024 */
+typedef struct {
+    int32_t shape;            /* 0 = box, 1 = sphere */
+    float half_extent[3];     /* cells; a sphere's radius is half_extent[0] (the others are ignored) */
+    float relative_density;   /* body density / fluid density, finite and > 0 */
+    float centre[3];          /* grid cells */
+    float rotation[4];        /* unit quaternion (w, x, y, z), body -> grid */
+    float velocity[3];        /* cells/s */
+    float angular_velocity[3];/* rad/s, grid axes */
+} BlubBody;
+typedef struct {
+    uint32_t step;            /* blub_fluid_step_count before the step that wrote the record */
+    uint32_t wetted_faces;
+    int64_t force_fx[3];      /* force * 2^16, per unit fluid density (BlubSolidLoad's fixed point) */
+    int64_t torque_fx[3];     /* torque about the centre * 2^8 */
+    float centre[3], rotation[4], velocity[3], angular_velocity[3]; /* the pose after the step's integration */
+    uint32_t reserved;
+} BlubBodyRecord;
+#ifdef __cplusplus
+static_assert(sizeof(BlubBody) == 72 && sizeof(BlubBodyRecord) == 112, "BlubBody / BlubBodyRecord layout");
+#else
+_Static_assert(sizeof(BlubBody) == 72 && sizeof(BlubBodyRecord) == 112, "BlubBody / BlubBodyRecord layout");
+#endif
+/* Replaces the whole body set (0 clears it), resets the history and drops the cached step graphs; the quaternions are stored normalised.
+ * BLUB_ERR_INVALID_ARGUMENT, changing nothing: more than 16 bodies, a non-finite value, a shape other than 0 / 1, a half extent or radius
+ * below 1 cell, relative_density <= 0, a quaternion whose norm is not within 1e-3 of 1, a bounding box outside [1, dim - 1], a z-slab rank,
+ * or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_bodies(BlubFluid *fluid, const BlubBody *bodies, uint32_t num_bodies);
+/* The newest min(capacity, recorded, 1024) records of body `body`, oldest first; *count receives their number.  Synchronises.
+ * BLUB_ERR_INVALID_ARGUMENT: a body index outside the set. */
+int blub_fluid_body_history(BlubFluid *fluid, uint32_t body, BlubBodyRecord *out, uint32_t capacity, uint32_t *count);
+/* The current bodies (the pose the next step writes); writes at most `capacity` and sets *count to the number in the set.  Synchronises. */
+int blub_fluid_bodies(BlubFluid *fluid, BlubBody *out, uint32_t capacity, uint32_t *count);
+/* The scene's optional fluid.bodies in grid cells and cells/s ((p - world_position) / grid_to_world_scale, Euler angles as for
+ * static_objects).  Writes at most `capacity` bodies and sets *count to the number the scene holds.  blub_scene_load sets them. */
+int blub_scene_bodies(const char *scene_json_path, BlubBody *out, uint32_t capacity, uint32_t *count);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their
@@ -352,7 +403,8 @@ int blub_enable_peer_access(int device, int peer);
 enum {
     BLUB_TAP_PARTICLE_POS = 0, BLUB_TAP_PARTICLE_VX = 1, BLUB_TAP_PARTICLE_VY = 2, BLUB_TAP_PARTICLE_VZ = 3,
     BLUB_TAP_GRID_VX = 4, BLUB_TAP_GRID_VY = 5, BLUB_TAP_GRID_VZ = 6, BLUB_TAP_MARKER = 7,
-    BLUB_TAP_PRESSURE_VELOCITY = 8, BLUB_TAP_PRESSURE_DENSITY = 9, BLUB_TAP_RESIDUAL = 10
+    BLUB_TAP_PRESSURE_VELOCITY = 8, BLUB_TAP_PRESSURE_DENSITY = 9, BLUB_TAP_RESIDUAL = 10,
+    BLUB_TAP_SOLID_VOXELS = 11 /* the solid volume the step reads: the composite one with bodies, else the borrowed one (download only) */
 };
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);

@@ -84,6 +84,46 @@ def tight_solver(*fluids, tol=1e-4, max_it=128):
         f.set_solver_config(1, tol, max_it, 4)
 
 
+def dilate(mask):
+    """mask dilated by one cell in every direction (Chebyshev), without wrap-around."""
+    out = mask.copy()
+    for dz in (-1, 0, 1):
+        for dy in (-1, 0, 1):
+            for dx in (-1, 0, 1):
+                src = [slice(max(0, -d), mask.shape[k] - max(0, d)) for k, d in enumerate((dz, dy, dx))]
+                dst = [slice(max(0, d), mask.shape[k] - max(0, -d)) for k, d in enumerate((dz, dy, dx))]
+                out[tuple(dst)] |= mask[tuple(src)]
+    return out
+
+
+def solid_contact(marker, vox, positions):
+    """How much of a solid test actually reaches the fluid: (FLUID cells with a face neighbour that is SOLID because of the solid volume -- not a
+    border wall -- and whose solid velocity is not zero, particles inside or within one cell of a solid voxel).  A solid test asserts a
+    minimum of both, so that a geometry that misses the fluid cannot pass quietly.  vox: [nz, ny, nx, 4] (any float type)."""
+    marker = np.asarray(marker)
+    vox = np.asarray(vox, dtype=np.float32)
+    solid = vox[..., 3] != 0
+    interior = np.zeros_like(solid)
+    interior[1:-1, 1:-1, 1:-1] = True
+    moving = (marker == O.SOLID) & solid & interior & (vox[..., :3] != 0).any(axis=-1)
+    fl = marker == O.FLUID
+    touch = np.zeros_like(fl)
+    for ax in range(3):
+        for sh in (1, -1):
+            nb = np.zeros_like(moving)
+            src = [slice(None)] * 3
+            dst = [slice(None)] * 3
+            src[ax] = slice(max(0, sh), moving.shape[ax] + min(0, sh))
+            dst[ax] = slice(max(0, -sh), moving.shape[ax] + min(0, -sh))
+            nb[tuple(dst)] = moving[tuple(src)]  # nb[g] = moving[g + sh e_ax]
+            touch |= nb
+    c = np.floor(np.asarray(positions, dtype=np.float64)[:, :3]).astype(np.int64)
+    for k, n in enumerate((marker.shape[2], marker.shape[1], marker.shape[0])):
+        c[:, k] = np.clip(c[:, k], 0, n - 1)
+    near = dilate(solid)
+    return int((fl & touch).sum()), int(near[c[:, 2], c[:, 1], c[:, 0]].sum())
+
+
 def near_fluid(marker):
     """Cells within one cell (Chebyshev) of a FLUID cell: the region the grid passes of the CUDA path visit.  Further away nothing reads the
     faces (P2G rewrites every face a particle can reach, extrapolation fills the one-cell ring G2P can reach) and the reference's P2G leaves

@@ -34,6 +34,23 @@ struct Quirks {
     int precond_mode = 0; // 0: z = r/diag^2 ("LOD-1 fetch returns 0"), 1: as written with clamped LOD (SURVEY B1)
 };
 
+// A mesh as the host holds it before it becomes a mesh body: present == false for a box or sphere.
+struct HostMesh {
+    bool present = false;
+    float scale = 0.0f; // cells per model unit
+    std::vector<float> positions;
+    std::vector<uint32_t> indices;
+};
+
+// A body slot's host copy of a mesh body (DESIGN.md §8 "Mesh bodies"): its properties as stored, the float32 body-frame vertices and its
+// indices; no vertices for a box or sphere.
+struct MeshBodyHost {
+    BlubMeshBodyProperties props{};
+    float mid[3] = {0, 0, 0}; // (lo + hi) / 2 of the body-frame bounds
+    std::vector<float> vertices;
+    std::vector<uint32_t> indices;
+};
+
 // A padded device array of grid cells (see GridDim).
 template <class T> struct GridArray {
     T *base = nullptr; // allocation
@@ -262,6 +279,14 @@ class HybridFluid {
     uint32_t body_history(uint32_t body, BlubBodyRecord *out, uint32_t capacity);
     // the solid volume the step reads: the composite one while there are bodies, else the borrowed one (may be nullptr)
     const uint2 *solid_volume() const { return num_bodies_ ? composite_ : voxels_; }
+    // set_bodies with mesh bodies (DESIGN.md §8 "Mesh bodies"): meshes[i] != nullptr makes body i a mesh body scaled by scales[i].  Copies
+    // the geometry; refuses what set_bodies and make_mesh_body refuse, a mesh on another device and sets over the vertex / triangle limits.
+    void set_bodies_meshes(const BlubBody *bodies, const BlubMesh *const *meshes, const float *scales, uint32_t num_bodies);
+    // the same with host meshes, one per body (meshes.size() bodies)
+    void set_bodies_host(const BlubBody *bodies, const std::vector<HostMesh> &meshes);
+    // the properties of mesh body `body` as stored; throws std::invalid_argument when it is not a mesh body
+    BlubMeshBodyProperties body_mass_properties(uint32_t body) const;
+    bool has_mesh_bodies() const { return !mesh_bodies_.empty(); }
 
   private:
     BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
@@ -270,7 +295,11 @@ class HybridFluid {
     uint2 *composite_ = nullptr;
     uint32_t num_bodies_ = 0, body_cube_ = 0;
     std::deque<uint32_t> body_steps_; // step numbers of the records in the body ring, oldest first
-    void restore_bodies(const std::vector<BlubBody> &bodies); // a validated set (set_bodies, state file load)
+    // a validated set (set_bodies, state file load); meshes: one host copy per body when the set has mesh bodies, else empty
+    void restore_bodies(const std::vector<BlubBody> &bodies, std::vector<MeshBodyHost> meshes = {});
+    std::vector<MeshBodyHost> mesh_bodies_; // one per body while the set has a mesh body, else empty
+    MeshBodySet mesh_;                      // device arrays, reallocated by every set with mesh bodies
+    void free_mesh_bodies();
     LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
     BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
     uint32_t num_load_probes_ = 0, load_max_cells_ = 0;
@@ -400,6 +429,27 @@ LoadProbeBox clamp_load_probe(const uint32_t dim[3], const BlubLoadProbe &probe)
 // (loaded == false) normalises the quaternions; a state file's bodies (loaded == true) are kept bit for bit and their bounding boxes may
 // leave [1, dim - 1] by the rounding of the integrator's clamp (1e-3 cells).
 std::vector<BlubBody> make_body_set(const uint32_t dim[3], const BlubBody *bodies, uint32_t num_bodies, bool loaded);
+
+// Mesh bodies (mesh_body.cpp, DESIGN.md §8 "Mesh bodies").
+// Checks a mesh and computes its mass properties and principal frame (blub_mesh_body_properties); throws std::invalid_argument.
+// body_vertices (if given) receives the float32 body-frame vertices.
+BlubMeshBodyProperties mesh_body_properties(const float *positions, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, float scale,
+                                            std::vector<float> *body_vertices);
+// A mesh body placed by `placement` (centre and rotation: the model origin and axes in the grid): its host copy and, in `stored`, the BlubBody
+// the device keeps (centre of mass, model rotation * principal rotation, half extents of the body-frame bounds).  Checks the placement as
+// set_bodies does and the bounding box against [1, dim - 1] (skipped when dim == nullptr); throws std::invalid_argument.
+MeshBodyHost make_mesh_body(const uint32_t dim[3], const BlubBody &placement, const float *positions, uint32_t num_vertices, const uint32_t *indices,
+                            uint32_t num_indices, float scale, BlubBody &stored);
+// A body set with mesh bodies checked against the rules of set_bodies_meshes: `set` receives the stored bodies; returns one host copy per body,
+// or none when no body has a mesh.  Throws std::invalid_argument.
+std::vector<MeshBodyHost> make_mesh_body_set(const uint32_t dim[3], const BlubBody *bodies, const std::vector<HostMesh> &meshes, std::vector<BlubBody> &set);
+// The setter's view of a mesh body's grid-axis bounding box: e = its half extents, off = R mid its centre relative to the centre of mass.
+// Not bit-exact with the device: off is float64 rounded once, not the device's float32 dot3, so a pose within rounding of [1, dim - 1] may be
+// accepted here and then moved by the first step's clamp.
+void mesh_body_box(const BlubBody &b, const float mid[3], float e[3], float off[3]);
+// The launch cube side of a mesh body: from the farthest corner of its body-frame bounds to the centre of mass.
+uint32_t mesh_body_cube_side(const float h[3], const float mid[3]);
+void quat_rotation_f64(const double q[4], double R[9]);
 // cgmath's Quaternion::from(Euler<Deg>) as (w, x, y, z) (solids.cu)
 void quat_from_euler_deg_wxyz(const float deg[3], float q[4]);
 // A flow set from the public boxes (grid units), clamped like add_fluid_cube; throws std::invalid_argument when it breaks a rule of set_flow
@@ -418,6 +468,9 @@ void rigid_state_at(const BlubRigidObject &o, float grid_to_world_scale, const f
 BlubMesh *mesh_create(const float *positions, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, int device);
 void mesh_destroy(BlubMesh *mesh);
 void mesh_info(const BlubMesh &mesh, uint32_t &num_vertices, uint32_t &num_triangles);
+int mesh_device(const BlubMesh &mesh);
+// the mesh's positions and indices, copied to the host (synchronous)
+void mesh_download(const BlubMesh &mesh, std::vector<float> &positions, std::vector<uint32_t> &indices);
 void voxelize_mesh(void *rgba16f, const uint32_t dim[3], BlubMesh &mesh, const BlubRigidObject &o, float grid_to_world_scale, const float fluid_world_position[3],
                    double total_time, double delta, int clear_first, cudaStream_t stream, BlubRigidState *state_out);
 void read_obj(const std::string &path, std::vector<float> &positions, std::vector<uint32_t> &indices);
@@ -440,7 +493,9 @@ struct SceneLoadProbe {
     bool has_pivot = false; // without one the pivot is the box centre
 };
 struct SceneBody {
-    int32_t shape = 0;            // "box" 0, "sphere" 1
+    int32_t shape = 0;            // "box" 0, "sphere" 1, "mesh" 2
+    std::string model;            // a mesh body's OBJ file, resolved against the scene file's directory
+    float model_scale = 1.0f;     // a mesh body's world units per model unit
     float position[3], half_extent[3], rotation_angles_deg[3] = {0, 0, 0}, relative_density = 1.0f;
     float velocity[3] = {0, 0, 0}, angular_velocity[3] = {0, 0, 0}; // m/s, rad/s
 };
@@ -464,6 +519,8 @@ std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
 // the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a
 // quaternion (quat_from_euler_deg_wxyz), the angular velocity unchanged
 std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg);
+// the scene's bodies' meshes (read from their OBJ files; scale in cells per model unit = model_scale / grid_to_world_scale), one per body
+std::vector<HostMesh> scene_body_meshes(const SceneConfig &cfg);
 // Scene::create_fluid_from_config, src/scene/mod.rs:109-144
 std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, int device, cudaStream_t stream);
 

@@ -457,6 +457,37 @@ int blub_fluid_bodies(BlubFluid *fluid, BlubBody *out, uint32_t capacity, uint32
     return guarded([&] { *count = fluid->impl->bodies(out, capacity); return BLUB_OK; });
 }
 
+int blub_mesh_body_properties(const float *positions, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, float scale,
+                              BlubMeshBodyProperties *out) {
+    if (!out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL output");
+    return guarded([&] { *out = blub::mesh_body_properties(positions, num_vertices, indices, num_indices, scale, nullptr); return BLUB_OK; });
+}
+
+int blub_mesh_body_vertices(const float *positions, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, float scale, float *out) {
+    if (!out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL output");
+    return guarded([&] {
+        std::vector<float> vb;
+        blub::mesh_body_properties(positions, num_vertices, indices, num_indices, scale, &vb);
+        std::copy(vb.begin(), vb.end(), out);
+        return BLUB_OK;
+    });
+}
+
+int blub_fluid_set_bodies_meshes(BlubFluid *fluid, const BlubBody *bodies, const BlubMeshBodyShape *shapes, uint32_t num_bodies) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    if (!shapes) return blub_fluid_set_bodies(fluid, bodies, num_bodies);
+    if (num_bodies > BLUB_BODIES_MAX) return fail(BLUB_ERR_INVALID_ARGUMENT, "set_bodies: at most 16 bodies");
+    const BlubMesh *meshes[BLUB_BODIES_MAX];
+    float scales[BLUB_BODIES_MAX];
+    for (uint32_t i = 0; i < num_bodies; ++i) meshes[i] = shapes[i].mesh, scales[i] = shapes[i].scale;
+    return guarded([&] { fluid->impl->set_bodies_meshes(bodies, meshes, scales, num_bodies); return BLUB_OK; });
+}
+
+int blub_fluid_body_mass_properties(BlubFluid *fluid, uint32_t body, BlubMeshBodyProperties *out) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *out = fluid->impl->body_mass_properties(body); return BLUB_OK; });
+}
+
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
 
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {
@@ -497,6 +528,20 @@ int blub_scene_bodies(const char *path, BlubBody *out, uint32_t capacity, uint32
         const std::vector<BlubBody> bodies = blub::scene_bodies_grid(blub::parse_scene_file(path));
         for (size_t k = 0; k < bodies.size() && k < capacity; ++k) out[k] = bodies[k];
         *count = (uint32_t)bodies.size();
+        return BLUB_OK;
+    });
+}
+
+int blub_scene_body_model(const char *path, uint32_t body, char *model_path_out, size_t capacity, float *scale_out) {
+    if (!path) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig c = blub::parse_scene_file(path);
+        if (body >= c.bodies.size() || c.bodies[body].shape != 2) throw std::invalid_argument("scene body_model: not a mesh body");
+        if (model_path_out && capacity) {
+            std::strncpy(model_path_out, c.bodies[body].model.c_str(), capacity - 1);
+            model_path_out[capacity - 1] = 0;
+        }
+        if (scale_out) *scale_out = c.bodies[body].model_scale / c.grid_to_world_scale;
         return BLUB_OK;
     });
 }

@@ -154,12 +154,41 @@ constexpr uint32_t BODY_HISTORY_LENGTH = BLUB_BODY_HISTORY_LENGTH;
 // The cells a launch walks around each body: a cube of `cube` cells per side from floor(c - e), sized at set time from the largest bounding
 // sphere, so that a captured graph stays valid while the bodies move and turn.
 uint32_t body_cube_side(const BlubBody &b);
+// Mesh bodies (shape 2, DESIGN.md §8 "Mesh bodies"): what the device needs of body slot i beyond its BlubBody.
+struct MeshBodyDev {
+    float mass, inertia[3]; // per unit fluid density: the integrator's m and I_b
+    float mid[3];           // (lo + hi) / 2 of the body-frame bounds; the BlubBody's half_extent is (hi - lo) / 2
+    uint32_t first_vertex, num_vertices, first_triangle, num_triangles; // into the set's arrays; num_triangles == 0: a box or sphere
+};
+// What the body kernels read of the mesh bodies: info == nullptr when the set has none.  bits: num_bodies x cube x cube rows of `words`
+// 32-bit words over each body's launch cube, bit x of row (z, y) = the cell's centre lies inside the mesh.
+struct MeshBodies {
+    const MeshBodyDev *info = nullptr;
+    const uint32_t *bits = nullptr;
+    uint32_t words = 0;
+    const int *origin = nullptr; // 3 per body: the first cell of its launch cube at the step's pose, written with the bits
+};
+// The device arrays of a set with mesh bodies (allocated by HybridFluid::restore_bodies).
+struct MeshBodySet {
+    MeshBodyDev *info = nullptr;    // BODIES_MAX slots
+    float *body_vertices = nullptr; // xyz per vertex, body frame
+    float *grid_vertices = nullptr; // xyz per vertex at the current pose: stage 0 scratch
+    uint32_t *indices = nullptr;    // 3 per triangle, into the vertex arrays
+    uint32_t *bits = nullptr;
+    int *origin = nullptr;          // BODIES_MAX x 3
+    uint32_t words = 0, max_vertices = 0, max_triangles = 0; // the largest body's counts size the launches
+    MeshBodies view() const { return {info, bits, words, origin}; }
+};
+// Stage 0, before the composite kernel: zero the bits, move every mesh body's vertices to the grid, flip the crossing bit of every covered
+// cell-centre row, then turn each row into its crossing parity.
+void launch_mesh_body_fill(cudaStream_t st, const GridDim &g, int num_bodies, uint32_t cube, const BlubBody *bodies, const MeshBodySet &mesh);
 // Stage 0: the composite solid volume (n cells of RGBA16F) = the borrowed volume (or zero when vox == nullptr), then every body written over it.
-void launch_body_composite(cudaStream_t st, const GridDim &g, const uint2 *vox, uint2 *composite, int num_bodies, uint32_t cube, const BlubBody *bodies);
+void launch_body_composite(cudaStream_t st, const GridDim &g, const uint2 *vox, uint2 *composite, int num_bodies, uint32_t cube, const BlubBody *bodies,
+                           const MeshBodies &mesh);
 // End of stage 2: every body's wetted-face sums into sums[8 * body] (zero on entry), then the integrator: it reads and re-zeroes the sums,
 // moves every body and writes its record into ring[body * BODY_HISTORY_LENGTH + params->step_count % BODY_HISTORY_LENGTH].
 void launch_body_step(cudaStream_t st, const GridDim &g, const StepParams *params, int num_bodies, uint32_t cube, BlubBody *bodies, const int8_t *marker,
-                      const float *p_vel, unsigned long long *sums, BlubBodyRecord *ring);
+                      const float *p_vel, unsigned long long *sums, BlubBodyRecord *ring, const MeshBodies &mesh);
 // Host twins of the device rules the setter checks a body against: the half extents of its grid-axis bounding box at its pose.
 void body_bounding_extents(const BlubBody &b, float e[3]);
 

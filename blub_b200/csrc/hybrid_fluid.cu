@@ -217,6 +217,7 @@ HybridFluid::~HybridFluid() {
     cudaFree(body_sums_);
     cudaFree(body_ring_);
     cudaFree(composite_);
+    free_mesh_bodies();
     cudaFree(mig_counters_);
     if (slab_error_host_) cudaFreeHost(slab_error_host_);
     cudaFree(params_dev_);
@@ -465,7 +466,8 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 0: // transfer particle velocity to grid (:806-833)
         if (num_bodies_ > 0) { // before the flow prologue: sources do not emit into bodies
             const NvtxScope body_scope("floating bodies: composite solid volume");
-            launch_body_composite(stream_, grid_, voxels_, composite_, (int)num_bodies_, body_cube_, bodies_dev_);
+            if (!mesh_bodies_.empty()) launch_mesh_body_fill(stream_, grid_, (int)num_bodies_, body_cube_, bodies_dev_, mesh_);
+            launch_body_composite(stream_, grid_, voxels_, composite_, (int)num_bodies_, body_cube_, bodies_dev_, mesh_.view());
         }
         if (flow_active_) {
             const NvtxScope flow_scope("fluid sources & drains");
@@ -504,7 +506,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         }
         if (num_bodies_ > 0) { // after the probes: the integrator moves the bodies the probes saw
             launch_body_step(stream_, grid_, params_dev_, (int)num_bodies_, body_cube_, bodies_dev_, marker_.ptr, field_velocity_->pressure(), body_sums_,
-                             body_ring_);
+                             body_ring_, mesh_.view());
             if (!capturing_) note_record(body_steps_, step_counter_, BODY_HISTORY_LENGTH);
         }
         break;
@@ -941,7 +943,7 @@ std::vector<BlubBody> make_body_set(const uint32_t dim[3], const BlubBody *bodie
         float e[3];
         body_bounding_extents(b, e);
         const float slack = loaded ? 1e-3f : 0.0f;
-        for (int k = 0; k < 3; ++k)
+        for (int k = 0; k < 3 && dim; ++k)
             if (b.centre[k] - e[k] < 1.0f - slack || b.centre[k] + e[k] > (float)dim[k] - 1.0f + slack)
                 throw std::invalid_argument("set_bodies: a body's bounding box leaves [1, dim - 1]");
     }
@@ -955,11 +957,114 @@ void HybridFluid::set_bodies(const BlubBody *bodies, uint32_t num_bodies) {
     restore_bodies(make_body_set(dim, bodies, num_bodies, false));
 }
 
-void HybridFluid::restore_bodies(const std::vector<BlubBody> &set) {
+void HybridFluid::set_bodies_meshes(const BlubBody *bodies, const BlubMesh *const *meshes, const float *scales, uint32_t num_bodies) {
+    if (num_bodies > (uint32_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
+    if (num_bodies && (!bodies || !meshes || !scales)) throw std::invalid_argument("set_bodies: NULL body, mesh or scale array");
+    std::vector<HostMesh> host(num_bodies);
+    for (uint32_t i = 0; i < num_bodies; ++i) {
+        if (!meshes[i]) continue;
+        if (mesh_device(*meshes[i]) != device_) throw std::invalid_argument("set_bodies: a mesh lives on another device");
+        host[i].present = true;
+        host[i].scale = scales[i];
+        mesh_download(*meshes[i], host[i].positions, host[i].indices);
+    }
+    set_bodies_host(bodies, host);
+}
+
+void HybridFluid::set_bodies_host(const BlubBody *bodies, const std::vector<HostMesh> &meshes) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_bodies: z-slab ranks have no floating bodies");
+    if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    const uint32_t num_bodies = (uint32_t)meshes.size();
+    if (num_bodies > (uint32_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
+    if (num_bodies && !bodies) throw std::invalid_argument("set_bodies: NULL body array");
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    std::vector<BlubBody> set(num_bodies);
+    std::vector<MeshBodyHost> host = make_mesh_body_set(dim, bodies, meshes, set);
+    restore_bodies(set, std::move(host));
+}
+
+std::vector<MeshBodyHost> make_mesh_body_set(const uint32_t dim[3], const BlubBody *bodies, const std::vector<HostMesh> &meshes, std::vector<BlubBody> &set) {
+    const size_t n = meshes.size();
+    set.assign(n, BlubBody{});
+    std::vector<MeshBodyHost> host(n);
+    size_t vertices = 0, triangles = 0;
+    bool any = false;
+    for (size_t i = 0; i < n; ++i) {
+        if (!meshes[i].present) {
+            set[i] = make_body_set(dim, bodies + i, 1, false)[0];
+            continue;
+        }
+        const HostMesh &m = meshes[i];
+        host[i] = make_mesh_body(dim, bodies[i], m.positions.data(), (uint32_t)(m.positions.size() / 3), m.indices.data(), (uint32_t)m.indices.size(),
+                                 m.scale, set[i]);
+        vertices += m.positions.size() / 3;
+        triangles += m.indices.size() / 3;
+        any = true;
+    }
+    if (vertices > (size_t)BLUB_MESH_BODY_MAX_VERTICES || triangles > (size_t)BLUB_MESH_BODY_MAX_TRIANGLES)
+        throw std::invalid_argument("set_bodies: the mesh bodies hold more than " + std::to_string(BLUB_MESH_BODY_MAX_VERTICES) + " vertices or " +
+                                    std::to_string(BLUB_MESH_BODY_MAX_TRIANGLES) + " triangles");
+    if (!any) host.clear();
+    return host;
+}
+
+BlubMeshBodyProperties HybridFluid::body_mass_properties(uint32_t body) const {
+    if (body >= num_bodies_ || mesh_bodies_.empty() || mesh_bodies_[body].vertices.empty())
+        throw std::invalid_argument("body_mass_properties: not a mesh body");
+    return mesh_bodies_[body].props;
+}
+
+void HybridFluid::free_mesh_bodies() {
+    cudaFree(mesh_.info);
+    cudaFree(mesh_.body_vertices);
+    cudaFree(mesh_.grid_vertices);
+    cudaFree(mesh_.indices);
+    cudaFree(mesh_.bits);
+    cudaFree(mesh_.origin);
+    mesh_ = MeshBodySet{};
+    mesh_bodies_.clear();
+}
+
+void HybridFluid::restore_bodies(const std::vector<BlubBody> &set, std::vector<MeshBodyHost> meshes) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // no step in flight reads the old bodies or writes the ring
     uint32_t cube = 0;
-    for (const BlubBody &b : set) cube = std::max(cube, body_cube_side(b));
+    for (size_t i = 0; i < set.size(); ++i)
+        cube = std::max(cube, meshes.empty() || meshes[i].vertices.empty() ? body_cube_side(set[i]) : mesh_body_cube_side(set[i].half_extent, meshes[i].mid));
+    free_mesh_bodies();
+    if (!meshes.empty()) {
+        std::vector<MeshBodyDev> info(BODIES_MAX, MeshBodyDev{});
+        std::vector<float> vb;
+        std::vector<uint32_t> idx;
+        for (size_t i = 0; i < meshes.size(); ++i) {
+            const MeshBodyHost &m = meshes[i];
+            MeshBodyDev &d = info[i];
+            d.first_vertex = (uint32_t)(vb.size() / 3);
+            d.first_triangle = (uint32_t)(idx.size() / 3);
+            d.num_vertices = (uint32_t)(m.vertices.size() / 3);
+            d.num_triangles = (uint32_t)(m.indices.size() / 3);
+            d.mass = m.props.mass;
+            for (int k = 0; k < 3; ++k) d.inertia[k] = m.props.moments[k], d.mid[k] = m.mid[k];
+            vb.insert(vb.end(), m.vertices.begin(), m.vertices.end());
+            for (uint32_t v : m.indices) idx.push_back(d.first_vertex + v);
+            mesh_.max_vertices = std::max(mesh_.max_vertices, d.num_vertices);
+            mesh_.max_triangles = std::max(mesh_.max_triangles, d.num_triangles);
+        }
+        mesh_.words = (cube + 31) / 32;
+        const size_t bit_words = set.size() * (size_t)cube * cube * mesh_.words;
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.info, BODIES_MAX * sizeof(MeshBodyDev)));
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.body_vertices, vb.size() * sizeof(float)));
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.grid_vertices, vb.size() * sizeof(float)));
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.indices, idx.size() * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.bits, bit_words * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&mesh_.origin, BODIES_MAX * 3 * sizeof(int)));
+        BLUB_CUDA_CHECK(cudaMemset(mesh_.origin, 0, BODIES_MAX * 3 * sizeof(int)));
+        BLUB_CUDA_CHECK(cudaMemcpy(mesh_.info, info.data(), BODIES_MAX * sizeof(MeshBodyDev), cudaMemcpyHostToDevice));
+        BLUB_CUDA_CHECK(cudaMemcpy(mesh_.body_vertices, vb.data(), vb.size() * sizeof(float), cudaMemcpyHostToDevice));
+        BLUB_CUDA_CHECK(cudaMemcpy(mesh_.indices, idx.data(), idx.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        BLUB_CUDA_CHECK(cudaMemset(mesh_.bits, 0, bit_words * sizeof(uint32_t)));
+        mesh_bodies_ = std::move(meshes);
+    }
     if (!set.empty()) {
         const size_t ring_bytes = (size_t)BODIES_MAX * BODY_HISTORY_LENGTH * sizeof(BlubBodyRecord);
         if (!bodies_dev_) {
@@ -1038,7 +1143,10 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
     }
     if (!cfg.bodies.empty()) {
         const std::vector<BlubBody> bodies = scene_bodies_grid(cfg);
-        f->set_bodies(bodies.data(), (uint32_t)bodies.size());
+        bool mesh = false;
+        for (const SceneBody &b : cfg.bodies) mesh = mesh || b.shape == 2;
+        if (mesh) f->set_bodies_host(bodies.data(), scene_body_meshes(cfg));
+        else f->set_bodies(bodies.data(), (uint32_t)bodies.size());
     }
     return f;
 }
@@ -1058,6 +1166,18 @@ std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg) {
             b.angular_velocity[k] = s.angular_velocity[k];
         }
         quat_from_euler_deg_wxyz(s.rotation_angles_deg, b.rotation);
+    }
+    return out;
+}
+
+std::vector<HostMesh> scene_body_meshes(const SceneConfig &cfg) {
+    std::vector<HostMesh> out(cfg.bodies.size());
+    for (size_t i = 0; i < out.size(); ++i) {
+        const SceneBody &s = cfg.bodies[i];
+        if (s.shape != 2) continue;
+        out[i].present = true;
+        out[i].scale = s.model_scale / cfg.grid_to_world_scale;
+        read_obj(s.model, out[i].positions, out[i].indices);
     }
     return out;
 }

@@ -137,6 +137,16 @@ void mesh_info(const BlubMesh &m, uint32_t &num_vertices, uint32_t &num_triangle
     num_triangles = m.num_triangles;
 }
 
+int mesh_device(const BlubMesh &m) { return m.device; }
+
+void mesh_download(const BlubMesh &m, std::vector<float> &positions, std::vector<uint32_t> &indices) {
+    positions.resize(3 * (size_t)m.num_vertices);
+    indices.resize(3 * (size_t)m.num_triangles);
+    BLUB_CUDA_CHECK(cudaSetDevice(m.device));
+    if (m.num_vertices) BLUB_CUDA_CHECK(cudaMemcpy(positions.data(), m.positions, positions.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    if (m.num_triangles) BLUB_CUDA_CHECK(cudaMemcpy(indices.data(), m.indices, indices.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+}
+
 void mesh_destroy(BlubMesh *m) {
     if (!m) return;
     if (m->positions) cudaFree(m->positions);

@@ -223,13 +223,22 @@ SceneConfig parse_scene_file(const std::string &path) {
             if (o.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.bodies` entry is not an object");
             SceneBody b;
             const JsonValue &shape = need(o, "shape");
-            if (shape.kind != JsonValue::String || (shape.string != "box" && shape.string != "sphere"))
-                throw std::runtime_error("scene JSON: `bodies.shape` must be \"box\" or \"sphere\"");
-            b.shape = shape.string == "sphere" ? 1 : 0;
+            if (shape.kind != JsonValue::String || (shape.string != "box" && shape.string != "sphere" && shape.string != "mesh"))
+                throw std::runtime_error("scene JSON: `bodies.shape` must be \"box\", \"sphere\" or \"mesh\"");
+            b.shape = shape.string == "mesh" ? 2 : shape.string == "sphere" ? 1 : 0;
             vec3(need(o, "position"), "bodies.position", b.position);
-            const JsonValue &ext = need(o, "half_extent"); // a sphere's radius: a number, or {x, y, z} with the radius in x
-            if (ext.kind == JsonValue::Number) b.half_extent[0] = b.half_extent[1] = b.half_extent[2] = num_f32(ext, "bodies.half_extent");
-            else vec3(ext, "bodies.half_extent", b.half_extent);
+            if (b.shape == 2) { // a closed OBJ mesh: its path relative to the scene file's directory, scale in world units per model unit
+                const JsonValue &model = need(o, "model");
+                if (model.kind != JsonValue::String || model.string.empty()) throw std::runtime_error("scene JSON: `bodies.model` is not a path");
+                const size_t slash = path.find_last_of('/');
+                b.model = model.string[0] == '/' || slash == std::string::npos ? model.string : path.substr(0, slash + 1) + model.string;
+                b.model_scale = num_f32(need(o, "scale"), "bodies.scale");
+                for (float &h : b.half_extent) h = 0.0f;
+            } else {
+                const JsonValue &ext = need(o, "half_extent"); // a sphere's radius: a number, or {x, y, z} with the radius in x
+                if (ext.kind == JsonValue::Number) b.half_extent[0] = b.half_extent[1] = b.half_extent[2] = num_f32(ext, "bodies.half_extent");
+                else vec3(ext, "bodies.half_extent", b.half_extent);
+            }
             b.relative_density = num_f32(need(o, "relative_density"), "bodies.relative_density");
             if (const JsonValue *v = o.get("rotation_angles_deg")) vec3(*v, "bodies.rotation_angles_deg", b.rotation_angles_deg);
             if (const JsonValue *v = o.get("velocity")) vec3(*v, "bodies.velocity", b.velocity);
@@ -238,8 +247,15 @@ SceneConfig parse_scene_file(const std::string &path) {
         }
         try {
             const std::vector<BlubBody> grid = scene_bodies_grid(cfg);
-            make_body_set(cfg.grid_dimension, grid.data(), (uint32_t)grid.size(), false);
-        } catch (const std::invalid_argument &e) {
+            bool mesh = false;
+            for (const SceneBody &b : cfg.bodies) mesh = mesh || b.shape == 2;
+            if (!mesh) make_body_set(cfg.grid_dimension, grid.data(), (uint32_t)grid.size(), false);
+            else {
+                if (grid.size() > (size_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
+                std::vector<BlubBody> set;
+                make_mesh_body_set(cfg.grid_dimension, grid.data(), scene_body_meshes(cfg), set);
+            }
+        } catch (const std::exception &e) {
             throw std::runtime_error(std::string("scene JSON: `fluid.bodies`: ") + e.what());
         }
     }

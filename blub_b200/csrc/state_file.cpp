@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <cerrno>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 
@@ -23,14 +24,16 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters; version 4:
 // section 14 followed by the sources' particle tags (written only when one of them is not 0).  Version 3 is not a format: no build writes
 // it and readers refuse it.  Version 8: a fluid with floating bodies; the version-4 layout (section 14 may describe an empty flow set) plus
-// section 15, the bodies.  Versions 3, 5, 6 and 7 are not formats either.
-constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8;
-constexpr uint32_t kNumSections = 15; // at most
+// section 15, the bodies.  Versions 3, 5, 6 and 7 are not formats either.  Version 16: a fluid with at least one mesh body; the version-8
+// layout plus section 16, the mesh bodies' geometry and mass properties (its length is what the file holds beyond section 15).
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16;
+constexpr uint32_t kNumSections = 16; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
-    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES
+    SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
+    SEC_MESH_BODIES
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -54,6 +57,16 @@ struct BodySection {
     BlubBody body[16];
 };
 static_assert(sizeof(BodySection) == 1156 && BODIES_MAX == 16, "body section layout");
+// Section 16 (version 16): u32 num_mesh_bodies, u32 reserved, then per mesh body in body order this record followed by its float32 body-frame
+// vertices (3 per vertex) and its uint32 indices (3 per triangle, into its own vertices)
+struct MeshBodyRecordHead {
+    uint32_t body, num_vertices, num_triangles, reserved;
+    float mass, moments[3];           // as stored: the integrator's m and I_b
+    float bounds_lo[3], bounds_hi[3]; // body-frame bounds
+    float scale, reserved2;
+    double volume, centroid[3], principal_moments[3], principal_rotation[4], inertia[9];
+};
+static_assert(sizeof(MeshBodyRecordHead) == 224, "mesh body record layout");
 
 struct StateHeader {
     char magic[8];
@@ -95,9 +108,9 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
                                      {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
-                                     {SEC_BODIES, sizeof(BodySection)}};
+                                     {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}}; // section 16: the file's remaining bytes
     std::memcpy(out, s, sizeof(s));
-    return h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
+    return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -170,9 +183,9 @@ StateHeader read_header(File &f) {
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
-        h.format_version != kFormatVersionBodies)
+        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4 and 8)");
+                         " is not supported (this library reads versions 1, 2, 4, 8 and 16)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -193,13 +206,24 @@ StateHeader read_header(File &f) {
                          std::to_string(ns));
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
-    if (size != total)
+    // version 16: section 16 holds at least its count and one mesh body record
+    if (ns == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
         throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
 }
 
 // Reads one section whose id and length must be `s`, in chunks of at most one staging half; sink(slot, data, bytes, offset) receives
 // every chunk (it must be done with the half `slot` before that half's event is waited on again), then the CRC is checked.
+// the length of section 16 when the file has one: what the file holds beyond section 15, its head and its CRC
+uint64_t mesh_section_length(File &f, const StateHeader &h) {
+    if (h.format_version != kFormatVersionMeshBodies) return 0;
+    Section sec[kNumSections];
+    expected_sections(h, sec);
+    uint64_t total = sizeof(StateHeader);
+    for (uint32_t k = 0; k < 15; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
+    return f.size() - total - sizeof(SectionHead) - 4;
+}
+
 template <class Sink> void read_section(File &f, const Section &s, Staging &st, Sink sink) {
     SectionHead head;
     f.read(&head, sizeof(head));
@@ -253,9 +277,9 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
 }
 
 // The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.  tags: the sources'
-// particle tags (version 4), or nullptr.  Version 8 may describe an empty set.
+// particle tags (version 4), or nullptr.  Versions 8 and 16 may describe an empty set.
 FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHeader &h, const std::string &path) {
-    if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version != kFormatVersionBodies))
+    if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version < kFormatVersionBodies))
         throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
     std::vector<BlubFluidSource> src(fl.num_sources);
     std::vector<BlubFluidDrain> drn(fl.num_drains);
@@ -297,6 +321,91 @@ std::vector<BlubBody> body_set_of(const BodySection &bs, const StateHeader &h, c
     }
 }
 
+// Version 16: the bodies of section 15 with the mesh bodies of section 16 (bytes), kept bit for bit.  A mesh body's placement is checked as
+// set_bodies checks a body (bounding box within 1e-3 of [1, dim - 1], on the box centred on c + R mid), its record for sizes, index ranges,
+// finite values, positive mass and moments, bounds at least 1 cell thick that match its vertices and its half extents.
+std::vector<BlubBody> mesh_body_set_of(const BodySection &bs, const std::vector<char> &bytes, const StateHeader &h, const std::string &path,
+                                       std::vector<MeshBodyHost> &meshes) {
+    auto bad = [&](const std::string &what) { return ParseError(path + ": section 16: " + what); };
+    if (bs.num_bodies == 0 || bs.num_bodies > 16) throw ParseError(path + ": section 15 must hold 1 to 16 bodies");
+    uint32_t count = 0;
+    std::memcpy(&count, bytes.data(), 4);
+    if (count == 0) throw bad("a version-16 file holds at least one mesh body");
+    size_t off = 8;
+    meshes.assign(bs.num_bodies, MeshBodyHost{});
+    size_t vertices = 0, triangles = 0;
+    for (uint32_t r = 0; r < count; ++r) {
+        MeshBodyRecordHead m;
+        if (bytes.size() - off < sizeof(m)) throw bad("truncated record");
+        std::memcpy(&m, bytes.data() + off, sizeof(m));
+        off += sizeof(m);
+        if (m.body >= bs.num_bodies || bs.body[m.body].shape != 2 || !meshes[m.body].vertices.empty())
+            throw bad("a record names no mesh body of section 15, or one twice");
+        if (m.num_vertices == 0 || m.num_triangles == 0 || m.num_vertices > (uint32_t)BLUB_MESH_BODY_MAX_VERTICES ||
+            m.num_triangles > (uint32_t)BLUB_MESH_BODY_MAX_TRIANGLES)
+            throw bad("vertex or triangle count out of range");
+        vertices += m.num_vertices;
+        triangles += m.num_triangles;
+        const size_t need = 12ull * m.num_vertices + 12ull * m.num_triangles;
+        if (bytes.size() - off < need) throw bad("truncated geometry");
+        MeshBodyHost &host = meshes[m.body];
+        host.vertices.resize(3ull * m.num_vertices);
+        host.indices.resize(3ull * m.num_triangles);
+        std::memcpy(host.vertices.data(), bytes.data() + off, 12ull * m.num_vertices);
+        std::memcpy(host.indices.data(), bytes.data() + off + 12ull * m.num_vertices, 12ull * m.num_triangles);
+        off += need;
+        for (uint32_t v : host.indices)
+            if (v >= m.num_vertices) throw bad("an index is out of range");
+        float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+        for (size_t k = 0; k < host.vertices.size(); ++k) {
+            if (!std::isfinite(host.vertices[k])) throw bad("a vertex is not finite");
+            lo[k % 3] = std::min(lo[k % 3], host.vertices[k]);
+            hi[k % 3] = std::max(hi[k % 3], host.vertices[k]);
+        }
+        BlubMeshBodyProperties &p = host.props;
+        p.volume = m.volume;
+        std::memcpy(p.centroid, m.centroid, sizeof(p.centroid));
+        std::memcpy(p.inertia, m.inertia, sizeof(p.inertia));
+        std::memcpy(p.principal_moments, m.principal_moments, sizeof(p.principal_moments));
+        std::memcpy(p.principal_rotation, m.principal_rotation, sizeof(p.principal_rotation));
+        p.mass = m.mass;
+        p.scale = m.scale;
+        p.num_vertices = m.num_vertices;
+        p.num_triangles = m.num_triangles;
+        bool ok = std::isfinite(m.mass) && m.mass > 0.0f && std::isfinite(m.scale) && m.scale > 0.0f && m.volume > 0.0;
+        for (int k = 0; k < 3; ++k) {
+            p.moments[k] = m.moments[k];
+            p.bounds_lo[k] = m.bounds_lo[k];
+            p.bounds_hi[k] = m.bounds_hi[k];
+            ok = ok && std::isfinite(m.moments[k]) && m.moments[k] > 0.0f && m.bounds_lo[k] == lo[k] && m.bounds_hi[k] == hi[k] &&
+                 hi[k] - lo[k] >= 1.0f && bs.body[m.body].half_extent[k] == 0.5f * (hi[k] - lo[k]);
+            host.mid[k] = 0.5f * (lo[k] + hi[k]);
+        }
+        if (!ok) throw bad("a mass, moment, scale or bound is out of range or does not match the vertices");
+    }
+    if (off != bytes.size()) throw bad("bytes beyond the last record");
+    if (vertices > (size_t)BLUB_MESH_BODY_MAX_VERTICES || triangles > (size_t)BLUB_MESH_BODY_MAX_TRIANGLES) throw bad("over the vertex or triangle limit");
+    std::vector<BlubBody> set(bs.body, bs.body + bs.num_bodies);
+    for (uint32_t i = 0; i < bs.num_bodies; ++i) {
+        const bool mesh = set[i].shape == 2;
+        if (mesh != !meshes[i].vertices.empty()) throw bad("a mesh body of section 15 has no record");
+        BlubBody b = set[i];
+        if (mesh) b.shape = 0, b.half_extent[0] = b.half_extent[1] = b.half_extent[2] = 1.0f; // its shape was checked above
+        try {
+            make_body_set(mesh ? nullptr : h.grid_dimension, &b, 1, true); // a mesh body's box is checked below
+        } catch (const std::invalid_argument &e) {
+            throw ParseError(path + ": section 15: " + e.what());
+        }
+        if (!mesh) continue;
+        float e[3], o[3];
+        mesh_body_box(set[i], meshes[i].mid, e, o);
+        for (int k = 0; k < 3; ++k)
+            if (set[i].centre[k] + o[k] - e[k] < 1.0f - 1e-3f || set[i].centre[k] + o[k] + e[k] > (float)h.grid_dimension[k] - 1.0f + 1e-3f)
+                throw ParseError(path + ": section 15: a body's bounding box leaves [1, dim - 1]");
+    }
+    return set;
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
@@ -311,10 +420,16 @@ StateInfo read_state_info(const std::string &path) {
         read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
         flow_set_of(fl.flow, fl.source_tags, h, f.path);
     }
-    if (ns == 15) {
+    if (ns >= 15) {
         BodySection bs{};
         read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
-        body_set_of(bs, h, f.path);
+        if (ns == 15) body_set_of(bs, h, f.path);
+        else {
+            std::vector<char> bytes(mesh_section_length(f, h));
+            read_section(f, {SEC_MESH_BODIES, bytes.size()}, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(bytes.data() + off, data, n); });
+            std::vector<MeshBodyHost> meshes;
+            mesh_body_set_of(bs, bytes, h, f.path, meshes);
+        }
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -336,7 +451,7 @@ void HybridFluid::save_state(const std::string &path) {
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
     const bool with_bodies = num_bodies_ > 0;
-    h.format_version = with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    h.format_version = has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -355,7 +470,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = with_bodies ? 15 : flow_active_ ? 14 : 13;
+    h.num_sections = has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13;
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -406,6 +521,39 @@ void HybridFluid::save_state(const std::string &path) {
             BodySection bs{};
             bs.num_bodies = bodies(bs.body, BODIES_MAX);
             write_host_section(f, SEC_BODIES, &bs, sizeof(bs));
+        }
+        if (has_mesh_bodies()) {
+            std::vector<char> bytes(8, 0);
+            uint32_t count = 0;
+            for (const MeshBodyHost &m : mesh_bodies_) count += m.vertices.empty() ? 0 : 1;
+            std::memcpy(bytes.data(), &count, 4);
+            for (uint32_t i = 0; i < (uint32_t)mesh_bodies_.size(); ++i) {
+                const MeshBodyHost &m = mesh_bodies_[i];
+                if (m.vertices.empty()) continue;
+                const BlubMeshBodyProperties &p = m.props;
+                MeshBodyRecordHead r{};
+                r.body = i;
+                r.num_vertices = (uint32_t)(m.vertices.size() / 3);
+                r.num_triangles = (uint32_t)(m.indices.size() / 3);
+                r.mass = p.mass;
+                r.scale = p.scale;
+                r.volume = p.volume;
+                for (int k = 0; k < 3; ++k) {
+                    r.moments[k] = p.moments[k];
+                    r.bounds_lo[k] = p.bounds_lo[k];
+                    r.bounds_hi[k] = p.bounds_hi[k];
+                    r.centroid[k] = p.centroid[k];
+                    r.principal_moments[k] = p.principal_moments[k];
+                }
+                std::memcpy(r.principal_rotation, p.principal_rotation, sizeof(r.principal_rotation));
+                std::memcpy(r.inertia, p.inertia, sizeof(r.inertia));
+                const char *rb = reinterpret_cast<const char *>(&r);
+                bytes.insert(bytes.end(), rb, rb + sizeof(r));
+                const char *vb = reinterpret_cast<const char *>(m.vertices.data()), *ib = reinterpret_cast<const char *>(m.indices.data());
+                bytes.insert(bytes.end(), vb, vb + m.vertices.size() * sizeof(float));
+                bytes.insert(bytes.end(), ib, ib + m.indices.size() * sizeof(uint32_t));
+            }
+            write_host_section(f, SEC_MESH_BODIES, bytes.data(), bytes.size());
         }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
@@ -470,10 +618,17 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
         if (fs.num_sources + fs.num_drains > 0) x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
     }
-    if (ns == 15) { // the history ring is not state: a loaded fluid starts with an empty one
+    if (ns >= 15) { // the history ring is not state: a loaded fluid starts with an empty one
         BodySection bs{};
         to_host(sec[14], &bs);
-        x.restore_bodies(body_set_of(bs, h, f.path));
+        if (ns == 15) x.restore_bodies(body_set_of(bs, h, f.path));
+        else {
+            std::vector<char> bytes(mesh_section_length(f, h));
+            to_host({SEC_MESH_BODIES, bytes.size()}, bytes.data());
+            std::vector<MeshBodyHost> meshes;
+            const std::vector<BlubBody> set = mesh_body_set_of(bs, bytes, h, f.path, meshes);
+            x.restore_bodies(set, std::move(meshes));
+        }
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

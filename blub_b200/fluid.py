@@ -143,7 +143,9 @@ class Body(C.Structure):
     def from_dict(cls, d):
         b = cls()
         shape = d.get("shape", "box")
-        b.shape = {"box": 0, "sphere": 1}.get(shape, shape) if isinstance(shape, str) else int(shape)
+        if isinstance(shape, str) and shape not in ("box", "sphere", "mesh"):
+            raise BlubError(f"body shape {shape!r}: must be \"box\", \"sphere\" or \"mesh\"")
+        b.shape = {"box": 0, "sphere": 1, "mesh": 2}[shape] if isinstance(shape, str) else int(shape)
         ext = d["half_extent"]
         b.half_extent[:] = [float(ext)] * 3 if np.ndim(ext) == 0 else [float(v) for v in ext]
         b.relative_density = float(d["relative_density"])
@@ -154,9 +156,57 @@ class Body(C.Structure):
         return b
 
     def to_dict(self):
-        return {"shape": "sphere" if self.shape == 1 else "box", "half_extent": tuple(self.half_extent), "relative_density": self.relative_density,
+        return {"shape": {1: "sphere", 2: "mesh"}.get(self.shape, "box"), "half_extent": tuple(self.half_extent), "relative_density": self.relative_density,
                 "centre": tuple(self.centre), "rotation": tuple(self.rotation), "velocity": tuple(self.velocity),
                 "angular_velocity": tuple(self.angular_velocity)}
+
+
+class MeshBodyProperties(C.Structure):
+    """BlubMeshBodyProperties: a mesh body's volume, centre of mass, inertia, principal frame and body-frame bounds (DESIGN.md §8)."""
+
+    _fields_ = [("volume", C.c_double), ("centroid", C.c_double * 3), ("inertia", C.c_double * 9), ("principal_moments", C.c_double * 3),
+                ("principal_rotation", C.c_double * 4), ("bounds_lo", C.c_float * 3), ("bounds_hi", C.c_float * 3), ("mass", C.c_float),
+                ("moments", C.c_float * 3), ("scale", C.c_float), ("num_vertices", C.c_uint32), ("num_triangles", C.c_uint32)]
+
+    def to_dict(self):
+        out = {name: getattr(self, name) for name in ("volume", "mass", "scale", "num_vertices", "num_triangles")}
+        for name in ("centroid", "principal_moments", "principal_rotation", "bounds_lo", "bounds_hi", "moments"):
+            out[name] = tuple(getattr(self, name))
+        out["inertia"] = np.array(list(self.inertia)).reshape(3, 3)
+        return out
+
+
+class MeshBodyShape(C.Structure):
+    _fields_ = [("mesh", C.c_void_p), ("scale", C.c_float)]
+
+
+def quat_matrix(q):
+    """The float64 rotation matrix of the quaternion q = (w, x, y, z)."""
+    w, x, y, z = [float(v) for v in q]
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                     [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                     [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+
+
+def mesh_body_properties(positions, triangles, scale):
+    """blub_mesh_body_properties (host only): checks a closed mesh and returns its mass properties and principal frame as a dict (mass and
+    moments for relative density 1).  Raises BlubError on a mesh a mesh body cannot take."""
+    pos = np.ascontiguousarray(positions, dtype=np.float32).reshape(-1, 3)
+    idx = np.ascontiguousarray(triangles, dtype=np.uint32).reshape(-1)
+    p = MeshBodyProperties()
+    _check(lib().blub_mesh_body_properties(pos.ctypes.data_as(C.c_void_p), pos.shape[0], idx.ctypes.data_as(C.c_void_p), idx.shape[0], float(scale),
+                                           C.byref(p)))
+    return p.to_dict()
+
+
+def mesh_body_vertices(positions, triangles, scale):
+    """blub_mesh_body_vertices (host only): the float32 body-frame vertices [n, 3] a mesh body of this mesh and scale stores."""
+    pos = np.ascontiguousarray(positions, dtype=np.float32).reshape(-1, 3)
+    idx = np.ascontiguousarray(triangles, dtype=np.uint32).reshape(-1)
+    out = np.zeros_like(pos)
+    _check(lib().blub_mesh_body_vertices(pos.ctypes.data_as(C.c_void_p), pos.shape[0], idx.ctypes.data_as(C.c_void_p), idx.shape[0], float(scale),
+                                         out.ctypes.data_as(C.c_void_p)))
+    return out
 
 
 class BodyRecord(C.Structure):
@@ -243,6 +293,11 @@ def lib():
         "blub_fluid_body_history": (C.c_int, [vp, u32, C.POINTER(BodyRecord), u32, C.POINTER(u32)]),
         "blub_fluid_bodies": (C.c_int, [vp, C.POINTER(Body), u32, C.POINTER(u32)]),
         "blub_scene_bodies": (C.c_int, [C.c_char_p, C.POINTER(Body), u32, C.POINTER(u32)]),
+        "blub_mesh_body_properties": (C.c_int, [vp, u32, vp, u32, C.c_float, C.POINTER(MeshBodyProperties)]),
+        "blub_mesh_body_vertices": (C.c_int, [vp, u32, vp, u32, C.c_float, vp]),
+        "blub_fluid_set_bodies_meshes":(C.c_int, [vp, C.POINTER(Body), C.POINTER(MeshBodyShape), u32]),
+        "blub_fluid_body_mass_properties": (C.c_int, [vp, u32, C.POINTER(MeshBodyProperties)]),
+        "blub_scene_body_model": (C.c_int, [C.c_char_p, u32, C.c_char_p, C.c_size_t, C.POINTER(C.c_float)]),
         "blub_last_error": (C.c_char_p, []),
         "blub_version": (C.c_char_p, []),
         "blub_scene_load": (C.c_int, [C.POINTER(vp), C.c_char_p, C.c_int, vp]),
@@ -400,6 +455,14 @@ def scene_bodies(path):
     return [b.to_dict() for b in arr[:min(count.value, BODIES_MAX)]]
 
 
+def scene_body_model(path, body):
+    """(resolved OBJ path, scale in cells per model unit) of the scene's mesh body `body` (host only)."""
+    buf = C.create_string_buffer(4096)
+    scale = C.c_float(0.0)
+    _check(lib().blub_scene_body_model(os.fsencode(path), int(body), buf, len(buf), C.byref(scale)))
+    return buf.value.decode(), scale.value
+
+
 def state_info(path):
     """Validates a state file written by HybridFluid.save_state (host only) and returns its StateInfo."""
     info = StateInfo()
@@ -414,6 +477,7 @@ class HybridFluid:
 
     def __init__(self, nx, ny, nz, max_num_particles, device=0, cuda_stream=None, _handle=None):
         self.L = lib()
+        self.device = device
         if _handle is None:
             h = C.c_void_p()
             _check(self.L.blub_fluid_create(C.byref(h), nx, ny, nz, max_num_particles, device, cuda_stream))
@@ -456,7 +520,7 @@ class HybridFluid:
         L = lib()
         h = C.c_void_p()
         _check(L.blub_scene_load(C.byref(h), os.fsencode(path), device, cuda_stream))
-        return cls(0, 0, 0, 0, _handle=h)
+        return cls(0, 0, 0, 0, device=device, _handle=h)
 
     @classmethod
     def from_state(cls, path, device=0, cuda_stream=None):
@@ -465,7 +529,7 @@ class HybridFluid:
         L = lib()
         h = C.c_void_p()
         _check(L.blub_fluid_load_state(C.byref(h), os.fsencode(path), device, cuda_stream))
-        return cls(0, 0, 0, 0, _handle=h)
+        return cls(0, 0, 0, 0, device=device, _handle=h)
 
     def save_state(self, path):
         """Waits for the enqueued steps, then writes everything a later step depends on to `path` (atomically)."""
@@ -668,11 +732,40 @@ class HybridFluid:
         """Replaces the floating bodies: dicts {"shape": "box" | "sphere", "half_extent": (hx, hy, hz) or a radius, "relative_density",
         "centre", "rotation" (w, x, y, z; default identity), "velocity", "angular_velocity"} in grid cells, cells/s and rad/s (at most 16).
         Resets the history; an empty list clears the set.  Raises BlubError (and changes nothing) on a body that breaks a rule of
-        blub_fluid_set_bodies, z-slab ranks and a fluid inside a step."""
+        blub_fluid_set_bodies, z-slab ranks and a fluid inside a step.
+        A mesh body is {"shape": "mesh", "mesh": Mesh or (positions [n, 3], triangles [m, 3]), "scale": cells per model unit, "relative_density",
+        "centre", "rotation", ...}: centre and rotation place the mesh's model origin and axes (DESIGN.md §8 "Mesh bodies"); it goes through
+        blub_fluid_set_bodies_meshes, which also refuses what blub_mesh_body_properties refuses."""
         arr = (Body * max(len(bodies), 1))()
+        shapes = (MeshBodyShape * max(len(bodies), 1))()
+        keep = []  # meshes made here live until the set has copied them
         for k, b in enumerate(bodies):
-            arr[k] = b if isinstance(b, Body) else Body.from_dict(b)
-        _check(self.L.blub_fluid_set_bodies(self.h, arr, len(bodies)))
+            if not isinstance(b, Body) and b.get("mesh") is not None:
+                m = b["mesh"]
+                if not isinstance(m, Mesh):
+                    m = Mesh(m[0], m[1], device=self.device)
+                keep.append(m)
+                arr[k] = Body.from_dict(dict(b, shape=2, half_extent=(1.0, 1.0, 1.0)))
+                shapes[k].mesh, shapes[k].scale = m.h, float(b["scale"])
+            else:
+                arr[k] = b if isinstance(b, Body) else Body.from_dict(b)
+        if keep:
+            _check(self.L.blub_fluid_set_bodies_meshes(self.h, arr, shapes, len(bodies)))
+        else:
+            _check(self.L.blub_fluid_set_bodies(self.h, arr, len(bodies)))
+
+    def body_mass_properties(self, body):
+        """The mass properties of mesh body `body` as stored (see mesh_body_properties; mass and moments with its relative density)."""
+        p = MeshBodyProperties()
+        _check(self.L.blub_fluid_body_mass_properties(self.h, int(body), C.byref(p)))
+        return p.to_dict()
+
+    def mesh_body_model_pose(self, body):
+        """(origin, R_model): where the current pose of mesh body `body` puts the mesh's model origin and model axes (R_model maps model
+        to grid coordinates): R_model = R_body R_p^T, origin = c - R_model (scale * centroid), in float64."""
+        b, p = self.bodies()[int(body)], self.body_mass_properties(body)
+        R = quat_matrix(b["rotation"]) @ quat_matrix(p["principal_rotation"]).T
+        return np.asarray(b["centre"], dtype=np.float64) - R @ (float(p["scale"]) * np.asarray(p["centroid"])), R
 
     def bodies(self):
         """The current bodies as dicts (the pose the next step writes).  Synchronises."""

@@ -245,7 +245,7 @@ int blub_load_probe_cells(const uint32_t dim[3], const BlubLoadProbe *probe, uin
  * pose: a bounding box leaving [1, dim - 1] is shifted back and the outward velocity component zeroed (a clamp, not a collision model);
  * bodies do not collide with each other.  The new pose is what the next step writes.  The coupling is explicit: it was measured stable for
  * relative densities 0.5 and 0.75 (a floating box) and 2 (a sinking one); lighter bodies were not measured.  Bodies are state: a fluid with
- * bodies saves format version 8. */
+ * bodies saves format version 8, with a mesh body version 16. */
 #define BLUB_BODIES_MAX 16
 #define BLUB_BODY_HISTORY_LENGTH 1024 /* records per body in the device ring: slot = step % 1024 */
 typedef struct {
@@ -283,6 +283,55 @@ int blub_fluid_bodies(BlubFluid *fluid, BlubBody *out, uint32_t capacity, uint32
 /* The scene's optional fluid.bodies in grid cells and cells/s ((p - world_position) / grid_to_world_scale, Euler angles as for
  * static_objects).  Writes at most `capacity` bodies and sets *count to the number the scene holds.  blub_scene_load sets them. */
 int blub_scene_bodies(const char *scene_json_path, BlubBody *out, uint32_t capacity, uint32_t *count);
+
+/* ---- triangle-mesh bodies (shape 2; rules: DESIGN.md section 8 "Mesh bodies") ------------------------------------------------
+ * A mesh body is a closed, consistently oriented triangle mesh (either winding) scaled by `scale` cells per model unit.  The library moves
+ * it to its body frame: origin at the centre of mass, axes along the principal axes of inertia.  The stored BlubBody has centre = the centre
+ * of mass in the grid, rotation = model rotation * principal rotation and half_extent = (hi - lo) / 2 of the body-frame bounds; mass and
+ * principal moments come from the mesh (float64 on the host, rounded to float32 once).  A mesh body covers the cells whose centre lies
+ * inside the mesh at the body's current pose, filled on the GPU every step by crossing parity along +x.  Self-intersecting meshes are not
+ * detected.  A fluid with a mesh body saves state format version 16 (version 8 plus section 16, the mesh bodies as stored).  The scene key
+ * fluid.bodies takes {shape: "mesh", model: OBJ path relative to the scene file, scale: world units per model unit, position,
+ * rotation_angles_deg?, relative_density, velocity?, angular_velocity?}; position and rotation place the model origin and axes. */
+#define BLUB_MESH_BODY_MAX_VERTICES 262144   /* over all mesh bodies of a set */
+#define BLUB_MESH_BODY_MAX_TRIANGLES 524288  /* over all mesh bodies of a set */
+typedef struct {
+    double volume;                 /* cells^3, > 0 for either winding */
+    double centroid[3];            /* the centre of mass in model units (model frame) */
+    double inertia[9];             /* about the centre of mass per unit body density, cells^5, model axes, row major */
+    double principal_moments[3];   /* per unit body density: the diagonal of the inertia in the principal frame */
+    double principal_rotation[4];  /* unit quaternion (w, x, y, z): principal frame -> model frame, R_p */
+    float bounds_lo[3], bounds_hi[3]; /* body-frame bounding box of the float32 body-frame vertices, cells */
+    float mass;                    /* float32(relative_density * volume) per unit fluid density (relative_density = 1 for blub_mesh_body_properties) */
+    float moments[3];              /* float32(relative_density * principal_moments) */
+    float scale;                   /* cells per model unit */
+    uint32_t num_vertices, num_triangles;
+} BlubMeshBodyProperties;
+typedef struct {
+    const struct BlubMesh *mesh;   /* NULL: the body is a box or sphere (BlubBody.shape 0 / 1) */
+    float scale;                   /* cells per model unit, finite and > 0 */
+} BlubMeshBodyShape;
+/* Host only, no device needed: checks a mesh and computes its mass properties and principal frame.  BLUB_ERR_INVALID_ARGUMENT: no
+ * triangles, num_indices not a multiple of 3, an index out of range, a triangle repeating a vertex, a directed edge occurring other than
+ * exactly once or without its reverse (not closed and consistently oriented), a non-finite position, zero volume, a scale that is not finite
+ * and > 0, a body-frame bounding box thinner than 1 cell on some axis, or more than BLUB_MESH_BODY_MAX_VERTICES / _TRIANGLES. */
+int blub_mesh_body_properties(const float *positions_xyz, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, float scale,
+                              BlubMeshBodyProperties *out);
+/* Host only: the float32 body-frame vertices (xyz, num_vertices of them) a mesh body of this mesh and scale stores: R_p^T (scale p - com).
+ * Refuses what blub_mesh_body_properties refuses. */
+int blub_mesh_body_vertices(const float *positions_xyz, uint32_t num_vertices, const uint32_t *indices, uint32_t num_indices, float scale,
+                            float *out_xyz);
+/* blub_fluid_set_bodies with triangle-mesh bodies: shapes[i].mesh != NULL makes body i a mesh body (bodies[i].shape and half_extent are
+ * ignored; centre and rotation place the mesh's model origin and axes in the grid).  The geometry is copied, so the meshes may be destroyed
+ * afterwards.  Refuses everything blub_fluid_set_bodies refuses (but shape 2 with a mesh), what blub_mesh_body_properties refuses, a mesh on
+ * another device and more than the vertex / triangle limits over the set, changing nothing.  shapes == NULL: blub_fluid_set_bodies. */
+int blub_fluid_set_bodies_meshes(BlubFluid *fluid, const BlubBody *bodies, const BlubMeshBodyShape *shapes, uint32_t num_bodies);
+/* The mass properties of mesh body `body` as stored (mass and moments with its relative density).  A renderer recovers the model pose
+ * from the body's pose: R_model = R_body R_p^T, origin = c - R_model (scale * centroid).  BLUB_ERR_INVALID_ARGUMENT: not a mesh body. */
+int blub_fluid_body_mass_properties(BlubFluid *fluid, uint32_t body, BlubMeshBodyProperties *out);
+/* The resolved OBJ path (NUL-terminated, truncated to capacity - 1) and the scale in cells per model unit of the scene's mesh body `body`.
+ * BLUB_ERR_INVALID_ARGUMENT: not a mesh body of the scene; the scene's own errors as blub_scene_info. */
+int blub_scene_body_model(const char *scene_json_path, uint32_t body, char *model_path_out, size_t capacity, float *scale_out);
 
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every

@@ -159,6 +159,7 @@ def compare_one_step(orc, gpu, robust=False, vox=None, min_contact=(1, 1)):
         report["contact7"] = util.solid_contact(m_o, vox, p_o)
         assert all(c >= lo for c, lo in zip(report["contact7"], min_contact)), (report["contact7"], min_contact)
         report["branches"] = {k: int(branches[k].sum()) for k in ("eaten", "wall", "voxel", "push")}
+        report["advect_ref"] = branches
     gpu.set_particles(np.c_[p_o, np.zeros(npart, np.float32)], orc.particles(O.ARR_ROWX), orc.particles(O.ARR_ROWY), orc.particles(O.ARR_ROWZ))
     gpu.upload_grid(F.TAP_MARKER, orc.grid(O.ARR_MARKER))
     run(9, 10)  # rhs 2
@@ -183,4 +184,5 @@ def compare_one_step(orc, gpu, robust=False, vox=None, min_contact=(1, 1)):
         report["correct"] = particles_close(p_o[~flips], p_g[~flips], "corrected positions", 2e-4)
         report["correct_flips"] = int(flips.sum())
         report["correct_hits"] = {k: int(corr[k].sum()) for k in ("wall", "marker")}
+        report["correct_ref"] = corr
     return report

@@ -25,8 +25,11 @@ __device__ __forceinline__ float signf(float x) { return x > 0.0f ? 1.0f : (x < 
 // All grid passes work on the 1-bit-per-cell FLUID mask (FluidBits, rebuilt with every finished marker volume): one thread per 32-cell
 // word of a row decides from a handful of mask words whether any of its cells has anything to do (in a dam break ~85 % of the words
 // have not), then the WARP walks the words that have, lane = cell, so that the loads and stores of a word are coalesced.  Cells that
-// are more than one cell away from every FLUID cell are not visited at all: nothing reads their faces (P2G rewrites every face a
-// particle can reach, the extrapolation fills the one-cell ring G2P can reach), the reference leaves them stale as well (SURVEY B6).
+// are more than one cell away from every FLUID cell are not visited at all: the reference's full-grid passes write 0 there, and no
+// particle in a FLUID cell reads them (the extrapolation fills the one-cell ring G2P can reach).  With a solid volume a particle can sit
+// in a SOLID cell: an eaten one is moved one cell before G2P and reads faces up to two cells from its own, one left in a solid by the
+// advection's push reads faces one cell from its own in the correction.  So the projection also visits the cells within two cells of a
+// SOLID cell that holds a particle, the position change those within one (near_stray_word), and writes there what the reference writes.
 __device__ __forceinline__ unsigned fbits(const GridDim &g, const FluidBits &b, int xw, int y, int z) {
     if (xw < 0 || xw >= b.wpr || y < 0 || y >= g.ny || z < 0 || z >= g.nz) return 0u;
     return __ldg(b.words + (z * g.ny + y) * b.wpr + xw);
@@ -56,6 +59,27 @@ __device__ __forceinline__ unsigned near_fluid_word(const GridDim &g, const Flui
         for (int dy = -1; dy <= 1; ++dy) {
             const unsigned f = fbits(g, b, p.xw, p.y + dy, p.z + dz);
             near |= f | (f << 1) | (f >> 1) | (fbits(g, b, p.xw - 1, p.y + dy, p.z + dz) >> 31) | (fbits(g, b, p.xw + 1, p.y + dy, p.z + dz) << 31);
+        }
+    return near & cells_mask(p);
+}
+// SOLID cells that hold a particle (particle words of the last marker pass minus the FLUID bits), dilated by R cells in every dimension
+__device__ __forceinline__ unsigned stray_bits(const GridDim &g, const FluidBits &b, const uint32_t *__restrict__ pw, int xw, int y, int z) {
+    if (xw < 0 || xw >= b.wpr || y < 0 || y >= g.ny || z < 0 || z >= g.nz) return 0u;
+    const int w = (z * g.ny + y) * b.wpr + xw;
+    return __ldg(pw + w) & ~__ldg(b.words + w);
+}
+template <int R>
+__device__ __forceinline__ unsigned near_stray_word(const GridDim &g, const FluidBits &b, const uint32_t *__restrict__ pw, const WordPos &p) {
+    unsigned near = 0;
+#pragma unroll
+    for (int dz = -R; dz <= R; ++dz)
+#pragma unroll
+        for (int dy = -R; dy <= R; ++dy) {
+            const unsigned s = stray_bits(g, b, pw, p.xw, p.y + dy, p.z + dz);
+            const unsigned l = stray_bits(g, b, pw, p.xw - 1, p.y + dy, p.z + dz), r = stray_bits(g, b, pw, p.xw + 1, p.y + dy, p.z + dz);
+            near |= s;
+#pragma unroll
+            for (int k = 1; k <= R; ++k) near |= (s << k) | (s >> k) | (l >> (32 - k)) | (r << (32 - k));
         }
     return near & cells_mask(p);
 }
@@ -100,12 +124,14 @@ __global__ void __launch_bounds__(PT) divergence_compute_kernel(GridDim g, Fluid
     });
 }
 
-// divergence_remove.comp:19-49, on the cells within one cell of the fluid
+// divergence_remove.comp:19-49, on the cells within one cell of the fluid and (pw: particle words, with a solid volume) within two
+// cells of a SOLID cell that holds a particle
 __global__ void __launch_bounds__(PT) divergence_remove_kernel(GridDim g, FluidBits b, const int8_t *__restrict__ marker,
                                                                const float *__restrict__ p, const uint2 *__restrict__ vox,
-                                                               float *__restrict__ ux, float *__restrict__ uy, float *__restrict__ uz) {
+                                                               const uint32_t *__restrict__ pw, float *__restrict__ ux, float *__restrict__ uy,
+                                                               float *__restrict__ uz) {
     const WordPos wp = word_of_thread(g, b);
-    const unsigned todo = wp.inside ? near_fluid_word(g, b, wp) : 0u;
+    const unsigned todo = wp.inside ? (near_fluid_word(g, b, wp) | (pw != nullptr ? near_stray_word<2>(g, b, pw, wp) : 0u)) : 0u;
     warp_walk(g, todo, wp, [&](unsigned on, int x, int y, int z, int) {
         if (!on) return;
         const int i = lin(g, x, y, z);
@@ -137,12 +163,13 @@ __global__ void __launch_bounds__(PT) divergence_remove_kernel(GridDim g, FluidB
 }
 
 // density_projection_position_change.comp:18-51 (writes the displacement field INTO the velocity volumes), on the cells within one
-// cell of the fluid
+// cell of the fluid and (pw: particle words, with a solid volume) within one cell of a SOLID cell that holds a particle
 __global__ void __launch_bounds__(PT) position_change_kernel(GridDim g, FluidBits b, const StepParams *__restrict__ params,
                                                              const int8_t *__restrict__ marker, const float *__restrict__ p,
-                                                             float *__restrict__ ux, float *__restrict__ uy, float *__restrict__ uz) {
+                                                             const uint32_t *__restrict__ pw, float *__restrict__ ux, float *__restrict__ uy,
+                                                             float *__restrict__ uz) {
     const WordPos wp = word_of_thread(g, b);
-    const unsigned todo = wp.inside ? near_fluid_word(g, b, wp) : 0u;
+    const unsigned todo = wp.inside ? (near_fluid_word(g, b, wp) | (pw != nullptr ? near_stray_word<1>(g, b, pw, wp) : 0u)) : 0u;
     const float dt = params->dt;
     warp_walk(g, todo, wp, [&](unsigned on, int x, int y, int z, int) {
         if (!on) return;
@@ -517,8 +544,9 @@ void launch_divergence_compute(cudaStream_t st, const GridDim &g, const FluidBit
     BLUB_LAUNCH(divergence_compute_kernel, word_blocks(g, bits), PT, 0, st, g, bits, marker, u[0], u[1], u[2], vox, rhs);
 }
 
-void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox, float *const u[3]) {
-    BLUB_LAUNCH(divergence_remove_kernel, word_blocks(g, bits), PT, 0, st, g, bits, marker, p, vox, u[0], u[1], u[2]);
+void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox,
+                              const uint32_t *particle_words, float *const u[3]) {
+    BLUB_LAUNCH(divergence_remove_kernel, word_blocks(g, bits), PT, 0, st, g, bits, marker, p, vox, particle_words, u[0], u[1], u[2]);
 }
 
 void launch_extrapolate(cudaStream_t st, const GridDim &g, const FluidBits &bits, float *const u[3]) {
@@ -541,8 +569,9 @@ void launch_advect_migrate(cudaStream_t st, const GridDim &g, const StepParams *
     BLUB_LAUNCH(advect_kernel<true>, particle_blocks(np_upper), PT, 0, st, g, params, pos, row[0], row[1], row[2], u[0], u[1], u[2], vox, marker, mig);
 }
 
-void launch_position_change(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker, const float *p, float *const u[3]) {
-    BLUB_LAUNCH(position_change_kernel, word_blocks(g, bits), PT, 0, st, g, bits, params, marker, p, u[0], u[1], u[2]);
+void launch_position_change(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker, const float *p,
+                            const uint32_t *particle_words, float *const u[3]) {
+    BLUB_LAUNCH(position_change_kernel, word_blocks(g, bits), PT, 0, st, g, bits, params, marker, p, particle_words, u[0], u[1], u[2]);
 }
 
 void launch_correct_particles(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos,

@@ -57,7 +57,9 @@ void launch_scatter_schedule(cudaStream_t st, const GridDim &g, const CellLists 
 void configure_transfer_kernels(); // once per device, before the first launch (dynamic shared memory opt-in)
 // clamp_lo: 1.0 velocity transfer, 0.5 density transfer, 0.0 binning (see transfer_position)
 void launch_cell_lists(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, float clamp_lo, const CellLists &l);
-void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits);
+// particle_words (nullable): 1 bit per cell "a particle is in this cell", before the boundary rule
+void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits,
+                              uint32_t *particle_words);
 void launch_p2g_gather(cudaStream_t st, const GridDim &g, const StepParams *params, const CellLists &l, const float4 *pos, float4 *const row[3],
                        const int8_t *marker, float *const u[3]);
 // scatter form of P2G / density in two halves, for callers that exchange halos in between (z-slab sharding).  sched: the brick schedule, or
@@ -80,16 +82,21 @@ void launch_fluid_bits(cudaStream_t st, const GridDim &g, const int8_t *marker, 
 int binning_scan_blocks(const GridDim &g);
 void launch_binning(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *src, float4 *dst, const CellLists &l);
 
-// grid passes: they visit the cells within one cell of the fluid only (FluidBits), everything further away keeps its previous value
+// grid passes: they visit the cells within one cell of the fluid (FluidBits) and, with a solid volume, divergence_remove / position_change also
+// those within two / one cells of a SOLID cell that holds a particle (DESIGN section 3.3); every other cell keeps its previous value
 void launch_divergence_compute(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, float *const u[3], const uint2 *vox, float *rhs);
-void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox, float *const u[3]);
+// particle_words (with a solid volume; nullptr without one): the words of the last marker pass -- the projection also visits the cells within
+// two cells, the position change those within one cell of a SOLID cell that holds a particle (the faces such a particle reads)
+void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox,
+                              const uint32_t *particle_words, float *const u[3]);
 void launch_extrapolate(cudaStream_t st, const GridDim &g, const FluidBits &bits, float *const u[3]);
 void launch_clear_marker(cudaStream_t st, const GridDim &g, int8_t *marker);
 void launch_advect(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos, float4 *const row[3],
                    float *const u[3], const uint2 *vox, int8_t *marker);
 void launch_advect_migrate(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos, float4 *const row[3],
                            float *const u[3], const uint2 *vox, int8_t *marker, const MigrateOut &mig);
-void launch_position_change(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker, const float *p, float *const u[3]);
+void launch_position_change(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker, const float *p,
+                            const uint32_t *particle_words, float *const u[3]);
 void launch_correct_particles(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos,
                               const int8_t *marker, float *const u[3]);
 

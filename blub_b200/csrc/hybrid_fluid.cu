@@ -476,7 +476,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         if (!shard && !use_scatter_) {
             // cell lists -> marker (+ FLUID bits) -> one gather per component; deterministic, no accumulator volumes
             launch_cell_lists(stream_, grid_, params_dev_, np, pos_[cur_], 1.0f, lists_);
-            launch_marker_from_lists(stream_, grid_, lists_, marker_.ptr, vox, bits);
+            launch_marker_from_lists(stream_, grid_, lists_, marker_.ptr, vox, bits, vox ? particle_words_ : nullptr);
             fluid_bits_stale_ = false;
             if (np > 0) launch_p2g_gather(stream_, grid_, params_dev_, lists_, pos_[cur_], row_, marker_.ptr, u);
             else for (int c = 0; c < 3; ++c) BLUB_CUDA_CHECK(cudaMemsetAsync(u[c], 0, (size_t)grid_.n * sizeof(float), stream_));
@@ -521,7 +521,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 4: // make velocity grid divergence free (:901-904)
         refresh_fluid_bits();
-        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, u);
+        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, vox ? particle_words_ : nullptr, u);
         break;
     case 5: // extrapolate velocity grid (:906-909)
         refresh_fluid_bits();
@@ -545,7 +545,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         }
         break;
     case 8: // density projection: set boundary marker (:923-927)
-        launch_boundary_marker(stream_, grid_, marker_.ptr, vox, bits);
+        launch_boundary_marker(stream_, grid_, marker_.ptr, vox, bits, vox ? particle_words_ : nullptr); // with a solid volume: the particle words stage 11 visits around
         fluid_bits_stale_ = false;
         break;
     case 9: // density projection: compute density error (:928-932)
@@ -564,7 +564,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 11: // compute position change (:959-962)
         refresh_fluid_bits();
-        launch_position_change(stream_, grid_, bits, params_dev_, marker_.ptr, field_density_->pressure(), u);
+        launch_position_change(stream_, grid_, bits, params_dev_, marker_.ptr, field_density_->pressure(), vox ? particle_words_ : nullptr, u);
         break;
     case 12: // extrapolate (:963-966)
         refresh_fluid_bits();

@@ -274,7 +274,7 @@ __device__ __forceinline__ unsigned solid_rule_mask(const GridDim &g, const uint
 // marker <- f(cell lists): a cell is FLUID iff a particle lies in it (transfer_build_linkedlist.comp:17-19) unless the boundary rule
 // makes it SOLID; everything else is AIR (transfer_clear.comp).  One thread per 32-cell word of a row; also writes the FLUID bit mask.
 __global__ void __launch_bounds__(PT) marker_from_lists_kernel(GridDim g, FluidBits bits, const uint32_t *__restrict__ cell_start, int8_t *__restrict__ marker,
-                                                               const uint2 *__restrict__ vox) {
+                                                               const uint2 *__restrict__ vox, uint32_t *__restrict__ particle_words) {
     const int w = blockIdx.x * PT + threadIdx.x;
     if (w >= bits.wpr * g.ny * g.nz) return;
     const int xw = w % bits.wpr, rowi = w / bits.wpr, y = rowi % g.ny, z = rowi / g.ny;
@@ -292,6 +292,7 @@ __global__ void __launch_bounds__(PT) marker_from_lists_kernel(GridDim g, FluidB
         prev = d;
     }
     const unsigned solid = solid_rule_mask(g, vox, xw, y, z, cells);
+    if (particle_words) particle_words[w] = fluid; // cells that hold a particle, whatever the boundary rule makes of them
     fluid &= ~solid;
     for (int k8 = 0; k8 < cells; k8 += 8) { // rows start on multiples of 8 cells: 8-byte stores
         unsigned long long m = 0;
@@ -1243,8 +1244,9 @@ void launch_cell_lists(cudaStream_t st, const GridDim &g, const StepParams *para
     BLUB_LAUNCH(crowded_canonicalize_kernel, 2 * device_sm_count(), PT, 0, st, l.cell_start, l.arrival, l.order, l.crowd); // 2 blocks per SM
 }
 
-void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits) {
-    BLUB_LAUNCH(marker_from_lists_kernel, blocks_for((int64_t)bits.wpr * g.ny * g.nz, PT), PT, 0, st, g, bits, l.cell_start, marker, vox);
+void launch_marker_from_lists(cudaStream_t st, const GridDim &g, const CellLists &l, int8_t *marker, const uint2 *vox, const FluidBits &bits,
+                              uint32_t *particle_words) {
+    BLUB_LAUNCH(marker_from_lists_kernel, blocks_for((int64_t)bits.wpr * g.ny * g.nz, PT), PT, 0, st, g, bits, l.cell_start, marker, vox, particle_words);
 }
 
 void launch_boundary_marker(cudaStream_t st, const GridDim &g, int8_t *marker, const uint2 *vox, const FluidBits &bits, uint32_t *particle_words) {

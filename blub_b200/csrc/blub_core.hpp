@@ -99,6 +99,8 @@ class PressureField {
     void enqueue_error_buffer_read(cudaStream_t stream, float simulation_delta);
     // blocking read of the device scalars (tests only)
     void read_last_solve(cudaStream_t stream, float *max_error, int *iterations);
+    // blocking read of the scalars the last solve left: {alpha, beta, sigma} (tests only; conventions in blub_fluid.h)
+    void read_last_scalars(cudaStream_t stream, float out[3]);
 
     PcgScalars *scalars = nullptr; // device
     bool touched = false;          // "timestamp_last_iteration == 0" of :601-603

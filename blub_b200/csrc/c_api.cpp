@@ -612,6 +612,15 @@ int blub_fluid_last_solve(BlubFluid *fluid, int which, float *max_error, int32_t
     });
 }
 
+int blub_fluid_last_solve_scalars(BlubFluid *fluid, int which, float out[3]) {
+    if (!fluid || which < 0 || which > 1 || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad argument");
+    return guarded([&] {
+        BLUB_CUDA_CHECK(cudaSetDevice(fluid->impl->device()));
+        fluid->impl->field(which).read_last_scalars(fluid->impl->stream(), out);
+        return BLUB_OK;
+    });
+}
+
 int blub_fluid_solver_work(BlubFluid *fluid, uint32_t out[4]) {
     if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad argument");
     return guarded([&] {

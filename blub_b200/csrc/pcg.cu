@@ -1617,6 +1617,15 @@ void PressureField::read_last_solve(cudaStream_t stream, float *max_error, int *
     *iterations = h.num_iterations;
 }
 
+void PressureField::read_last_scalars(cudaStream_t stream, float out[3]) {
+    PcgScalars h;
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(&h, scalars, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream));
+    out[0] = h.alpha;
+    out[1] = h.beta;
+    out[2] = h.sigma;
+}
+
 namespace {
 // 3-D tensor maps (x fastest).  The encoder lives in libcuda; it is fetched through the runtime so that libblubcore.so
 // does not link against the driver library.

@@ -309,6 +309,7 @@ def lib():
         "blub_fluid_solve_only": (C.c_int, [vp, C.c_int, C.c_double]),
         "blub_fluid_last_solve": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
         "blub_fluid_solver_work": (C.c_int, [vp, C.POINTER(u32)]),
+        "blub_fluid_last_solve_scalars": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float)]),
         "blub_fluid_time_solve": (C.c_int, [vp, C.c_int, C.c_double, C.c_int, C.POINTER(C.c_float)]),
         "blub_fluid_time_steps": (C.c_int, [vp, C.c_double, C.c_int, C.POINTER(C.c_float)]),
         "blub_fluid_step_timed": (C.c_int, [vp, C.c_double, C.POINTER(C.c_float)]),
@@ -640,6 +641,12 @@ class HybridFluid:
         e, it = C.c_float(0), C.c_int32(0)
         _check(self.L.blub_fluid_last_solve(self.h, which, C.byref(e), C.byref(it)))
         return float(e.value), int(it.value)
+
+    def last_solve_scalars(self, which):
+        """(alpha, beta, sigma) the last solve of a field left, as float32 values (conventions per solver path: blub_fluid.h)."""
+        out = (C.c_float * 3)()
+        _check(self.L.blub_fluid_last_solve_scalars(self.h, which, out))
+        return tuple(np.float32(out[k]) for k in range(3))
 
     def solver_work(self):
         """{tiles, columns, cells_per_tile, cells_per_column} of the most recent solve's work lists."""

@@ -470,6 +470,15 @@ int blub_fluid_last_solve(BlubFluid *fluid, int which, float *max_error, int32_t
 /* work list of the most recent solve (diagnostics for the in-step roofline; synchronises): out[0] = tiles walked by the tile body,
  * out[1] = quad columns walked by the column body, out[2] = cells per tile, out[3] = cells per column */
 int blub_fluid_solver_work(BlubFluid *fluid, uint32_t out[4]);
+/* scalars the last finished solve of a field left (diagnostics for tests of the solver; synchronises): out = {alpha, beta, sigma}.
+ * A solve that stops after iteration K (0-based) leaves, by the kernels that actually run it (not the path that was requested: without
+ * cooperative launch, or with BLUB_PCG=multikernel, paths 1, 2, 4 and 6 run the three-kernel code too)
+ *   the persistent solvers (paths 1, 2, 4, 6, z-slab ranks) and the three-kernel code with precond_mode 1: (alpha_K, beta_{K-1}, sigma_K),
+ *     beta_{-1} = 0;
+ *   the three-kernel code with precond_mode 0, whose update kernel forms beta and sigma after it stops the solve: (alpha_K, beta_K,
+ *     sigma_{K+1}).
+ * Here sigma_k = z_k . r_k, alpha_k = sigma_k / (s_k . A s_k +- eps) and beta_k = sigma_{k+1} / (sigma_k +- eps). */
+int blub_fluid_last_solve_scalars(BlubFluid *fluid, int which, float out[3]);
 /* PCG micro-benchmark: `repetitions` times { restore the rhs that is in the residual tap now, zero the pressure field,
  * solve } with CUDA events around each solve on the fluid's stream; ms_each[repetitions] receives device milliseconds.
  * Synchronises. */

@@ -54,6 +54,7 @@ typedef struct {
 typedef struct {
     float error; /* max|r| (NOT yet multiplied by dt) */
     int iteration_count;
+    float alpha, beta, sigma; /* of the last iteration: alpha_K, beta_{K-1}, sigma_K (beta_{-1} = 0) */
 } OrcSolveResult;
 
 typedef struct OrcFluid {
@@ -115,7 +116,9 @@ OrcFluid *orc_create(int nx, int ny, int nz, uint32_t max_particles) {
     f->aux = (float *)calloc(f->n, sizeof(float));
     f->aux_temp = (float *)calloc(f->n, sizeof(float));
     f->search = (float *)calloc(f->n, sizeof(float));
-    f->reduce0 = (float *)calloc(f->n, sizeof(float));
+    /* reduce_addr places cells in 8 x 8 groups: x and y round up to multiples of 8 (reduce_all still reads the first n entries, as the
+     * reference does -- grids whose nx or ny is not a multiple of 8 lose terms there) */
+    f->reduce0 = (float *)calloc((size_t)((nx + 7) / 8 * 8) * ((ny + 7) / 8 * 8) * nz, sizeof(float));
     f->reduce1 = (float *)calloc(f->n / 16384 + 1024, sizeof(float));
     for (int k = 0; k < 2; ++k) {
         f->pressure[k] = (float *)calloc(f->n, sizeof(float));
@@ -228,6 +231,9 @@ void orc_set_voxels(OrcFluid *f, const float *rgba) { memcpy(f->voxel, rgba, f->
 uint32_t orc_num_particles(const OrcFluid *f) { return f->num_particles; }
 uint32_t orc_step_counter(const OrcFluid *f) { return f->step_counter; }
 void orc_last_solve(const OrcFluid *f, int which, float *err, int *iters) { *err = f->last[which].error; *iters = f->last[which].iteration_count; }
+void orc_last_scalars(const OrcFluid *f, int which, float out[3]) {
+    out[0] = f->last[which].alpha; out[1] = f->last[which].beta; out[2] = f->last[which].sigma;
+}
 
 /* array accessor for the Python harness */
 void *orc_array(OrcFluid *f, int which) {
@@ -505,7 +511,7 @@ void orc_solve(OrcFluid *f, int which, float dt) {
     /* init: precondition r straight into the search vector, sigma = z.r (:625-649) */
     precond_pass(f, f->residual, f->aux_temp, 0);
     precond_pass(f, f->aux_temp, f->search, 1);
-    float alphabeta = 0.0f;
+    float alphabeta = 0.0f, last_beta = 0.0f;
     float sigma = reduce_all(f, 0);
     for (int i = 0;; ++i) {
         /* pressure_apply_coeff.comp:19-30 */
@@ -556,6 +562,7 @@ void orc_solve(OrcFluid *f, int which, float dt) {
         alphabeta = zr / (sigma + (sigma < 0.0f ? -EPS : EPS)); /* :77-80 */
         sigma = zr;
         const float beta = alphabeta;
+        last_beta = beta;
         /* pressure_update_search.comp:13-24 */
 #pragma omp parallel for
         for (size_t g = 0; g < f->n; ++g)
@@ -563,6 +570,9 @@ void orc_solve(OrcFluid *f, int which, float dt) {
     }
     f->last[which].error = max_error;
     f->last[which].iteration_count = num_iterations;
+    f->last[which].alpha = alphabeta;
+    f->last[which].beta = last_beta;
+    f->last[which].sigma = sigma;
 }
 
 /* ------------------------------------------------------------------ A4: projection

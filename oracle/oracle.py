@@ -73,6 +73,7 @@ def lib():
         L.orc_step_counter.restype = C.c_uint32
         L.orc_step_counter.argtypes = [C.c_void_p]
         L.orc_last_solve.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int)]
+        L.orc_last_scalars.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float)]
         L.orc_array.restype = C.c_void_p
         L.orc_array.argtypes = [C.c_void_p, C.c_int]
         L.orc_step.argtypes = [C.c_void_p, C.c_float]
@@ -167,6 +168,12 @@ class OracleFluid:
         e, it = C.c_float(0), C.c_int(0)
         self.L.orc_last_solve(self.h, which, C.byref(e), C.byref(it))
         return float(e.value), int(it.value)
+
+    def last_scalars(self, which):
+        """(alpha_K, beta_{K-1}, sigma_K) of the last iteration K of the last solve, as float32 values."""
+        out = (C.c_float * 3)()
+        self.L.orc_last_scalars(self.h, which, out)
+        return tuple(np.float32(out[k]) for k in range(3))
 
     # -- stepping ---------------------------------------------------------------------------
     def step(self, dt=DT_120HZ):

@@ -1306,6 +1306,17 @@ bool scatter_schedule_enabled() {
     return on;
 }
 
+// How many waves of 4 blocks per SM the work items must fill before P2G walks them: P2G_MIN_ITEM_WAVES, or BLUB_P2G_ITEM_WAVES=N (0..8,
+// read once; a test hook: 0 walks the items whenever the schedule is valid, so that small grids reach the item path).
+static uint32_t p2g_item_waves() {
+    static const uint32_t waves = [] {
+        const char *e = std::getenv("BLUB_P2G_ITEM_WAVES");
+        if (e && e[0] >= '0' && e[0] <= '0' + P2G_MIN_ITEM_WAVES && e[1] == '\0') return (uint32_t)(e[0] - '0');
+        return (uint32_t)P2G_MIN_ITEM_WAVES;
+    }();
+    return waves;
+}
+
 int scatter_schedule_bricks(const GridDim &g) {
     return ((g.nx + SCHED_BX - 1) / SCHED_BX) * ((g.ny + SCHED_BY - 1) / SCHED_BY) * ((g.nz + SCHED_BZ - 1) / SCHED_BZ);
 }
@@ -1331,7 +1342,7 @@ void launch_p2g_scatter(cudaStream_t st, const GridDim &g, const StepParams *par
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? p2g_scatter_kernel<true, true> : p2g_scatter_kernel<true, false>;
     BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, P2G_TILE_BYTES, st, g, params, pos, row[0], row[1], row[2], nw[0], nw[1], nw[2], marker, sched,
-                (uint32_t)(P2G_MIN_ITEM_WAVES * 4 * device_sm_count()));
+                p2g_item_waves() * 4u * (uint32_t)device_sm_count());
 }
 
 void launch_p2g_finish(cudaStream_t st, const GridDim &g, const StepParams *params, float *const u[3], longlong2 *const nw[3], int8_t *marker,

@@ -2,7 +2,8 @@
 processes, once as built and once with BLUB_SCATTER_SCHEDULE=off (read once per process: the scatter then walks the 256-particle chunks
 only), and the density rhs, the P2G velocities and marker and the particles must be equal bit for bit.  20 steps span the
 re-sorts of steps 0, 8 and 16; a fluid loaded from a state file runs the chunks until its next re-sort.  The P2G scatter walks the work items
-only when they fill several waves of resident blocks, which the small scenes do not: the dam_256 case (16.4 M particles) covers that path.
+only when they fill several waves of resident blocks, which the small scenes do not: the dam_256 case (16.4 M particles) covers that path over
+steps 0-9, 56, 57 and 230, and crowded_items (BLUB_P2G_ITEM_WAVES=0) on bricks that hold several work items each.
 Arrays are compared by their SHA-256 digests."""
 import hashlib
 import os
@@ -50,11 +51,17 @@ def run_case(case, tmp):
 
     p2g = (("ux", F.TAP_UX), ("uy", F.TAP_UY), ("uz", F.TAP_UZ), ("marker", F.TAP_MARKER))
     end = (("pos", F.TAP_POS), ("ux_end", F.TAP_UX))
-    if case in ("eager", "crowded", "dam_256"):
+    if case in ("eager", "crowded", "crowded_items", "dam_256"):
         # stage by stage: the P2G result after stage 0, the density rhs (the solver residual) after stage 9
-        f = {"eager": lambda: _fluid("dam_small"), "crowded": _crowded, "dam_256": lambda: _fluid("dam_256")}[case]()
+        f = {"eager": lambda: _fluid("dam_small"), "crowded": _crowded, "crowded_items": _crowded, "dam_256": lambda: _fluid("dam_256")}[case]()
         f.set_graph_replay(False)
-        for k in range(STEPS if case != "dam_256" else 10):  # dam_256: the re-sorts of steps 0 and 8
+        # dam_256: the re-sorts of steps 0 and 8, then step 56 (the most decayed order of the window of step 48), 57 (the first P2G on the
+        # schedule of step 56) and 230 (the step bench.py times stage by stage); the steps in between are not recorded
+        checked = range(STEPS) if case != "dam_256" else [*range(10), 56, 57, 230]
+        for k in range(checked[-1] + 1):
+            if k not in checked:
+                f.step(DT)
+                continue
             f.step_stages(DT, 0, 1)
             record(f, k, p2g)
             f.step_stages(DT, 1, 10)
@@ -90,6 +97,9 @@ def run_case(case, tmp):
 def _run(case, tmp_path, schedule):
     out = str(tmp_path / f"{case}_{schedule}.npz")
     env = dict(os.environ)
+    env.pop("BLUB_P2G_ITEM_WAVES", None)
+    if case == "crowded_items":  # P2G walks the work items whenever the schedule is valid, as at millions of particles
+        env["BLUB_P2G_ITEM_WAVES"] = "0"
     if schedule == "off":
         env["BLUB_SCATTER_SCHEDULE"] = "off"
     else:
@@ -101,7 +111,7 @@ def _run(case, tmp_path, schedule):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["eager", "graph", "tap", "resume", "norebin", "crowded", "dam_256"])
+@pytest.mark.parametrize("case", ["eager", "graph", "tap", "resume", "norebin", "crowded", "crowded_items", "dam_256"])
 def test_schedule_changes_no_bit(case, tmp_path):
     a, b = _run(case, tmp_path, "on"), _run(case, tmp_path, "off")
     assert sorted(a) == sorted(b) and len(a) > 0

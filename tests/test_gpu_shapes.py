@@ -8,8 +8,9 @@ those pieces at their edges; every test below runs on every row (sections 4 and 
 word, the last gather block and the last brick of its rows (assert_edges).
 
 The P2G scatter walks the brick schedule's work items only when they fill several waves of resident blocks (P2G_MIN_ITEM_WAVES, millions of
-particles); at these sizes it runs its 256-particle chunks, and the item windows of P2G are covered by test_gpu_scatter_schedule.py's dam_256
-case.  The density scatter walks the items at every size: the schedule-on steps below check it against the float64 reference."""
+particles); at these sizes it runs its 256-particle chunks, and test_schedule_steps_on_work_items_match_float64_reference runs the schedule
+steps again with BLUB_P2G_ITEM_WAVES=0, which sends P2G through the items here too.  The density scatter walks the items at every size:
+the schedule-on steps below check it against the float64 reference."""
 import hashlib
 import os
 import subprocess
@@ -272,7 +273,9 @@ def test_p2g_and_density_match_float64_reference(dims, order, scatter):
 @shape_params()
 def test_schedule_steps_match_float64_reference(dims, scatter):
     """Ten steps with the default re-sorts (steps 0 and 8): every step's P2G and density rhs against the float64 reference of the particles it
-    read.  The density scatter runs the brick schedule's work items from the re-sort of step 0 on, the P2G scatter its chunks."""
+    read.  The density scatter runs the brick schedule's work items from the re-sort of step 0 on; the P2G scatter runs its chunks, or under
+    BLUB_P2G_ITEM_WAVES=0 (test_schedule_steps_on_work_items_match_float64_reference) the work items too, whose count is then restated from
+    the cell order the re-sort of step 0 left and must be non-zero."""
     import blub_b200
     from blub_b200 import fluid as F
     from tests.util import DT
@@ -288,10 +291,29 @@ def test_schedule_steps_match_float64_reference(dims, scatter):
         rows = [gpu.download_particles(t) for t in (F.TAP_VX, F.TAP_VY, F.TAP_VZ)]
         gpu.step_stages(DT, 0, 1)
         check_p2g(gpu, pos, rows, scatter, gravity_dt(g, DT), f"{dims} step {k}")
-        gpu.step_stages(DT, 1, 10)
+        gpu.step_stages(DT, 1, 4)
+        if k == 0 and scatter and os.environ.get("BLUB_P2G_ITEM_WAVES") == "0":  # the items the next steps' P2G walks
+            from tests.test_gpu_bench_scale import schedule
+
+            items = int(schedule(gpu.download_particles(), dims)["brick_items"].sum())
+            assert items > 0, f"{dims}: no work item after the re-sort of step 0"
+            print(f"{dims}: {items} work items for P2G from step 1 on")
+        gpu.step_stages(DT, 4, 10)
         check_rhs(gpu, DT, f"{dims} step {k}")
         gpu.step_stages(DT, 10, 14)
     print_bound_ratios(f"{dims} schedule steps {'scatter' if scatter else 'gather'}")
+
+
+@pytest.mark.gpu
+def test_schedule_steps_on_work_items_match_float64_reference():
+    """test_schedule_steps_match_float64_reference on every row and path again under BLUB_P2G_ITEM_WAVES=0 (read once per process, hence a
+    fresh pytest): the P2G scatter then walks the brick schedule's work items from the re-sort of step 0 on, so that its item path meets the
+    brick edges the rows were chosen for."""
+    env = dict(os.environ, BLUB_P2G_ITEM_WAVES="0")
+    res = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu",
+                          f"{os.path.abspath(__file__)}::test_schedule_steps_match_float64_reference"], cwd=ROOT, env=env, capture_output=True,
+                         text=True, timeout=1800)
+    assert res.returncode == 0 and f"{2 * len(SHAPES)} passed" in res.stdout, res.stdout[-6000:] + res.stderr[-2000:]
 
 
 # ------------------------------------------------------------------------------------------------ 4. particle counts at warp and chunk edges

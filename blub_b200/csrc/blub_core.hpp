@@ -170,6 +170,7 @@ class PressureSolver {
     void *tma_maps_ = nullptr;       // PcgTmaMaps (tensor maps of r, s0, s1, codes)
     int tma_blocks_ = 0, column_blocks_ = 0;
     int code_slots_ = 0;              // column solver: passes per thread whose code words stay in shared memory
+    int p_slots_ = 0;                 // column solver, single GPU: passes per thread whose p stays in shared memory
     bool dense_setup_ = false;        // BLUB_PCG_SETUP=dense (test hook): the column solver prepares every tile on every solve
     int *tile_cols_ = nullptr;        // column solver: per-tile column counts | exclusive offsets | total
     int *col_list_ = nullptr;         // compacted quad columns (linear index of the quad in its tile's first plane)

@@ -574,6 +574,7 @@ struct PcgSolveArgs {
     const int *col_list;    // column solver: compacted quad columns (4 cells x PCG_TZ planes) of the sparsely filled tiles, see pcg_solve_columns_kernel
     const int *num_cols;
     int code_slots;         // column solver: passes per thread whose code words stay in shared memory (see pass_codes)
+    int p_slots;            // column solver: passes per thread whose p stays in shared memory (see p_slot); 0 on the other paths
     float *p, *r, *s0, *s1;
     PcgScalars *scal;
     float *partials;        // 3 x gridDim.x
@@ -694,9 +695,11 @@ __device__ __forceinline__ bool warp_has_no_fluid(const unsigned (&w)[PCG_TZ + 2
     return !__any_sync(0xffffffffu, any != 0u);
 }
 
-// r <- b - A p, partial z.r  (pressure_init.comp:45-83)
+// r <- b - A p, partial z.r  (pressure_init.comp:45-83).  ps (column solver, see p_slot): the thread's slot that keeps its own p quads
+// on chip for the rest of the solve, filled here with the quads of planes 0 .. PCG_TZ - 1.
 template <bool SKIP>
-__device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *p, float *r, float &acc) {
+__device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *p, float *r, float &acc,
+                                          float4 *ps = nullptr) {
     const GridDim &g = e.g;
     int i = c.i;
     float4 pm = zero4(), p0 = zero4(), pp = zero4();
@@ -704,6 +707,7 @@ __device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, co
 #pragma unroll
     for (int k = 0; k < PCG_TZ; ++k, i += g.sz) {
         float left = __shfl_up_sync(0xffffffffu, p0.w, 1), right = __shfl_down_sync(0xffffffffu, p0.x, 1);
+        if (ps) ps[k * PCG_THREADS] = p0;
         if (c.valid) pp = ld4w<SKIP>(p, i + g.sz, w[k + 2]);
         if (c.valid && (!SKIP || w[k + 1] != 0u)) {
             if (c.first) left = p[i - 1];
@@ -767,10 +771,11 @@ __device__ __forceinline__ void search_tile(const TileEnv &e, const TileCtx &c, 
     }
 }
 
-// phase B: p += alpha s', r -= alpha A s' (pressure_update_pressure_and_residual.comp), partial z.r and max|r|
+// phase B: p += alpha s', r -= alpha A s' (pressure_update_pressure_and_residual.comp), partial z.r and max|r|.  With a p slot (ps) the
+// thread's p quads are read and updated there instead of in memory.
 template <bool SKIP>
 __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *s, float *p, float *r,
-                                            float alpha, float &acc, float &err) {
+                                            float alpha, float &acc, float &err, float4 *ps = nullptr) {
     const GridDim &g = e.g;
     int i = c.i;
     float4 sm = zero4(), s0 = zero4(), sp = zero4();
@@ -784,7 +789,7 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
         if (act) {
             ym = ld4(s + i - g.sy);
             yp = ld4(s + i + g.sy);
-            p4 = ld4(p + i);
+            p4 = ps ? ps[k * PCG_THREADS] : ld4(p + i);
             r4 = ld4(r + i);
         }
         if (act) {
@@ -797,7 +802,8 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
             r4.y -= alpha * (code.y ? As.y : 0.0f);
             r4.z -= alpha * (code.z ? As.z : 0.0f);
             r4.w -= alpha * (code.w ? As.w : 0.0f);
-            st4(p + i, p4);
+            if (ps) ps[k * PCG_THREADS] = p4;
+            else st4(p + i, p4);
             st4(r + i, r4);
             if (e.sharded) {
                 if (k == 0 && c.tz == e.tz_first && e.peer_r_lo) st4(e.peer_r_lo + i + e.push, r4);
@@ -810,6 +816,15 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
         sm = s0;
         s0 = sp;
     }
+}
+
+// End of a solve: the slotted p quads go to memory on exactly the planes update_tile stores, so that p is still written only inside
+// the active tiles (the sparse set-up and PressureField::p_tiles rely on that)
+template <bool SKIP>
+__device__ __forceinline__ void store_p_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], float *p, const float4 *ps) {
+#pragma unroll
+    for (int k = 0; k < PCG_TZ; ++k)
+        if (c.valid && (!SKIP || w[k + 1] != 0u)) st4(p + c.i + k * e.g.sz, ps[k * PCG_THREADS]);
 }
 
 // Formed from the kernel parameters where a phase needs it, not kept in the walkers: values derived from parameters are re-read from the
@@ -832,7 +847,8 @@ __device__ __forceinline__ TileEnv make_tile_env(const PcgSolveArgs &a) {
 // ---------------------------------------------------------------------------------------------------------------
 // The solve, written once for the three persistent kernels.  A kernel hands it
 //   a walker:  init(acc), search(it, beta, acc) = phase A, update(it, alpha, acc, err) = phase B -- the kernel's share of the work of a
-//              phase -- and each_tile(f), which calls f(c) for every tile (and column) of that share;
+//              phase --, store_p(), which writes back the p kept on chip (column solver), and each_tile(f), which calls f(c) for every
+//              tile (and column) of that share;
 //   a reducer: the grid-wide sums, on z-slab ranks followed by or fused with the all-rank round: open(psum) and close(psum) are empty
 //              rounds, sum(psum, acc, tot) a sum, sum_max(psum, pmax, acc, err, tot, gmax) a sum and a maximum.
 // Partial buffers (gridDim.x floats each): init on 1, phase A on 0, phase B on 1 + 2 for the maximum (a fast block never overwrites
@@ -891,6 +907,7 @@ __device__ __forceinline__ void pcg_solve(const PcgSolveArgs &a, Walker &wk, Red
         beta = guarded_div(zr, sigma); // RESULTMODE_BETA, pressure_reduce.comp:77-80
         sigma = zr;
     }
+    wk.store_p();
     if (sharded) {
         // hand the boundary planes of the solution to the neighbours (warm start of their next init, pressure gradient across the slab
         // face), then one more round so that nobody leaves before its ghost planes are complete
@@ -963,30 +980,37 @@ struct SyncReduce {
     for (int li_ = blockIdx.x, tile = li_ < nact ? a.tile_list_flagged[li_] : 0, next_ = 0; li_ < nact; li_ += gridDim.x, tile = next_) \
         if ((next_ = li_ + (int)gridDim.x < nact ? a.tile_list_flagged[li_ + gridDim.x] : 0), true)
 
-// Phases of the register-marching kernels (tile and column solver): Walk::passes(fill, body) calls body(c, w, sparse) for every pass of
-// the thread -- a tile or a column with its code words w; sparse: std::true_type for the sparse body -- and fill is set in the first
-// phase of a solve.
+// Phases of the register-marching kernels (tile and column solver): Walk::passes(fill, body) calls body(c, w, sparse, ps) for every pass
+// of the thread -- a tile or a column with its code words w; sparse: std::true_type for the sparse body; ps: the pass's p slot or null --
+// and fill is set in the first phase of a solve.
 template <class Walk>
 struct MarchWalker : Walk {
     __device__ __forceinline__ void init(float &acc) const {
         const TileEnv e = make_tile_env(this->a);
-        this->passes(true, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
-            init_tile<decltype(sparse)::value>(e, c, w, this->a.p, this->a.r, acc);
+        this->passes(true, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *ps) {
+            init_tile<decltype(sparse)::value>(e, c, w, this->a.p, this->a.r, acc, ps);
         });
     }
     __device__ __forceinline__ void search(int it, float beta, float &acc) const {
         const float *s_in = (it & 1) ? this->a.s1 : this->a.s0;
         float *s_out = (it & 1) ? this->a.s0 : this->a.s1;
         const TileEnv e = make_tile_env(this->a);
-        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
+        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *) {
             search_tile<decltype(sparse)::value>(e, c, w, this->a.r, s_in, s_out, beta, acc);
         });
     }
     __device__ __forceinline__ void update(int it, float alpha, float &acc, float &err) const {
         const float *s = (it & 1) ? this->a.s0 : this->a.s1;
         const TileEnv e = make_tile_env(this->a);
-        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse) {
-            update_tile<decltype(sparse)::value>(e, c, w, s, this->a.p, this->a.r, alpha, acc, err);
+        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *ps) {
+            update_tile<decltype(sparse)::value>(e, c, w, s, this->a.p, this->a.r, alpha, acc, err, ps);
+        });
+    }
+    __device__ __forceinline__ void store_p() const {
+        if (this->a.p_slots == 0) return;
+        const TileEnv e = make_tile_env(this->a);
+        this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *ps) {
+            if (ps) store_p_tile<decltype(sparse)::value>(e, c, w, this->a.p, ps);
         });
     }
 };
@@ -1006,8 +1030,8 @@ struct TileWalk {
             unsigned w[PCG_TZ + 2];
             load_column_codes(e, c, w);
             if (SKIP && warp_has_no_fluid(w)) continue;
-            if (!SKIP || (tile & TILE_DENSE_BIT)) body(c, w, std::false_type{});
-            else body(c, w, std::true_type{});
+            if (!SKIP || (tile & TILE_DENSE_BIT)) body(c, w, std::false_type{}, nullptr);
+            else body(c, w, std::true_type{}, nullptr);
         }
     }
 };
@@ -1274,12 +1298,29 @@ __device__ __forceinline__ void pass_codes(const TileEnv &e, const TileCtx &c, u
     }
 }
 constexpr int PCG_CODE_SLOT_BYTES = (PCG_TZ + 2) * PCG_THREADS * 4; // 6 KB
-// 8 slots = 48 KB per block, ~150 KB of shared memory per SM at three blocks: the 256^3 dam break ran 4 and 8 slots alike (126.6-126.8
-// steps/s), 12 slots shrink L1 to ~28 KB and ran 112.9 (H100 SXM at 400 W, profiles/h100_pcg_setup.json)
-constexpr int PCG_CODE_SLOTS = 8;
 
-// Work of the column solver: the dense tiles by the tile body, then the column list by the sparse body, code words of the first passes
-// kept in shared memory (pass_codes)
+// p of a thread's pass (tile or column) number `pass`, for the whole solve.  Nobody else reads a cell's p during a solve: init reads the
+// neighbours' p before any of it changes, phase B reads and writes the thread's own quads only, and only the closing push of a z-slab rank
+// (no p slots there) reads p after the loop.  So init keeps the p quads of its own planes in a slot of dynamic shared memory that only
+// this thread uses ([pass][plane][thread] float4: conflict-free), phase B updates them there, and store_p writes them back once at the
+// end: 24 instead of 32 B of own-cell traffic per cell and iteration, and one operand load less in phase B.  Passes beyond the slots
+// keep p in memory.
+// The p slots follow the code slots (sh_cw: 6 KB slots, so 16-byte aligned).
+__device__ __forceinline__ float4 *p_slot(unsigned *sh_cw, const PcgSolveArgs &a, int pass) {
+    return pass < a.p_slots ? reinterpret_cast<float4 *>(sh_cw + a.code_slots * (PCG_TZ + 2) * PCG_THREADS) + pass * PCG_TZ * PCG_THREADS + linear_tid()
+                            : nullptr;
+}
+constexpr int PCG_P_SLOT_BYTES = PCG_TZ * PCG_THREADS * 16; // 16 KB
+
+// Slots per block, code words and p (PressureSolver searches down from this pair for one that keeps the resident blocks per SM).  2 + 2 =
+// 44 KB per block ran the 256^3 dam break fastest of the pairs measured: 153.3 steps/s, 150.0-150.2 for 4 + 2 and 2 + 3, 139.3-140.1 for
+// 8 or 4 code slots without p slots (H100 SXM at 700 W, profiles/h100_pcg_onchip.json).  12 code slots alone (72 KB) shrink L1 to ~28 KB
+// and ran 112.9 against 126.7 steps/s for 8 (400 W, profiles/h100_pcg_setup.json).
+constexpr int PCG_CODE_SLOTS = 2, PCG_P_SLOTS = 2;
+constexpr int PCG_MAX_CODE_SLOTS = 8, PCG_MAX_P_SLOTS = 4; // largest counts the test hooks may ask for
+
+// Work of the column solver: the dense tiles by the tile body, then the column list by the sparse body, code words and p of the first
+// passes kept in shared memory (pass_codes, p_slot)
 struct ColumnWalk {
     const PcgSolveArgs &a;
     int nact, ncols;
@@ -1295,13 +1336,13 @@ struct ColumnWalk {
         PCG_FOR_EACH_TILE(tile) {
             const TileCtx c = tile_ctx_id(e.g, a.t, tile & (TILE_DENSE_BIT - 1));
             unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, fill);
-            body(c, w, std::false_type{});
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass, fill);
+            body(c, w, std::false_type{}, p_slot(sh_cw, a, pass++));
         }
         PCG_FOR_EACH_COLUMN(c) {
             unsigned w[PCG_TZ + 2];
-            pass_codes(e, c, w, sh_cw, a.code_slots, pass++, fill);
-            body(c, w, std::true_type{});
+            pass_codes(e, c, w, sh_cw, a.code_slots, pass, fill);
+            body(c, w, std::true_type{}, p_slot(sh_cw, a, pass++));
         }
     }
 };
@@ -1309,7 +1350,7 @@ struct ColumnWalk {
 // Three resident blocks per SM (up to 85 registers): for sm_90a, a four-block bound (64 registers) spills the column body to local memory,
 // and on an H100 SXM (700 W limit) the 256^3 dam break runs 100.9 instead of 97.7 steps/s with three blocks (profiles/h100_choices.json).
 __global__ void __launch_bounds__(PCG_THREADS, 3) pcg_solve_columns_kernel(PcgSolveArgs a) {
-    extern __shared__ unsigned sh_cw[]; // a.code_slots x (PCG_TZ + 2) x PCG_THREADS code words
+    extern __shared__ unsigned sh_cw[]; // a.code_slots x (PCG_TZ + 2) x PCG_THREADS code words, then a.p_slots x PCG_TZ x PCG_THREADS p quads
     __shared__ ReduceScratch sc;
     __shared__ double sh_csum[SLAB_MAX_WORLD];
     __shared__ float sh_cmax[SLAB_MAX_WORLD];
@@ -1391,6 +1432,7 @@ struct TmaWalk {
     template <class F> __device__ __forceinline__ void each_tile(F f) const {
         for (int li = blockIdx.x; li < nact; li += gridDim.x) f(tile_ctx_id(a.g, a.t, a.tile_list[li]));
     }
+    __device__ __forceinline__ void store_p() const {} // p stays in memory
     // init as in the register-marching kernels (runs once, plain loads)
     __device__ __forceinline__ void init(float &acc) const {
         const TileEnv e = make_tile_env(a);
@@ -1703,18 +1745,30 @@ PressureSolver::PressureSolver(const GridDim &grid, void *external_residual) : g
         BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, pcg_solve_columns_kernel, PCG_THREADS, 0));
         column_blocks_ = sms * per;
         if (column_blocks_ > 2048) column_blocks_ = 2048;
-        // as many code slots as leave the number of resident blocks (and with it the grouping of the partial sums) unchanged.  The
-        // attribute is the largest size any solver asks for, so that solvers with different slot counts can live in one process.
-        // BLUB_PCG_CODE_SLOTS=N (0..8, test hook) starts the search at N: the grid and every sum stay the same, passes beyond N reload.
-        int max_slots = PCG_CODE_SLOTS;
-        const char *slots_env = std::getenv("BLUB_PCG_CODE_SLOTS");
-        if (slots_env && slots_env[0] >= '0' && slots_env[0] <= '0' + PCG_CODE_SLOTS && slots_env[1] == '\0') max_slots = slots_env[0] - '0';
-        BLUB_CUDA_CHECK(cudaFuncSetAttribute(pcg_solve_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PCG_CODE_SLOTS * PCG_CODE_SLOT_BYTES));
-        for (code_slots_ = max_slots; code_slots_ > 0; --code_slots_) {
-            const int bytes = code_slots_ * PCG_CODE_SLOT_BYTES;
-            int per_slots = 0;
-            BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_slots, pcg_solve_columns_kernel, PCG_THREADS, bytes));
-            if (per_slots == per) break;
+        // as many code and p slots as leave the number of resident blocks (and with it the grouping of the partial sums) unchanged: p slots
+        // are kept longest, code slots give way first.  The attribute is the largest size any solver asks for, so that solvers with
+        // different slot counts can live in one process.  Test hooks BLUB_PCG_CODE_SLOTS=N (0..8) and BLUB_PCG_P_SLOTS=N (0..4) start the
+        // search at N: the grid and every sum stay the same, passes beyond the slots reload their code words / keep p in memory.
+        auto hook = [](const char *name, int dflt, int most) {
+            const char *v = std::getenv(name);
+            return v && v[0] >= '0' && v[0] <= '0' + most && v[1] == '\0' ? v[0] - '0' : dflt;
+        };
+        const int max_code = hook("BLUB_PCG_CODE_SLOTS", PCG_CODE_SLOTS, PCG_MAX_CODE_SLOTS), max_p = hook("BLUB_PCG_P_SLOTS", PCG_P_SLOTS, PCG_MAX_P_SLOTS);
+        BLUB_CUDA_CHECK(cudaFuncSetAttribute(pcg_solve_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             PCG_MAX_CODE_SLOTS * PCG_CODE_SLOT_BYTES + PCG_MAX_P_SLOTS * PCG_P_SLOT_BYTES));
+        code_slots_ = p_slots_ = 0;
+        for (int ps = max_p, found = 0; ps >= 0 && !found; --ps) {
+            for (int cs = max_code; cs >= 0; --cs) {
+                int per_slots = 0;
+                BLUB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_slots, pcg_solve_columns_kernel, PCG_THREADS,
+                                                                              cs * PCG_CODE_SLOT_BYTES + ps * PCG_P_SLOT_BYTES));
+                if (per_slots == per) {
+                    code_slots_ = cs;
+                    p_slots_ = ps;
+                    found = 1;
+                    break;
+                }
+            }
         }
     }
     use_columns = column_blocks_ > 0 && !(env && std::string(env) == "tiles");
@@ -1808,6 +1862,8 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
         args.params = dparams; args.which = which; args.max_iterations = max_it; args.check_frequency = freq;
         args.comm = comm;
         args.col_list = col_list_; args.num_cols = num_cols; args.barrier = barrier_; args.code_slots = code_slots_;
+        // z-slab ranks keep p in memory: their closing push reads it
+        args.p_slots = columns && comm.world == 1 ? p_slots_ : 0;
         void *args_only[] = {&args}, *args_and_maps[] = {&args, tma_maps_};
         void **kargs = args_only;
         const void *kernel;
@@ -1817,7 +1873,7 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
             BLUB_LAUNCH(pcg_column_fill_kernel, grid, block, 0, stream, g, t, st, ta, col_offset, ghost_tiles, t.ntiles - ghost_tiles, col_list_);
             kernel = (const void *)pcg_solve_columns_kernel;
             nblocks = column_blocks_;
-            smem = (size_t)code_slots_ * PCG_CODE_SLOT_BYTES;
+            smem = (size_t)code_slots_ * PCG_CODE_SLOT_BYTES + (size_t)args.p_slots * PCG_P_SLOT_BYTES;
         } else if (use_tma && tma_blocks_ > 0) {
             kernel = (const void *)pcg_solve_tma_kernel;
             kargs = args_and_maps;

@@ -76,6 +76,10 @@ template <class T> struct GridArray {
     }
 };
 
+// The setting of a fluid without viscosity, and the setter's range rules (std::invalid_argument names the field).
+constexpr BlubViscosity kViscosityOff = {0.0f, 1e-4f, 200, 0u};
+void check_viscosity(const BlubViscosity &v);
+
 class PressureSolver;
 
 // PressureField, pressure_solver.rs:84-210: one pressure volume (kept between steps = warm start), its solver
@@ -291,6 +295,16 @@ class HybridFluid {
     BlubMeshBodyProperties body_mass_properties(uint32_t body) const;
     bool has_mesh_bodies() const { return !mesh_bodies_.empty(); }
 
+    // Viscous liquids (viscosity_kernels.cu): nullptr or a kinematic viscosity of 0 turns the stage off.  Stream-ordered; the working volumes are
+    // allocated with the first viscosity above zero, and only a change between off and on drops the step graphs.  Throws std::invalid_argument
+    // and changes nothing on a value check_viscosity refuses, a z-slab rank or a fluid inside a step.
+    void set_viscosity(const BlubViscosity *v);
+    const BlubViscosity &viscosity() const { return viscosity_; }
+    // iterations and max |r| per component of the last viscosity solve (synchronises); zeros before the first one
+    void last_viscosity_solve(int32_t *iterations, float max_error[3]);
+    // test hook: the viscosity stage on the grid velocity and marker as they are
+    void viscosity_only(double simulation_delta_seconds);
+
   private:
     BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
     unsigned long long *body_sums_ = nullptr; // composite volume, allocated with the first non-empty set
@@ -303,6 +317,9 @@ class HybridFluid {
     std::vector<MeshBodyHost> mesh_bodies_; // one per body while the set has a mesh body, else empty
     MeshBodySet mesh_;                      // device arrays, reallocated by every set with mesh bodies
     void free_mesh_bodies();
+    BlubViscosity viscosity_ = kViscosityOff;
+    ViscosityWork visc_;
+    void run_viscosity();
     LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
     BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
     uint32_t num_load_probes_ = 0, load_max_cells_ = 0;
@@ -513,12 +530,15 @@ struct SceneConfig {
     std::vector<SceneBox> drains;
     std::vector<SceneLoadProbe> load_probes; // optional fluid.load_probes (world units)
     std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
+    float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };
 SceneConfig parse_scene_file(const std::string &path);
 // the scene's load probes in grid cells: corners and pivot / grid_to_world_scale, pivot (min + max) / 2 when the scene gives none
 std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
+// the scene's kinematic viscosity in cells^2/s: viscosity / grid_to_world_scale^2
+float scene_viscosity_grid(const SceneConfig &cfg);
 // the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a
 // quaternion (quat_from_euler_deg_wxyz), the angular velocity unchanged
 std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg);

@@ -279,6 +279,15 @@ int main(int argc, char **argv) {
             std::fprintf(f, ", \"flow\": {\"emitted\": %llu, \"drained\": %llu, \"refused\": %llu}", (unsigned long long)c[0], (unsigned long long)c[1],
                          (unsigned long long)c[2]);
         }
+        BlubViscosity visc;
+        if (blub_fluid_viscosity(fluid, &visc)) die("cannot read the viscosity");
+        if (visc.kinematic_viscosity > 0.0f) {
+            int32_t it = 0;
+            float e[3] = {0, 0, 0};
+            if (blub_fluid_last_viscosity_solve(fluid, &it, e)) die("cannot read the last viscosity solve");
+            std::fprintf(f, ", \"viscosity\": {\"kinematic_viscosity\": %.9g, \"last_iterations\": %d, \"last_max_error\": [%.9g, %.9g, %.9g]}",
+                         visc.kinematic_viscosity, it, e[0], e[1], e[2]);
+        }
         std::fprintf(f, "}\n");
         std::fclose(f);
     }

@@ -488,6 +488,27 @@ int blub_fluid_body_mass_properties(BlubFluid *fluid, uint32_t body, BlubMeshBod
     return guarded([&] { *out = fluid->impl->body_mass_properties(body); return BLUB_OK; });
 }
 
+int blub_fluid_set_viscosity(BlubFluid *fluid, const BlubViscosity *viscosity) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_viscosity(viscosity); return BLUB_OK; });
+}
+
+int blub_fluid_viscosity(const BlubFluid *fluid, BlubViscosity *out) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *out = fluid->impl->viscosity();
+    return BLUB_OK;
+}
+
+int blub_fluid_last_viscosity_solve(BlubFluid *fluid, int32_t *iterations, float max_error[3]) {
+    if (!fluid || !iterations || !max_error) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->last_viscosity_solve(iterations, max_error); return BLUB_OK; });
+}
+
+int blub_scene_viscosity(const char *path, float *cells2_per_s) {
+    if (!path || !cells2_per_s) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *cells2_per_s = blub::scene_viscosity_grid(blub::parse_scene_file(path)); return BLUB_OK; });
+}
+
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
 
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {
@@ -599,6 +620,11 @@ int blub_fluid_step_stages(BlubFluid *fluid, double dt, int from, int to) {
 int blub_fluid_solve_only(BlubFluid *fluid, int which, double dt) {
     if (!fluid || which < 0 || which > 1) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad argument");
     return guarded([&] { fluid->impl->solve_only(which, dt); return BLUB_OK; });
+}
+
+int blub_fluid_viscosity_only(BlubFluid *fluid, double dt) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->viscosity_only(dt); return BLUB_OK; });
 }
 
 int blub_fluid_last_solve(BlubFluid *fluid, int which, float *max_error, int32_t *iterations) {

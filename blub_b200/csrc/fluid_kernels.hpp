@@ -199,4 +199,30 @@ void launch_body_step(cudaStream_t st, const GridDim &g, const StepParams *param
 // Host twins of the device rules the setter checks a body against: the half extents of its grid-axis bounding box at its pose.
 void body_bounding_extents(const BlubBody &b, float e[3]);
 
+// ---- viscous liquids (viscosity_kernels.cu, DESIGN.md §8 "Viscous liquids") ----
+// What the last viscosity solve left on the device.
+struct ViscositySolveInfo {
+    int iterations;
+    float max_error[3]; // max |r| per component, cells/s
+};
+// Working memory of the viscosity stage, allocated with the first viscosity above zero: 28 bytes per cell.
+struct ViscosityWork {
+    uint32_t *codes = nullptr;                   // n: three 10-bit face codes per cell
+    float *r[3] = {nullptr, nullptr, nullptr};   // n each: the right-hand side, then the residual
+    float *s[3] = {nullptr, nullptr, nullptr};   // n each: the search direction
+    uint32_t *word_flags = nullptr;              // words + 1: "the word holds a live face", then their exclusive scan (last entry: the number of active words)
+    uint32_t *words = nullptr;                   // the active 32-cell words, ascending
+    uint32_t *scan_sums = nullptr;               // block sums of the scan
+    float *partials = nullptr;                   // 2 x 6 x blocks: the blocks' partial sums and maxima, alternating between rounds
+    unsigned *barrier = nullptr;                 // arrival counter of the solve's grid-wide rounds
+    BlubViscosity *block = nullptr;              // what the kernels read of the setting: a change does not invalidate a captured graph
+    ViscositySolveInfo *info = nullptr;
+    int blocks = 0;                              // the solve's resident grid
+};
+int viscosity_solve_blocks(); // SMs x resident blocks per SM; throws CudaError without cooperative launch
+// The whole stage: classify the faces and list the active words from the FLUID bits and the marker, then solve all three components in one
+// cooperative launch; k = block->kinematic_viscosity * params->dt is formed on the device.  Writes live faces of u only.
+void launch_viscosity(cudaStream_t st, const GridDim &g, const StepParams *params, const FluidBits &bits, const int8_t *marker, const uint2 *vox,
+                      float *const u[3], const ViscosityWork &w);
+
 } // namespace blub

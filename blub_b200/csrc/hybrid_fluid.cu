@@ -210,6 +210,18 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.scan_sums);
     cudaFree(flow_scratch_.scalars);
     cudaFree(flow_scratch_.counters);
+    cudaFree(visc_.codes);
+    for (int c = 0; c < 3; ++c) {
+        cudaFree(visc_.r[c]);
+        cudaFree(visc_.s[c]);
+    }
+    cudaFree(visc_.word_flags);
+    cudaFree(visc_.words);
+    cudaFree(visc_.scan_sums);
+    cudaFree(visc_.partials);
+    cudaFree(visc_.barrier);
+    cudaFree(visc_.block);
+    cudaFree(visc_.info);
     cudaFree(census_dev_);
     cudaFree(load_probes_dev_);
     cudaFree(load_ring_);
@@ -491,6 +503,7 @@ void HybridFluid::run_stage(int stage, float dt) {
             launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, vox, bits, particle_words_);
             fluid_bits_stale_ = false;
         }
+        if (viscosity_.kinematic_viscosity > 0.0f) run_viscosity();
         break;
     case 1: // compute divergence -> PCG residual (:835-840)
         refresh_fluid_bits();
@@ -693,6 +706,73 @@ void HybridFluid::step_timed(double simulation_delta_seconds, float ms[14]) {
     BLUB_CUDA_CHECK(cudaEventSynchronize(ev[14]));
     for (int s = 0; s < 14; ++s) BLUB_CUDA_CHECK(cudaEventElapsedTime(&ms[s], ev[s], ev[s + 1]));
     for (auto &e : ev) cudaEventDestroy(e);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Viscous liquids (viscosity_kernels.cu).  Not in the reference.
+void check_viscosity(const BlubViscosity &v) {
+    if (!std::isfinite(v.kinematic_viscosity) || v.kinematic_viscosity < 0.0f) throw std::invalid_argument("viscosity: kinematic_viscosity must be finite and not negative");
+    if (!std::isfinite(v.error_tolerance) || !(v.error_tolerance > 0.0f)) throw std::invalid_argument("viscosity: error_tolerance must be finite and above 0");
+    if (v.max_num_iterations < 1 || v.max_num_iterations > 10000) throw std::invalid_argument("viscosity: max_num_iterations must lie in [1, 10000]");
+    if (v.reserved != 0u) throw std::invalid_argument("viscosity: reserved must be 0");
+}
+
+void HybridFluid::set_viscosity(const BlubViscosity *v) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_viscosity: z-slab ranks have no viscosity");
+    if (mid_step_) throw std::invalid_argument("set_viscosity: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    const BlubViscosity next = v ? *v : kViscosityOff;
+    check_viscosity(next);
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const bool on = next.kinematic_viscosity > 0.0f;
+    if (on && !visc_.block) {
+        ViscosityWork w;
+        w.blocks = viscosity_solve_blocks();
+        const size_t n = (size_t)grid_.n, words = (size_t)fluid_bits_.wpr * grid_.ny * grid_.nz;
+        BLUB_CUDA_CHECK(cudaMalloc(&w.codes, n * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMemsetAsync(w.codes, 0, n * sizeof(uint32_t), stream_));
+        for (int c = 0; c < 3; ++c) {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.r[c], n * sizeof(float)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.s[c], n * sizeof(float)));
+        }
+        BLUB_CUDA_CHECK(cudaMalloc(&w.word_flags, (words + 1) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.words, words * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks((int64_t)words + 1) + 1024) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.partials, 2 * 6 * (size_t)w.blocks * sizeof(float)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.barrier, 256));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(BlubViscosity)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.info, sizeof(ViscositySolveInfo)));
+        BLUB_CUDA_CHECK(cudaMemsetAsync(w.info, 0, sizeof(ViscositySolveInfo), stream_));
+        visc_ = w;
+    }
+    // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
+    if (visc_.block) BLUB_CUDA_CHECK(cudaMemcpyAsync(visc_.block, &next, sizeof(next), cudaMemcpyHostToDevice, stream_));
+    if (on != (viscosity_.kinematic_viscosity > 0.0f)) destroy_graphs();
+    viscosity_ = next;
+}
+
+void HybridFluid::run_viscosity() {
+    const NvtxScope scope("apply viscosity");
+    float *u[3] = {u_[0].ptr, u_[1].ptr, u_[2].ptr};
+    launch_viscosity(stream_, grid_, params_dev_, fluid_bits_, marker_.ptr, solid_volume(), u, visc_);
+}
+
+void HybridFluid::last_viscosity_solve(int32_t *iterations, float max_error[3]) {
+    ViscositySolveInfo info{};
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (visc_.info) BLUB_CUDA_CHECK(cudaMemcpyAsync(&info, visc_.info, sizeof(info), cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    *iterations = info.iterations;
+    for (int c = 0; c < 3; ++c) max_error[c] = info.max_error[c];
+}
+
+void HybridFluid::viscosity_only(double simulation_delta_seconds) {
+    if (!(viscosity_.kinematic_viscosity > 0.0f)) throw std::invalid_argument("viscosity_only: the fluid has no viscosity");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const float dt = (float)simulation_delta_seconds;
+    if (!(dt > 0.0f)) throw std::invalid_argument("simulation delta must be positive");
+    upload_step_params(dt);
+    refresh_fluid_bits();
+    run_viscosity();
 }
 
 void HybridFluid::solve_only(int which, double simulation_delta_seconds) {
@@ -1136,6 +1216,11 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
                 drn[i].max_grid[k] = cfg.drains[i].max[k] / scale;
             }
         f->set_flow(src.data(), tags.data(), (uint32_t)src.size(), drn.data(), (uint32_t)drn.size());
+    }
+    if (cfg.viscosity > 0.0f) {
+        BlubViscosity v = kViscosityOff;
+        v.kinematic_viscosity = scene_viscosity_grid(cfg);
+        f->set_viscosity(&v);
     }
     if (!cfg.load_probes.empty()) {
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);

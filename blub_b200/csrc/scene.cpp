@@ -145,6 +145,8 @@ uint32_t tag_of(const JsonValue &obj, const char *what) {
 
 } // namespace
 
+float scene_viscosity_grid(const SceneConfig &cfg) { return cfg.viscosity / (cfg.grid_to_world_scale * cfg.grid_to_world_scale); }
+
 SceneConfig parse_scene_file(const std::string &path) {
     std::ifstream in(path, std::ios::binary);
     if (!in) throw std::ios_base::failure("cannot open scene file " + path);
@@ -196,6 +198,13 @@ SceneConfig parse_scene_file(const std::string &path) {
             vec3(need(d, "max"), "drains.max", b.max);
             cfg.drains.push_back(b);
         }
+    }
+    // kinematic viscosity (not in the reference): a number in m^2/s
+    if (const JsonValue *nu = fluid.get("viscosity")) {
+        if (nu->kind != JsonValue::Number) throw std::runtime_error("scene JSON: `fluid.viscosity` is not a number");
+        cfg.viscosity = num_f32(*nu, "viscosity");
+        if (!std::isfinite(cfg.viscosity) || cfg.viscosity < 0.0f || !std::isfinite(scene_viscosity_grid(cfg)))
+            throw std::runtime_error("scene JSON: `fluid.viscosity` must be finite and not negative");
     }
     // solid load probes (not in the reference): world units, the pivot optional
     if (const JsonValue *probes = fluid.get("load_probes")) {

@@ -25,15 +25,17 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // section 14 followed by the sources' particle tags (written only when one of them is not 0).  Version 3 is not a format: no build writes
 // it and readers refuse it.  Version 8: a fluid with floating bodies; the version-4 layout (section 14 may describe an empty flow set) plus
 // section 15, the bodies.  Versions 3, 5, 6 and 7 are not formats either.  Version 16: a fluid with at least one mesh body; the version-8
-// layout plus section 16, the mesh bodies' geometry and mass properties (its length is what the file holds beyond section 15).
-constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16;
-constexpr uint32_t kNumSections = 16; // at most
+// layout plus section 16, the mesh bodies' geometry and mass properties (its length is what the file holds beyond section 15).  Version 32: a
+// fluid with viscosity; the layout it would otherwise have, promoted to 13 sections, or 14 (section 14 in its version-4 form, possibly an empty
+// set), 15 or 16, plus a last section 17, the viscosity setting: num_sections (14 to 17) tells which.  Versions 17 to 31 are not formats.
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32;
+constexpr uint32_t kNumSections = 17; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES
+    SEC_MESH_BODIES, SEC_VISCOSITY
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -67,6 +69,8 @@ struct MeshBodyRecordHead {
     double volume, centroid[3], principal_moments[3], principal_rotation[4], inertia[9];
 };
 static_assert(sizeof(MeshBodyRecordHead) == 224, "mesh body record layout");
+// Section 17 (version 32): the BlubViscosity as set, kinematic_viscosity > 0
+static_assert(sizeof(BlubViscosity) == 16, "viscosity section layout");
 
 struct StateHeader {
     char magic[8];
@@ -100,7 +104,12 @@ struct Section {
     uint64_t length;
 };
 
-// The sections of a file in their order, with the lengths its header implies; returns their number.
+// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32 header whose
+// num_sections names no layout).  The base sections come first: base_sections() of them, then section 17 in a version-32 file.
+uint32_t base_sections(const StateHeader &h) {
+    if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
+    return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
+}
 uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const Section s[kNumSections] = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
@@ -108,9 +117,13 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
                                      {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
-                                     {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}}; // section 16: the file's remaining bytes
+                                     {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
+                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}};
     std::memcpy(out, s, sizeof(s));
-    return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
+    const uint32_t nb = base_sections(h);
+    if (h.format_version != kFormatVersionViscosity || nb == 0) return nb;
+    out[nb] = s[16];
+    return nb + 1;
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -183,9 +196,9 @@ StateHeader read_header(File &f) {
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
-        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies)
+        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8 and 16)");
+                         " is not supported (this library reads versions 1, 2, 4, 8, 16 and 32)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -203,11 +216,11 @@ StateHeader read_header(File &f) {
     const uint32_t ns = expected_sections(h, sec);
     if (h.num_sections != ns)
         throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(h.format_version) + " has " +
-                         std::to_string(ns));
+                         (ns ? std::to_string(ns) : std::string("14 to 17")));
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
     // version 16: section 16 holds at least its count and one mesh body record
-    if (ns == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
+    if (base_sections(h) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
         throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
 }
@@ -216,12 +229,12 @@ StateHeader read_header(File &f) {
 // every chunk (it must be done with the half `slot` before that half's event is waited on again), then the CRC is checked.
 // the length of section 16 when the file has one: what the file holds beyond section 15, its head and its CRC
 uint64_t mesh_section_length(File &f, const StateHeader &h) {
-    if (h.format_version != kFormatVersionMeshBodies) return 0;
+    if (base_sections(h) != 16) return 0;
     Section sec[kNumSections];
-    expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec);
     uint64_t total = sizeof(StateHeader);
-    for (uint32_t k = 0; k < 15; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
-    return f.size() - total - sizeof(SectionHead) - 4;
+    for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4; // section 16 counted empty
+    return f.size() - total;
 }
 
 template <class Sink> void read_section(File &f, const Section &s, Staging &st, Sink sink) {
@@ -277,7 +290,7 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
 }
 
 // The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.  tags: the sources'
-// particle tags (version 4), or nullptr.  Versions 8 and 16 may describe an empty set.
+// particle tags (version 4), or nullptr.  Versions 8, 16 and 32 may describe an empty set.
 FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHeader &h, const std::string &path) {
     if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version < kFormatVersionBodies))
         throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
@@ -406,30 +419,46 @@ std::vector<BlubBody> mesh_body_set_of(const BodySection &bs, const std::vector<
     return set;
 }
 
+// The setting of section 17, checked with the rules of set_viscosity; a version-32 file has viscosity.
+BlubViscosity viscosity_of(const BlubViscosity &v, const std::string &path) {
+    try {
+        check_viscosity(v);
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": section 17: " + e.what());
+    }
+    if (!(v.kinematic_viscosity > 0.0f)) throw ParseError(path + ": section 17: a version-32 file holds a viscosity above 0");
+    return v;
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
     File f(path, "rb");
     const StateHeader h = read_header(f);
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec), nb = base_sections(h);
     Staging st(false);
     for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
-    if (ns >= 14) {
+    if (nb >= 14) {
         FlowSectionTagged fl{};
         read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
         flow_set_of(fl.flow, fl.source_tags, h, f.path);
     }
-    if (ns >= 15) {
+    if (nb >= 15) {
         BodySection bs{};
         read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
-        if (ns == 15) body_set_of(bs, h, f.path);
+        if (nb == 15) body_set_of(bs, h, f.path);
         else {
             std::vector<char> bytes(mesh_section_length(f, h));
             read_section(f, {SEC_MESH_BODIES, bytes.size()}, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(bytes.data() + off, data, n); });
             std::vector<MeshBodyHost> meshes;
             mesh_body_set_of(bs, bytes, h, f.path, meshes);
         }
+    }
+    if (ns > nb) {
+        BlubViscosity v{};
+        read_section(f, sec[nb], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&v) + off, data, n); });
+        viscosity_of(v, f.path);
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -451,7 +480,8 @@ void HybridFluid::save_state(const std::string &path) {
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
     const bool with_bodies = num_bodies_ > 0;
-    h.format_version = has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool viscous = viscosity_.kinematic_viscosity > 0.0f;
+    h.format_version = viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -470,7 +500,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13;
+    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -515,7 +545,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous ? sizeof(tagged) : sizeof(fl));
         }
         if (with_bodies) {
             BodySection bs{};
@@ -555,6 +585,7 @@ void HybridFluid::save_state(const std::string &path) {
             }
             write_host_section(f, SEC_MESH_BODIES, bytes.data(), bytes.size());
         }
+        if (viscous) write_host_section(f, SEC_VISCOSITY, &viscosity_, sizeof(viscosity_));
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
         f.f = nullptr;
@@ -570,7 +601,7 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     File f(path, "rb");
     const StateHeader h = read_header(f); // every size is checked before anything is allocated
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec), nb = base_sections(h);
     std::unique_ptr<HybridFluid> fluid(
         new HybridFluid(h.grid_dimension[0], h.grid_dimension[1], h.grid_dimension[2], h.max_num_particles, device, stream));
     HybridFluid &x = *fluid;
@@ -611,17 +642,17 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         x.field(which).stats.assign(samples.begin(), samples.end());
     }
     x.fluid_bits_stale_ = true; // rebuilt from the restored marker volume before the next grid pass that reads it
-    if (ns >= 14) {
+    if (nb >= 14) {
         FlowSectionTagged fl{};
         to_host(sec[13], &fl);
         const FlowSet fs = flow_set_of(fl.flow, fl.source_tags, h, f.path);
         BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
         if (fs.num_sources + fs.num_drains > 0) x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
     }
-    if (ns >= 15) { // the history ring is not state: a loaded fluid starts with an empty one
+    if (nb >= 15) { // the history ring is not state: a loaded fluid starts with an empty one
         BodySection bs{};
         to_host(sec[14], &bs);
-        if (ns == 15) x.restore_bodies(body_set_of(bs, h, f.path));
+        if (nb == 15) x.restore_bodies(body_set_of(bs, h, f.path));
         else {
             std::vector<char> bytes(mesh_section_length(f, h));
             to_host({SEC_MESH_BODIES, bytes.size()}, bytes.data());
@@ -629,6 +660,12 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
             const std::vector<BlubBody> set = mesh_body_set_of(bs, bytes, h, f.path, meshes);
             x.restore_bodies(set, std::move(meshes));
         }
+    }
+    if (ns > nb) { // the working volumes and the last solve are not state
+        BlubViscosity v{};
+        to_host(sec[nb], &v);
+        v = viscosity_of(v, f.path);
+        x.set_viscosity(&v);
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

@@ -121,6 +121,12 @@ class TagCensus(C.Structure):
                 ("cell_max", C.c_int32 * 3)]
 
 
+class Viscosity(C.Structure):
+    """BlubViscosity: kinematic viscosity in cells^2/s, the solve's absolute tolerance (cells/s) and iteration cap."""
+
+    _fields_ = [("kinematic_viscosity", C.c_float), ("error_tolerance", C.c_float), ("max_num_iterations", C.c_int32), ("reserved", C.c_uint32)]
+
+
 class LoadProbe(C.Structure):
     """BlubLoadProbe: a box of cells and a pivot, in grid cells."""
 
@@ -289,6 +295,11 @@ def lib():
         "blub_fluid_load_history": (C.c_int, [vp, u32, C.POINTER(SolidLoad), u32, C.POINTER(u32)]),
         "blub_load_probe_cells": (C.c_int, [C.POINTER(u32), C.POINTER(LoadProbe), C.POINTER(u32), C.POINTER(u32)]),
         "blub_scene_load_probes": (C.c_int, [C.c_char_p, C.POINTER(LoadProbe), u32, C.POINTER(u32)]),
+        "blub_fluid_set_viscosity": (C.c_int, [vp, C.POINTER(Viscosity)]),
+        "blub_fluid_viscosity": (C.c_int, [vp, C.POINTER(Viscosity)]),
+        "blub_fluid_last_viscosity_solve": (C.c_int, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
+        "blub_fluid_viscosity_only": (C.c_int, [vp, C.c_double]),
+        "blub_scene_viscosity": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
         "blub_fluid_set_bodies": (C.c_int, [vp, C.POINTER(Body), u32]),
         "blub_fluid_body_history": (C.c_int, [vp, u32, C.POINTER(BodyRecord), u32, C.POINTER(u32)]),
         "blub_fluid_bodies": (C.c_int, [vp, C.POINTER(Body), u32, C.POINTER(u32)]),
@@ -446,6 +457,13 @@ def scene_load_probes(path):
     arr = (LoadProbe * LOAD_PROBES_MAX)()
     _check(lib().blub_scene_load_probes(os.fsencode(path), arr, LOAD_PROBES_MAX, C.byref(count)))
     return [(tuple(p.min_grid), tuple(p.max_grid), tuple(p.pivot_grid)) for p in arr[:count.value]]
+
+
+def scene_viscosity(path):
+    """The scene's fluid.viscosity (m^2/s) in cells^2/s: value / grid_to_world_scale^2, 0.0 without the key (host only)."""
+    out = C.c_float(0)
+    _check(lib().blub_scene_viscosity(os.fsencode(path), C.byref(out)))
+    return float(out.value)
 
 
 def scene_bodies(path):
@@ -713,6 +731,30 @@ class HybridFluid:
         return res
 
     # -- solid load probes --------------------------------------------------------------------
+    def set_viscosity(self, nu, error_tolerance=1e-4, max_num_iterations=200):
+        """Kinematic viscosity in cells^2/s (m^2/s / grid_to_world_scale^2); 0 turns the stage off.  Every step then ends its stage 0 with
+        the implicit diffusion of the grid velocity, solved to max |residual| <= error_tolerance (cells/s) or max_num_iterations.  Raises
+        BlubError (and changes nothing) on a negative or non-finite nu, a tolerance that is not finite and above 0, a cap outside
+        [1, 10000], z-slab ranks and a fluid inside a step."""
+        v = Viscosity(float(nu), float(error_tolerance), int(max_num_iterations), 0)
+        _check(self.L.blub_fluid_set_viscosity(self.h, C.byref(v)))
+
+    def viscosity(self):
+        """(kinematic viscosity in cells^2/s, error_tolerance, max_num_iterations); a viscosity of 0.0 means off."""
+        v = Viscosity()
+        _check(self.L.blub_fluid_viscosity(self.h, C.byref(v)))
+        return float(v.kinematic_viscosity), float(v.error_tolerance), int(v.max_num_iterations)
+
+    def last_viscosity_solve(self):
+        """(iterations, [max |residual| per component]) of the last viscosity solve.  Synchronises."""
+        it, e = C.c_int32(0), (C.c_float * 3)()
+        _check(self.L.blub_fluid_last_viscosity_solve(self.h, C.byref(it), e))
+        return int(it.value), [float(x) for x in e]
+
+    def viscosity_only(self, dt=DT_120HZ):
+        """Test hook: the viscosity stage on the grid velocity and marker as they are (tap uploads), nothing else."""
+        _check(self.L.blub_fluid_viscosity_only(self.h, dt))
+
     def set_load_probes(self, probes=()):
         """Replaces the load probe set: probes = [(min, max[, pivot])] in grid cells (at most 16; pivot default: the box centre).  Resets the
         history.  An empty list clears the set.  Raises BlubError (and changes nothing) on too many probes, non-finite values, boxes empty

@@ -333,6 +333,32 @@ int blub_fluid_body_mass_properties(BlubFluid *fluid, uint32_t body, BlubMeshBod
  * BLUB_ERR_INVALID_ARGUMENT: not a mesh body of the scene; the scene's own errors as blub_scene_info. */
 int blub_scene_body_model(const char *scene_json_path, uint32_t body, char *model_path_out, size_t capacity, float *scale_out);
 
+/* ---- viscous liquids (not part of the reference surface; rules: DESIGN.md section 8) ------------------------------------------------
+ * With a kinematic viscosity above zero every step ends its stage 0 with an implicit diffusion of the grid velocity,
+ * (I - nu dt Laplace) u_c = u_c* per component, solved by Jacobi-preconditioned CG in one persistent kernel: solids (the tank walls, the
+ * solid volume, floating bodies) are no-slip with their own velocity, the free surface carries du_c/dn = 0, gravity's increment is left out
+ * of the diffusion (a tank at rest stays bit for bit what it is without viscosity).  kinematic_viscosity is in cells^2/s (m^2/s divided by
+ * grid_to_world_scale^2); error_tolerance is the absolute bound on max |residual| in cells/s at which the solve stops, max_num_iterations
+ * its cap.  Viscosity is part of the saved state (format version 32). */
+typedef struct {
+    float kinematic_viscosity;
+    float error_tolerance;
+    int32_t max_num_iterations;
+    uint32_t reserved; /* 0 */
+} BlubViscosity;
+/* NULL or kinematic_viscosity == 0 turns the stage off: the step is then the step of a fluid that never had viscosity.  Stream-ordered;
+ * turning it on or off drops the cached step graphs, a change between two positive settings does not.  BLUB_ERR_INVALID_ARGUMENT, changing
+ * nothing: a negative or non-finite viscosity, a tolerance that is not finite or not above 0, max_num_iterations outside [1, 10000],
+ * reserved != 0, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_viscosity(BlubFluid *fluid, const BlubViscosity *viscosity);
+/* the current setting (kinematic_viscosity 0: off) */
+int blub_fluid_viscosity(const BlubFluid *fluid, BlubViscosity *out);
+/* the last viscosity solve, synchronously: its iterations and max |residual| per component (cells/s); zeros before the first solve */
+int blub_fluid_last_viscosity_solve(BlubFluid *fluid, int32_t *iterations, float max_error[3]);
+/* The scene's optional fluid.viscosity (m^2/s) in cells^2/s: value / grid_to_world_scale^2, 0 without the key.  blub_scene_load sets it on
+ * the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
+int blub_scene_viscosity(const char *scene_json_path, float *cells2_per_s);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their
@@ -465,6 +491,9 @@ int blub_fluid_set_particles(BlubFluid *fluid, uint32_t count, const float *pos4
 int blub_fluid_step_stages(BlubFluid *fluid, double simulation_delta_seconds, int from, int to);
 /* PCG only: solve for the rhs currently in the residual tap with the current markers; warm start from the field */
 int blub_fluid_solve_only(BlubFluid *fluid, int which, double simulation_delta_seconds);
+/* viscosity only: applies the viscosity stage to the grid velocity and marker as they are (tap uploads), nothing else;
+ * BLUB_ERR_INVALID_ARGUMENT without a viscosity above zero */
+int blub_fluid_viscosity_only(BlubFluid *fluid, double simulation_delta_seconds);
 /* last finished solve of a field, synchronously: max|r| (not multiplied by dt) and iteration count */
 int blub_fluid_last_solve(BlubFluid *fluid, int which, float *max_error, int32_t *iterations);
 /* work list of the most recent solve (diagnostics for the in-step roofline; synchronises): out[0] = tiles walked by the tile body,

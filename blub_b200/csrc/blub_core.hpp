@@ -305,7 +305,15 @@ class HybridFluid {
     // test hook: the viscosity stage on the grid velocity and marker as they are
     void viscosity_only(double simulation_delta_seconds);
 
+    // CFL-limited substeps (cfl_kernels.cu): max |v_c| over the live particles per axis (one kernel, then synchronises), and the next substep
+    // of `remaining_ns` by cfl_substep_ns with this fluid's gravity (max_velocity_out, may be nullptr, receives the measurement even when the
+    // rule refuses it).  Both throw std::invalid_argument on a z-slab rank or a fluid inside a step; plan_substep checks its arguments before it
+    // launches anything.  The 12-byte result is allocated with the first measurement.
+    void max_particle_velocity(float out[3]);
+    uint64_t plan_substep(uint64_t remaining_ns, const BlubTimeStepping &ts, float max_velocity_out[3]);
+
   private:
+    uint32_t *max_velocity_dev_ = nullptr;
     BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
     unsigned long long *body_sums_ = nullptr; // composite volume, allocated with the first non-empty set
     BlubBodyRecord *body_ring_ = nullptr;
@@ -436,6 +444,13 @@ struct IoError : std::runtime_error {
 struct ParseError : std::runtime_error {
     explicit ParseError(const std::string &what) : std::runtime_error(what) {}
 };
+// A CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns (BLUB_ERR_UNSTABLE).
+struct UnstableError : std::runtime_error {
+    explicit UnstableError(const std::string &what) : std::runtime_error(what) {}
+};
+// CFL-limited substeps (cfl_kernels.cu, DESIGN.md §8): the config's range rules (std::invalid_argument), and the host rule of blub_cfl_substep_ns.
+void check_time_stepping(const BlubTimeStepping &ts);
+uint64_t cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping &ts);
 struct StateInfo {
     uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
 };

@@ -25,6 +25,12 @@
 //   --models DIR   where the scene's static_objects find their OBJ files (the reference reads `models/<model>`,
 //                  src/scene/models.rs:253).  Every step then runs Scene::step's order (src/scene/mod.rs:192-211): animate the
 //                  models at the already advanced simulation time, voxelize their hulls, step the fluid.
+//   --cfl C        CFL-limited substeps (not in the reference): every fixed step of 1 / hz becomes an interval that planned substeps cover
+//                  (blub_fluid_plan_substep with CFL number C, max_dt = the interval, min_dt = interval / 256, so at most 258 substeps).  The
+//                  static objects are voxelized at each substep's time with that substep's delta; the clock at interval boundaries is the
+//                  fixed run's, --steps counts intervals (also with --record), and the load and body histories are collected after every
+//                  interval.  --stats gains "time_stepping" with every substep's length and measured velocity.  Refused with --load-state:
+//                  the clock of a resumed adaptive run is not step_count * dt.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -52,16 +58,17 @@ int main(int argc, char **argv) {
                              "                [--stats out.json] [--trace out.json] [--dump particles.f32] [--models DIR] [--record FPS PREFIX]\n"
                              "                [--solver TOLERANCE MAX_ITERATIONS CHECK_FREQUENCY] [--rebin EVERY_N_STEPS]\n"
                              "                [--save-state FILE [--checkpoint-every N]] [--load-state FILE] [--loads out.json]\n"
-                             "                [--bodies out.json]\n");
+                             "                [--bodies out.json] [--cfl C]\n");
         return 2;
     }
     const char *scene = argv[1];
     int steps = 160, batch = 16, device = 0, graph = 1;
     long hz = 120;
     std::string bodies_path, loads_path, stats_path, trace_path, dump_path, models_dir = "models", record_prefix, save_path, load_path;
-    double record_fps = 0.0;
+    double record_fps = 0.0, cfl = 0.0;
     float solver_tol = -1.0f;
     int solver_max = 0, solver_freq = 0, rebin = -1, checkpoint_every = 0;
+    bool adaptive = false; // --cfl
     for (int i = 2; i < argc; ++i) {
         auto next = [&](const char *flag) -> const char * {
             if (i + 1 >= argc) { std::fprintf(stderr, "blub_run: %s needs a value\n", flag); std::exit(2); }
@@ -84,6 +91,7 @@ int main(int argc, char **argv) {
         else if (!std::strcmp(argv[i], "--checkpoint-every")) checkpoint_every = std::atoi(next("--checkpoint-every"));
         else if (!std::strcmp(argv[i], "--load-state")) load_path = next("--load-state");
         else if (!std::strcmp(argv[i], "--record")) { record_fps = std::atof(next("--record")); record_prefix = next("--record"); }
+        else if (!std::strcmp(argv[i], "--cfl")) { cfl = std::atof(next("--cfl")); adaptive = true; }
         else { std::fprintf(stderr, "blub_run: unknown option %s\n", argv[i]); return 2; }
     }
     if (steps < 1 || batch < 1 || hz < 1) { std::fprintf(stderr, "blub_run: bad --steps/--batch/--hz\n"); return 2; }
@@ -103,6 +111,19 @@ int main(int argc, char **argv) {
     if (checkpoint_every < 0 || (checkpoint_every > 0 && save_path.empty())) {
         std::fprintf(stderr, "blub_run: --checkpoint-every needs a positive N and --save-state FILE\n");
         return 2;
+    }
+    const BlubTimeStepping time_stepping = {(float)cfl, 0u, dt_ns, dt_ns / 256 > 0 ? dt_ns / 256 : 1};
+    if (adaptive) {
+        const float zero[3] = {0.0f, 0.0f, 0.0f};
+        uint64_t probe_ns = 0;
+        if (blub_cfl_substep_ns(dt_ns, zero, zero, &time_stepping, &probe_ns) != BLUB_OK) {
+            std::fprintf(stderr, "blub_run: bad --cfl: %s\n", blub_last_error());
+            return 2;
+        }
+        if (!load_path.empty()) {
+            std::fprintf(stderr, "blub_run: --cfl cannot resume a --load-state file (the clock of an adaptive run is not step_count * dt)\n");
+            return 2;
+        }
     }
 
     BlubSceneInfo info;
@@ -161,14 +182,40 @@ int main(int argc, char **argv) {
     }
     // Timer::total_simulated_time / total_rendered_time; a resumed run continues the clock, so that animated solids are where they were
     uint64_t simulated_ns = (uint64_t)blub_fluid_step_count(fluid) * dt_ns, rendered_ns = 0;
-    auto scene_step = [&]() {
-        simulated_ns += dt_ns; // advanced BEFORE the step it belongs to (src/timer.rs:122-124)
-        const double simulated = (double)blub_duration_as_secs_f32(simulated_ns);
+    // one step of `delta_ns` ending at simulated_ns: the solids at that time, then the fluid
+    auto voxelize_and_step = [&](uint64_t delta_ns) {
+        const double simulated = (double)blub_duration_as_secs_f32(simulated_ns), delta = (double)blub_duration_as_secs_f32(delta_ns);
         for (size_t k = 0; k < solids.size(); ++k)
             if (blub_solid_voxelize_mesh(voxels, info.grid_dimension, solids[k].mesh, &solids[k].placement, info.grid_to_world_scale, info.world_position,
-                                         simulated, dt, k == 0, blub_fluid_stream(fluid), nullptr))
+                                         simulated, delta, k == 0, blub_fluid_stream(fluid), nullptr))
                 die("voxelization failed");
-        if (blub_fluid_step(fluid, dt)) die("step failed");
+        if (blub_fluid_step(fluid, delta)) die("step failed");
+    };
+    // --cfl: every substep's length and the velocity it was planned from, per interval
+    struct Interval {
+        std::vector<uint64_t> dt_ns;
+        std::vector<float> max_velocity; // 3 per substep
+    };
+    std::vector<Interval> intervals;
+    auto scene_step = [&]() {
+        if (!adaptive) {
+            simulated_ns += dt_ns; // advanced BEFORE the step it belongs to (src/timer.rs:122-124)
+            voxelize_and_step(dt_ns);
+            return;
+        }
+        const uint64_t start_ns = simulated_ns;
+        Interval rec;
+        for (uint64_t covered = 0; covered < dt_ns;) {
+            uint64_t sub_ns = 0;
+            float v[3];
+            if (blub_fluid_plan_substep(fluid, dt_ns - covered, &time_stepping, &sub_ns, v)) die("cannot plan a substep");
+            covered += sub_ns;
+            simulated_ns = start_ns + covered;
+            voxelize_and_step(sub_ns);
+            rec.dt_ns.push_back(sub_ns);
+            rec.max_velocity.insert(rec.max_velocity.end(), v, v + 3);
+        }
+        intervals.push_back(std::move(rec));
     };
 
     auto write_particles = [&](const std::string &path) {
@@ -211,6 +258,15 @@ int main(int argc, char **argv) {
         }
     };
 
+    // one fixed step, or with --cfl one interval and then the histories (up to 258 substeps must not overrun the 1024-record rings)
+    auto scene_interval = [&]() {
+        scene_step();
+        if (adaptive) {
+            collect_loads();
+            collect_bodies();
+        }
+    };
+
     const bool has_flow = blub_fluid_has_flow(fluid) == 1;
     int done = 0, saved_at = -1;
     auto save_state = [&]() {
@@ -229,7 +285,7 @@ int main(int argc, char **argv) {
         for (int frame = 0; done < steps; ++frame) {
             uint32_t n = blub_timer_steps_in_frame(&rendered_ns, &clock_ns, frame_ns, dt_ns);
             if ((int)n > steps - done) n = (uint32_t)(steps - done);
-            for (uint32_t k = 0; k < n; ++k) scene_step();
+            for (uint32_t k = 0; k < n; ++k) scene_interval();
             if (blub_fluid_synchronize(fluid)) die("synchronize failed");
             blub_fluid_update_statistics(fluid);
             done += (int)n;
@@ -244,7 +300,7 @@ int main(int argc, char **argv) {
     }
     while (done < steps) { // MAX_FAST_FORWARD_SIMULATION_BATCH_SIZE = 16, then wait for the GPU
         const int n = steps - done < batch ? steps - done : batch;
-        for (int k = 0; k < n; ++k) scene_step();
+        for (int k = 0; k < n; ++k) scene_interval();
         if (blub_fluid_synchronize(fluid)) die("synchronize failed");
         blub_fluid_update_statistics(fluid);
         done += n;
@@ -287,6 +343,20 @@ int main(int argc, char **argv) {
             if (blub_fluid_last_viscosity_solve(fluid, &it, e)) die("cannot read the last viscosity solve");
             std::fprintf(f, ", \"viscosity\": {\"kinematic_viscosity\": %.9g, \"last_iterations\": %d, \"last_max_error\": [%.9g, %.9g, %.9g]}",
                          visc.kinematic_viscosity, it, e[0], e[1], e[2]);
+        }
+        if (adaptive) {
+            std::fprintf(f, ", \"time_stepping\": {\"cfl\": %.9g, \"interval_ns\": %llu, \"min_dt_ns\": %llu, \"intervals\": [", (double)time_stepping.cfl_number,
+                         (unsigned long long)dt_ns, (unsigned long long)time_stepping.min_dt_ns);
+            for (size_t i = 0; i < intervals.size(); ++i) {
+                const Interval &r = intervals[i];
+                std::fprintf(f, "%s\n {\"dt_ns\": [", i ? "," : "");
+                for (size_t k = 0; k < r.dt_ns.size(); ++k) std::fprintf(f, "%s%llu", k ? ", " : "", (unsigned long long)r.dt_ns[k]);
+                std::fprintf(f, "], \"max_velocity\": [");
+                for (size_t k = 0; k < r.dt_ns.size(); ++k)
+                    std::fprintf(f, "%s[%.9g, %.9g, %.9g]", k ? ", " : "", r.max_velocity[3 * k], r.max_velocity[3 * k + 1], r.max_velocity[3 * k + 2]);
+                std::fprintf(f, "]}");
+            }
+            std::fprintf(f, "\n]}");
         }
         std::fprintf(f, "}\n");
         std::fclose(f);

@@ -39,6 +39,8 @@ template <class F> int guarded(F &&f) {
         return fail(BLUB_ERR_IO, e.what());
     } catch (const blub::ParseError &e) {
         return fail(BLUB_ERR_PARSE, e.what());
+    } catch (const blub::UnstableError &e) {
+        return fail(BLUB_ERR_UNSTABLE, e.what());
     } catch (const std::exception &e) {
         return fail(BLUB_ERR_PARSE, e.what());
     } catch (...) {
@@ -507,6 +509,21 @@ int blub_fluid_last_viscosity_solve(BlubFluid *fluid, int32_t *iterations, float
 int blub_scene_viscosity(const char *path, float *cells2_per_s) {
     if (!path || !cells2_per_s) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] { *cells2_per_s = blub::scene_viscosity_grid(blub::parse_scene_file(path)); return BLUB_OK; });
+}
+
+int blub_fluid_max_particle_velocity(BlubFluid *fluid, float out[3]) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->max_particle_velocity(out); return BLUB_OK; });
+}
+
+int blub_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping *config, uint64_t *dt_ns) {
+    if (!max_velocity || !gravity_grid || !config || !dt_ns) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *dt_ns = blub::cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, *config); return BLUB_OK; });
+}
+
+int blub_fluid_plan_substep(BlubFluid *fluid, uint64_t remaining_ns, const BlubTimeStepping *config, uint64_t *dt_ns, float max_velocity_out[3]) {
+    if (!fluid || !config || !dt_ns) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *dt_ns = fluid->impl->plan_substep(remaining_ns, *config, max_velocity_out); return BLUB_OK; });
 }
 
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }

@@ -225,4 +225,9 @@ int viscosity_solve_blocks(); // SMs x resident blocks per SM; throws CudaError 
 void launch_viscosity(cudaStream_t st, const GridDim &g, const StepParams *params, const FluidBits &bits, const int8_t *marker, const uint2 *vox,
                       float *const u[3], const ViscosityWork &w);
 
+// ---- CFL-limited substeps (cfl_kernels.cu, DESIGN.md §8 "CFL-limited substeps") ----
+// out[c] = the bits of max |v_c| over the particles (params->num_particles when `params` is not null, else n_host; np_upper sizes the launch).
+// Zeroes the three words first.
+void launch_max_particle_velocity(cudaStream_t st, const StepParams *params, uint32_t n_host, uint32_t np_upper, float4 *const row[3], uint32_t *out);
+
 } // namespace blub

@@ -223,6 +223,7 @@ HybridFluid::~HybridFluid() {
     cudaFree(visc_.block);
     cudaFree(visc_.info);
     cudaFree(census_dev_);
+    cudaFree(max_velocity_dev_);
     cudaFree(load_probes_dev_);
     cudaFree(load_ring_);
     cudaFree(bodies_dev_);
@@ -928,6 +929,30 @@ void HybridFluid::tag_census(uint32_t first, uint32_t num_tags, BlubTagCensus *o
                       row_, census_dev_);
     BLUB_CUDA_CHECK(cudaMemcpyAsync(out, census_dev_, bytes, cudaMemcpyDeviceToHost, stream_));
     BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// CFL-limited substeps (cfl_kernels.cu).  Not in the reference.  The count follows the tags' rule: the device count in device-count mode.
+void HybridFluid::max_particle_velocity(float out[3]) {
+    if (slab_world_ > 1) throw std::invalid_argument("max_particle_velocity: z-slab ranks cannot plan substeps");
+    if (mid_step_) throw std::invalid_argument("max_particle_velocity: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (!max_velocity_dev_) BLUB_CUDA_CHECK(cudaMalloc(&max_velocity_dev_, 3 * sizeof(uint32_t)));
+    const bool dev = device_count_mode();
+    launch_max_particle_velocity(stream_, dev ? params_dev_ : nullptr, num_particles_, dev ? max_num_particles_ : num_particles_, row_, max_velocity_dev_);
+    uint32_t bits[3];
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(bits, max_velocity_dev_, sizeof(bits), cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    std::memcpy(out, bits, sizeof(bits));
+}
+
+uint64_t HybridFluid::plan_substep(uint64_t remaining_ns, const BlubTimeStepping &ts, float max_velocity_out[3]) {
+    check_time_stepping(ts);
+    if (remaining_ns == 0) throw std::invalid_argument("plan_substep: remaining_ns must be above 0");
+    float v[3];
+    max_particle_velocity(v);
+    if (max_velocity_out) std::memcpy(max_velocity_out, v, sizeof(v));
+    return cfl_substep_ns(remaining_ns, v, gravity_, ts);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -25,6 +25,7 @@ STAGES = [
 TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, TAP_P_DEN, TAP_RESIDUAL, TAP_SOLID_VOXELS = range(12)
 
 BLUB_OK = 0
+BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
 BLUB_WARN_TRUNCATED = 100
 TAG_CENSUS_FRAC_BITS = 16  # BLUB_TAG_CENSUS_FRAC_BITS: census sums are sums of rint(value * 2^16)
 TAG_CENSUS_MAX = 256       # tags per census
@@ -125,6 +126,12 @@ class Viscosity(C.Structure):
     """BlubViscosity: kinematic viscosity in cells^2/s, the solve's absolute tolerance (cells/s) and iteration cap."""
 
     _fields_ = [("kinematic_viscosity", C.c_float), ("error_tolerance", C.c_float), ("max_num_iterations", C.c_int32), ("reserved", C.c_uint32)]
+
+
+class TimeStepping(C.Structure):
+    """BlubTimeStepping: the CFL number C in (0, 16] and the longest and shortest substep in nanoseconds (1 <= min <= max)."""
+
+    _fields_ = [("cfl_number", C.c_float), ("reserved", C.c_uint32), ("max_dt_ns", C.c_uint64), ("min_dt_ns", C.c_uint64)]
 
 
 class LoadProbe(C.Structure):
@@ -300,6 +307,9 @@ def lib():
         "blub_fluid_last_viscosity_solve": (C.c_int, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
         "blub_fluid_viscosity_only": (C.c_int, [vp, C.c_double]),
         "blub_scene_viscosity": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
+        "blub_fluid_max_particle_velocity": (C.c_int, [vp, f3]),
+        "blub_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
+        "blub_fluid_plan_substep": (C.c_int, [vp, C.c_uint64, C.POINTER(TimeStepping), C.POINTER(C.c_uint64), f3]),
         "blub_fluid_set_bodies": (C.c_int, [vp, C.POINTER(Body), u32]),
         "blub_fluid_body_history": (C.c_int, [vp, u32, C.POINTER(BodyRecord), u32, C.POINTER(u32)]),
         "blub_fluid_bodies": (C.c_int, [vp, C.POINTER(Body), u32, C.POINTER(u32)]),
@@ -464,6 +474,21 @@ def scene_viscosity(path):
     out = C.c_float(0)
     _check(lib().blub_scene_viscosity(os.fsencode(path), C.byref(out)))
     return float(out.value)
+
+
+def time_stepping(cfl, max_dt_ns, min_dt_ns):
+    """A BlubTimeStepping (the library checks its ranges where it is used)."""
+    return TimeStepping(float(cfl), 0, int(max_dt_ns), int(min_dt_ns))
+
+
+def cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, cfl=1.0, max_dt_ns=None, min_dt_ns=1):
+    """blub_cfl_substep_ns (host only): the length in ns of the next substep of `remaining_ns` for the largest particle velocity per axis
+    `max_velocity` (cells/s) under gravity `gravity_grid` (cells/s^2); max_dt_ns defaults to remaining_ns.  Raises BlubError on a bad config
+    or remaining_ns == 0 (error 1), and on a non-finite velocity or a CFL step below min_dt_ns (error 6, BLUB_ERR_UNSTABLE)."""
+    out = C.c_uint64(0)
+    ts = time_stepping(cfl, remaining_ns if max_dt_ns is None else max_dt_ns, min_dt_ns)
+    _check(lib().blub_cfl_substep_ns(int(remaining_ns), _f3(max_velocity), _f3(gravity_grid), C.byref(ts), C.byref(out)))
+    return int(out.value)
 
 
 def scene_bodies(path):
@@ -754,6 +779,38 @@ class HybridFluid:
     def viscosity_only(self, dt=DT_120HZ):
         """Test hook: the viscosity stage on the grid velocity and marker as they are (tap uploads), nothing else."""
         _check(self.L.blub_fluid_viscosity_only(self.h, dt))
+
+    # -- CFL-limited substeps -----------------------------------------------------------------
+    def max_particle_velocity(self):
+        """[max |v_x|, max |v_y|, max |v_z|] over the live particles in cells/s, exact (float32 values).  One kernel, then synchronises."""
+        out = (C.c_float * 3)()
+        _check(self.L.blub_fluid_max_particle_velocity(self.h, out))
+        return [float(x) for x in out]
+
+    def plan_substep(self, remaining_ns, cfl=1.0, max_dt_ns=None, min_dt_ns=1):
+        """(dt_ns, max_velocity): the measured largest particle velocity per axis and the next substep of `remaining_ns` by the CFL rule
+        (cfl_substep_ns) with this fluid's gravity; max_dt_ns defaults to remaining_ns.  Raises BlubError as cfl_substep_ns does, and on a
+        z-slab rank or a fluid inside a step."""
+        ts = time_stepping(cfl, remaining_ns if max_dt_ns is None else max_dt_ns, min_dt_ns)
+        dt, v = C.c_uint64(0), (C.c_float * 3)()
+        _check(self.L.blub_fluid_plan_substep(self.h, int(remaining_ns), C.byref(ts), C.byref(dt), v))
+        return int(dt.value), [float(x) for x in v]
+
+    def advance(self, interval_ns, cfl=1.0, max_dt_ns=None, min_dt_ns=None):
+        """Covers `interval_ns` with CFL-limited substeps: plan, then step(duration_as_secs_f32(dt_ns)), until the substeps add up to the
+        interval.  Defaults: max_dt_ns = interval_ns, min_dt_ns = max(1, interval_ns // 256).  Returns [(dt_ns, max_velocity)], one per
+        substep.  Every plan synchronises; raises BlubError (BLUB_ERR_UNSTABLE: error 6) when a substep cannot be planned, after the substeps
+        already taken."""
+        interval_ns = int(interval_ns)
+        max_dt_ns = interval_ns if max_dt_ns is None else int(max_dt_ns)
+        min_dt_ns = max(1, interval_ns // 256) if min_dt_ns is None else int(min_dt_ns)
+        done, out = 0, []
+        while done < interval_ns:
+            dt_ns, v = self.plan_substep(interval_ns - done, cfl, max_dt_ns, min_dt_ns)
+            self.step(float(self.L.blub_duration_as_secs_f32(dt_ns)))
+            done += dt_ns
+            out.append((dt_ns, v))
+        return out
 
     def set_load_probes(self, probes=()):
         """Replaces the load probe set: probes = [(min, max[, pivot])] in grid cells (at most 16; pivot default: the box centre).  Resets the

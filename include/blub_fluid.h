@@ -359,6 +359,37 @@ int blub_fluid_last_viscosity_solve(BlubFluid *fluid, int32_t *iterations, float
  * the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
 int blub_scene_viscosity(const char *scene_json_path, float *cells2_per_s);
 
+/* ---- CFL-limited substeps (not part of the reference surface, whose clock is a fixed 120 Hz; rules: DESIGN.md section 8) -----------
+ * The library can choose the length of the next step from the particles' largest velocity.  An adaptive run is an ordinary sequence of
+ * blub_fluid_step calls: plan a substep of the time still to cover, step it as blub_fluid_step(fluid, blub_duration_as_secs_f32(dt_ns))
+ * (the conversion blub_run uses for its fixed step), repeat until the interval is covered.  The step itself, its graphs and the state file are
+ * unchanged, and a fluid that never plans launches and allocates nothing for it.
+ * The rule (float64, integer nanoseconds): u = max_c |max_velocity[c]|; s = u + sqrt(5 |g|) with |g| the Euclidean norm of the gravity in
+ * cells/s^2 (Bridson's margin for the speed one step of gravity adds, dx = 1 cell); d = cfl_number / s seconds (+infinity when s = 0);
+ * d_ns = min(max_dt_ns, floor(d * 1e9)), saturating.  d_ns < min_dt_ns is refused with BLUB_ERR_UNSTABLE.  Otherwise, with R the time
+ * still to cover: dt = R when R <= d_ns, R - R / 2 (integer division) when R < 2 d_ns (the interval does not end in a sliver), else d_ns.
+ * Each particle then moves at most cfl_number cells along each axis at its current velocity (a per-axis bound, not a Euclidean one), and the
+ * substeps of an interval add up to it exactly. */
+#define BLUB_ERR_UNSTABLE 6 /* a non-finite particle velocity, or a CFL step below min_dt_ns: nothing was stepped */
+typedef struct {
+    float cfl_number;   /* C: finite, in (0, 16] */
+    uint32_t reserved;  /* 0 */
+    uint64_t max_dt_ns; /* the longest substep */
+    uint64_t min_dt_ns; /* 1 <= min_dt_ns <= max_dt_ns: a CFL step below it is refused */
+} BlubTimeStepping;
+/* out[c] = max |v_c| over the live particles (v_c = the .w word of velocity row c; the device-resident count while a flow set is active),
+ * exact: +0 without particles, infinity and NaN as themselves.  Runs one kernel, then synchronises.  BLUB_ERR_INVALID_ARGUMENT: a z-slab rank
+ * or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_max_particle_velocity(BlubFluid *fluid, float out[3]);
+/* Host only, no device needed: the rule above applied to a measured max_velocity (cells/s per axis) and gravity (cells/s^2).
+ * BLUB_ERR_INVALID_ARGUMENT: a bad config (cfl_number not finite or outside (0, 16], reserved != 0, not 1 <= min_dt_ns <= max_dt_ns),
+ * remaining_ns == 0 or a non-finite gravity.  BLUB_ERR_UNSTABLE: a non-finite velocity or d_ns < min_dt_ns; blub_last_error names the case
+ * and the velocity. */
+int blub_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping *config, uint64_t *dt_ns);
+/* blub_fluid_max_particle_velocity, then blub_cfl_substep_ns with the fluid's gravity.  max_velocity_out (may be NULL) receives the measurement,
+ * also when the rule refuses it.  Refuses what both refuse, checking the config and remaining_ns before anything is launched. */
+int blub_fluid_plan_substep(BlubFluid *fluid, uint64_t remaining_ns, const BlubTimeStepping *config, uint64_t *dt_ns, float max_velocity_out[3]);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their

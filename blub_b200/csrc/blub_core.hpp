@@ -312,6 +312,15 @@ class HybridFluid {
     void max_particle_velocity(float out[3]);
     uint64_t plan_substep(uint64_t remaining_ns, const BlubTimeStepping &ts, float max_velocity_out[3]);
 
+    // Surface tension (surface_tension_kernels.cu): a kinematic surface tension in cells^3/s^2, 0 turns it off.  Stream-ordered; the working
+    // volumes are allocated with the first value above zero, and only a change between off and on drops the step graphs.  Throws
+    // std::invalid_argument and changes nothing on a negative or non-finite value, a z-slab rank or a fluid inside a step.  While it is on,
+    // plan_substep holds every substep to capillary_limit_ns.
+    void set_surface_tension(float cells3_per_s2);
+    float surface_tension() const { return surface_tension_; }
+    float *curvature() const { return st_.kappa; }             // nullptr before the first surface tension above zero
+    long long *density_accumulator() const { return density_.ptr; }
+
   private:
     uint32_t *max_velocity_dev_ = nullptr;
     BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
@@ -327,6 +336,8 @@ class HybridFluid {
     void free_mesh_bodies();
     BlubViscosity viscosity_ = kViscosityOff;
     ViscosityWork visc_;
+    float surface_tension_ = 0.0f;
+    SurfaceTensionWork st_;
     void run_viscosity();
     LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
     BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
@@ -450,6 +461,9 @@ struct UnstableError : std::runtime_error {
 };
 // CFL-limited substeps (cfl_kernels.cu, DESIGN.md §8): the config's range rules (std::invalid_argument), and the host rule of blub_cfl_substep_ns.
 void check_time_stepping(const BlubTimeStepping &ts);
+// Brackbill's capillary step limit with dx = 1 cell and the mean of the liquid and air densities: floor(1e9 sqrt(1 / (4 pi s))) ns for a
+// kinematic surface tension s > 0 (cells^3/s^2), saturating at UINT64_MAX.
+uint64_t capillary_limit_ns(float cells3_per_s2);
 uint64_t cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping &ts);
 struct StateInfo {
     uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
@@ -546,6 +560,7 @@ struct SceneConfig {
     std::vector<SceneLoadProbe> load_probes; // optional fluid.load_probes (world units)
     std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
     float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
+    float surface_tension = 0.0f;            // optional fluid.surface_tension: kinematic, m^3/s^2
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };
@@ -554,6 +569,8 @@ SceneConfig parse_scene_file(const std::string &path);
 std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
 // the scene's kinematic viscosity in cells^2/s: viscosity / grid_to_world_scale^2
 float scene_viscosity_grid(const SceneConfig &cfg);
+// the scene's kinematic surface tension in cells^3/s^2: surface_tension / grid_to_world_scale^3
+float scene_surface_tension_grid(const SceneConfig &cfg);
 // the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a
 // quaternion (quat_from_euler_deg_wxyz), the angular velocity unchanged
 std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg);

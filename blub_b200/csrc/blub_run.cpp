@@ -344,6 +344,9 @@ int main(int argc, char **argv) {
             std::fprintf(f, ", \"viscosity\": {\"kinematic_viscosity\": %.9g, \"last_iterations\": %d, \"last_max_error\": [%.9g, %.9g, %.9g]}",
                          visc.kinematic_viscosity, it, e[0], e[1], e[2]);
         }
+        float sigma = 0.0f;
+        if (blub_fluid_surface_tension(fluid, &sigma)) die("cannot read the surface tension");
+        if (sigma > 0.0f) std::fprintf(f, ", \"surface_tension\": %.9g", sigma);
         if (adaptive) {
             std::fprintf(f, ", \"time_stepping\": {\"cfl\": %.9g, \"interval_ns\": %llu, \"min_dt_ns\": %llu, \"intervals\": [", (double)time_stepping.cfl_number,
                          (unsigned long long)dt_ns, (unsigned long long)time_stepping.min_dt_ns);

@@ -69,6 +69,8 @@ Tap tap_of(BlubFluid *f, int tap) {
     case BLUB_TAP_PRESSURE_DENSITY: return {h.field(1).pressure(), n * 4};
     case BLUB_TAP_RESIDUAL: return {h.solver().residual(), n * 4};
     case BLUB_TAP_SOLID_VOXELS: return {const_cast<uint2 *>(h.solid_volume()), n * 8};
+    case BLUB_TAP_CURVATURE: return {h.curvature(), n * 4}; // nullptr before the first surface tension above zero: zeros
+    case BLUB_TAP_DENSITY: return {h.density_accumulator(), n * 8};
     default: return {nullptr, 0};
     }
 }
@@ -516,6 +518,22 @@ int blub_fluid_max_particle_velocity(BlubFluid *fluid, float out[3]) {
     return guarded([&] { fluid->impl->max_particle_velocity(out); return BLUB_OK; });
 }
 
+int blub_fluid_set_surface_tension(BlubFluid *fluid, float cells3_per_s2) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_surface_tension(cells3_per_s2); return BLUB_OK; });
+}
+
+int blub_fluid_surface_tension(const BlubFluid *fluid, float *cells3_per_s2) {
+    if (!fluid || !cells3_per_s2) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *cells3_per_s2 = fluid->impl->surface_tension();
+    return BLUB_OK;
+}
+
+int blub_scene_surface_tension(const char *path, float *cells3_per_s2) {
+    if (!path || !cells3_per_s2) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *cells3_per_s2 = blub::scene_surface_tension_grid(blub::parse_scene_file(path)); return BLUB_OK; });
+}
+
 int blub_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping *config, uint64_t *dt_ns) {
     if (!max_velocity || !gravity_grid || !config || !dt_ns) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] { *dt_ns = blub::cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, *config); return BLUB_OK; });
@@ -601,6 +619,11 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
     if (!fluid || !host_dst) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
+        if (tap == BLUB_TAP_CURVATURE && !t.ptr) {
+            if (bytes > (size_t)fluid->impl->grid_dimension().n * 4) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
+            std::memset(host_dst, 0, bytes);
+            return BLUB_OK;
+        }
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
         BLUB_CUDA_CHECK(cudaSetDevice(fluid->impl->device()));
         BLUB_CUDA_CHECK(cudaMemcpyAsync(host_dst, t.ptr, bytes, cudaMemcpyDeviceToHost, fluid->impl->stream()));
@@ -611,7 +634,8 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
 
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes) {
     if (!fluid || !host_src) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
-    if (tap == BLUB_TAP_SOLID_VOXELS) return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume tap is download only");
+    if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY)
+        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature and density taps are download only");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");

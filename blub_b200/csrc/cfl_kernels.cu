@@ -71,6 +71,11 @@ void check_time_stepping(const BlubTimeStepping &ts) {
     if (ts.min_dt_ns < 1u || ts.min_dt_ns > ts.max_dt_ns) throw std::invalid_argument("time stepping: 1 <= min_dt_ns <= max_dt_ns is required");
 }
 
+uint64_t capillary_limit_ns(float s) {
+    const double d_scaled = std::floor(1e9 * std::sqrt(1.0 / (4.0 * M_PI * (double)s)));
+    return d_scaled < 18446744073709551616.0 ? (uint64_t)d_scaled : UINT64_MAX;
+}
+
 uint64_t cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping &ts) {
     check_time_stepping(ts);
     if (remaining_ns == 0) throw std::invalid_argument("cfl substep: remaining_ns must be above 0");

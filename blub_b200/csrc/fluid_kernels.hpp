@@ -230,4 +230,22 @@ void launch_viscosity(cudaStream_t st, const GridDim &g, const StepParams *param
 // Zeroes the three words first.
 void launch_max_particle_velocity(cudaStream_t st, const StepParams *params, uint32_t n_host, uint32_t np_upper, float4 *const row[3], uint32_t *out);
 
+// ---- surface tension (surface_tension_kernels.cu, DESIGN.md §8 "Surface tension") ----
+// Working memory, allocated with the first surface tension above zero: 12 bytes per cell.
+struct SurfaceTensionWork {
+    long long *psi = nullptr; // n: the wall-ruled splat (2^-32 particle weights), valid within 3 cells of FLUID
+    float *kappa = nullptr;   // n: the curvature of the last stage 1 in the band (cells^-1), 0 elsewhere
+    float *sigma = nullptr;   // the kinematic surface tension the kernels read (cells^3/s^2): a change does not invalidate a captured graph
+};
+// Stage 1: the wall rule on the splat in `density`, the smoothed field phi written back into `density` (within 2 cells of FLUID), the
+// curvature into w.kappa.  `density` must hold the splat of the current positions (launch_density_scatter).
+void launch_surface_curvature(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, long long *density,
+                              const SurfaceTensionWork &w);
+// Stage 1, after the divergence: rhs += the ghost values of every FLUID cell's AIR faces.  Writes FLUID cells only.
+void launch_surface_rhs(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
+                        const SurfaceTensionWork &w, float *rhs);
+// Stage 4, after the projection: the FLUID-AIR faces get the ghost value the solve assumed.
+void launch_surface_faces(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
+                          const SurfaceTensionWork &w, float *const u[3]);
+
 } // namespace blub

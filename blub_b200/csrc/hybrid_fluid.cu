@@ -34,6 +34,28 @@ void note_record(std::deque<uint32_t> &steps, uint32_t step, uint32_t length) {
     // a slot holds the newest of the steps that map to it
     while (steps.size() > length || (uint64_t)steps.front() + length <= step) steps.pop_front();
 }
+// Frees what an allocation of the working memory got to (cudaFree(nullptr) is a no-op): the destructor, and a first allocation that failed halfway.
+void free_work(ViscosityWork &w) {
+    cudaFree(w.codes);
+    for (int c = 0; c < 3; ++c) {
+        cudaFree(w.r[c]);
+        cudaFree(w.s[c]);
+    }
+    cudaFree(w.word_flags);
+    cudaFree(w.words);
+    cudaFree(w.scan_sums);
+    cudaFree(w.partials);
+    cudaFree(w.barrier);
+    cudaFree(w.block);
+    cudaFree(w.info);
+    w = ViscosityWork{};
+}
+void free_work(SurfaceTensionWork &w) {
+    cudaFree(w.psi);
+    cudaFree(w.kappa);
+    cudaFree(w.sigma);
+    w = SurfaceTensionWork{};
+}
 } // namespace
 
 HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num_particles, int device, cudaStream_t stream, int slab_rank,
@@ -210,18 +232,8 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.scan_sums);
     cudaFree(flow_scratch_.scalars);
     cudaFree(flow_scratch_.counters);
-    cudaFree(visc_.codes);
-    for (int c = 0; c < 3; ++c) {
-        cudaFree(visc_.r[c]);
-        cudaFree(visc_.s[c]);
-    }
-    cudaFree(visc_.word_flags);
-    cudaFree(visc_.words);
-    cudaFree(visc_.scan_sums);
-    cudaFree(visc_.partials);
-    cudaFree(visc_.barrier);
-    cudaFree(visc_.block);
-    cudaFree(visc_.info);
+    free_work(visc_);
+    free_work(st_);
     cudaFree(census_dev_);
     cudaFree(max_velocity_dev_);
     cudaFree(load_probes_dev_);
@@ -509,6 +521,14 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 1: // compute divergence -> PCG residual (:835-840)
         refresh_fluid_bits();
         launch_divergence_compute(stream_, grid_, bits, marker_.ptr, u, vox, solver_->residual());
+        if (surface_tension_ > 0.0f) {
+            const NvtxScope st_scope("surface tension: curvature");
+            // The density accumulator is free until stage 9 memsets it.  On the scheduled path the splat rewrites sched_.item_box, the boxes
+            // the next P2G reads: harmless, because stage 9 of this step rewrites them before that P2G.
+            launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr, sched_);
+            launch_surface_curvature(stream_, grid_, bits, marker_.ptr, density_.ptr, st_);
+            launch_surface_rhs(stream_, grid_, bits, params_dev_, marker_.ptr, st_, solver_->residual());
+        }
         break;
     case 2: // primary pressure solver (:843-852)
         solver_->solve(stream_, *field_velocity_, 0, marker_.ptr, params_dev_, quirks);
@@ -536,6 +556,10 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 4: // make velocity grid divergence free (:901-904)
         refresh_fluid_bits();
         launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, vox ? particle_words_ : nullptr, u);
+        if (surface_tension_ > 0.0f) {
+            const NvtxScope st_scope("surface tension: pressure jump");
+            launch_surface_faces(stream_, grid_, bits, params_dev_, marker_.ptr, st_, u);
+        }
         break;
     case 5: // extrapolate velocity grid (:906-909)
         refresh_fluid_bits();
@@ -729,20 +753,26 @@ void HybridFluid::set_viscosity(const BlubViscosity *v) {
         ViscosityWork w;
         w.blocks = viscosity_solve_blocks();
         const size_t n = (size_t)grid_.n, words = (size_t)fluid_bits_.wpr * grid_.ny * grid_.nz;
-        BLUB_CUDA_CHECK(cudaMalloc(&w.codes, n * sizeof(uint32_t)));
-        BLUB_CUDA_CHECK(cudaMemsetAsync(w.codes, 0, n * sizeof(uint32_t), stream_));
-        for (int c = 0; c < 3; ++c) {
-            BLUB_CUDA_CHECK(cudaMalloc(&w.r[c], n * sizeof(float)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.s[c], n * sizeof(float)));
+        try {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.codes, n * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.codes, 0, n * sizeof(uint32_t), stream_));
+            for (int c = 0; c < 3; ++c) {
+                BLUB_CUDA_CHECK(cudaMalloc(&w.r[c], n * sizeof(float)));
+                BLUB_CUDA_CHECK(cudaMalloc(&w.s[c], n * sizeof(float)));
+            }
+            BLUB_CUDA_CHECK(cudaMalloc(&w.word_flags, (words + 1) * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.words, words * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks((int64_t)words + 1) + 1024) * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.partials, 2 * 6 * (size_t)w.blocks * sizeof(float)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.barrier, 256));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(BlubViscosity)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.info, sizeof(ViscositySolveInfo)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.info, 0, sizeof(ViscositySolveInfo), stream_));
+        } catch (...) {
+            cudaStreamSynchronize(stream_); // the memsets may be in flight
+            free_work(w);
+            throw;
         }
-        BLUB_CUDA_CHECK(cudaMalloc(&w.word_flags, (words + 1) * sizeof(uint32_t)));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.words, words * sizeof(uint32_t)));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks((int64_t)words + 1) + 1024) * sizeof(uint32_t)));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.partials, 2 * 6 * (size_t)w.blocks * sizeof(float)));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.barrier, 256));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(BlubViscosity)));
-        BLUB_CUDA_CHECK(cudaMalloc(&w.info, sizeof(ViscositySolveInfo)));
-        BLUB_CUDA_CHECK(cudaMemsetAsync(w.info, 0, sizeof(ViscositySolveInfo), stream_));
         visc_ = w;
     }
     // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
@@ -952,7 +982,44 @@ uint64_t HybridFluid::plan_substep(uint64_t remaining_ns, const BlubTimeStepping
     float v[3];
     max_particle_velocity(v);
     if (max_velocity_out) std::memcpy(max_velocity_out, v, sizeof(v));
-    return cfl_substep_ns(remaining_ns, v, gravity_, ts);
+    if (!(surface_tension_ > 0.0f)) return cfl_substep_ns(remaining_ns, v, gravity_, ts);
+    const uint64_t cap = capillary_limit_ns(surface_tension_);
+    if (cap < ts.min_dt_ns)
+        throw UnstableError("plan_substep: the capillary step limit of " + std::to_string(cap) + " ns at a surface tension of " + std::to_string(surface_tension_) +
+                            " cells^3/s^2 is below min_dt_ns = " + std::to_string(ts.min_dt_ns) + " ns");
+    BlubTimeStepping capped = ts;
+    capped.max_dt_ns = std::min(ts.max_dt_ns, cap);
+    return cfl_substep_ns(remaining_ns, v, gravity_, capped);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Surface tension (surface_tension_kernels.cu).  Not in the reference.
+void HybridFluid::set_surface_tension(float s) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_surface_tension: z-slab ranks have no surface tension");
+    if (mid_step_) throw std::invalid_argument("set_surface_tension: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    if (!std::isfinite(s) || s < 0.0f) throw std::invalid_argument("set_surface_tension: the surface tension must be finite and not negative");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const bool on = s > 0.0f;
+    if (on && !st_.sigma) {
+        SurfaceTensionWork w;
+        const size_t n = (size_t)grid_.n;
+        try {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.psi, n * sizeof(long long)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.kappa, n * sizeof(float)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.kappa, 0, n * sizeof(float), stream_));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.sigma, sizeof(float)));
+        } catch (...) {
+            cudaStreamSynchronize(stream_); // the memset may be in flight
+            free_work(w);
+            throw;
+        }
+        st_ = w;
+    }
+    // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
+    if (st_.sigma) BLUB_CUDA_CHECK(cudaMemcpyAsync(st_.sigma, &s, sizeof(s), cudaMemcpyHostToDevice, stream_));
+    if (!on && st_.kappa) BLUB_CUDA_CHECK(cudaMemsetAsync(st_.kappa, 0, (size_t)grid_.n * sizeof(float), stream_)); // the tap reads zeros when off
+    if (on != (surface_tension_ > 0.0f)) destroy_graphs();
+    surface_tension_ = s;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1247,6 +1314,7 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
         v.kinematic_viscosity = scene_viscosity_grid(cfg);
         f->set_viscosity(&v);
     }
+    if (cfg.surface_tension > 0.0f) f->set_surface_tension(scene_surface_tension_grid(cfg));
     if (!cfg.load_probes.empty()) {
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);
         f->set_load_probes(probes.data(), (uint32_t)probes.size());

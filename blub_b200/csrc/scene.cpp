@@ -146,6 +146,9 @@ uint32_t tag_of(const JsonValue &obj, const char *what) {
 } // namespace
 
 float scene_viscosity_grid(const SceneConfig &cfg) { return cfg.viscosity / (cfg.grid_to_world_scale * cfg.grid_to_world_scale); }
+float scene_surface_tension_grid(const SceneConfig &cfg) {
+    return cfg.surface_tension / (cfg.grid_to_world_scale * cfg.grid_to_world_scale * cfg.grid_to_world_scale);
+}
 
 SceneConfig parse_scene_file(const std::string &path) {
     std::ifstream in(path, std::ios::binary);
@@ -205,6 +208,13 @@ SceneConfig parse_scene_file(const std::string &path) {
         cfg.viscosity = num_f32(*nu, "viscosity");
         if (!std::isfinite(cfg.viscosity) || cfg.viscosity < 0.0f || !std::isfinite(scene_viscosity_grid(cfg)))
             throw std::runtime_error("scene JSON: `fluid.viscosity` must be finite and not negative");
+    }
+    // kinematic surface tension sigma / density (not in the reference): a number in m^3/s^2
+    if (const JsonValue *st = fluid.get("surface_tension")) {
+        if (st->kind != JsonValue::Number) throw std::runtime_error("scene JSON: `fluid.surface_tension` is not a number");
+        cfg.surface_tension = num_f32(*st, "surface_tension");
+        if (!std::isfinite(cfg.surface_tension) || cfg.surface_tension < 0.0f || !std::isfinite(scene_surface_tension_grid(cfg)))
+            throw std::runtime_error("scene JSON: `fluid.surface_tension` must be finite and not negative");
     }
     // solid load probes (not in the reference): world units, the pivot optional
     if (const JsonValue *probes = fluid.get("load_probes")) {

@@ -28,14 +28,18 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // layout plus section 16, the mesh bodies' geometry and mass properties (its length is what the file holds beyond section 15).  Version 32: a
 // fluid with viscosity; the layout it would otherwise have, promoted to 13 sections, or 14 (section 14 in its version-4 form, possibly an empty
 // set), 15 or 16, plus a last section 17, the viscosity setting: num_sections (14 to 17) tells which.  Versions 17 to 31 are not formats.
-constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32;
-constexpr uint32_t kNumSections = 17; // at most
+// Version 64: a fluid with surface tension; the layout it would otherwise have (13 to 16 base sections as in version 32, then section 17 when
+// it is viscous) plus a last section 18, the setting.  The header cannot tell 13 + 17 + 18 from 14 + 18 apart: the reader walks the section
+// heads (their stored lengths) after section 13 and finds section 17 by its id.  Versions 33 to 63 are not formats.
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32,
+                   kFormatVersionSurfaceTension = 64;
+constexpr uint32_t kNumSections = 18; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES, SEC_VISCOSITY
+    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -71,6 +75,12 @@ struct MeshBodyRecordHead {
 static_assert(sizeof(MeshBodyRecordHead) == 224, "mesh body record layout");
 // Section 17 (version 32): the BlubViscosity as set, kinematic_viscosity > 0
 static_assert(sizeof(BlubViscosity) == 16, "viscosity section layout");
+// Section 18 (version 64): the kinematic surface tension as set, above 0 (cells^3/s^2)
+struct SurfaceTensionSection {
+    float surface_tension;
+    uint32_t reserved; // 0
+};
+static_assert(sizeof(SurfaceTensionSection) == 8, "surface tension section layout");
 
 struct StateHeader {
     char magic[8];
@@ -104,13 +114,18 @@ struct Section {
     uint64_t length;
 };
 
-// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32 header whose
-// num_sections names no layout).  The base sections come first: base_sections() of them, then section 17 in a version-32 file.
-uint32_t base_sections(const StateHeader &h) {
+// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32 or -64 header whose
+// num_sections names no layout).  The base sections come first: base_sections() of them, then section 17 in a version-32 file, sections 17
+// (when viscous64: a version-64 file that holds it) and 18 in a version-64 file.
+uint32_t base_sections(const StateHeader &h, bool viscous64) {
     if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
+    if (h.format_version == kFormatVersionSurfaceTension) {
+        const uint32_t extra = viscous64 ? 2 : 1;
+        return h.num_sections >= 13 + extra && h.num_sections <= 16 + extra ? h.num_sections - extra : 0;
+    }
     return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
 }
-uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
+uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], bool viscous64) {
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const Section s[kNumSections] = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
                                      {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
@@ -118,12 +133,18 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections]) {
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
                                      {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
-                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}};
+                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)}};
     std::memcpy(out, s, sizeof(s));
-    const uint32_t nb = base_sections(h);
-    if (h.format_version != kFormatVersionViscosity || nb == 0) return nb;
-    out[nb] = s[16];
-    return nb + 1;
+    const uint32_t nb = base_sections(h, viscous64);
+    if (nb == 0) return 0;
+    uint32_t ns = nb;
+    if (h.format_version == kFormatVersionViscosity || (h.format_version == kFormatVersionSurfaceTension && viscous64)) out[ns++] = s[16];
+    if (h.format_version == kFormatVersionSurfaceTension) out[ns++] = s[17];
+    return ns;
+}
+// whether the file has a viscosity section: a version-32 file always, a version-64 file when section 17 follows its base sections
+bool has_viscosity_section(const StateHeader &h, bool viscous64) {
+    return h.format_version == kFormatVersionViscosity || (h.format_version == kFormatVersionSurfaceTension && viscous64);
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -155,7 +176,32 @@ struct File {
         if (fstat(fileno(f), &st) != 0) throw IoError("cannot stat " + path + ": " + errno_text());
         return (uint64_t)st.st_size;
     }
+    uint64_t tell() { return (uint64_t)ftello(f); }
+    void seek(uint64_t at) {
+        if (fseeko(f, (off_t)at, SEEK_SET) != 0) throw IoError("cannot seek in " + path + ": " + errno_text());
+    }
 };
+
+// A version-64 file: whether a section 17 lies among the sections after section 13, found by walking their heads with their stored lengths
+// (at most four of them before section 18).  Leaves `f` where it was.  The lengths are checked later, section by section.
+bool version64_viscous(File &f, const StateHeader &h) {
+    const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
+    const uint64_t base[13] = {np, np, np, np, 4 * n, 4 * n, 4 * n, n, 4 * n, 4 * n, 2 * sizeof(PcgScalars), 8ull * h.num_stats[0], 8ull * h.num_stats[1]};
+    const uint64_t here = f.tell(), size = f.size();
+    uint64_t at = here;
+    for (uint64_t len : base) at += sizeof(SectionHead) + len + 4;
+    bool viscous = false;
+    for (int k = 0; k < 5 && at + sizeof(SectionHead) <= size; ++k) {
+        SectionHead head;
+        f.seek(at);
+        f.read(&head, sizeof(head));
+        if (head.id == SEC_VISCOSITY) viscous = true;
+        if (head.id == SEC_SURFACE_TENSION || head.length > size) break;
+        at += sizeof(SectionHead) + head.length + 4;
+    }
+    f.seek(here);
+    return viscous;
+}
 
 // Staging memory of the array sections: pinned halves with an event each when the arrays come from / go to the device, plain host memory
 // for the host-only reader.
@@ -188,17 +234,19 @@ struct Staging {
     }
 };
 
-// Header checks: everything a reader needs to trust before it allocates anything.  Leaves `f` at the first section.
-StateHeader read_header(File &f) {
+// Header checks: everything a reader needs to trust before it allocates anything.  Leaves `f` at the first section.  viscous64: whether a
+// version-64 file holds section 17 (false for every other version).
+StateHeader read_header(File &f, bool &viscous64) {
     StateHeader h;
     const uint64_t size = f.size();
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
-        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity)
+        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity &&
+        h.format_version != kFormatVersionSurfaceTension)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8, 16 and 32)");
+                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32 and 64)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -212,15 +260,16 @@ StateHeader read_header(File &f) {
         throw ParseError(f.path + ": precond_mode, transfer path or graph replay flag out of range");
     const uint32_t sp = h.solver_path;
     if (sp > 6 || sp == 3 || sp == 5 || (sp == 2 && d[0] % 128)) throw ParseError(f.path + ": solver path out of range");
+    viscous64 = h.format_version == kFormatVersionSurfaceTension && version64_viscous(f, h);
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec, viscous64);
     if (h.num_sections != ns)
         throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(h.format_version) + " has " +
-                         (ns ? std::to_string(ns) : std::string("14 to 17")));
+                         (ns ? std::to_string(ns) : viscous64 ? std::string("15 to 18") : std::string("14 to 17")));
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
     // version 16: section 16 holds at least its count and one mesh body record
-    if (base_sections(h) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
+    if (base_sections(h, viscous64) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
         throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
 }
@@ -228,10 +277,10 @@ StateHeader read_header(File &f) {
 // Reads one section whose id and length must be `s`, in chunks of at most one staging half; sink(slot, data, bytes, offset) receives
 // every chunk (it must be done with the half `slot` before that half's event is waited on again), then the CRC is checked.
 // the length of section 16 when the file has one: what the file holds beyond section 15, its head and its CRC
-uint64_t mesh_section_length(File &f, const StateHeader &h) {
-    if (base_sections(h) != 16) return 0;
+uint64_t mesh_section_length(File &f, const StateHeader &h, bool viscous64) {
+    if (base_sections(h, viscous64) != 16) return 0;
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec);
+    const uint32_t ns = expected_sections(h, sec, viscous64);
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4; // section 16 counted empty
     return f.size() - total;
@@ -426,17 +475,25 @@ BlubViscosity viscosity_of(const BlubViscosity &v, const std::string &path) {
     } catch (const std::invalid_argument &e) {
         throw ParseError(path + ": section 17: " + e.what());
     }
-    if (!(v.kinematic_viscosity > 0.0f)) throw ParseError(path + ": section 17: a version-32 file holds a viscosity above 0");
+    if (!(v.kinematic_viscosity > 0.0f)) throw ParseError(path + ": section 17: a version-32 or -64 file's section 17 holds a viscosity above 0");
     return v;
+}
+
+// The setting of section 18, checked with the rules of set_surface_tension; a version-64 file has surface tension.
+float surface_tension_of(const SurfaceTensionSection &s, const std::string &path) {
+    if (!std::isfinite(s.surface_tension) || !(s.surface_tension > 0.0f)) throw ParseError(path + ": section 18: the surface tension must be finite and above 0");
+    if (s.reserved != 0u) throw ParseError(path + ": section 18: reserved must be 0");
+    return s.surface_tension;
 }
 
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
     File f(path, "rb");
-    const StateHeader h = read_header(f);
+    bool viscous64 = false;
+    const StateHeader h = read_header(f, viscous64);
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec), nb = base_sections(h);
+    const uint32_t ns = expected_sections(h, sec, viscous64), nb = base_sections(h, viscous64);
     Staging st(false);
     for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
     if (nb >= 14) {
@@ -449,16 +506,22 @@ StateInfo read_state_info(const std::string &path) {
         read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
         if (nb == 15) body_set_of(bs, h, f.path);
         else {
-            std::vector<char> bytes(mesh_section_length(f, h));
+            std::vector<char> bytes(mesh_section_length(f, h, viscous64));
             read_section(f, {SEC_MESH_BODIES, bytes.size()}, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(bytes.data() + off, data, n); });
             std::vector<MeshBodyHost> meshes;
             mesh_body_set_of(bs, bytes, h, f.path, meshes);
         }
     }
-    if (ns > nb) {
+    uint32_t next = nb;
+    if (has_viscosity_section(h, viscous64)) {
         BlubViscosity v{};
-        read_section(f, sec[nb], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&v) + off, data, n); });
+        read_section(f, sec[next++], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&v) + off, data, n); });
         viscosity_of(v, f.path);
+    }
+    if (next < ns) {
+        SurfaceTensionSection s{};
+        read_section(f, sec[next], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&s) + off, data, n); });
+        surface_tension_of(s, f.path);
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -480,8 +543,8 @@ void HybridFluid::save_state(const std::string &path) {
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
     const bool with_bodies = num_bodies_ > 0;
-    const bool viscous = viscosity_.kinematic_viscosity > 0.0f;
-    h.format_version = viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool viscous = viscosity_.kinematic_viscosity > 0.0f, capillary = surface_tension_ > 0.0f;
+    h.format_version = capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -500,7 +563,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0);
+    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -545,7 +608,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary ? sizeof(tagged) : sizeof(fl));
         }
         if (with_bodies) {
             BodySection bs{};
@@ -586,6 +649,10 @@ void HybridFluid::save_state(const std::string &path) {
             write_host_section(f, SEC_MESH_BODIES, bytes.data(), bytes.size());
         }
         if (viscous) write_host_section(f, SEC_VISCOSITY, &viscosity_, sizeof(viscosity_));
+        if (capillary) {
+            const SurfaceTensionSection sts = {surface_tension_, 0u};
+            write_host_section(f, SEC_SURFACE_TENSION, &sts, sizeof(sts));
+        }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
         f.f = nullptr;
@@ -599,9 +666,10 @@ void HybridFluid::save_state(const std::string &path) {
 
 std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, int device, cudaStream_t stream) {
     File f(path, "rb");
-    const StateHeader h = read_header(f); // every size is checked before anything is allocated
+    bool viscous64 = false;
+    const StateHeader h = read_header(f, viscous64); // every size is checked before anything is allocated
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec), nb = base_sections(h);
+    const uint32_t ns = expected_sections(h, sec, viscous64), nb = base_sections(h, viscous64);
     std::unique_ptr<HybridFluid> fluid(
         new HybridFluid(h.grid_dimension[0], h.grid_dimension[1], h.grid_dimension[2], h.max_num_particles, device, stream));
     HybridFluid &x = *fluid;
@@ -654,18 +722,24 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         to_host(sec[14], &bs);
         if (nb == 15) x.restore_bodies(body_set_of(bs, h, f.path));
         else {
-            std::vector<char> bytes(mesh_section_length(f, h));
+            std::vector<char> bytes(mesh_section_length(f, h, viscous64));
             to_host({SEC_MESH_BODIES, bytes.size()}, bytes.data());
             std::vector<MeshBodyHost> meshes;
             const std::vector<BlubBody> set = mesh_body_set_of(bs, bytes, h, f.path, meshes);
             x.restore_bodies(set, std::move(meshes));
         }
     }
-    if (ns > nb) { // the working volumes and the last solve are not state
+    uint32_t next = nb;
+    if (has_viscosity_section(h, viscous64)) { // the working volumes and the last solve are not state
         BlubViscosity v{};
-        to_host(sec[nb], &v);
+        to_host(sec[next++], &v);
         v = viscosity_of(v, f.path);
         x.set_viscosity(&v);
+    }
+    if (next < ns) { // the curvature is not state: stage 1 measures it again
+        SurfaceTensionSection s{};
+        to_host(sec[next], &s);
+        x.set_surface_tension(surface_tension_of(s, f.path));
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

@@ -23,6 +23,8 @@ STAGES = [
     "position_change", "extrapolate2", "correct_particles",
 ]
 TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, TAP_P_DEN, TAP_RESIDUAL, TAP_SOLID_VOXELS = range(12)
+# download only: the float32 curvature of the last stage 1; the int64 density accumulator (a diagnostic whose contents may change, see blub_fluid.h)
+TAP_CURVATURE, TAP_DENSITY = 12, 13
 
 BLUB_OK = 0
 BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
@@ -38,7 +40,9 @@ BODY_HISTORY_LENGTH = 1024      # BLUB_BODY_HISTORY_LENGTH: records per body in 
 
 
 class BlubError(RuntimeError):
-    pass
+    """A refused or failed library call; `code` is its BLUB_ERR_* value when the library returned one."""
+
+    code = None
 
 
 class SolverConfig(C.Structure):
@@ -307,6 +311,9 @@ def lib():
         "blub_fluid_last_viscosity_solve": (C.c_int, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
         "blub_fluid_viscosity_only": (C.c_int, [vp, C.c_double]),
         "blub_scene_viscosity": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
+        "blub_fluid_set_surface_tension": (C.c_int, [vp, C.c_float]),
+        "blub_fluid_surface_tension": (C.c_int, [vp, C.POINTER(C.c_float)]),
+        "blub_scene_surface_tension": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
         "blub_fluid_max_particle_velocity": (C.c_int, [vp, f3]),
         "blub_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
         "blub_fluid_plan_substep": (C.c_int, [vp, C.c_uint64, C.POINTER(TimeStepping), C.POINTER(C.c_uint64), f3]),
@@ -349,7 +356,9 @@ def lib():
 
 def _check(rc, allow=(BLUB_OK,)):
     if rc not in allow:
-        raise BlubError(f"libblubcore error {rc}: {lib().blub_last_error().decode()}")
+        err = BlubError(f"libblubcore error {rc}: {lib().blub_last_error().decode()}")
+        err.code = rc  # the BLUB_ERR_* value
+        raise err
     return rc
 
 
@@ -467,6 +476,13 @@ def scene_load_probes(path):
     arr = (LoadProbe * LOAD_PROBES_MAX)()
     _check(lib().blub_scene_load_probes(os.fsencode(path), arr, LOAD_PROBES_MAX, C.byref(count)))
     return [(tuple(p.min_grid), tuple(p.max_grid), tuple(p.pivot_grid)) for p in arr[:count.value]]
+
+
+def scene_surface_tension(path):
+    """The scene's fluid.surface_tension (m^3/s^2) in cells^3/s^2: value / grid_to_world_scale^3, 0.0 without the key (host only)."""
+    out = C.c_float(0)
+    _check(lib().blub_scene_surface_tension(os.fsencode(path), C.byref(out)))
+    return float(out.value)
 
 
 def scene_viscosity(path):
@@ -652,7 +668,7 @@ class HybridFluid:
 
     # -- taps ---------------------------------------------------------------------------------
     def download_grid(self, tap):
-        dt = np.int8 if tap == TAP_MARKER else np.float32
+        dt = np.int8 if tap == TAP_MARKER else np.int64 if tap == TAP_DENSITY else np.float32
         out = np.empty((self.nz, self.ny, self.nx), dtype=dt)
         _check(self.L.blub_fluid_download(self.h, tap, out.ctypes.data_as(C.c_void_p), out.nbytes))
         return out
@@ -780,6 +796,19 @@ class HybridFluid:
         """Test hook: the viscosity stage on the grid velocity and marker as they are (tap uploads), nothing else."""
         _check(self.L.blub_fluid_viscosity_only(self.h, dt))
 
+    # -- surface tension ----------------------------------------------------------------------
+    def set_surface_tension(self, sigma):
+        """Kinematic surface tension sigma / density in cells^3/s^2 (m^3/s^2 / grid_to_world_scale^3; water: 7.28e-5 m^3/s^2); 0 turns it
+        off.  Every step then applies the capillary pressure jump at the free surface, and plan_substep / advance respect the capillary step
+        limit.  Raises BlubError (and changes nothing) on a negative or non-finite value, z-slab ranks and a fluid inside a step."""
+        _check(self.L.blub_fluid_set_surface_tension(self.h, float(sigma)))
+
+    def surface_tension(self):
+        """The kinematic surface tension in cells^3/s^2 (0.0: off)."""
+        out = C.c_float(0)
+        _check(self.L.blub_fluid_surface_tension(self.h, C.byref(out)))
+        return float(out.value)
+
     # -- CFL-limited substeps -----------------------------------------------------------------
     def max_particle_velocity(self):
         """[max |v_x|, max |v_y|, max |v_z|] over the live particles in cells/s, exact (float32 values).  One kernel, then synchronises."""
@@ -789,7 +818,8 @@ class HybridFluid:
 
     def plan_substep(self, remaining_ns, cfl=1.0, max_dt_ns=None, min_dt_ns=1):
         """(dt_ns, max_velocity): the measured largest particle velocity per axis and the next substep of `remaining_ns` by the CFL rule
-        (cfl_substep_ns) with this fluid's gravity; max_dt_ns defaults to remaining_ns.  Raises BlubError as cfl_substep_ns does, and on a
+        (cfl_substep_ns) with this fluid's gravity, max_dt_ns lowered to the capillary limit while the fluid has surface tension; max_dt_ns
+        defaults to remaining_ns.  Raises BlubError as cfl_substep_ns does, and on a
         z-slab rank or a fluid inside a step."""
         ts = time_stepping(cfl, remaining_ns if max_dt_ns is None else max_dt_ns, min_dt_ns)
         dt, v = C.c_uint64(0), (C.c_float * 3)()

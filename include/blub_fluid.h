@@ -386,9 +386,27 @@ int blub_fluid_max_particle_velocity(BlubFluid *fluid, float out[3]);
  * remaining_ns == 0 or a non-finite gravity.  BLUB_ERR_UNSTABLE: a non-finite velocity or d_ns < min_dt_ns; blub_last_error names the case
  * and the velocity. */
 int blub_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping *config, uint64_t *dt_ns);
-/* blub_fluid_max_particle_velocity, then blub_cfl_substep_ns with the fluid's gravity.  max_velocity_out (may be NULL) receives the measurement,
- * also when the rule refuses it.  Refuses what both refuse, checking the config and remaining_ns before anything is launched. */
+/* blub_fluid_max_particle_velocity, then blub_cfl_substep_ns with the fluid's gravity and, while the fluid has surface tension s > 0, with
+ * max_dt_ns lowered to the capillary limit floor(1e9 sqrt(1 / (4 pi s))) (a limit below min_dt_ns: BLUB_ERR_UNSTABLE).  max_velocity_out (may be
+ * NULL) receives the measurement, also when the rule refuses it.  Refuses what both refuse, checking the config and remaining_ns before anything is launched. */
 int blub_fluid_plan_substep(BlubFluid *fluid, uint64_t remaining_ns, const BlubTimeStepping *config, uint64_t *dt_ns, float max_velocity_out[3]);
+
+/* ---- surface tension (not part of the reference surface; rules: DESIGN.md section 8 "Surface tension") --------------------------------
+ * With a kinematic surface tension s = sigma / density above zero (cells^3/s^2: m^3/s^2 divided by grid_to_world_scale^3; water is
+ * 7.28e-5 m^3/s^2) the free surface carries the pressure jump P_liquid - P_air = sigma kappa.  Stage 1 of every step measures the curvature
+ * kappa of a smoothed particle density (integer arithmetic, bit-reproducible) in the band of cells on both sides of the surface and moves the
+ * velocity solve's Dirichlet value on AIR from 0 to the ghost value g = -dt s (kappa_i + kappa_j) / 2 of each FLUID-AIR face; stage 4 adds g
+ * to those faces.  Walls are neutrally wetting (contact angle 90 degrees).  While s > 0 blub_fluid_plan_substep also holds every substep
+ * to the capillary limit floor(1e9 sqrt(1 / (4 pi s))) ns.  Surface tension is part of the saved state (format version 64). */
+/* 0 turns it off: the step is then the step of a fluid that never had surface tension.  Stream-ordered; turning it on or off drops the cached
+ * step graphs, a change between two positive values does not.  BLUB_ERR_INVALID_ARGUMENT, changing nothing: a negative or non-finite value,
+ * a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_surface_tension(BlubFluid *fluid, float cells3_per_s2);
+/* the current setting (0: off) */
+int blub_fluid_surface_tension(const BlubFluid *fluid, float *cells3_per_s2);
+/* The scene's optional fluid.surface_tension (m^3/s^2) in cells^3/s^2: value / grid_to_world_scale^3, 0 without the key.  blub_scene_load
+ * sets it on the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
+int blub_scene_surface_tension(const char *scene_json_path, float *cells3_per_s2);
 
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
@@ -510,7 +528,13 @@ enum {
     BLUB_TAP_PARTICLE_POS = 0, BLUB_TAP_PARTICLE_VX = 1, BLUB_TAP_PARTICLE_VY = 2, BLUB_TAP_PARTICLE_VZ = 3,
     BLUB_TAP_GRID_VX = 4, BLUB_TAP_GRID_VY = 5, BLUB_TAP_GRID_VZ = 6, BLUB_TAP_MARKER = 7,
     BLUB_TAP_PRESSURE_VELOCITY = 8, BLUB_TAP_PRESSURE_DENSITY = 9, BLUB_TAP_RESIDUAL = 10,
-    BLUB_TAP_SOLID_VOXELS = 11 /* the solid volume the step reads: the composite one with bodies, else the borrowed one (download only) */
+    BLUB_TAP_SOLID_VOXELS = 11, /* the solid volume the step reads: the composite one with bodies, else the borrowed one (download only) */
+    BLUB_TAP_CURVATURE = 12,    /* float per cell: the curvature (cells^-1) of the last stage 1 in the surface band, 0 elsewhere; zeros while
+                                   surface tension is off (download only) */
+    BLUB_TAP_DENSITY = 13       /* DIAGNOSTIC, not a stable interface: the step's internal scratch density accumulator as the last stage that
+                                   wrote it left it (int64 per cell: the stage-9 splat in 2^-40 particle weights, or after a stage 1 with surface
+                                   tension the smoothed field phi within 2 cells of FLUID).  Its contents and layout may change with the step's
+                                   implementation; it exists so that tests can restate stage 1 bit for bit (download only) */
 };
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);

@@ -707,14 +707,30 @@ struct TileWindow {
     int ox, oy, oz; // face (x, y, z) of tile entry 0
     int ex, ey, ez; // extent; ex * ey * ez <= the tile's capacity (ex may be 0: no tile)
 };
-__device__ __forceinline__ void tile_add(uint32_t *lo, uint32_t *hi, long long q) {
+// tile_add_lo adds the low word of q and returns what the high word still needs: the high half of q plus the carry out of the low word.
+// The scatters' fast paths issue the low-word adds of several faces back to back and only then the high-word adds, so that the round
+// trips overlap; they add zeros rather than branch around them (q == 0 leaves both words as they are).
+__device__ __forceinline__ uint32_t tile_add_lo(uint32_t *lo, long long q) {
     const uint32_t ql = (uint32_t)q;
     const uint32_t old = atomicAdd(lo, ql);
-    const uint32_t h = (uint32_t)((unsigned long long)q >> 32) + (old + ql < old ? 1u : 0u);
+    return (uint32_t)((unsigned long long)q >> 32) + (old + ql < old ? 1u : 0u);
+}
+__device__ __forceinline__ void tile_add(uint32_t *lo, uint32_t *hi, long long q) {
+    const uint32_t h = tile_add_lo(lo, q);
     if (h != 0u) atomicAdd(hi, h);
 }
 __device__ __forceinline__ long long tile_word(const uint32_t *lo, const uint32_t *hi) {
     return (long long)(((unsigned long long)*hi << 32) | *lo);
+}
+// Zeroes the first `size` entries of PLANES word planes of CAP entries with 128-bit stores (the tile is 16-byte aligned and CAP % 4 == 0,
+// so the range rounded up to 4 entries stays inside each plane; no face adds to the entries past `size`).  The flushes keep 32-bit loads:
+// lane = entry keeps a warp's global reductions on adjacent cells.
+template <int PLANES, int CAP>
+__device__ __forceinline__ void tile_zero(uint32_t *tile, int size) {
+    static_assert(CAP % 4 == 0, "128-bit tile stores");
+    for (int t = 4 * threadIdx.x; t < size; t += 4 * PT)
+#pragma unroll
+        for (int k = 0; k < PLANES; ++k) *reinterpret_cast<uint4 *>(tile + k * CAP + t) = make_uint4(0u, 0u, 0u, 0u);
 }
 // The window of the chunk starting at particle b, from the primal cells of its particles (every thread of the block calls this, `cell`
 // of its own particle, `valid` whether it has one).  It covers the faces [min - 1, max + 1] of those cells in every dimension, which
@@ -757,6 +773,12 @@ __device__ __forceinline__ int tile_entry(const TileWindow &w, int x, int y, int
     const int rx = x - w.ox, ry = y - w.oy, rz = z - w.oz;
     return ((unsigned)rx < (unsigned)w.ex && (unsigned)ry < (unsigned)w.ey && (unsigned)rz < (unsigned)w.ez) ? (rz * w.ey + ry) * w.ex + rx : -1;
 }
+// tile entry of face (x, y, z) if the whole box of faces x..x+1, y..y+1, z..z+1 lies inside the window (its eight entries are then this one
+// plus 0, 1, ex, ex + 1, ex * ey, ...), or -1
+__device__ __forceinline__ int tile_box_entry(const TileWindow &w, int x, int y, int z) {
+    const int rx = x - w.ox, ry = y - w.oy, rz = z - w.oz;
+    return (rx >= 0 && ry >= 0 && rz >= 0 && rx + 1 < w.ex && ry + 1 < w.ey && rz + 1 < w.ez) ? (rz * w.ey + ry) * w.ex + rx : -1;
+}
 // global cell index of tile entry t
 __device__ __forceinline__ int tile_cell(const GridDim &g, const TileWindow &w, int t) {
     const int q = t / w.ex;
@@ -767,6 +789,7 @@ __device__ __forceinline__ int tile_cell(const GridDim &g, const TileWindow &w, 
 constexpr int P2G_TILE = 1184;
 constexpr int P2G_TILE_BYTES = 12 * P2G_TILE * 4; // 56,832 B: with the 1 KB the hardware reserves per block, 4 blocks fit into 228 KB
 constexpr int DENSITY_TILE = 2048;                // density tile: {low, high} word planes (16 KB)
+constexpr int P2G_CARRY_BATCH = 4;                // P2G faces whose low-word adds (value and weight) are issued before their carries
 
 // ---- brick schedule of the density and P2G scatters (built at every re-sort, DESIGN.md §3.2)
 // After a re-sort the particles are in x-fastest cell order, so a chunk of 256 consecutive particles covers one short run of a cell row and
@@ -910,14 +933,16 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
     const bool valid = i < np;     // no per-lane early return: every lane of a live warp takes part in the shuffles
     if (MARK && valid) marker[cell_of_position(g, p)] = (int8_t)CELL_FLUID; // transfer_build_linkedlist.comp:17-19
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 rows[3] = {valid ? rowx[i] : zero, valid ? rowy[i] : zero, valid ? rowz[i] : zero};
-    longlong2 *const nw[3] = {nwx, nwy, nwz};
-#pragma unroll
+    // one copy of the component body, not three: unrolled (and inlined twice, by the item and the chunk path) the loop makes the kernel
+    // about 8,000 instructions, and the scatter runs measurably slower out of the instruction caches
+#pragma unroll 1
     for (int c = 0; c < 3; ++c) {
+        const float4 *const row = c == 0 ? rowx : c == 1 ? rowy : rowz;
+        longlong2 *const nwc = c == 0 ? nwx : c == 1 ? nwy : nwz;
         const float ox = c == 0 ? 1.0f : 0.5f, oy = c == 1 ? 1.0f : 0.5f, oz = c == 2 ? 1.0f : 0.5f;
         const int dx = (int)(p.x - ox), dy = (int)(p.y - oy), dz = (int)(p.z - oz);
         const float qx = (float)dx + ox, qy = (float)dy + oy, qz = (float)dz + oz; // sample point of face (dx,dy,dz)
-        const float4 r = rows[c];
+        const float4 r = valid ? row[i] : zero;
         const float tx[2] = {qx - p.x, qx + 1.0f - p.x}, ty[2] = {qy - p.y, qy + 1.0f - p.y}, tz[2] = {qz - p.z, qz + 1.0f - p.z};
         const float wxs[2] = {saturatef(1.0f - fabsf(tx[0])), saturatef(1.0f - fabsf(tx[1]))};
         const float wys[2] = {saturatef(1.0f - fabsf(ty[0])), saturatef(1.0f - fabsf(ty[1]))};
@@ -932,9 +957,35 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
             acc[2 * k] = w > 0.0f ? w * v : 0.0f;
             acc[2 * k + 1] = w > 0.0f ? w : 0.0f;
         }
-        const bool head = warp_group_sum<MATCH, 16>(valid ? base : -1 - (int)(threadIdx.x & 31), acc);
-        if (head && valid) {
-            uint32_t *const t = tile + 4 * c * P2G_TILE; // planes: value low, value high, weight low, weight high
+        const bool live = warp_group_sum<MATCH, 16>(valid ? base : -1 - (int)(threadIdx.x & 31), acc) && valid; // a head issues the adds
+        const int e0 = tile_box_entry(win, dx, dy, dz);
+        if (__all_sync(0xffffffffu, e0 >= 0 || !live)) { // warp-uniform: every head's eight faces go to the tile
+            // the same sums as below without a branch per face, P2G_CARRY_BATCH faces at a time: their low-word adds (value and weight)
+            // first, then the high words they carry into.  A weight that rounds to 0 leaves its value out, as below: both add 0.
+            if (live) {
+                uint32_t *const t = tile + 4 * c * P2G_TILE + e0; // planes: value low, value high, weight low, weight high
+                const int sy = win.ex, sz = win.ex * win.ey;
+#pragma unroll
+                for (int k0 = 0; k0 < 8; k0 += P2G_CARRY_BATCH) {
+                    uint32_t hv[P2G_CARRY_BATCH], hw[P2G_CARRY_BATCH];
+#pragma unroll
+                    for (int j = 0; j < P2G_CARRY_BATCH; ++j) {
+                        const int k = k0 + j, o = (k & 1) + ((k >> 1) & 1) * sy + (k >> 2) * sz;
+                        const long long wq = to_fixed<FIXED_WEIGHT_BITS>(acc[2 * k + 1]);
+                        const long long num = wq > 0 ? to_fixed<FIXED_VALUE_BITS>(acc[2 * k]) : 0;
+                        hv[j] = tile_add_lo(t + o, num);
+                        hw[j] = tile_add_lo(t + 2 * P2G_TILE + o, wq > 0 ? wq : 0);
+                    }
+#pragma unroll
+                    for (int j = 0; j < P2G_CARRY_BATCH; ++j) {
+                        const int k = k0 + j, o = (k & 1) + ((k >> 1) & 1) * sy + (k >> 2) * sz;
+                        atomicAdd(t + P2G_TILE + o, hv[j]);
+                        atomicAdd(t + 3 * P2G_TILE + o, hw[j]);
+                    }
+                }
+            }
+        } else if (live) {
+            uint32_t *const t = tile + 4 * c * P2G_TILE;
 #pragma unroll
             for (int k = 0; k < 8; ++k)
             {
@@ -947,7 +998,7 @@ __device__ __forceinline__ void p2g_scatter_kernel_one(uint32_t i, GridDim g, co
                         if (num != 0) tile_add(t + e, t + P2G_TILE + e, num);
                         tile_add(t + 2 * P2G_TILE + e, t + 3 * P2G_TILE + e, wq);
                     } else {
-                        longlong2 *const f = nw[c] + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz;
+                        longlong2 *const f = nwc + base + (k & 1) + ((k >> 1) & 1) * g.sy + (k >> 2) * g.sz;
                         if (num != 0) fixed_add(&f->x, num);
                         fixed_add(&f->y, wq);
                     }
@@ -964,7 +1015,7 @@ __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const Ste
                                                          const float4 *__restrict__ rowz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
                                                          longlong2 *__restrict__ nwz, int8_t *__restrict__ marker, ScatterSchedule sched,
                                                          uint32_t min_items) {
-    extern __shared__ uint32_t tile[]; // [12][P2G_TILE]
+    extern __shared__ __align__(16) uint32_t tile[]; // [12][P2G_TILE]
     __shared__ int scratch[PT / 32 + 1][8];
     __shared__ TileWindow shared_win;
     longlong2 *const nw[3] = {nwx, nwy, nwz};
@@ -980,9 +1031,7 @@ __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const Ste
         __syncthreads();
         const TileWindow win = shared_win;
         const int size = win.ex * win.ey * win.ez;
-        for (int t = threadIdx.x; t < size; t += PT)
-#pragma unroll
-            for (int k = 0; k < 12; ++k) tile[k * P2G_TILE + t] = 0u;
+        tile_zero<12, P2G_TILE>(tile, size);
         __syncthreads();
         const uint32_t w0 = sched.item_start[it], w1 = it + 1 < items ? sched.item_start[it + 1] : tail / 32u;
         for (uint32_t k = w0 + (threadIdx.x >> 5); k < w1; k += PT / 32) { // warp-uniform
@@ -1014,9 +1063,7 @@ __global__ void __launch_bounds__(PT, 4) p2g_scatter_kernel(GridDim g, const Ste
         const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
         const TileWindow win = scatter_window<P2G_TILE>(b, np_, valid, cell, scratch, &shared_win);
         const int size = win.ex * win.ey * win.ez;
-        for (int t = threadIdx.x; t < size; t += PT)
-#pragma unroll
-            for (int k = 0; k < 12; ++k) tile[k * P2G_TILE + t] = 0u;
+        tile_zero<12, P2G_TILE>(tile, size);
         __syncthreads();
         p2g_scatter_kernel_one<MARK, MATCH>(i, g, params, p, rowx, rowy, rowz, nwx, nwy, nwz, marker, win, tile);
         __syncthreads();
@@ -1116,8 +1163,19 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
     float acc[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) acc[k] = valid ? wx[k & 1] * wy[(k >> 1) & 1] * wz[k >> 2] : 0.0f;
-    const bool head = warp_group_sum<MATCH, 8>(valid ? base : -1 - (int)(threadIdx.x & 31), acc);
-    if (head && valid) {
+    const bool live = warp_group_sum<MATCH, 8>(valid ? base : -1 - (int)(threadIdx.x & 31), acc) && valid; // a head issues the adds
+    const int e0 = tile_box_entry(win, dx, dy, dz);
+    if (__all_sync(0xffffffffu, e0 >= 0 || !live)) { // warp-uniform: every head's eight cells go to the tile; low words first, as in P2G
+        if (live) {
+            uint32_t *const t = tile + e0;
+            const int sy = win.ex, sz = win.ex * win.ey;
+            uint32_t h[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) h[k] = tile_add_lo(t + (k & 1) + ((k >> 1) & 1) * sy + (k >> 2) * sz, acc[k] > 0.0f ? to_fixed<FIXED_WEIGHT_BITS>(acc[k]) : 0);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) atomicAdd(t + DENSITY_TILE + (k & 1) + ((k >> 1) & 1) * sy + (k >> 2) * sz, h[k]);
+        }
+    } else if (live) {
 #pragma unroll
         for (int k = 0; k < 8; ++k)
             if (acc[k] > 0.0f) {
@@ -1131,7 +1189,7 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
 template <bool MATCH>
 __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
                                                              long long *__restrict__ density, ScatterSchedule sched) {
-    __shared__ uint32_t tile[2 * DENSITY_TILE]; // low words, high words
+    __shared__ __align__(16) uint32_t tile[2 * DENSITY_TILE]; // low words, high words
     __shared__ int scratch[PT / 32 + 1][8];
     __shared__ TileWindow shared_win;
     const uint32_t np_ = params->num_particles;
@@ -1143,7 +1201,7 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
         const uint32_t w0 = sched.item_start[it], w1 = it + 1 < items ? sched.item_start[it + 1] : tail / 32u;
         const TileWindow win = item_window<DENSITY_TILE>(g, sched, it, w0, w1, np_, pos, 0.5f, scratch, &shared_win);
         const int size = win.ex * win.ey * win.ez;
-        for (int t = threadIdx.x; t < size; t += PT) tile[t] = tile[DENSITY_TILE + t] = 0u;
+        tile_zero<2, DENSITY_TILE>(tile, size);
         __syncthreads();
         for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
             const uint32_t i = 32u * sched.warps[k] + lane;
@@ -1166,7 +1224,7 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
         const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
         const TileWindow win = scatter_window<DENSITY_TILE>(b, np_, valid, cell, scratch, &shared_win);
         const int size = win.ex * win.ey * win.ez;
-        for (int t = threadIdx.x; t < size; t += PT) tile[t] = tile[DENSITY_TILE + t] = 0u;
+        tile_zero<2, DENSITY_TILE>(tile, size);
         __syncthreads();
         density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
         __syncthreads();

@@ -79,6 +79,10 @@ template <class T> struct GridArray {
 // The setting of a fluid without viscosity, and the setter's range rules (std::invalid_argument names the field).
 constexpr BlubViscosity kViscosityOff = {0.0f, 1e-4f, 200, 0u};
 void check_viscosity(const BlubViscosity &v);
+// A moving tank's frame (tank_kernels.cu): check_tank_frame throws std::invalid_argument on a non-finite value or a rotation that is not
+// orthonormal with det +1 to 1e-6; tank_frame_rotates: omega or alpha is not zero.
+void check_tank_frame(const BlubTankFrame &f);
+bool tank_frame_rotates(const BlubTankFrame &f);
 
 class PressureSolver;
 
@@ -318,10 +322,18 @@ class HybridFluid {
     // plan_substep holds every substep to capillary_limit_ns.
     void set_surface_tension(float cells3_per_s2);
     float surface_tension() const { return surface_tension_; }
+    // Moving tanks (tank_kernels.cu): the frame of the following steps (nullptr: at rest).  Not state.  Throws std::invalid_argument and changes
+    // nothing on a frame check_tank_frame refuses, a rotating frame while the fluid has bodies, a z-slab rank or a fluid inside a step.  Only a
+    // change between rotating and not rotating drops the step graphs.
+    void set_tank_frame(const BlubTankFrame *frame);
+    const BlubTankFrame *tank_frame() const { return has_tank_frame_ ? &tank_frame_ : nullptr; }
     float *curvature() const { return st_.kappa; }             // nullptr before the first surface tension above zero
     long long *density_accumulator() const { return density_.ptr; }
 
   private:
+    BlubTankFrame tank_frame_{};
+    bool has_tank_frame_ = false;
+    bool tank_rotating() const { return has_tank_frame_ && tank_frame_rotates(tank_frame_); }
     uint32_t *max_velocity_dev_ = nullptr;
     BlubBody *bodies_dev_ = nullptr;          // BODIES_MAX bodies, BODIES_MAX x 8 sums, BODIES_MAX x BODY_HISTORY_LENGTH records and the
     unsigned long long *body_sums_ = nullptr; // composite volume, allocated with the first non-empty set
@@ -465,6 +477,12 @@ void check_time_stepping(const BlubTimeStepping &ts);
 // kinematic surface tension s > 0 (cells^3/s^2), saturating at UINT64_MAX.
 uint64_t capillary_limit_ns(float cells3_per_s2);
 uint64_t cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping &ts);
+// Moving tanks (tank_kernels.cu, DESIGN.md §8 "Moving tanks"): the host rules of blub_tank_frame_at, blub_tank_step_constants and
+// blub_tank_cfl_substep_ns (frame == nullptr: cfl_substep_ns).
+BlubTankFrame tank_frame_at(const BlubTankMotion &m, double t_seconds);
+BlubTankStepConstants tank_step_constants(const BlubTankFrame &f, const float gravity_grid[3], float dt);
+uint64_t tank_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTankFrame *frame,
+                             const uint32_t dim[3], const BlubTimeStepping &ts);
 struct StateInfo {
     uint32_t grid_dimension[3], max_num_particles, num_particles, step_count, format_version;
 };
@@ -561,12 +579,16 @@ struct SceneConfig {
     std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
     float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
     float surface_tension = 0.0f;            // optional fluid.surface_tension: kinematic, m^3/s^2
+    bool has_tank_motion = false;            // optional fluid.tank_motion (world units, Hz, rad, rad/s; directions and axis normalised)
+    BlubTankMotion tank_motion{};
     uint32_t num_static_objects = 0;
     std::vector<SceneStaticObject> static_objects;
 };
 SceneConfig parse_scene_file(const std::string &path);
 // the scene's load probes in grid cells: corners and pivot / grid_to_world_scale, pivot (min + max) / 2 when the scene gives none
 std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
+// the scene's tank motion in grid cells: pivot and amplitudes / grid_to_world_scale (in float32, as the load probes' pivots), the rest as parsed
+BlubTankMotion scene_tank_motion_grid(const SceneConfig &cfg);
 // the scene's kinematic viscosity in cells^2/s: viscosity / grid_to_world_scale^2
 float scene_viscosity_grid(const SceneConfig &cfg);
 // the scene's kinematic surface tension in cells^3/s^2: surface_tension / grid_to_world_scale^3

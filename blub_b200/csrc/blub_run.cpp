@@ -31,6 +31,8 @@
 //                  fixed run's, --steps counts intervals (also with --record), and the load and body histories are collected after every
 //                  interval.  --stats gains "time_stepping" with every substep's length and measured velocity.  Refused with --load-state:
 //                  the clock of a resumed adaptive run is not step_count * dt.
+//   fluid.tank_motion  a moving tank (not in the reference): before every step (and every --cfl substep) the runner sets the tank frame at the
+//                  time the static objects are voxelized at (blub_tank_frame_at); a --load-state run continues the clock at step_count * dt.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -182,9 +184,16 @@ int main(int argc, char **argv) {
     }
     // Timer::total_simulated_time / total_rendered_time; a resumed run continues the clock, so that animated solids are where they were
     uint64_t simulated_ns = (uint64_t)blub_fluid_step_count(fluid) * dt_ns, rendered_ns = 0;
-    // one step of `delta_ns` ending at simulated_ns: the solids at that time, then the fluid
+    BlubTankMotion tank_motion;
+    int32_t has_tank_motion = 0;
+    if (blub_scene_tank_motion(scene, &tank_motion, &has_tank_motion)) die("cannot read the scene's tank motion");
+    // one step of `delta_ns` ending at simulated_ns: the solids and the tank frame at that time, then the fluid
     auto voxelize_and_step = [&](uint64_t delta_ns) {
         const double simulated = (double)blub_duration_as_secs_f32(simulated_ns), delta = (double)blub_duration_as_secs_f32(delta_ns);
+        if (has_tank_motion) {
+            BlubTankFrame frame;
+            if (blub_tank_frame_at(&tank_motion, simulated, &frame) || blub_fluid_set_tank_frame(fluid, &frame)) die("cannot set the tank frame");
+        }
         for (size_t k = 0; k < solids.size(); ++k)
             if (blub_solid_voxelize_mesh(voxels, info.grid_dimension, solids[k].mesh, &solids[k].placement, info.grid_to_world_scale, info.world_position,
                                          simulated, delta, k == 0, blub_fluid_stream(fluid), nullptr))

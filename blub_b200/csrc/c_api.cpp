@@ -544,6 +544,43 @@ int blub_fluid_plan_substep(BlubFluid *fluid, uint64_t remaining_ns, const BlubT
     return guarded([&] { *dt_ns = fluid->impl->plan_substep(remaining_ns, *config, max_velocity_out); return BLUB_OK; });
 }
 
+int blub_tank_frame_at(const BlubTankMotion *motion, double t_seconds, BlubTankFrame *out) {
+    if (!motion || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *out = blub::tank_frame_at(*motion, t_seconds); return BLUB_OK; });
+}
+
+int blub_tank_step_constants(const BlubTankFrame *frame, const float gravity_grid[3], float dt, BlubTankStepConstants *out) {
+    if (!frame || !gravity_grid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *out = blub::tank_step_constants(*frame, gravity_grid, dt); return BLUB_OK; });
+}
+
+int blub_fluid_set_tank_frame(BlubFluid *fluid, const BlubTankFrame *frame) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_tank_frame(frame); return BLUB_OK; });
+}
+
+int blub_fluid_tank_frame(const BlubFluid *fluid, BlubTankFrame *out) {
+    const BlubTankFrame *f = fluid ? fluid->impl->tank_frame() : nullptr;
+    if (f && out) *out = *f;
+    return f ? 1 : 0;
+}
+
+int blub_tank_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTankFrame *frame,
+                             const uint32_t grid_dimension[3], const BlubTimeStepping *config, uint64_t *dt_ns) {
+    if (!max_velocity || !gravity_grid || !grid_dimension || !config || !dt_ns) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *dt_ns = blub::tank_cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, frame, grid_dimension, *config); return BLUB_OK; });
+}
+
+int blub_scene_tank_motion(const char *path, BlubTankMotion *out, int32_t *has_motion) {
+    if (!path || !out || !has_motion) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig cfg = blub::parse_scene_file(path);
+        *has_motion = cfg.has_tank_motion ? 1 : 0;
+        *out = cfg.has_tank_motion ? blub::scene_tank_motion_grid(cfg) : BlubTankMotion{};
+        return BLUB_OK;
+    });
+}
+
 int blub_fluid_has_flow(const BlubFluid *fluid) { return fluid && fluid->impl->has_flow() ? 1 : 0; }
 
 int blub_fluid_flow_counters(BlubFluid *fluid, uint64_t out[3]) {

@@ -91,6 +91,9 @@ struct StepParams {
     float inv_dt;
     float gravity[3];       // GravityGridSpace itself (the floating bodies' integrator)
     uint32_t step_count;    // whole steps taken before this one (seeds the source emission)
+    float tank_q[9];        // moving tanks, row major: the Coriolis rotation Q of the step (identity at rest; read only by tank_frame_kernel)
+    float tank_k[9];        //   the position-dependent velocity increment K (zero at rest)
+    float tank_pivot[3];    //   the frame's pivot, grid cells
     uint32_t num_particles; // last: left alone by the upload when the count lives on the device
 };
 

@@ -230,6 +230,12 @@ void launch_viscosity(cudaStream_t st, const GridDim &g, const StepParams *param
 // Zeroes the three words first.
 void launch_max_particle_velocity(cudaStream_t st, const StepParams *params, uint32_t n_host, uint32_t np_upper, float4 *const row[3], uint32_t *out);
 
+// ---- moving tanks (tank_kernels.cu, DESIGN.md §8 "Moving tanks") ----
+// Stage 0 of a rotating frame, before P2G: every live particle's rows rotated by params->tank_q, plus the force params->tank_k (x - tank_pivot).
+// The count: params->num_particles when device_count, else n_host; np_upper sizes the launch.
+void launch_tank_frame(cudaStream_t st, const StepParams *params, bool device_count, uint32_t n_host, uint32_t np_upper, const float4 *pos,
+                       float4 *const row[3]);
+
 // ---- surface tension (surface_tension_kernels.cu, DESIGN.md §8 "Surface tension") ----
 // Working memory, allocated with the first surface tension above zero: 12 bytes per cell.
 struct SurfaceTensionWork {

@@ -433,10 +433,19 @@ void HybridFluid::upload_step_params(float dt) {
     BLUB_CUDA_CHECK(cudaEventSynchronize(param_events_[slot]));
     h->dt = dt;
     h->inv_dt = 1.0f / dt;
+    // a moving tank's frame: g_eff replaces the gravity of this step only (gravity_ keeps the configured value), Q and K reach tank_frame_kernel
+    BlubTankStepConstants tank{};
+    if (has_tank_frame_) tank = tank_step_constants(tank_frame_, gravity_, dt);
     for (int c = 0; c < 3; ++c) {
-        h->gravity_dt[c] = gravity_[c] * dt;
-        h->gravity[c] = gravity_[c];
+        const float g = has_tank_frame_ ? tank.gravity[c] : gravity_[c];
+        h->gravity_dt[c] = g * dt;
+        h->gravity[c] = g;
     }
+    for (int i = 0; i < 9; ++i) {
+        h->tank_q[i] = has_tank_frame_ ? tank.coriolis[i] : (i % 4 == 0 ? 1.0f : 0.0f);
+        h->tank_k[i] = tank.force[i];
+    }
+    for (int c = 0; c < 3; ++c) h->tank_pivot[c] = tank.pivot[c];
     h->tolerance[0] = field_velocity_->config.error_tolerance / dt; // pressure_solver.rs:193-201
     h->tolerance[1] = field_density_->config.error_tolerance / dt;
     h->step_count = step_counter_;
@@ -497,6 +506,10 @@ void HybridFluid::run_stage(int stage, float dt) {
         if (flow_active_) {
             const NvtxScope flow_scope("fluid sources & drains");
             run_flow_prologue();
+        }
+        if (tank_rotating()) { // after the prologue: emitted particles start with the source velocity in the tank frame, then feel the frame
+            const NvtxScope tank_scope("moving tank: frame forces");
+            launch_tank_frame(stream_, params_dev_, device_count_mode(), num_particles_, np, pos_[cur_], row_);
         }
         if (!shard && !use_scatter_) {
             // cell lists -> marker (+ FLUID bits) -> one gather per component; deterministic, no accumulator volumes
@@ -982,14 +995,32 @@ uint64_t HybridFluid::plan_substep(uint64_t remaining_ns, const BlubTimeStepping
     float v[3];
     max_particle_velocity(v);
     if (max_velocity_out) std::memcpy(max_velocity_out, v, sizeof(v));
-    if (!(surface_tension_ > 0.0f)) return cfl_substep_ns(remaining_ns, v, gravity_, ts);
+    const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
+    if (!(surface_tension_ > 0.0f)) return tank_cfl_substep_ns(remaining_ns, v, gravity_, tank_frame(), dim, ts);
     const uint64_t cap = capillary_limit_ns(surface_tension_);
     if (cap < ts.min_dt_ns)
         throw UnstableError("plan_substep: the capillary step limit of " + std::to_string(cap) + " ns at a surface tension of " + std::to_string(surface_tension_) +
                             " cells^3/s^2 is below min_dt_ns = " + std::to_string(ts.min_dt_ns) + " ns");
     BlubTimeStepping capped = ts;
     capped.max_dt_ns = std::min(ts.max_dt_ns, cap);
-    return cfl_substep_ns(remaining_ns, v, gravity_, capped);
+    return tank_cfl_substep_ns(remaining_ns, v, gravity_, tank_frame(), dim, capped);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Moving tanks (tank_kernels.cu).  Not in the reference.  The frame is host state only: every upload_step_params turns it into the step's
+// constants, so a captured graph follows a new frame without a recapture; only the launch of tank_frame_kernel depends on whether it rotates.
+void HybridFluid::set_tank_frame(const BlubTankFrame *frame) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_tank_frame: z-slab ranks cannot move their tank");
+    if (mid_step_) throw std::invalid_argument("set_tank_frame: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    if (frame) {
+        check_tank_frame(*frame);
+        if (num_bodies_ > 0 && tank_frame_rotates(*frame))
+            throw std::invalid_argument("set_tank_frame: a rotating frame is not supported with floating bodies (translation-only frames are)");
+    }
+    const bool was_rotating = tank_rotating();
+    has_tank_frame_ = frame != nullptr;
+    if (frame) tank_frame_ = *frame;
+    if (tank_rotating() != was_rotating) destroy_graphs();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1125,6 +1156,7 @@ std::vector<BlubBody> make_body_set(const uint32_t dim[3], const BlubBody *bodie
 void HybridFluid::set_bodies(const BlubBody *bodies, uint32_t num_bodies) {
     if (slab_world_ > 1) throw std::invalid_argument("set_bodies: z-slab ranks have no floating bodies");
     if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    if (num_bodies > 0 && tank_rotating()) throw std::invalid_argument("set_bodies: floating bodies are not supported in a rotating tank frame");
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
     restore_bodies(make_body_set(dim, bodies, num_bodies, false));
 }
@@ -1147,6 +1179,7 @@ void HybridFluid::set_bodies_host(const BlubBody *bodies, const std::vector<Host
     if (slab_world_ > 1) throw std::invalid_argument("set_bodies: z-slab ranks have no floating bodies");
     if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     const uint32_t num_bodies = (uint32_t)meshes.size();
+    if (num_bodies > 0 && tank_rotating()) throw std::invalid_argument("set_bodies: floating bodies are not supported in a rotating tank frame");
     if (num_bodies > (uint32_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
     if (num_bodies && !bodies) throw std::invalid_argument("set_bodies: NULL body array");
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};

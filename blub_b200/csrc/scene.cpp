@@ -150,6 +150,14 @@ float scene_surface_tension_grid(const SceneConfig &cfg) {
     return cfg.surface_tension / (cfg.grid_to_world_scale * cfg.grid_to_world_scale * cfg.grid_to_world_scale);
 }
 
+BlubTankMotion scene_tank_motion_grid(const SceneConfig &cfg) {
+    const float scale = cfg.grid_to_world_scale;
+    BlubTankMotion m = cfg.tank_motion;
+    for (int k = 0; k < 3; ++k) m.pivot[k] = (float)cfg.tank_motion.pivot[k] / scale;
+    for (uint32_t i = 0; i < m.num_translations; ++i) m.translations[i].amplitude = (float)cfg.tank_motion.translations[i].amplitude / scale;
+    return m;
+}
+
 SceneConfig parse_scene_file(const std::string &path) {
     std::ifstream in(path, std::ios::binary);
     if (!in) throw std::ios_base::failure("cannot open scene file " + path);
@@ -215,6 +223,53 @@ SceneConfig parse_scene_file(const std::string &path) {
         cfg.surface_tension = num_f32(*st, "surface_tension");
         if (!std::isfinite(cfg.surface_tension) || cfg.surface_tension < 0.0f || !std::isfinite(scene_surface_tension_grid(cfg)))
             throw std::runtime_error("scene JSON: `fluid.surface_tension` must be finite and not negative");
+    }
+    // a moving tank (not in the reference): pivot and amplitudes in world units, frequencies in Hz, phases in rad, the rate in rad/s; checked
+    // here against the rules of blub_tank_frame_at
+    if (const JsonValue *tm = fluid.get("tank_motion")) {
+        if (tm->kind != JsonValue::Object) throw std::runtime_error("scene JSON: `fluid.tank_motion` is not an object");
+        BlubTankMotion &m = cfg.tank_motion;
+        m = BlubTankMotion{};
+        float v[3];
+        auto unit = [&](const JsonValue &obj, const char *what, double out[3]) {
+            vec3(obj, what, v);
+            const double n = std::sqrt((double)v[0] * v[0] + (double)v[1] * v[1] + (double)v[2] * v[2]);
+            if (!(n > 0.0) || !std::isfinite(n)) throw std::runtime_error(std::string("scene JSON: `") + what + "` must be a finite vector that is not zero");
+            for (int k = 0; k < 3; ++k) out[k] = v[k] / n;
+        };
+        auto opt = [&](const JsonValue &obj, const char *key, const char *what) -> double {
+            const JsonValue *x = obj.get(key);
+            return x ? (double)num_f32(*x, what) : 0.0;
+        };
+        vec3(need(*tm, "pivot"), "tank_motion.pivot", v);
+        for (int k = 0; k < 3; ++k) m.pivot[k] = v[k];
+        if (const JsonValue *trs = tm->get("translations")) {
+            if (trs->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.tank_motion.translations` is not an array");
+            if (trs->array.size() > (size_t)BLUB_TANK_TRANSLATIONS_MAX) throw std::runtime_error("scene JSON: `fluid.tank_motion.translations` holds more than 4");
+            for (const JsonValue &t : trs->array) {
+                if (t.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.tank_motion.translations` entry is not an object");
+                BlubTankTranslation &tr = m.translations[m.num_translations++];
+                unit(need(t, "direction"), "tank_motion.translations.direction", tr.direction);
+                tr.amplitude = num_f32(need(t, "amplitude"), "tank_motion.translations.amplitude");
+                tr.frequency = num_f32(need(t, "frequency"), "tank_motion.translations.frequency");
+                tr.phase = opt(t, "phase", "tank_motion.translations.phase");
+            }
+        }
+        m.axis[1] = 1.0; // no rotation: theta = 0 about any unit axis
+        if (const JsonValue *rot = tm->get("rotation")) {
+            if (rot->kind != JsonValue::Object) throw std::runtime_error("scene JSON: `fluid.tank_motion.rotation` is not an object");
+            unit(need(*rot, "axis"), "tank_motion.rotation.axis", m.axis);
+            m.amplitude = opt(*rot, "amplitude", "tank_motion.rotation.amplitude");
+            m.frequency = opt(*rot, "frequency", "tank_motion.rotation.frequency");
+            m.phase = opt(*rot, "phase", "tank_motion.rotation.phase");
+            m.rate = opt(*rot, "rate", "tank_motion.rotation.rate");
+        }
+        cfg.has_tank_motion = true;
+        try {
+            tank_frame_at(scene_tank_motion_grid(cfg), 0.0);
+        } catch (const std::exception &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.tank_motion`: ") + e.what());
+        }
     }
     // solid load probes (not in the reference): world units, the pivot optional
     if (const JsonValue *probes = fluid.get("load_probes")) {

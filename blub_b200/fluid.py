@@ -197,6 +197,115 @@ class MeshBodyShape(C.Structure):
     _fields_ = [("mesh", C.c_void_p), ("scale", C.c_float)]
 
 
+class TankFrame(C.Structure):
+    """BlubTankFrame: a moving tank's kinematics -- rotation R (tank -> world, row major), the pivot's acceleration A (world axes, cells/s^2),
+    angular velocity and acceleration (tank axes, rad/s and rad/s^2) and the pivot (grid cells), all float64."""
+
+    _fields_ = [("rotation", C.c_double * 9), ("acceleration", C.c_double * 3), ("angular_velocity", C.c_double * 3),
+                ("angular_acceleration", C.c_double * 3), ("pivot", C.c_double * 3)]
+
+    @classmethod
+    def from_dict(cls, d):
+        f = cls()
+        f.rotation[:] = [float(v) for v in np.asarray(d.get("rotation", np.eye(3)), dtype=np.float64).reshape(9)]
+        for name in ("acceleration", "angular_velocity", "angular_acceleration", "pivot"):
+            getattr(f, name)[:] = [float(v) for v in d.get(name, (0.0, 0.0, 0.0))]
+        return f
+
+    def to_dict(self):
+        return {"rotation": np.array(list(self.rotation)).reshape(3, 3), "acceleration": np.array(list(self.acceleration)),
+                "angular_velocity": np.array(list(self.angular_velocity)), "angular_acceleration": np.array(list(self.angular_acceleration)),
+                "pivot": np.array(list(self.pivot))}
+
+
+class TankTranslation(C.Structure):
+    _fields_ = [("direction", C.c_double * 3), ("amplitude", C.c_double), ("frequency", C.c_double), ("phase", C.c_double)]
+
+
+TANK_TRANSLATIONS_MAX = 4  # BLUB_TANK_TRANSLATIONS_MAX
+
+
+class TankMotion(C.Structure):
+    """BlubTankMotion: up to 4 harmonic translations of the pivot and one rotation theta(t) = amplitude sin(2 pi f t + phase) + rate t about a
+    fixed unit axis (grid cells, Hz, rad, rad/s)."""
+
+    _fields_ = [("pivot", C.c_double * 3), ("num_translations", C.c_uint32), ("reserved", C.c_uint32),
+                ("translations", TankTranslation * TANK_TRANSLATIONS_MAX), ("axis", C.c_double * 3), ("amplitude", C.c_double),
+                ("frequency", C.c_double), ("phase", C.c_double), ("rate", C.c_double)]
+
+    @classmethod
+    def from_dict(cls, d):
+        """{"pivot", "translations": [{"direction", "amplitude", "frequency", "phase"?}], "rotation": {"axis", "amplitude"?, "frequency"?,
+        "phase"?, "rate"?}?}; the library checks the values where they are used."""
+        m = cls()
+        m.pivot[:] = [float(v) for v in d["pivot"]]
+        trs = list(d.get("translations", ()))
+        m.num_translations = len(trs)
+        for k, t in enumerate(trs[:TANK_TRANSLATIONS_MAX]):
+            m.translations[k].direction[:] = [float(v) for v in t["direction"]]
+            m.translations[k].amplitude, m.translations[k].frequency = float(t["amplitude"]), float(t["frequency"])
+            m.translations[k].phase = float(t.get("phase", 0.0))
+        rot = d.get("rotation") or {"axis": (0.0, 1.0, 0.0)}
+        m.axis[:] = [float(v) for v in rot["axis"]]
+        m.amplitude, m.frequency = float(rot.get("amplitude", 0.0)), float(rot.get("frequency", 0.0))
+        m.phase, m.rate = float(rot.get("phase", 0.0)), float(rot.get("rate", 0.0))
+        return m
+
+    def to_dict(self):
+        trs = [{"direction": tuple(t.direction), "amplitude": t.amplitude, "frequency": t.frequency, "phase": t.phase}
+               for t in self.translations[:min(self.num_translations, TANK_TRANSLATIONS_MAX)]]
+        return {"pivot": tuple(self.pivot), "translations": trs,
+                "rotation": {"axis": tuple(self.axis), "amplitude": self.amplitude, "frequency": self.frequency, "phase": self.phase, "rate": self.rate}}
+
+
+class TankStepConstants(C.Structure):
+    """BlubTankStepConstants: the float32 constants of one step under a frame (g_eff, Q, K, pivot) and whether it rotates."""
+
+    _fields_ = [("gravity", C.c_float * 3), ("coriolis", C.c_float * 9), ("force", C.c_float * 9), ("pivot", C.c_float * 3), ("rotating", C.c_int32)]
+
+
+def _tank_frame(frame):
+    return frame if isinstance(frame, TankFrame) else TankFrame.from_dict(frame)
+
+
+def _tank_motion(motion):
+    return motion if isinstance(motion, TankMotion) else TankMotion.from_dict(motion)
+
+
+def tank_frame_at(motion, t):
+    """blub_tank_frame_at (host only): the TankFrame of a motion (TankMotion or dict) at t seconds, as a dict of float64 arrays."""
+    out = TankFrame()
+    _check(lib().blub_tank_frame_at(C.byref(_tank_motion(motion)), float(t), C.byref(out)))
+    return out.to_dict()
+
+
+def tank_step_constants(frame, gravity_grid, dt):
+    """blub_tank_step_constants (host only): {"gravity" [3], "coriolis" [3, 3], "force" [3, 3], "pivot" [3]} as float32 arrays and "rotating"
+    for a frame (TankFrame or dict), the fluid's gravity (cells/s^2) and the step's float32 dt."""
+    out = TankStepConstants()
+    _check(lib().blub_tank_step_constants(C.byref(_tank_frame(frame)), _f3(gravity_grid), float(np.float32(dt)), C.byref(out)))
+    return {"gravity": np.array(list(out.gravity), dtype=np.float32), "coriolis": np.array(list(out.coriolis), dtype=np.float32).reshape(3, 3),
+            "force": np.array(list(out.force), dtype=np.float32).reshape(3, 3), "pivot": np.array(list(out.pivot), dtype=np.float32),
+            "rotating": bool(out.rotating)}
+
+
+def tank_cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, frame, grid_dimension, cfl=1.0, max_dt_ns=None, min_dt_ns=1):
+    """blub_tank_cfl_substep_ns (host only): cfl_substep_ns under a tank frame (None: exactly cfl_substep_ns)."""
+    out = C.c_uint64(0)
+    ts = time_stepping(cfl, remaining_ns if max_dt_ns is None else max_dt_ns, min_dt_ns)
+    fr = None if frame is None else C.byref(_tank_frame(frame))
+    _check(lib().blub_tank_cfl_substep_ns(int(remaining_ns), _f3(max_velocity), _f3(gravity_grid), fr, (C.c_uint32 * 3)(*[int(v) for v in grid_dimension]),
+                                          C.byref(ts), C.byref(out)))
+    return int(out.value)
+
+
+def scene_tank_motion(path):
+    """The scene's fluid.tank_motion in grid cells as a dict (see TankMotion.from_dict), or None without the key (host only)."""
+    m, has = TankMotion(), C.c_int32(0)
+    _check(lib().blub_scene_tank_motion(os.fsencode(path), C.byref(m), C.byref(has)))
+    return m.to_dict() if has.value else None
+
+
 def quat_matrix(q):
     """The float64 rotation matrix of the quaternion q = (w, x, y, z)."""
     w, x, y, z = [float(v) for v in q]
@@ -317,6 +426,12 @@ def lib():
         "blub_fluid_max_particle_velocity": (C.c_int, [vp, f3]),
         "blub_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
         "blub_fluid_plan_substep": (C.c_int, [vp, C.c_uint64, C.POINTER(TimeStepping), C.POINTER(C.c_uint64), f3]),
+        "blub_tank_frame_at": (C.c_int, [C.POINTER(TankMotion), C.c_double, C.POINTER(TankFrame)]),
+        "blub_tank_step_constants": (C.c_int, [C.POINTER(TankFrame), f3, C.c_float, C.POINTER(TankStepConstants)]),
+        "blub_fluid_set_tank_frame": (C.c_int, [vp, C.POINTER(TankFrame)]),
+        "blub_fluid_tank_frame": (C.c_int, [vp, C.POINTER(TankFrame)]),
+        "blub_tank_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TankFrame), C.POINTER(u32), C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
+        "blub_scene_tank_motion": (C.c_int, [C.c_char_p, C.POINTER(TankMotion), C.POINTER(C.c_int32)]),
         "blub_fluid_set_bodies": (C.c_int, [vp, C.POINTER(Body), u32]),
         "blub_fluid_body_history": (C.c_int, [vp, u32, C.POINTER(BodyRecord), u32, C.POINTER(u32)]),
         "blub_fluid_bodies": (C.c_int, [vp, C.POINTER(Body), u32, C.POINTER(u32)]),
@@ -809,6 +924,18 @@ class HybridFluid:
         _check(self.L.blub_fluid_surface_tension(self.h, C.byref(out)))
         return float(out.value)
 
+    # -- moving tanks -------------------------------------------------------------------------
+    def set_tank_frame(self, frame):
+        """The tank frame of the following steps (TankFrame, a dict as for TankFrame.from_dict, or None: at rest).  Set it before each step.
+        Raises BlubError (and changes nothing) on a non-finite frame, a rotation that is not orthonormal with det +1, a rotating frame while
+        the fluid has floating bodies, z-slab ranks and a fluid inside a step."""
+        _check(self.L.blub_fluid_set_tank_frame(self.h, None if frame is None else C.byref(_tank_frame(frame))))
+
+    def tank_frame(self):
+        """The frame as a dict (see TankFrame.to_dict), or None at rest."""
+        out = TankFrame()
+        return out.to_dict() if self.L.blub_fluid_tank_frame(self.h, C.byref(out)) == 1 else None
+
     # -- CFL-limited substeps -----------------------------------------------------------------
     def max_particle_velocity(self):
         """[max |v_x|, max |v_y|, max |v_z|] over the live particles in cells/s, exact (float32 values).  One kernel, then synchronises."""
@@ -818,7 +945,8 @@ class HybridFluid:
 
     def plan_substep(self, remaining_ns, cfl=1.0, max_dt_ns=None, min_dt_ns=1):
         """(dt_ns, max_velocity): the measured largest particle velocity per axis and the next substep of `remaining_ns` by the CFL rule
-        (cfl_substep_ns) with this fluid's gravity, max_dt_ns lowered to the capillary limit while the fluid has surface tension; max_dt_ns
+        (cfl_substep_ns; tank_cfl_substep_ns while a tank frame is set) with this fluid's gravity, max_dt_ns lowered to the capillary limit
+        while the fluid has surface tension; max_dt_ns
         defaults to remaining_ns.  Raises BlubError as cfl_substep_ns does, and on a
         z-slab rank or a fluid inside a step."""
         ts = time_stepping(cfl, remaining_ns if max_dt_ns is None else max_dt_ns, min_dt_ns)

@@ -408,6 +408,79 @@ int blub_fluid_surface_tension(const BlubFluid *fluid, float *cells3_per_s2);
  * sets it on the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
 int blub_scene_surface_tension(const char *scene_json_path, float *cells3_per_s2);
 
+/* ---- moving tanks (not part of the reference surface; rules: DESIGN.md section 8 "Moving tanks") ----------------------------------
+ * The liquid is simulated in the tank's own frame: the grid, the walls, the solid volume, probes, sources and drains are fixed in it, and the
+ * fluid feels f = R^T (g - A) - alpha x r - omega x (omega x r) - 2 omega x v with r = x - pivot (all lengths in grid cells).  The library keeps
+ * no clock: the caller sets the frame of the next steps with blub_fluid_set_tank_frame, as it rewrites the solid volume before each step.
+ * The frame is not state: a saved file is the same with or without one, and a loaded fluid starts at rest. */
+typedef struct {
+    double rotation[9];             /* R: tank -> world, row major; orthonormal with det +1 (to 1e-6) */
+    double acceleration[3];         /* A: the pivot's acceleration, world axes, cells/s^2 */
+    double angular_velocity[3];     /* omega: tank axes, rad/s */
+    double angular_acceleration[3]; /* alpha: tank axes, rad/s^2 */
+    double pivot[3];                /* grid cells */
+} BlubTankFrame;
+/* One harmonic translation of the pivot: amplitude * direction * sin(2 pi frequency t + phase). */
+typedef struct {
+    double direction[3];            /* unit vector (to 1e-6), world axes */
+    double amplitude;               /* cells */
+    double frequency;               /* Hz, >= 0 */
+    double phase;                   /* rad */
+} BlubTankTranslation;
+#define BLUB_TANK_TRANSLATIONS_MAX 4
+/* A prescribed motion the library evaluates but never stores: up to 4 harmonic translations and one rotation about the fixed unit axis n
+ * through the pivot by theta(t) = amplitude sin(2 pi frequency t + phase) + rate t. */
+typedef struct {
+    double pivot[3];                /* grid cells */
+    uint32_t num_translations;      /* <= BLUB_TANK_TRANSLATIONS_MAX */
+    uint32_t reserved;              /* 0 */
+    BlubTankTranslation translations[BLUB_TANK_TRANSLATIONS_MAX];
+    double axis[3];                 /* n: unit vector (to 1e-6) */
+    double amplitude;               /* rad */
+    double frequency;               /* Hz, >= 0 */
+    double phase;                   /* rad */
+    double rate;                    /* rad/s */
+} BlubTankMotion;
+/* The float32 constants one step uses, computed in float64 and rounded once (blub_tank_step_constants). */
+typedef struct {
+    float gravity[3];               /* g_eff = R^T (g - A) */
+    float coriolis[9];              /* Q = Rot(omega / |omega|, -2 |omega| dt), row major: the exact solution of dv/dt = -2 omega x v over dt */
+    float force[9];                 /* K = dt (|omega|^2 I - omega omega^T - [alpha]x), row major: the velocity increment per cell of r */
+    float pivot[3];
+    int32_t rotating;               /* 1 when omega or alpha is not zero: the step then runs tank_frame_kernel */
+} BlubTankStepConstants;
+#ifdef __cplusplus
+static_assert(sizeof(BlubTankFrame) == 168 && sizeof(BlubTankMotion) == 280 && sizeof(BlubTankStepConstants) == 100, "tank layouts");
+#else
+_Static_assert(sizeof(BlubTankFrame) == 168 && sizeof(BlubTankMotion) == 280 && sizeof(BlubTankStepConstants) == 100, "tank layouts");
+#endif
+/* Host only: the frame of `motion` at t_seconds, in closed form in float64: R = Rot(n, theta), omega = theta' n, alpha = theta'' n, A = the second
+ * derivative of the translations, pivot = motion->pivot.  BLUB_ERR_INVALID_ARGUMENT: a NULL pointer, a non-finite value or t, a direction or
+ * axis that is not a unit vector, a negative frequency, more than 4 translations or reserved != 0. */
+int blub_tank_frame_at(const BlubTankMotion *motion, double t_seconds, BlubTankFrame *out);
+/* Host only: the step constants of `frame` for a fluid of float32 gravity gravity_grid and a step of dt seconds (the step's float32 delta).
+ * BLUB_ERR_INVALID_ARGUMENT: a NULL pointer, a frame blub_fluid_set_tank_frame refuses, a non-finite gravity or dt <= 0. */
+int blub_tank_step_constants(const BlubTankFrame *frame, const float gravity_grid[3], float dt, BlubTankStepConstants *out);
+/* The frame of the following steps (NULL: at rest).  Every step then uses the constants above with the fluid's gravity: StepParams' gravity
+ * becomes g_eff (a frame with omega = alpha = 0 launches nothing new and steps exactly as blub_fluid_set_gravity_grid(g_eff) would), and a
+ * rotating frame runs tank_frame_kernel on every live particle in stage 0, between the sources and drains and the P2G.  Turning rotation on
+ * or off drops the cached step graphs; a new frame of the same kind does not.  BLUB_ERR_INVALID_ARGUMENT, changing nothing: a frame that is not
+ * finite or whose rotation is not orthonormal with det +1 to 1e-6, a rotating frame while the fluid has floating bodies, a z-slab rank, or a
+ * fluid left inside a step by blub_fluid_step_stages.  While a frame is set blub_fluid_plan_substep plans with blub_tank_cfl_substep_ns. */
+int blub_fluid_set_tank_frame(BlubFluid *fluid, const BlubTankFrame *frame);
+/* 1 and *out = the frame when one is set, 0 when the fluid is at rest (or fluid is NULL) */
+int blub_fluid_tank_frame(const BlubFluid *fluid, BlubTankFrame *out);
+/* Host only: blub_cfl_substep_ns under a frame (NULL: exactly blub_cfl_substep_ns).  The gravity passed to the rule has the norm
+ * |g_eff| + (|omega|^2 + |alpha|) r_max, r_max = the distance from the pivot to the farthest corner of the grid_dimension box; while omega is not
+ * zero the velocity passed is the Euclidean norm of max_velocity (the Coriolis rotation moves speed between axes).  Both rounded to float32. */
+int blub_tank_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTankFrame *frame,
+                             const uint32_t grid_dimension[3], const BlubTimeStepping *config, uint64_t *dt_ns);
+/* The scene's optional fluid.tank_motion in grid cells: {pivot, translations: [{direction, amplitude, frequency, phase?}],
+ * rotation?: {axis, amplitude?, frequency?, phase?, rate?}} in world units (pivot and amplitudes / grid_to_world_scale, as the load probes'
+ * pivots), Hz, rad and rad/s; directions and the axis are normalised.  *has_motion = 0 without the key.  A bad value makes every scene call fail
+ * with BLUB_ERR_PARSE. */
+int blub_scene_tank_motion(const char *scene_json_path, BlubTankMotion *out, int32_t *has_motion);
+
 /* ---- scene JSON surface (src/scene/mod.rs:19-43,109-144; src/scene/models.rs:11-46) ------------------------- */
 /* Scene::new + create_fluid_from_config: parses an unchanged blub scene file, creates the fluid, seeds every
  * fluid cube (world / grid_to_world_scale) and sets gravity.  static_objects are parsed (blub_scene_static_object) but their

@@ -16,7 +16,7 @@ SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu
 # the mesh voxelizer shares its arithmetic with a host twin and a NumPy restatement, the curvature with a NumPy restatement: no FMA
 # contraction, so that they agree bit for bit
 EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"], "surface_tension_kernels.cu": ["-fmad=false"]}
-HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "voxelize_core.hpp", "xoshiro.hpp", "grid_words.cuh", "grid_reduce.cuh", os.path.join("..", "..", "include", "blub_fluid.h")]
+HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "advect.cuh", "voxelize_core.hpp", "xoshiro.hpp", "grid_words.cuh", "grid_reduce.cuh", os.path.join("..", "..", "include", "blub_fluid.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

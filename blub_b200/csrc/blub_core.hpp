@@ -418,6 +418,7 @@ class HybridFluid {
     struct GraphRolesAfter {
         int cur, row_parity;
         uint32_t exchanges;
+        bool density_zero;
     };
     GraphRolesAfter graph_roles_after_[2][2][2][2] = {};
     bool capturing_ = false;
@@ -437,6 +438,12 @@ class HybridFluid {
     float4 *row_[3] = {nullptr, nullptr, nullptr};
     GridArray<float> u_[3];
     GridArray<long long> density_;     // density scatter accumulator, 64-bit fixed point (common.cuh: to_fixed)
+    // Stage 7 scatters the density of the new positions along with the advection (launch_advect_density) on one GPU and grids of 2^21 cells
+    // or more (BLUB_DENSITY_FUSE=off / on, read when the fluid is created, decides for any grid); stage 9 then only finishes it on the
+    // particles' cells and leaves the volume zero.
+    bool density_fuse_ = true;
+    bool density_fused_ = false; // stage 7 of the running step / step_stages call scattered the density of the positions as they are now
+    bool density_zero_ = true;   // the density volume is all zero once the enqueued work has run: the fused stage 7 needs no memset
     GridArray<longlong2> numw_[3];     // scatter-form P2G accumulators: (sum w*value, sum w) per face, 64-bit fixed point
     FluidBits fluid_bits_ = {nullptr, 0}; // 1 bit per cell "FLUID", rebuilt with every finished marker volume
     bool fluid_bits_stale_ = false;       // the marker volume was written through a tap since

@@ -77,6 +77,13 @@ void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams 
 void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs);
 void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos,
                         const int8_t *marker, long long *density, float *rhs, const ScatterSchedule &sched);
+// Stage 7 with the density scatter fused in (one GPU): launch_advect, and the scatter of the new positions into `density`, which must be all
+// zero.  launch_density_finish_sparse then writes the right-hand side of the FLUID cells and puts the density words back to zero, visiting
+// the one-cell dilation of particle_words only: the words of a marker pass over the marker this advection left (launch_boundary_marker).
+void launch_advect_density(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos, float4 *const row[3],
+                           float *const u[3], const uint2 *vox, int8_t *marker, long long *density, const ScatterSchedule &sched);
+void launch_density_finish_sparse(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const FluidBits &bits,
+                                  const uint32_t *particle_words, long long *density, float *rhs);
 void launch_boundary_marker(cudaStream_t st, const GridDim &g, int8_t *marker, const uint2 *vox, const FluidBits &bits, uint32_t *particle_words = nullptr);
 void launch_fluid_bits(cudaStream_t st, const GridDim &g, const int8_t *marker, const FluidBits &bits);
 int binning_scan_blocks(const GridDim &g);

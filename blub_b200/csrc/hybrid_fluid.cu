@@ -180,6 +180,11 @@ HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num
     if (const char *rs = std::getenv("BLUB_RESORT_EVERY")) internal_resort_every_ = (uint32_t)std::atoi(rs);
     const char *ng = std::getenv("BLUB_NO_GRAPH");
     if (ng && ng[0] == '1') use_graph = false;
+    // The fused stage 7 pays where its blocks' tile atomics can hide under other blocks' advection traffic: on grids of 2^21 cells and more.
+    // On the 128 x 64 x 64 scenes it measured 1.3-1.5 % slower than the separate kernels.  BLUB_DENSITY_FUSE=off / on (a test hook) decides
+    // for every grid.
+    const char *df = std::getenv("BLUB_DENSITY_FUSE");
+    density_fuse_ = df && std::string(df) == "off" ? false : (df && std::string(df) == "on") || grid_.n >= (int64_t(1) << 21);
 }
 
 void HybridFluid::destroy_graphs() {
@@ -536,9 +541,10 @@ void HybridFluid::run_stage(int stage, float dt) {
         launch_divergence_compute(stream_, grid_, bits, marker_.ptr, u, vox, solver_->residual());
         if (surface_tension_ > 0.0f) {
             const NvtxScope st_scope("surface tension: curvature");
-            // The density accumulator is free until stage 9 memsets it.  On the scheduled path the splat rewrites sched_.item_box, the boxes
-            // the next P2G reads: harmless, because stage 9 of this step rewrites them before that P2G.
+            // The density accumulator is free until stage 7 or 9 clears it.  On the scheduled path the splat rewrites sched_.item_box, the boxes
+            // the next P2G reads: harmless, because stage 7 or 9 of this step rewrites them before that P2G.
             launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr, sched_);
+            density_zero_ = false;
             launch_surface_curvature(stream_, grid_, bits, marker_.ptr, density_.ptr, st_);
             launch_surface_rhs(stream_, grid_, bits, params_dev_, marker_.ptr, st_, solver_->residual());
         }
@@ -586,7 +592,12 @@ void HybridFluid::run_stage(int stage, float dt) {
         launch_clear_marker(stream_, grid_, marker_.ptr);
         break;
     case 7: // advect particles (:917-921)
-        if (!shard) {
+        if (!shard && density_fuse_) { // + the density scatter of stage 9
+            if (!density_zero_) BLUB_CUDA_CHECK(cudaMemsetAsync(density_.ptr, 0, (size_t)grid_.n * sizeof(long long), stream_));
+            launch_advect_density(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, vox, marker_.ptr, density_.ptr, sched_);
+            density_fused_ = true;
+            density_zero_ = false;
+        } else if (!shard) {
             launch_advect(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, vox, marker_.ptr);
         } else {
             launch_advect_migrate(stream_, grid_, params_dev_, np, pos_[cur_], row_, u, vox, marker_.ptr, slab_migrate_targets());
@@ -596,17 +607,24 @@ void HybridFluid::run_stage(int stage, float dt) {
         }
         break;
     case 8: // density projection: set boundary marker (:923-927)
-        launch_boundary_marker(stream_, grid_, marker_.ptr, vox, bits, vox ? particle_words_ : nullptr); // with a solid volume: the particle words stage 11 visits around
+        // the particle words: with a solid volume the cells stage 11 visits around, after a fused stage 7 the cells stage 9 finishes around
+        launch_boundary_marker(stream_, grid_, marker_.ptr, vox, bits, vox || density_fused_ ? particle_words_ : nullptr);
         fluid_bits_stale_ = false;
         break;
     case 9: // density projection: compute density error (:928-932)
-        if (!shard) {
+        if (density_fused_) {
+            launch_density_finish_sparse(stream_, grid_, params_dev_, marker_.ptr, bits, particle_words_, density_.ptr, solver_->residual());
+            density_fused_ = false;
+            density_zero_ = true;
+        } else if (!shard) { // the positions may have changed since a fused stage 7 (a step_stages window, an upload): scatter them afresh
             launch_density_rhs(stream_, grid_, params_dev_, np, pos_[cur_], marker_.ptr, density_.ptr, solver_->residual(), sched_);
+            density_zero_ = false;
         } else {
             launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr, sched_);
             const SlabHaloItem items[1] = {{density_.ptr, sizeof(long long), 0}};
             slab_halo_exchange(items, 1); // X4
             launch_density_finish(stream_, grid_, params_dev_, marker_.ptr, density_.ptr, solver_->residual());
+            density_zero_ = false;
         }
         break;
     case 10: // secondary pressure solver (:940-949)
@@ -647,9 +665,15 @@ void HybridFluid::step(double simulation_delta_seconds) {
     field_velocity_->retrieve_new_error_samples(); // pressure_solver.rs:614
     field_density_->retrieve_new_error_samples();
     upload_step_params(dt);
+    density_fused_ = false;
     if (!use_graph) {
         for (int s = 0; s < 14; ++s) run_stage(s, dt);
         return;
+    }
+    // a graph is recorded from an all-zero density volume, so that its stage 7 needs no memset when it fuses
+    if (density_fuse_ && !density_zero_) {
+        BLUB_CUDA_CHECK(cudaMemsetAsync(density_.ptr, 0, (size_t)grid_.n * sizeof(long long), stream_));
+        density_zero_ = true;
     }
     GraphSignature sig;
     sig.num_particles = flow_active_ ? 0xFFFFFFFEu : num_particles_; // with sources / drains the launches do not depend on the count
@@ -667,13 +691,14 @@ void HybridFluid::step(double simulation_delta_seconds) {
         int cur, row_parity;
         uint32_t exchange_index, step_counter;
         float4 *row[3], *row_alt[3];
+        bool density_zero;
     };
     auto save_roles = [&]() {
-        Roles r{cur_, row_parity_, slab_exchange_index_, step_counter_, {row_[0], row_[1], row_[2]}, {row_alt_[0], row_alt_[1], row_alt_[2]}};
+        Roles r{cur_, row_parity_, slab_exchange_index_, step_counter_, {row_[0], row_[1], row_[2]}, {row_alt_[0], row_alt_[1], row_alt_[2]}, density_zero_};
         return r;
     };
     auto restore_roles = [&](const Roles &r) {
-        cur_ = r.cur; row_parity_ = r.row_parity; slab_exchange_index_ = r.exchange_index; step_counter_ = r.step_counter;
+        cur_ = r.cur; row_parity_ = r.row_parity; slab_exchange_index_ = r.exchange_index; step_counter_ = r.step_counter; density_zero_ = r.density_zero;
         for (int k = 0; k < 3; ++k) { row_[k] = r.row[k]; row_alt_[k] = r.row_alt[k]; }
     };
     const Roles before = save_roles();
@@ -695,7 +720,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
             throw;
         }
         capturing_ = false;
-        graph_roles_after_[before.cur][kb][before.row_parity][kx] = {cur_, row_parity_, slab_exchange_index_ - before.exchange_index};
+        graph_roles_after_[before.cur][kb][before.row_parity][kx] = {cur_, row_parity_, slab_exchange_index_ - before.exchange_index, density_zero_};
         restore_roles(before); // capture only recorded; the replay below performs the step
         nodes_in_graph = g_kernel_launches.load() - launches0; // recorded, not launched
         g_kernel_launches.fetch_sub(nodes_in_graph);
@@ -714,6 +739,7 @@ void HybridFluid::step(double simulation_delta_seconds) {
         row_parity_ = after.row_parity;
     }
     slab_exchange_index_ = before.exchange_index + after.exchanges;
+    density_zero_ = after.density_zero;
     step_counter_ = before.step_counter + 1;
     if (num_load_probes_ > 0) note_load_record(before.step_counter);
     if (num_bodies_ > 0) note_record(body_steps_, before.step_counter, BODY_HISTORY_LENGTH);
@@ -726,6 +752,7 @@ void HybridFluid::step_stages(double simulation_delta_seconds, int from, int to)
     const float dt = (float)simulation_delta_seconds;
     if (!(dt > 0.0f)) throw std::invalid_argument("simulation delta must be positive");
     upload_step_params(dt);
+    density_fused_ = false; // what happened to the particles between two calls is unknown
     for (int s = from; s < to && s < 14; ++s) run_stage(s, dt);
     mid_step_ = to < 14;
 }
@@ -734,6 +761,7 @@ void HybridFluid::step_timed(double simulation_delta_seconds, float ms[14]) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     const float dt = (float)simulation_delta_seconds;
     upload_step_params(dt);
+    density_fused_ = false;
     cudaEvent_t ev[15];
     for (auto &e : ev) BLUB_CUDA_CHECK(cudaEventCreate(&e));
     BLUB_CUDA_CHECK(cudaEventRecord(ev[0], stream_));

@@ -31,14 +31,12 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "advect.cuh"
 #include "fluid_kernels.hpp"
 
 namespace blub {
 namespace {
 
-constexpr int PT = 256; // threads per block for particle and cell kernels
-
-__device__ __forceinline__ int lin(const GridDim &g, int x, int y, int z) { return (z * g.ny + y) * g.nx + x; }
 inline int blocks_for(int64_t n, int per_block) { return (int)((n + per_block - 1) / per_block); }
 // particle kernels: at most 128 blocks per SM (small enough for a negligible tail, few enough to launch quickly), a grid-stride loop over the rest
 inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), device_sm_count() * 128); }
@@ -877,26 +875,19 @@ __device__ __forceinline__ TileWindow box_window(const GridDim &g, const Scatter
     for (int d = 0; d < 3; ++d) o[d] = min(max(mid[d] - e[d] / 2, lo[d]), hi[d] - e[d] + 1);
     return TileWindow{o[0], o[1], o[2], e[0], e[1], e[2]};
 }
-// The window of work item `it` (its warps are s.warps[w0 .. w1)) for the density scatter, from the primal cells its particles are in NOW:
-// particles drift away from the brick they were sorted into, and a window fixed at the re-sort loses them within a few steps.  The box of
-// those cells is also kept in s.item_box: the next step's P2G scatter takes its window from it (the density correction in between moves
-// particles by a fraction of a cell; a face that leaves the window takes the global path).  Every thread of the block calls this; it ends
-// with __syncthreads().
-template <int CAP>
-__device__ __forceinline__ TileWindow item_window(const GridDim &g, const ScatterSchedule &s, uint32_t it, uint32_t w0, uint32_t w1, uint32_t np,
-                                                  const float4 *__restrict__ pos, float clamp_lo, int (*scratch)[8], TileWindow *shared_win) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int big = 0x3fffffff;
-    int mn[3] = {big, big, big}, mx[3] = {-big, -big, -big};
-    for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
-        const uint32_t i = 32u * s.warps[k] + lane;
-        if (i < np) {
-            const float3 p = transfer_position(g, pos[i], clamp_lo);
-            const int c[3] = {min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1)};
+// The box of primal cells a work item's particles are in, one thread's share: `p` a position as the scatter sees it (transfer_position)
+constexpr int BOX_EMPTY = 0x3fffffff;
+__device__ __forceinline__ void extend_box(const GridDim &g, const float3 &p, int mn[3], int mx[3]) {
+    const int c[3] = {min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1)};
 #pragma unroll
-            for (int d = 0; d < 3; ++d) { mn[d] = min(mn[d], c[d]); mx[d] = max(mx[d], c[d]); }
-        }
-    }
+    for (int d = 0; d < 3; ++d) { mn[d] = min(mn[d], c[d]); mx[d] = max(mx[d], c[d]); }
+}
+// The tile window of work item `it` from the threads' shares of its cell box (extend_box), which is also kept in s.item_box.  Every thread
+// of the block calls this; it ends with __syncthreads().
+template <int CAP>
+__device__ __forceinline__ TileWindow item_box_window(const GridDim &g, const ScatterSchedule &s, uint32_t it, int mn[3], int mx[3], int (*scratch)[8],
+                                                      TileWindow *shared_win) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
         mn[d] = __reduce_min_sync(0xffffffffu, mn[d]);
@@ -910,7 +901,7 @@ __device__ __forceinline__ TileWindow item_window(const GridDim &g, const Scatte
         int lo[3], hi[3];
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
-            lo[d] = big; hi[d] = -big;
+            lo[d] = BOX_EMPTY; hi[d] = -BOX_EMPTY;
             for (int w = 0; w < PT / 32; ++w) { lo[d] = min(lo[d], scratch[w][d]); hi[d] = max(hi[d], scratch[w][3 + d]); }
         }
         const int4 l = make_int4(lo[0], lo[1], lo[2], 0), h = make_int4(hi[0], hi[1], hi[2], 0);
@@ -920,6 +911,22 @@ __device__ __forceinline__ TileWindow item_window(const GridDim &g, const Scatte
     }
     __syncthreads();
     return *shared_win;
+}
+// The window of work item `it` (its warps are s.warps[w0 .. w1)) for the density scatter, from the primal cells its particles are in NOW:
+// particles drift away from the brick they were sorted into, and a window fixed at the re-sort loses them within a few steps.  The box of
+// those cells is also kept in s.item_box: the next step's P2G scatter takes its window from it (the density correction in between moves
+// particles by a fraction of a cell; a face that leaves the window takes the global path).  Every thread of the block calls this; it ends
+// with __syncthreads().
+template <int CAP>
+__device__ __forceinline__ TileWindow item_window(const GridDim &g, const ScatterSchedule &s, uint32_t it, uint32_t w0, uint32_t w1, uint32_t np,
+                                                  const float4 *__restrict__ pos, float clamp_lo, int (*scratch)[8], TileWindow *shared_win) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int mn[3] = {BOX_EMPTY, BOX_EMPTY, BOX_EMPTY}, mx[3] = {-BOX_EMPTY, -BOX_EMPTY, -BOX_EMPTY};
+    for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
+        const uint32_t i = 32u * s.warps[k] + lane;
+        if (i < np) extend_box(g, transfer_position(g, pos[i], clamp_lo), mn, mx);
+    }
+    return item_box_window<CAP>(g, s, it, mn, mx, scratch, shared_win);
 }
 
 template <bool MARK, bool MATCH>
@@ -1093,15 +1100,10 @@ __device__ __forceinline__ unsigned pbits(const GridDim &g, const uint32_t *__re
     if (xw < 0 || xw >= wpr || y < 0 || y >= g.ny || z < 0 || z >= g.nz) return 0u;
     return __ldg(pw + (z * g.ny + y) * wpr + xw);
 }
-__global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, const uint32_t *__restrict__ particle_words, const StepParams *__restrict__ params,
-                                                           const int8_t *__restrict__ marker, float *__restrict__ ux, float *__restrict__ uy,
-                                                           float *__restrict__ uz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
-                                                           longlong2 *__restrict__ nwz) {
-    const int nwords = wpr * g.ny * g.nz;
-    const int w = blockIdx.x * PT + threadIdx.x, lane = threadIdx.x & 31;
+// the cells of word w (xw, y, z) within one cell of a cell in particle_words; 0 for a thread beyond the last word
+__device__ __forceinline__ unsigned particle_dilation(const GridDim &g, const uint32_t *__restrict__ particle_words, int wpr, int w, int &xw, int &y, int &z) {
     unsigned touched = 0;
-    int xw = 0, y = 0, z = 0;
-    if (w < nwords) {
+    if (w < wpr * g.ny * g.nz) {
         xw = w % wpr;
         const int rowi = w / wpr;
         y = rowi % g.ny;
@@ -1116,6 +1118,15 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
         const int cells = min(32, g.nx - xw * 32);
         if (cells < 32) touched &= (1u << cells) - 1u;
     }
+    return touched;
+}
+__global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, const uint32_t *__restrict__ particle_words, const StepParams *__restrict__ params,
+                                                           const int8_t *__restrict__ marker, float *__restrict__ ux, float *__restrict__ uy,
+                                                           float *__restrict__ uz, longlong2 *__restrict__ nwx, longlong2 *__restrict__ nwy,
+                                                           longlong2 *__restrict__ nwz) {
+    const int w = blockIdx.x * PT + threadIdx.x, lane = threadIdx.x & 31;
+    int xw = 0, y = 0, z = 0;
+    const unsigned touched = particle_dilation(g, particle_words, wpr, w, xw, y, z);
     unsigned todo = __ballot_sync(0xffffffffu, touched != 0u);
     float *const u[3] = {ux, uy, uz};
     longlong2 *const nw[3] = {nwx, nwy, nwz};
@@ -1235,14 +1246,69 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
     }
 }
 
-// density_projection_gather_error.comp:99-199
-__global__ void __launch_bounds__(PT) density_rhs_kernel(GridDim g, const StepParams *__restrict__ params,
-                                                         const int8_t *__restrict__ marker, const long long *__restrict__ density,
-                                                         float *__restrict__ rhs) {
-    const int64_t i = (int64_t)blockIdx.x * PT + threadIdx.x;
-    if (i >= g.n) return;
-    if (marker[i] != CELL_FLUID) return;
-    float d = (float)from_fixed<FIXED_WEIGHT_BITS>(density[i]);
+// Stage 7 with the density scatter of stage 9 fused in behind it (one GPU): every particle is advected by advect_kernel_one and its new
+// position goes on to density_scatter_kernel_one from the block's registers and shared memory, never from the position array.  The work order
+// is density_scatter_kernel's -- the schedule's work items, 8 of an item's warps at a time, then 256-particle chunks for the rest -- so
+// every warp holds the particles it holds there and forms the same peer groups and integers.  An item's warps are advected first, their
+// positions kept in `moved`; the item's window (and s.item_box) come from them, then the tile is zeroed, scattered into and flushed.  One
+// block's tile atomics overlap another's advection traffic on the same SM, and the positions are not read a second time.  The density
+// volume must be all zero on entry (HybridFluid::density_zero_).
+template <bool MATCH>
+__global__ void __launch_bounds__(PT) advect_density_kernel(GridDim g, const StepParams *__restrict__ params, float4 *__restrict__ pos,
+                                                            float4 *__restrict__ rowx, float4 *__restrict__ rowy, float4 *__restrict__ rowz,
+                                                            const float *__restrict__ ux, const float *__restrict__ uy, const float *__restrict__ uz,
+                                                            const uint2 *__restrict__ vox, int8_t *__restrict__ marker, long long *__restrict__ density,
+                                                            ScatterSchedule sched) {
+    __shared__ __align__(16) uint32_t tile[2 * DENSITY_TILE]; // low words, high words
+    __shared__ float3 moved[SCHED_K * 32];                     // the new positions of an item's particles, as the scatter sees them
+    __shared__ int scratch[PT / 32 + 1][8];
+    __shared__ TileWindow shared_win;
+    const uint32_t np_ = params->num_particles;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t tail;
+    const uint32_t items = schedule_items(sched, tail);
+    for (uint32_t it = blockIdx.x; it < items; it += gridDim.x) { // block-uniform
+        const uint32_t w0 = sched.item_start[it], w1 = it + 1 < items ? sched.item_start[it + 1] : tail / 32u;
+        int mn[3] = {BOX_EMPTY, BOX_EMPTY, BOX_EMPTY}, mx[3] = {-BOX_EMPTY, -BOX_EMPTY, -BOX_EMPTY};
+        for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
+            const uint32_t i = 32u * sched.warps[k] + lane;
+            const float3 p = transfer_position(g, advect_kernel_one<false>(i, g, params, pos, rowx, rowy, rowz, ux, uy, uz, vox, marker, MigrateOut{}), 0.5f);
+            moved[(k - w0) * 32 + lane] = p;
+            if (i < np_) extend_box(g, p, mn, mx);
+        }
+        const TileWindow win = item_box_window<DENSITY_TILE>(g, sched, it, mn, mx, scratch, &shared_win);
+        const int size = win.ex * win.ey * win.ez;
+        tile_zero<2, DENSITY_TILE>(tile, size);
+        __syncthreads();
+        for (uint32_t k = w0 + warp; k < w1; k += PT / 32) // warp-uniform; each warp reads back only what it wrote
+            density_scatter_kernel_one<MATCH>(32u * sched.warps[k] + lane, g, params, moved[(k - w0) * 32 + lane], density, win, tile);
+        __syncthreads();
+        for (int t = threadIdx.x; t < size; t += PT) {
+            const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
+            if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
+        }
+    }
+    for (uint32_t b = tail + blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
+        const uint32_t i = b + threadIdx.x;
+        const float3 p = transfer_position(g, advect_kernel_one<false>(i, g, params, pos, rowx, rowy, rowz, ux, uy, uz, vox, marker, MigrateOut{}), 0.5f);
+        const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
+        const TileWindow win = scatter_window<DENSITY_TILE>(b, np_, i < np_, cell, scratch, &shared_win);
+        const int size = win.ex * win.ey * win.ez;
+        tile_zero<2, DENSITY_TILE>(tile, size);
+        __syncthreads();
+        density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
+        __syncthreads();
+        for (int t = threadIdx.x; t < size; t += PT) {
+            const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
+            if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
+        }
+    }
+}
+
+// density_projection_gather_error.comp:99-199: the right-hand side of FLUID cell i from its density sum q
+__device__ __forceinline__ float density_rhs_of(const GridDim &g, const StepParams *__restrict__ params, const int8_t *__restrict__ marker, int64_t i,
+                                                long long q) {
+    float d = (float)from_fixed<FIXED_WEIGHT_BITS>(q);
     const int m[6] = {marker[i + 1], marker[i + g.sy], marker[i + g.sz], marker[i - 1], marker[i - g.sy], marker[i - g.sz]};
     bool any_air = false;
 #pragma unroll
@@ -1254,7 +1320,37 @@ __global__ void __launch_bounds__(PT) density_rhs_kernel(GridDim g, const StepPa
     d = 1.0f - d / 8.0f;
     d = fminf(fmaxf(d, -0.5f), 0.5f);
     d /= params->dt;
-    rhs[i] = d;
+    return d;
+}
+__global__ void __launch_bounds__(PT) density_rhs_kernel(GridDim g, const StepParams *__restrict__ params,
+                                                         const int8_t *__restrict__ marker, const long long *__restrict__ density,
+                                                         float *__restrict__ rhs) {
+    const int64_t i = (int64_t)blockIdx.x * PT + threadIdx.x;
+    if (i >= g.n) return;
+    if (marker[i] != CELL_FLUID) return;
+    rhs[i] = density_rhs_of(g, params, marker, i, density[i]);
+}
+// The sparse finish after advect_density_kernel: the particles of stage 7 marked the cells in particle_words (stage 8), and each of them
+// added only to the cells within one cell of its own.  So the dilation of those cells holds every non-zero density word and every FLUID cell:
+// the warp walks it as p2g_normalize_kernel does, writes the right-hand side of the FLUID cells and puts the words back to zero.
+__global__ void __launch_bounds__(PT) density_finish_sparse_kernel(GridDim g, int wpr, const uint32_t *__restrict__ particle_words,
+                                                                   const StepParams *__restrict__ params, const int8_t *__restrict__ marker,
+                                                                   long long *__restrict__ density, float *__restrict__ rhs) {
+    const int w = blockIdx.x * PT + threadIdx.x, lane = threadIdx.x & 31;
+    int xw = 0, y = 0, z = 0;
+    const unsigned touched = particle_dilation(g, particle_words, wpr, w, xw, y, z);
+    unsigned todo = __ballot_sync(0xffffffffu, touched != 0u);
+    while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const unsigned tw = __shfl_sync(0xffffffffu, touched, src);
+        const int sxw = __shfl_sync(0xffffffffu, xw, src), sy = __shfl_sync(0xffffffffu, y, src), sz = __shfl_sync(0xffffffffu, z, src);
+        if (!((tw >> lane) & 1u)) continue;
+        const int i = lin(g, sxw * 32 + lane, sy, sz);
+        const long long q = density[i];
+        if (q != 0) density[i] = 0;
+        if (marker[i] == CELL_FLUID) rhs[i] = density_rhs_of(g, params, marker, i, q);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ binning
@@ -1426,6 +1522,18 @@ void launch_density_rhs(cudaStream_t st, const GridDim &g, const StepParams *par
                         const int8_t *marker, long long *density, float *rhs, const ScatterSchedule &sched) {
     launch_density_scatter(st, g, params, np_upper, pos, density, sched);
     launch_density_finish(st, g, params, marker, density, rhs);
+}
+
+void launch_advect_density(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos, float4 *const row[3],
+                           float *const u[3], const uint2 *vox, int8_t *marker, long long *density, const ScatterSchedule &sched) {
+    if (np_upper == 0) return;
+    const auto kernel = scatter_groups_by_match() ? advect_density_kernel<true> : advect_density_kernel<false>;
+    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, row[0], row[1], row[2], u[0], u[1], u[2], vox, marker, density, sched);
+}
+
+void launch_density_finish_sparse(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const FluidBits &bits,
+                                  const uint32_t *particle_words, long long *density, float *rhs) {
+    BLUB_LAUNCH(density_finish_sparse_kernel, blocks_for((int64_t)bits.wpr * g.ny * g.nz, PT), PT, 0, st, g, bits.wpr, particle_words, params, marker, density, rhs);
 }
 
 void launch_binning(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *src, float4 *dst, const CellLists &l) {

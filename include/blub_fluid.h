@@ -605,7 +605,8 @@ enum {
     BLUB_TAP_CURVATURE = 12,    /* float per cell: the curvature (cells^-1) of the last stage 1 in the surface band, 0 elsewhere; zeros while
                                    surface tension is off (download only) */
     BLUB_TAP_DENSITY = 13       /* DIAGNOSTIC, not a stable interface: the step's internal scratch density accumulator as the last stage that
-                                   wrote it left it (int64 per cell: the stage-9 splat in 2^-40 particle weights, or after a stage 1 with surface
+                                   wrote it left it (int64 per cell: the stage-9 splat in 2^-40 particle weights when stage 9 ran without stage 7 in the same call
+                                   -- after a whole step it is all zero --, or after a stage 1 with surface
                                    tension the smoothed field phi within 2 cells of FLUID).  Its contents and layout may change with the step's
                                    implementation; it exists so that tests can restate stage 1 bit for bit (download only) */
 };

@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libblubcore.so")
-SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu", "load_kernels.cu", "body_kernels.cu", "viscosity_kernels.cu", "cfl_kernels.cu", "surface_tension_kernels.cu", "tank_kernels.cu", "mesh_body.cpp", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
+SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu", "load_kernels.cu", "body_kernels.cu", "viscosity_kernels.cu", "cfl_kernels.cu", "surface_tension_kernels.cu", "tank_kernels.cu", "tag_density_kernels.cu", "mesh_body.cpp", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
            "c_api.cpp"]
 # the mesh voxelizer shares its arithmetic with a host twin and a NumPy restatement, the curvature with a NumPy restatement: no FMA
 # contraction, so that they agree bit for bit

@@ -83,6 +83,10 @@ void check_viscosity(const BlubViscosity &v);
 // orthonormal with det +1 to 1e-6; tank_frame_rotates: omega or alpha is not zero.
 void check_tank_frame(const BlubTankFrame &f);
 bool tank_frame_rotates(const BlubTankFrame &f);
+// Liquids of different densities (tag_density_kernels.cu): check_tag_densities throws std::invalid_argument on more than 16 entries, a tag listed
+// twice or a density that is not finite or outside [1/2, 2]; make_tag_density_block is the device block of a checked table.
+void check_tag_densities(const BlubTagDensity *table, uint32_t count);
+TagDensityBlock make_tag_density_block(const BlubTagDensity *table, uint32_t count);
 
 class PressureSolver;
 
@@ -137,9 +141,10 @@ class PressureSolver {
 
     float *residual() const { return residual_.ptr; } // the rhs is written straight into it (hybrid_fluid.rs:836-838)
 
-    // PressureSolver::solve, pressure_solver.rs:591-729.  Enqueue-only.
+    // PressureSolver::solve, pressure_solver.rs:591-729.  Enqueue-only.  weights (liquids of different densities): the variable-density
+    // operator, solved by pcg_solve_weighted_kernel whatever the path (precond_mode 0 and one GPU only); nullptr: the constant-density one.
     void solve(cudaStream_t stream, PressureField &field, int which, const int8_t *marker, const StepParams *dparams,
-               const Quirks &quirks);
+               const Quirks &quirks, const TagDensityWork *weights = nullptr);
     SlabComm comm; // filled by HybridFluid::attach_slab_peers; world == 1 when not sharded
     // {tiles walked by the tile body, quad columns walked by the column body, cells per tile, cells per column} of the last solve (blocking)
     void read_work(cudaStream_t stream, uint32_t out[4]);
@@ -329,8 +334,19 @@ class HybridFluid {
     const BlubTankFrame *tank_frame() const { return has_tank_frame_ ? &tank_frame_ : nullptr; }
     float *curvature() const { return st_.kappa; }             // nullptr before the first surface tension above zero
     long long *density_accumulator() const { return density_.ptr; }
+    // Liquids of different densities (tag_density_kernels.cu): replaces the table, count 0 turns the feature off.  Stream-ordered; the working
+    // volumes are allocated with the first non-empty table, and only a change between off and on drops the step graphs.  Throws
+    // std::invalid_argument and changes nothing on a table check_tag_densities refuses, a table while the surface tension is above 0 or floating bodies are set, precond_mode
+    // 1, a z-slab rank or a fluid inside a step.
+    void set_tag_densities(const BlubTagDensity *table, uint32_t count);
+    const std::vector<BlubTagDensity> &tag_densities() const { return tag_densities_; }
+    bool has_tag_densities() const { return !tag_densities_.empty(); }
+    float *cell_density() const { return td_.rho; } // nullptr before the first non-empty table
 
   private:
+    std::vector<BlubTagDensity> tag_densities_;
+    TagDensityWork td_;
+    const TagDensityWork *solve_weights() const { return tag_densities_.empty() ? nullptr : &td_; }
     BlubTankFrame tank_frame_{};
     bool has_tank_frame_ = false;
     bool tank_rotating() const { return has_tank_frame_ && tank_frame_rotates(tank_frame_); }
@@ -586,6 +602,7 @@ struct SceneConfig {
     std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
     float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
     float surface_tension = 0.0f;            // optional fluid.surface_tension: kinematic, m^3/s^2
+    std::vector<BlubTagDensity> tag_densities; // optional fluid.tag_densities, checked with the setter's rules
     bool has_tank_motion = false;            // optional fluid.tank_motion (world units, Hz, rad, rad/s; directions and axis normalised)
     BlubTankMotion tank_motion{};
     uint32_t num_static_objects = 0;

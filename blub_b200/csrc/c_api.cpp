@@ -71,6 +71,7 @@ Tap tap_of(BlubFluid *f, int tap) {
     case BLUB_TAP_SOLID_VOXELS: return {const_cast<uint2 *>(h.solid_volume()), n * 8};
     case BLUB_TAP_CURVATURE: return {h.curvature(), n * 4}; // nullptr before the first surface tension above zero: zeros
     case BLUB_TAP_DENSITY: return {h.density_accumulator(), n * 8};
+    case BLUB_TAP_CELL_DENSITY: return {h.cell_density(), n * 4}; // nullptr before the first table: zeros
     default: return {nullptr, 0};
     }
 }
@@ -361,6 +362,8 @@ int blub_fluid_view(const BlubFluid *fluid, BlubFluidView *out) {
 int blub_fluid_set_quirks(BlubFluid *fluid, const BlubQuirks *q) {
     if (!fluid || !q) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     if (q->precond_mode < 0 || q->precond_mode > 1) return fail(BLUB_ERR_INVALID_ARGUMENT, "precond_mode must be 0 or 1");
+    if (q->precond_mode != 0 && fluid->impl->has_tag_densities())
+        return fail(BLUB_ERR_INVALID_ARGUMENT, "precond_mode 1 is not supported with a tag density table");
     fluid->impl->quirks.precond_mode = q->precond_mode;
     return BLUB_OK;
 }
@@ -534,6 +537,29 @@ int blub_scene_surface_tension(const char *path, float *cells3_per_s2) {
     return guarded([&] { *cells3_per_s2 = blub::scene_surface_tension_grid(blub::parse_scene_file(path)); return BLUB_OK; });
 }
 
+int blub_fluid_set_tag_densities(BlubFluid *fluid, const BlubTagDensity *table, uint32_t count) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_tag_densities(table, count); return BLUB_OK; });
+}
+
+int blub_fluid_tag_densities(const BlubFluid *fluid, BlubTagDensity *out, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    const std::vector<BlubTagDensity> &t = fluid->impl->tag_densities();
+    for (size_t k = 0; k < t.size() && k < capacity; ++k) out[k] = t[k];
+    *count = (uint32_t)t.size();
+    return BLUB_OK;
+}
+
+int blub_scene_tag_densities(const char *path, BlubTagDensity *out, uint32_t capacity, uint32_t *count) {
+    if (!path || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig c = blub::parse_scene_file(path);
+        for (size_t k = 0; k < c.tag_densities.size() && k < capacity; ++k) out[k] = c.tag_densities[k];
+        *count = (uint32_t)c.tag_densities.size();
+        return BLUB_OK;
+    });
+}
+
 int blub_cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping *config, uint64_t *dt_ns) {
     if (!max_velocity || !gravity_grid || !config || !dt_ns) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] { *dt_ns = blub::cfl_substep_ns(remaining_ns, max_velocity, gravity_grid, *config); return BLUB_OK; });
@@ -656,7 +682,7 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
     if (!fluid || !host_dst) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
-        if (tap == BLUB_TAP_CURVATURE && !t.ptr) {
+        if ((tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_CELL_DENSITY) && !t.ptr) {
             if (bytes > (size_t)fluid->impl->grid_dimension().n * 4) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
             std::memset(host_dst, 0, bytes);
             return BLUB_OK;
@@ -671,8 +697,8 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
 
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes) {
     if (!fluid || !host_src) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
-    if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY)
-        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature and density taps are download only");
+    if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY || tap == BLUB_TAP_CELL_DENSITY)
+        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature, density and cell density taps are download only");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");

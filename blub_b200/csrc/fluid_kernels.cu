@@ -40,11 +40,13 @@ __global__ void __launch_bounds__(PT) divergence_compute_kernel(GridDim g, Fluid
 }
 
 // divergence_remove.comp:19-49, on the cells within one cell of the fluid and (pw: particle words, with a solid volume) within two
-// cells of a SOLID cell that holds a particle
+// cells of a SOLID cell that holds a particle.  bx, by, bz (liquids of different densities; nullptr: constant density): the face
+// coefficients, u = u* - beta (p_i - p_j) on the faces with a FLUID side and no SOLID side.
 __global__ void __launch_bounds__(PT) divergence_remove_kernel(GridDim g, FluidBits b, const int8_t *__restrict__ marker,
                                                                const float *__restrict__ p, const uint2 *__restrict__ vox,
                                                                const uint32_t *__restrict__ pw, float *__restrict__ ux, float *__restrict__ uy,
-                                                               float *__restrict__ uz) {
+                                                               float *__restrict__ uz, const float *__restrict__ bx, const float *__restrict__ by,
+                                                               const float *__restrict__ bz) {
     const WordPos wp = word_of_thread(g, b);
     const unsigned todo = wp.inside ? (near_fluid_word(g, b, wp) | (pw != nullptr ? near_stray_word<2>(g, b, pw, wp) : 0u)) : 0u;
     warp_walk(g, todo, wp, [&](unsigned on, int x, int y, int z, int) {
@@ -53,6 +55,7 @@ __global__ void __launch_bounds__(PT) divergence_remove_kernel(GridDim g, FluidB
         const int mc = marker[i];
         const float pc = mc == CELL_FLUID ? p[i] : 0.0f;
         float *const u[3] = {ux, uy, uz};
+        const float *const beta[3] = {bx, by, bz};
         const int nb[3] = {i + 1, i + g.sy, i + g.sz};
         const bool inb[3] = {x + 1 < g.nx, y + 1 < g.ny, z + 1 < g.nz};
 #pragma unroll
@@ -69,7 +72,8 @@ __global__ void __launch_bounds__(PT) divergence_remove_kernel(GridDim g, FluidB
                     v = c == 0 ? s.x : (c == 1 ? s.y : s.z);
                 } else {
                     const float pn = mn == CELL_FLUID ? p[nb[c]] : 0.0f;
-                    v = u[c][i] - (pc - pn);
+                    if (bx) v = __fsub_rn(u[c][i], __fmul_rn(beta[c][i], __fsub_rn(pc, pn)));
+                    else v = u[c][i] - (pc - pn);
                 }
             }
             u[c][i] = v;
@@ -274,8 +278,9 @@ void launch_divergence_compute(cudaStream_t st, const GridDim &g, const FluidBit
 }
 
 void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox,
-                              const uint32_t *particle_words, float *const u[3]) {
-    BLUB_LAUNCH(divergence_remove_kernel, word_blocks(g, bits), PT, 0, st, g, bits, marker, p, vox, particle_words, u[0], u[1], u[2]);
+                              const uint32_t *particle_words, float *const u[3], const float *const *beta) {
+    BLUB_LAUNCH(divergence_remove_kernel, word_blocks(g, bits), PT, 0, st, g, bits, marker, p, vox, particle_words, u[0], u[1], u[2],
+                beta ? beta[0] : nullptr, beta ? beta[1] : nullptr, beta ? beta[2] : nullptr);
 }
 
 void launch_extrapolate(cudaStream_t st, const GridDim &g, const FluidBits &bits, float *const u[3]) {

@@ -94,8 +94,9 @@ void launch_binning(cudaStream_t st, const GridDim &g, const StepParams *params,
 void launch_divergence_compute(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, float *const u[3], const uint2 *vox, float *rhs);
 // particle_words (with a solid volume; nullptr without one): the words of the last marker pass -- the projection also visits the cells within
 // two cells, the position change those within one cell of a SOLID cell that holds a particle (the faces such a particle reads)
+// beta (nullptr: every face 1, the constant-density projection): the variable-density face coefficients of launch_tag_density, u -= beta (p_i - p_j)
 void launch_divergence_remove(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const float *p, const uint2 *vox,
-                              const uint32_t *particle_words, float *const u[3]);
+                              const uint32_t *particle_words, float *const u[3], const float *const *beta = nullptr);
 void launch_extrapolate(cudaStream_t st, const GridDim &g, const FluidBits &bits, float *const u[3]);
 void launch_clear_marker(cudaStream_t st, const GridDim &g, int8_t *marker);
 void launch_advect(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, float4 *pos, float4 *const row[3],
@@ -260,5 +261,31 @@ void launch_surface_rhs(cudaStream_t st, const GridDim &g, const FluidBits &bits
 // Stage 4, after the projection: the FLUID-AIR faces get the ghost value the solve assumed.
 void launch_surface_faces(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
                           const SurfaceTensionWork &w, float *const u[3]);
+
+// ---- liquids of different densities (tag_density_kernels.cu, DESIGN.md §8 "Liquids of different densities") ----
+constexpr int TAG_DENSITIES_MAX = BLUB_TAG_DENSITIES_MAX;
+constexpr int TAG_DENSITY_FRAC_BITS = 20; // a particle adds rint(rho * 2^20) to its cell's sum
+// What the kernels read of the table: a change does not invalidate a captured graph.
+struct TagDensityBlock {
+    uint32_t count;
+    uint32_t tag[TAG_DENSITIES_MAX];
+    uint32_t q[TAG_DENSITIES_MAX]; // rint(relative_density * 2^20)
+};
+// Working memory, allocated with the first non-empty table: 36 bytes per cell.  The face arrays follow divergence_remove's layout: beta[c][i]
+// is the face between cell i and its +c neighbour.
+struct TagDensityWork {
+    unsigned long long *sum = nullptr; // n: sum of rint(rho * 2^20) over the cell's particles; zero between stages 0
+    uint32_t *count = nullptr;         // n: the cell's particles; zero between stages 0
+    float *rho = nullptr;              // padded: rho_i of the last stage 0 on FLUID cells, 0 elsewhere
+    float *beta[3] = {nullptr, nullptr, nullptr}; // padded: the face coefficients, 0 on faces with a SOLID side or no FLUID side
+    float *diag = nullptr;             // padded: D_i, the sum of a FLUID cell's face coefficients (0 elsewhere)
+    float *inv_diag2 = nullptr;        // padded: 1 / D_i^2 (1 where D_i = 0 and on every cell that is not FLUID)
+    TagDensityBlock *block = nullptr;
+    void *volumes = nullptr;           // the one allocation of the six padded float volumes above
+};
+// Stage 0, after P2G: the cell densities of the live particles (params->num_particles when device_count, else n_host; np_upper sizes the
+// launch), then the face coefficients, the diagonal and the preconditioner from them and the marker.  Leaves sum and count zero.
+void launch_tag_density(cudaStream_t st, const GridDim &g, const StepParams *params, bool device_count, uint32_t n_host, uint32_t np_upper,
+                        const float4 *pos, const int8_t *marker, const TagDensityWork &w);
 
 } // namespace blub

@@ -12,6 +12,17 @@ constexpr int PT = 256; // threads per block for particle and cell kernels
 // per-cell and per-particle kernels.
 __device__ __forceinline__ int lin(const GridDim &g, int x, int y, int z) { return (z * g.ny + y) * g.nx + x; }
 
+// The position a transfer sees: clamped so that every face / cell a particle touches exists (a simulated particle is always
+// inside [1.001, dim - 1.001], so this only ever changes particles handed in from outside the domain).  lo = 1.0 for the
+// velocity transfer, 0.5 for the density transfer, 0.0 for binning (which only needs a valid cell).
+__device__ __forceinline__ float3 transfer_position(const GridDim &g, const float4 &p, float lo) {
+    return make_float3(fminf(fmaxf(p.x, lo), (float)g.nx - 1.0f), fminf(fmaxf(p.y, lo), (float)g.ny - 1.0f), fminf(fmaxf(p.z, lo), (float)g.nz - 1.0f));
+}
+// the cell P2G marks FLUID for a particle at transfer position p (lo = 1.0)
+__device__ __forceinline__ int cell_of_position(const GridDim &g, const float3 &p) {
+    return lin(g, min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
+}
+
 // All grid passes work on the 1-bit-per-cell FLUID mask (FluidBits, rebuilt with every finished marker volume): one thread per 32-cell
 // word of a row decides from a handful of mask words whether any of its cells has anything to do (in a dam break ~85 % of the words
 // have not), then the WARP walks the words that have, lane = cell, so that the loads and stores of a word are coalesced.  Cells that

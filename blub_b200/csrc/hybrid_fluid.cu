@@ -56,6 +56,13 @@ void free_work(SurfaceTensionWork &w) {
     cudaFree(w.sigma);
     w = SurfaceTensionWork{};
 }
+void free_work(TagDensityWork &w) {
+    cudaFree(w.sum);
+    cudaFree(w.count);
+    cudaFree(w.volumes);
+    cudaFree(w.block);
+    w = TagDensityWork{};
+}
 } // namespace
 
 HybridFluid::HybridFluid(uint32_t nx, uint32_t ny, uint32_t nz, uint32_t max_num_particles, int device, cudaStream_t stream, int slab_rank,
@@ -239,6 +246,7 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.counters);
     free_work(visc_);
     free_work(st_);
+    free_work(td_);
     cudaFree(census_dev_);
     cudaFree(max_velocity_dev_);
     cudaFree(load_probes_dev_);
@@ -534,6 +542,10 @@ void HybridFluid::run_stage(int stage, float dt) {
             launch_p2g_finish(stream_, grid_, params_dev_, u, nw, marker_.ptr, vox, bits, particle_words_);
             fluid_bits_stale_ = false;
         }
+        if (!tag_densities_.empty()) { // the marker P2G finished: the cell densities and the coefficients of stages 2 and 4
+            const NvtxScope td_scope("liquids of different densities: cell density");
+            launch_tag_density(stream_, grid_, params_dev_, device_count_mode(), num_particles_, np, pos_[cur_], marker_.ptr, td_);
+        }
         if (viscosity_.kinematic_viscosity > 0.0f) run_viscosity();
         break;
     case 1: // compute divergence -> PCG residual (:835-840)
@@ -550,7 +562,7 @@ void HybridFluid::run_stage(int stage, float dt) {
         }
         break;
     case 2: // primary pressure solver (:843-852)
-        solver_->solve(stream_, *field_velocity_, 0, marker_.ptr, params_dev_, quirks);
+        solver_->solve(stream_, *field_velocity_, 0, marker_.ptr, params_dev_, quirks, solve_weights());
         if (!capturing_) field_velocity_->enqueue_error_buffer_read(stream_, dt); // the scalars live until this field's next solve
         if (num_load_probes_ > 0) { // the marker and pressure this solve used: stage 6 rewrites the marker
             launch_solid_loads(stream_, grid_, params_dev_, (int)num_load_probes_, load_max_cells_, load_probes_dev_, marker_.ptr, field_velocity_->pressure(),
@@ -574,7 +586,8 @@ void HybridFluid::run_stage(int stage, float dt) {
         break;
     case 4: // make velocity grid divergence free (:901-904)
         refresh_fluid_bits();
-        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, vox ? particle_words_ : nullptr, u);
+        launch_divergence_remove(stream_, grid_, bits, marker_.ptr, field_velocity_->pressure(), vox, vox ? particle_words_ : nullptr, u,
+                                 tag_densities_.empty() ? nullptr : td_.beta);
         if (surface_tension_ > 0.0f) {
             const NvtxScope st_scope("surface tension: pressure jump");
             launch_surface_faces(stream_, grid_, bits, params_dev_, marker_.ptr, st_, u);
@@ -851,7 +864,7 @@ void HybridFluid::solve_only(int which, double simulation_delta_seconds) {
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     const float dt = (float)simulation_delta_seconds;
     upload_step_params(dt);
-    solver_->solve(stream_, field(which), which, marker_.ptr, params_dev_, quirks);
+    solver_->solve(stream_, field(which), which, marker_.ptr, params_dev_, quirks, which == 0 ? solve_weights() : nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1057,6 +1070,8 @@ void HybridFluid::set_surface_tension(float s) {
     if (slab_world_ > 1) throw std::invalid_argument("set_surface_tension: z-slab ranks have no surface tension");
     if (mid_step_) throw std::invalid_argument("set_surface_tension: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     if (!std::isfinite(s) || s < 0.0f) throw std::invalid_argument("set_surface_tension: the surface tension must be finite and not negative");
+    if (s > 0.0f && !tag_densities_.empty())
+        throw std::invalid_argument("set_surface_tension: not supported with a tag density table (the interfacial tension is not modelled)");
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     const bool on = s > 0.0f;
     if (on && !st_.sigma) {
@@ -1079,6 +1094,53 @@ void HybridFluid::set_surface_tension(float s) {
     if (!on && st_.kappa) BLUB_CUDA_CHECK(cudaMemsetAsync(st_.kappa, 0, (size_t)grid_.n * sizeof(float), stream_)); // the tap reads zeros when off
     if (on != (surface_tension_ > 0.0f)) destroy_graphs();
     surface_tension_ = s;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Liquids of different densities (tag_density_kernels.cu).  Not in the reference.  The kernels read the table from a device block, so a new
+// non-empty table replays the captured graphs; turning the feature on or off changes the launches and drops them.
+void HybridFluid::set_tag_densities(const BlubTagDensity *table, uint32_t count) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_tag_densities: z-slab ranks have one density");
+    if (mid_step_) throw std::invalid_argument("set_tag_densities: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    check_tag_densities(table, count);
+    if (count && surface_tension_ > 0.0f)
+        throw std::invalid_argument("set_tag_densities: not supported with surface tension (the interfacial tension is not modelled)");
+    if (count && quirks.precond_mode != 0) throw std::invalid_argument("set_tag_densities: the variable-density solve needs precond_mode 0");
+    // the bodies' coupling was measured not to hold with a table (a 0.9 box rose through a 0.8 layer instead of settling on the water below)
+    if (count && num_bodies_ > 0) throw std::invalid_argument("set_tag_densities: not supported with floating bodies");
+    if (count && !solver_->persistent_available()) throw std::invalid_argument("set_tag_densities: the variable-density solve needs cooperative launch");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (count && !td_.block) {
+        TagDensityWork w;
+        const size_t n = (size_t)grid_.n, vol = GridArray<float>::bytes_for(grid_);
+        try {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.sum, n * sizeof(unsigned long long)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.sum, 0, n * sizeof(unsigned long long), stream_));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.count, n * sizeof(uint32_t)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.count, 0, n * sizeof(uint32_t), stream_));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.volumes, 6 * vol));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.volumes, 0, 6 * vol, stream_)); // the padding stays zero
+            float *v[6];
+            for (int k = 0; k < 6; ++k) v[k] = reinterpret_cast<float *>(static_cast<char *>(w.volumes) + k * vol) + grid_.pad;
+            w.rho = v[0];
+            for (int c = 0; c < 3; ++c) w.beta[c] = v[1 + c];
+            w.diag = v[4];
+            w.inv_diag2 = v[5];
+            BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(TagDensityBlock)));
+        } catch (...) {
+            cudaStreamSynchronize(stream_); // the memsets may be in flight
+            free_work(w);
+            throw;
+        }
+        td_ = w;
+    }
+    if (td_.block) { // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
+        const TagDensityBlock b = make_tag_density_block(table, count);
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(td_.block, &b, sizeof(b), cudaMemcpyHostToDevice, stream_));
+    }
+    if (!count && td_.rho) BLUB_CUDA_CHECK(cudaMemsetAsync(td_.rho, 0, (size_t)grid_.n * sizeof(float), stream_)); // the tap reads zeros when off
+    if ((count != 0) != !tag_densities_.empty()) destroy_graphs();
+    tag_densities_.assign(table, table + count);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1185,6 +1247,7 @@ void HybridFluid::set_bodies(const BlubBody *bodies, uint32_t num_bodies) {
     if (slab_world_ > 1) throw std::invalid_argument("set_bodies: z-slab ranks have no floating bodies");
     if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     if (num_bodies > 0 && tank_rotating()) throw std::invalid_argument("set_bodies: floating bodies are not supported in a rotating tank frame");
+    if (num_bodies > 0 && !tag_densities_.empty()) throw std::invalid_argument("set_bodies: floating bodies are not supported with a tag density table");
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
     restore_bodies(make_body_set(dim, bodies, num_bodies, false));
 }
@@ -1208,6 +1271,7 @@ void HybridFluid::set_bodies_host(const BlubBody *bodies, const std::vector<Host
     if (mid_step_) throw std::invalid_argument("set_bodies: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     const uint32_t num_bodies = (uint32_t)meshes.size();
     if (num_bodies > 0 && tank_rotating()) throw std::invalid_argument("set_bodies: floating bodies are not supported in a rotating tank frame");
+    if (num_bodies > 0 && !tag_densities_.empty()) throw std::invalid_argument("set_bodies: floating bodies are not supported with a tag density table");
     if (num_bodies > (uint32_t)BODIES_MAX) throw std::invalid_argument("set_bodies: at most 16 bodies");
     if (num_bodies && !bodies) throw std::invalid_argument("set_bodies: NULL body array");
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
@@ -1376,6 +1440,7 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
         f->set_viscosity(&v);
     }
     if (cfg.surface_tension > 0.0f) f->set_surface_tension(scene_surface_tension_grid(cfg));
+    if (!cfg.tag_densities.empty()) f->set_tag_densities(cfg.tag_densities.data(), (uint32_t)cfg.tag_densities.size());
     if (!cfg.load_probes.empty()) {
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);
         f->set_load_probes(probes.data(), (uint32_t)probes.size());

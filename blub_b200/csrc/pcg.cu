@@ -574,6 +574,8 @@ struct PcgSolveArgs {
     const StepParams *params;
     int which, max_iterations, check_frequency;
     SlabComm comm;          // world == 1: single GPU
+    // the variable-density solve (pcg_solve_weighted_kernel): TagDensityWork's face coefficients, diagonal and 1 / D^2; null on the other paths
+    const float *wbeta[3], *wdiag, *winv;
 };
 
 // ---- cross-GPU all-reduce through peer-mapped mailboxes (z-slab sharding, protocol in common.cuh) ----------------
@@ -611,16 +613,6 @@ __device__ __forceinline__ void comm_allreduce(const SlabComm &c, unsigned seq, 
     mailbox_gather(c, seq, sum, mx, sh_sum, sh_max, sh_dead);
 }
 
-// NOTE: r, s, p are written by other blocks between grid barriers: no __restrict__/read-only (LDG.NC) path for them.
-__device__ __forceinline__ float4 snew4(const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
-    const float4 r4 = ld4(r + i), s4 = ld4(s + i);
-    const uchar4 c = ldcode(codes + i);
-    return make_float4(precond_diag2(r4.x, c.x) + beta * s4.x, precond_diag2(r4.y, c.y) + beta * s4.y, precond_diag2(r4.z, c.z) + beta * s4.z,
-                       precond_diag2(r4.w, c.w) + beta * s4.w);
-}
-__device__ __forceinline__ float snew1(const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
-    return precond_diag2(r[i], codes[i]) + beta * s[i];
-}
 
 // every thread of every block returns the same value
 __device__ __forceinline__ double grid_sum(cooperative_groups::grid_group &grid, float *partials, float acc, float *sh, double *shd) {
@@ -648,17 +640,89 @@ __device__ __forceinline__ uchar4 cw_code(unsigned w) {
     return make_uchar4((unsigned char)(w & 0xffu), (unsigned char)((w >> 8) & 0xffu), (unsigned char)((w >> 16) & 0xffu), (unsigned char)(w >> 24));
 }
 template <bool SKIP>
-__device__ __forceinline__ float4 snew4w(const float *r, const float *s, int i, float beta, unsigned w) {
-    if (SKIP && w == 0u) return zero4();
-    const float4 r4 = ld4(r + i), s4 = ld4(s + i);
-    const uchar4 c = cw_code(w);
-    return make_float4(precond_diag2(r4.x, c.x) + beta * s4.x, precond_diag2(r4.y, c.y) + beta * s4.y, precond_diag2(r4.z, c.z) + beta * s4.z,
-                       precond_diag2(r4.w, c.w) + beta * s4.w);
-}
-template <bool SKIP>
 __device__ __forceinline__ float4 ld4w(const float *x, int i, unsigned w) {
     if (SKIP && w == 0u) return zero4();
     return ld4(x + i);
+}
+
+// The operator a tile body applies: the constant-density stencil (UnitOp: diagonal and preconditioner from the cell codes), or the
+// variable-density one of liquids of different densities (WeightedOp: face coefficients, D and 1 / D^2 from launch_tag_density).  apply(code,
+// i, ...) is A x for the quad at i, factors(code, i) the quad's preconditioner factors (z = r * factor).  With every coefficient 1 WeightedOp
+// does, operation for operation, what stencil_quad does: the products with the coefficients are rounded on their own (exact for 1), the sums
+// keep stencil_quad's order and D x - S is one fused multiply-add, as the compiler contracts it in stencil_quad (FFMA d, x, -S).
+struct UnitOp {
+    __device__ __forceinline__ UnitOp() {}
+    __device__ __forceinline__ explicit UnitOp(const PcgSolveArgs &) {}
+    __device__ __forceinline__ float4 apply(const uchar4 &code, int, const float4 &c, float left, float right, const float4 &ym, const float4 &yp,
+                                            const float4 &zm, const float4 &zp) const {
+        return stencil_quad(code, c, left, right, ym, yp, zm, zp);
+    }
+    __device__ __forceinline__ float4 factors(const uchar4 &code, int) const {
+        return make_float4(c_inv_diag2[code.x & 7u], c_inv_diag2[code.y & 7u], c_inv_diag2[code.z & 7u], c_inv_diag2[code.w & 7u]);
+    }
+    __device__ __forceinline__ float4 factors_at(const uint8_t *__restrict__ codes, int i) const { return factors(ldcode(codes + i), i); }
+    __device__ __forceinline__ float factor_at(const uint8_t *__restrict__ codes, int i) const { return c_inv_diag2[codes[i] & 7u]; }
+};
+struct WeightedOp {
+    const PcgSolveArgs &a;
+    __device__ __forceinline__ explicit WeightedOp(const PcgSolveArgs &args) : a(args) {}
+    __device__ __forceinline__ float4 apply(const uchar4 &, int i, const float4 &c, float left, float right, const float4 &ym, const float4 &yp,
+                                            const float4 &zm, const float4 &zp) const {
+        const float *bx = a.wbeta[0], *by = a.wbeta[1], *bz = a.wbeta[2];
+        const float4 d = ld4(a.wdiag + i), xp = ld4(bx + i), ymb = ld4(by + i - a.g.sy), ypb = ld4(by + i), zmb = ld4(bz + i - a.g.sz), zpb = ld4(bz + i);
+        const float xm = bx[i - 1];
+        float4 o;
+        o.x = __fmaf_rn(d.x, c.x, -(((__fmul_rn(xm, left) + __fmul_rn(xp.x, c.y)) + (__fmul_rn(ymb.x, ym.x) + __fmul_rn(ypb.x, yp.x))) +
+                                    (__fmul_rn(zmb.x, zm.x) + __fmul_rn(zpb.x, zp.x))));
+        o.y = __fmaf_rn(d.y, c.y, -(((__fmul_rn(xp.x, c.x) + __fmul_rn(xp.y, c.z)) + (__fmul_rn(ymb.y, ym.y) + __fmul_rn(ypb.y, yp.y))) +
+                                    (__fmul_rn(zmb.y, zm.y) + __fmul_rn(zpb.y, zp.y))));
+        o.z = __fmaf_rn(d.z, c.z, -(((__fmul_rn(xp.y, c.y) + __fmul_rn(xp.z, c.w)) + (__fmul_rn(ymb.z, ym.z) + __fmul_rn(ypb.z, yp.z))) +
+                                    (__fmul_rn(zmb.z, zm.z) + __fmul_rn(zpb.z, zp.z))));
+        o.w = __fmaf_rn(d.w, c.w, -(((__fmul_rn(xp.z, c.z) + __fmul_rn(xp.w, right)) + (__fmul_rn(ymb.w, ym.w) + __fmul_rn(ypb.w, yp.w))) +
+                                    (__fmul_rn(zmb.w, zm.w) + __fmul_rn(zpb.w, zp.w))));
+        return o;
+    }
+    __device__ __forceinline__ float4 factors(const uchar4 &, int i) const { return ld4(a.winv + i); }
+    __device__ __forceinline__ float4 factors_at(const uint8_t *__restrict__, int i) const { return ld4(a.winv + i); }
+    __device__ __forceinline__ float factor_at(const uint8_t *__restrict__, int i) const { return a.winv[i]; }
+};
+// z = r * factor, and s' = z + beta s, under an operator
+__device__ __forceinline__ float4 precond4(const float4 &r, const float4 &f) { return make_float4(r.x * f.x, r.y * f.y, r.z * f.z, r.w * f.w); }
+__device__ __forceinline__ float4 snew4f(const float4 &r4, const float4 &s4, const float4 &f, float beta) {
+    return make_float4(r4.x * f.x + beta * s4.x, r4.y * f.y + beta * s4.y, r4.z * f.z + beta * s4.z, r4.w * f.w + beta * s4.w);
+}
+template <bool SKIP, class Op>
+__device__ __forceinline__ float4 snew4w_op(const Op &op, const float *r, const float *s, int i, float beta, unsigned w) {
+    if (SKIP && w == 0u) return zero4();
+    const float4 r4 = ld4(r + i), s4 = ld4(s + i);
+    return snew4f(r4, s4, op.factors(cw_code(w), i), beta);
+}
+// NOTE: r, s, p are written by other blocks between grid barriers: no __restrict__/read-only (LDG.NC) path for them.
+template <class Op> __device__ __forceinline__ float4 snew4_op(const Op &op, const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
+    const float4 r4 = ld4(r + i), s4 = ld4(s + i);
+    return snew4f(r4, s4, op.factors_at(codes, i), beta);
+}
+template <class Op> __device__ __forceinline__ float snew1_op(const Op &op, const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
+    return r[i] * op.factor_at(codes, i) + beta * s[i];
+}
+// The same for WeightedOp, with the contraction of s' = r f + beta s written out: the one nvcc picks for UnitOp in the tile kernel of
+// solver path 6 (read from its SASS), so that with every coefficient 1 the weighted solve is path 6 bit for bit.  fma(beta, s, r f) for
+// the y-quads and for the .y, .z and .w cells of the own column's quads; fma(r, f, beta s) for their .x cells and for the single cells left
+// and right of a row segment.
+__device__ __forceinline__ float snew_rf(float r, float f, float beta, float s) { return __fmaf_rn(beta, s, __fmul_rn(r, f)); }
+__device__ __forceinline__ float snew_bs(float r, float f, float beta, float s) { return __fmaf_rn(r, f, __fmul_rn(beta, s)); }
+template <bool SKIP>
+__device__ __forceinline__ float4 snew4w_op(const WeightedOp &op, const float *r, const float *s, int i, float beta, unsigned w) {
+    if (SKIP && w == 0u) return zero4();
+    const float4 r4 = ld4(r + i), s4 = ld4(s + i), f = op.factors(cw_code(w), i);
+    return make_float4(snew_bs(r4.x, f.x, beta, s4.x), snew_rf(r4.y, f.y, beta, s4.y), snew_rf(r4.z, f.z, beta, s4.z), snew_rf(r4.w, f.w, beta, s4.w));
+}
+__device__ __forceinline__ float4 snew4_op(const WeightedOp &op, const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
+    const float4 r4 = ld4(r + i), s4 = ld4(s + i), f = op.factors_at(codes, i);
+    return make_float4(snew_rf(r4.x, f.x, beta, s4.x), snew_rf(r4.y, f.y, beta, s4.y), snew_rf(r4.z, f.z, beta, s4.z), snew_rf(r4.w, f.w, beta, s4.w));
+}
+__device__ __forceinline__ float snew1_op(const WeightedOp &op, const float *r, const float *s, const uint8_t *__restrict__ codes, int i, float beta) {
+    return snew_bs(r[i], op.factor_at(codes, i), beta, s[i]);
 }
 
 // What the tile bodies need besides their operands.
@@ -690,9 +754,9 @@ __device__ __forceinline__ bool warp_has_no_fluid(const unsigned (&w)[PCG_TZ + 2
 
 // r <- b - A p, partial z.r  (pressure_init.comp:45-83).  ps (column solver, see p_slot): the thread's slot that keeps its own p quads
 // on chip for the rest of the solve, filled here with the quads of planes 0 .. PCG_TZ - 1.
-template <bool SKIP>
+template <bool SKIP, class Op = UnitOp>
 __device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *p, float *r, float &acc,
-                                          float4 *ps = nullptr) {
+                                          float4 *ps = nullptr, const Op &op = Op()) {
     const GridDim &g = e.g;
     int i = c.i;
     float4 pm = zero4(), p0 = zero4(), pp = zero4();
@@ -708,7 +772,7 @@ __device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, co
             const uchar4 code = cw_code(w[k + 1]);
             const float4 ym = ld4(p + i - g.sy), yp = ld4(p + i + g.sy);
             float4 r4 = ld4(r + i);
-            const float4 Ap = stencil_quad(code, p0, left, right, ym, yp, pm, pp);
+            const float4 Ap = op.apply(code, i, p0, left, right, ym, yp, pm, pp);
             r4.x -= code.x ? Ap.x : 0.0f;
             r4.y -= code.y ? Ap.y : 0.0f;
             r4.z -= code.z ? Ap.z : 0.0f;
@@ -718,8 +782,8 @@ __device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, co
                 if (k == 0 && c.tz == e.tz_first && e.peer_r_lo) st4(e.peer_r_lo + i + e.push, r4);
                 if (k == PCG_TZ - 1 && c.tz == e.tz_last && e.peer_r_hi) st4(e.peer_r_hi + i - e.push, r4);
             }
-            acc += (precond_diag2(r4.x, code.x) * r4.x + precond_diag2(r4.y, code.y) * r4.y) +
-                   (precond_diag2(r4.z, code.z) * r4.z + precond_diag2(r4.w, code.w) * r4.w);
+            const float4 z = precond4(r4, op.factors(code, i));
+            acc += (z.x * r4.x + z.y * r4.y) + (z.z * r4.z + z.w * r4.w);
         }
         pm = p0;
         p0 = pp;
@@ -727,16 +791,16 @@ __device__ __forceinline__ void init_tile(const TileEnv &e, const TileCtx &c, co
 }
 
 // phase A: s' = z + beta s (pressure_update_search.comp) fused with s'.A s' (pressure_apply_coeff.comp)
-template <bool SKIP>
+template <bool SKIP, class Op = UnitOp>
 __device__ __forceinline__ void search_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *r, const float *s_in,
-                                            float *s_out, float beta, float &acc) {
+                                            float *s_out, float beta, float &acc, const Op &op = Op()) {
     const GridDim &g = e.g;
     const uint8_t *codes = e.codes;
     int i = c.i;
     float4 cm = zero4(), c0 = zero4(), cp = zero4();
     if (c.valid) {
-        cm = snew4w<SKIP>(r, s_in, i - g.sz, beta, w[0]);
-        c0 = snew4w<SKIP>(r, s_in, i, beta, w[1]);
+        cm = snew4w_op<SKIP>(op, r, s_in, i - g.sz, beta, w[0]);
+        c0 = snew4w_op<SKIP>(op, r, s_in, i, beta, w[1]);
         // ghost plane below an owned boundary tile: keep the recomputed s' so that phase B and the next
         // iteration find it locally (bit-identical to what the neighbour computes for its own plane)
         if (e.sharded && c.tz == e.tz_first && (!SKIP || w[0] != 0u)) st4(s_out + i - g.sz, cm);
@@ -744,17 +808,17 @@ __device__ __forceinline__ void search_tile(const TileEnv &e, const TileCtx &c, 
 #pragma unroll
     for (int k = 0; k < PCG_TZ; ++k, i += g.sz) {
         float left = __shfl_up_sync(0xffffffffu, c0.w, 1), right = __shfl_down_sync(0xffffffffu, c0.x, 1);
-        if (c.valid) cp = snew4w<SKIP>(r, s_in, i + g.sz, beta, w[k + 2]);
+        if (c.valid) cp = snew4w_op<SKIP>(op, r, s_in, i + g.sz, beta, w[k + 2]);
         const bool act = c.valid && (!SKIP || w[k + 1] != 0u);
         float4 ym = zero4(), yp = zero4();
         if (act) { // operand loads only: short enough to be predicated, so that the planes' loads can overlap
-            ym = snew4(r, s_in, codes, i - g.sy, beta);
-            yp = snew4(r, s_in, codes, i + g.sy, beta);
+            ym = snew4_op(op, r, s_in, codes, i - g.sy, beta);
+            yp = snew4_op(op, r, s_in, codes, i + g.sy, beta);
         }
         if (act) {
-            if (c.first) left = snew1(r, s_in, codes, i - 1, beta);
-            if (c.last) right = snew1(r, s_in, codes, i + 4, beta);
-            const float4 As = stencil_quad(cw_code(w[k + 1]), c0, left, right, ym, yp, cm, cp);
+            if (c.first) left = snew1_op(op, r, s_in, codes, i - 1, beta);
+            if (c.last) right = snew1_op(op, r, s_in, codes, i + 4, beta);
+            const float4 As = op.apply(cw_code(w[k + 1]), i, c0, left, right, ym, yp, cm, cp);
             acc += (c0.x * As.x + c0.y * As.y) + (c0.z * As.z + c0.w * As.w);
             st4(s_out + i, c0);
         }
@@ -766,9 +830,9 @@ __device__ __forceinline__ void search_tile(const TileEnv &e, const TileCtx &c, 
 
 // phase B: p += alpha s', r -= alpha A s' (pressure_update_pressure_and_residual.comp), partial z.r and max|r|.  With a p slot (ps) the
 // thread's p quads are read and updated there instead of in memory.
-template <bool SKIP>
+template <bool SKIP, class Op = UnitOp>
 __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], const float *s, float *p, float *r,
-                                            float alpha, float &acc, float &err, float4 *ps = nullptr) {
+                                            float alpha, float &acc, float &err, float4 *ps = nullptr, const Op &op = Op()) {
     const GridDim &g = e.g;
     int i = c.i;
     float4 sm = zero4(), s0 = zero4(), sp = zero4();
@@ -789,7 +853,7 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
             if (c.first) left = s[i - 1];
             if (c.last) right = s[i + 4];
             const uchar4 code = cw_code(w[k + 1]);
-            const float4 As = stencil_quad(code, s0, left, right, ym, yp, sm, sp);
+            const float4 As = op.apply(code, i, s0, left, right, ym, yp, sm, sp);
             p4.x += alpha * s0.x; p4.y += alpha * s0.y; p4.z += alpha * s0.z; p4.w += alpha * s0.w;
             r4.x -= alpha * (code.x ? As.x : 0.0f);
             r4.y -= alpha * (code.y ? As.y : 0.0f);
@@ -802,8 +866,8 @@ __device__ __forceinline__ void update_tile(const TileEnv &e, const TileCtx &c, 
                 if (k == 0 && c.tz == e.tz_first && e.peer_r_lo) st4(e.peer_r_lo + i + e.push, r4);
                 if (k == PCG_TZ - 1 && c.tz == e.tz_last && e.peer_r_hi) st4(e.peer_r_hi + i - e.push, r4);
             }
-            acc += (precond_diag2(r4.x, code.x) * r4.x + precond_diag2(r4.y, code.y) * r4.y) +
-                   (precond_diag2(r4.z, code.z) * r4.z + precond_diag2(r4.w, code.w) * r4.w);
+            const float4 z = precond4(r4, op.factors(code, i));
+            acc += (z.x * r4.x + z.y * r4.y) + (z.z * r4.z + z.w * r4.w);
             err = fmaxf(fmaxf(err, fmaxf(fabsf(r4.x), fabsf(r4.y))), fmaxf(fabsf(r4.z), fabsf(r4.w)));
         }
         sm = s0;
@@ -976,27 +1040,31 @@ struct SyncReduce {
 // Phases of the register-marching kernels (tile and column solver): Walk::passes(fill, body) calls body(c, w, sparse, ps) for every pass
 // of the thread -- a tile or a column with its code words w; sparse: std::true_type for the sparse body; ps: the pass's p slot or null --
 // and fill is set in the first phase of a solve.
-template <class Walk>
+// Op: the operator of the tile bodies (UnitOp, or WeightedOp for the variable-density solve).
+template <class Walk, class Op = UnitOp>
 struct MarchWalker : Walk {
     __device__ __forceinline__ void init(float &acc) const {
         const TileEnv e = make_tile_env(this->a);
+        const Op op(this->a);
         this->passes(true, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *ps) {
-            init_tile<decltype(sparse)::value>(e, c, w, this->a.p, this->a.r, acc, ps);
+            init_tile<decltype(sparse)::value>(e, c, w, this->a.p, this->a.r, acc, ps, op);
         });
     }
     __device__ __forceinline__ void search(int it, float beta, float &acc) const {
         const float *s_in = (it & 1) ? this->a.s1 : this->a.s0;
         float *s_out = (it & 1) ? this->a.s0 : this->a.s1;
         const TileEnv e = make_tile_env(this->a);
+        const Op op(this->a);
         this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *) {
-            search_tile<decltype(sparse)::value>(e, c, w, this->a.r, s_in, s_out, beta, acc);
+            search_tile<decltype(sparse)::value>(e, c, w, this->a.r, s_in, s_out, beta, acc, op);
         });
     }
     __device__ __forceinline__ void update(int it, float alpha, float &acc, float &err) const {
         const float *s = (it & 1) ? this->a.s0 : this->a.s1;
         const TileEnv e = make_tile_env(this->a);
+        const Op op(this->a);
         this->passes(false, [&](const TileCtx &c, const unsigned (&w)[PCG_TZ + 2], auto sparse, float4 *ps) {
-            update_tile<decltype(sparse)::value>(e, c, w, s, this->a.p, this->a.r, alpha, acc, err, ps);
+            update_tile<decltype(sparse)::value>(e, c, w, s, this->a.p, this->a.r, alpha, acc, err, ps, op);
         });
     }
     __device__ __forceinline__ void store_p() const {
@@ -1038,6 +1106,20 @@ __global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_persistent_kernel(Pc
     __shared__ float sh_cmax[SLAB_MAX_WORLD];
     __shared__ int sh_dead;
     MarchWalker<TileWalk<SKIP>> wk{{a, *a.num_active}};
+    SyncReduce rd{{a.comm, 0u, sh_csum, sh_cmax, &sh_dead}, cooperative_groups::this_grid(), sh, &shd, &shf};
+    pcg_solve(a, wk, rd);
+}
+
+// The variable-density velocity solve of liquids of different densities: the tile kernel of solver path 6 (same tiles, sparse bodies, blocks,
+// reductions and recurrence) with the weighted operator.
+__global__ void __launch_bounds__(PCG_THREADS, 4) pcg_solve_weighted_kernel(PcgSolveArgs a) {
+    __shared__ float sh[PCG_THREADS / 32];
+    __shared__ double shd;
+    __shared__ float shf;
+    __shared__ double sh_csum[SLAB_MAX_WORLD];
+    __shared__ float sh_cmax[SLAB_MAX_WORLD];
+    __shared__ int sh_dead;
+    MarchWalker<TileWalk<true>, WeightedOp> wk{{a, *a.num_active}};
     SyncReduce rd{{a.comm, 0u, sh_csum, sh_cmax, &sh_dead}, cooperative_groups::this_grid(), sh, &shd, &shf};
     pcg_solve(a, wk, rd);
 }
@@ -1717,7 +1799,7 @@ void PressureSolver::set_path(int path) {
 }
 
 void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which, const int8_t *marker, const StepParams *dparams,
-                           const Quirks &quirks) {
+                           const Quirks &quirks, const TagDensityWork *weights) {
     const GridDim g = grid_;
     const TileMap t = make_tilemap(g);
     const dim3 grid = t.grid(), block = t.block();
@@ -1733,12 +1815,15 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
 
     if (comm.world > 1 && !(mode == 0 && persistent_blocks_ > 0 && use_persistent))
         throw std::invalid_argument("the z-slab sharded solve needs the persistent solver with precond_mode 0");
-    const bool persistent = mode == 0 && persistent_blocks_ > 0 && use_persistent;
+    // the variable-density solve runs pcg_solve_weighted_kernel whatever the solver path
+    if (weights && (mode != 0 || persistent_blocks_ == 0 || comm.world > 1))
+        throw std::invalid_argument("the variable-density solve needs cooperative launch, precond_mode 0 and one GPU");
+    const bool persistent = weights || (mode == 0 && persistent_blocks_ > 0 && use_persistent);
     // Set-up sized by the fluid: only the tiles that hold FLUID now or were active in the previous solve (p: this field's previous
     // solve) are prepared.  Kept to the single-GPU column solver, whose kernels write inside the active tiles only; everything else,
     // the first solve and any solve after a write from outside the step prepare every tile, and so does the solve after them.
     // The choice is made on the device (dense_flags_), so that a captured step graph follows writes from outside the step.
-    const bool columns = persistent && use_columns && column_blocks_ > 0 && !use_tma && !use_dense;
+    const bool columns = !weights && persistent && use_columns && column_blocks_ > 0 && !use_tma && !use_dense;
     int *const flags = columns && comm.world == 1 && !dense_setup_ ? dense_flags_ : nullptr;
 
     BLUB_LAUNCH(pcg_reset_scalars_kernel, 1, 1, 0, stream, scal, barrier_);
@@ -1765,12 +1850,19 @@ void PressureSolver::solve(cudaStream_t stream, PressureField &field, int which,
         args.col_list = col_list_; args.num_cols = num_cols; args.barrier = barrier_; args.code_slots = code_slots_;
         // z-slab ranks keep p in memory: their closing push reads it
         args.p_slots = columns && comm.world == 1 ? p_slots_ : 0;
+        for (int c = 0; c < 3; ++c) args.wbeta[c] = weights ? weights->beta[c] : nullptr;
+        args.wdiag = weights ? weights->diag : nullptr;
+        args.winv = weights ? weights->inv_diag2 : nullptr;
         void *args_only[] = {&args}, *args_and_maps[] = {&args, tma_maps_};
         void **kargs = args_only;
         const void *kernel;
         int nblocks;
         size_t smem;
-        if (columns) { // dense tiles by the tile body, everything else column by column
+        if (weights) { // as many blocks as path 6 launches: the same grouping of every sum
+            kernel = (const void *)pcg_solve_weighted_kernel;
+            nblocks = persistent_blocks_ < t.ntiles ? persistent_blocks_ : t.ntiles;
+            smem = 0;
+        } else if (columns) { // dense tiles by the tile body, everything else column by column
             BLUB_LAUNCH(pcg_column_fill_kernel, grid, block, 0, stream, g, t, st, ta, col_offset, ghost_tiles, t.ntiles - ghost_tiles, col_list_);
             kernel = (const void *)pcg_solve_columns_kernel;
             nblocks = column_blocks_;

@@ -224,6 +224,26 @@ SceneConfig parse_scene_file(const std::string &path) {
         if (!std::isfinite(cfg.surface_tension) || cfg.surface_tension < 0.0f || !std::isfinite(scene_surface_tension_grid(cfg)))
             throw std::runtime_error("scene JSON: `fluid.surface_tension` must be finite and not negative");
     }
+    // liquids of different densities (not in the reference): [{"tag": n, "relative_density": x}], checked with the setter's rules
+    if (const JsonValue *td = fluid.get("tag_densities")) {
+        if (td->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.tag_densities` is not an array");
+        for (const JsonValue &e : td->array) {
+            if (e.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.tag_densities` entry is not an object");
+            BlubTagDensity d;
+            d.tag = num_u32(need(e, "tag"), "tag_densities.tag");
+            d.relative_density = num_f32(need(e, "relative_density"), "tag_densities.relative_density");
+            cfg.tag_densities.push_back(d);
+        }
+        try {
+            check_tag_densities(cfg.tag_densities.data(), (uint32_t)cfg.tag_densities.size());
+        } catch (const std::invalid_argument &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.tag_densities`: ") + e.what());
+        }
+        if (!cfg.tag_densities.empty() && cfg.surface_tension > 0.0f)
+            throw std::runtime_error("scene JSON: `fluid.tag_densities` is not supported together with `fluid.surface_tension` above 0");
+        if (!cfg.tag_densities.empty() && fluid.get("bodies") && !fluid.get("bodies")->array.empty())
+            throw std::runtime_error("scene JSON: `fluid.tag_densities` is not supported together with `fluid.bodies`");
+    }
     // a moving tank (not in the reference): pivot and amplitudes in world units, frequencies in Hz, phases in rad, the rate in rad/s; checked
     // here against the rules of blub_tank_frame_at
     if (const JsonValue *tm = fluid.get("tank_motion")) {

@@ -31,15 +31,18 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // Version 64: a fluid with surface tension; the layout it would otherwise have (13 to 16 base sections as in version 32, then section 17 when
 // it is viscous) plus a last section 18, the setting.  The header cannot tell 13 + 17 + 18 from 14 + 18 apart: the reader walks the section
 // heads (their stored lengths) after section 13 and finds section 17 by its id.  Versions 33 to 63 are not formats.
+// Version 128: a fluid with a tag density table (liquids of different densities, never together with surface tension); the layout it would
+// otherwise have (13 to 16 base sections, then section 17 when it is viscous) plus a last section 19, the table.  Section 17 is found as in
+// version 64.  Versions 65 to 127 are not formats.
 constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32,
-                   kFormatVersionSurfaceTension = 64;
-constexpr uint32_t kNumSections = 18; // at most
+                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128;
+constexpr uint32_t kNumSections = 19; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION
+    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -81,6 +84,13 @@ struct SurfaceTensionSection {
     uint32_t reserved; // 0
 };
 static_assert(sizeof(SurfaceTensionSection) == 8, "surface tension section layout");
+// Section 19 (version 128): the tag density table in the order it was set, unused entries zero
+struct TagDensitySection {
+    uint32_t count;
+    uint32_t reserved; // 0
+    BlubTagDensity entry[16];
+};
+static_assert(sizeof(TagDensitySection) == 136 && TAG_DENSITIES_MAX == 16, "tag density section layout");
 
 struct StateHeader {
     char magic[8];
@@ -114,12 +124,16 @@ struct Section {
     uint64_t length;
 };
 
-// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32 or -64 header whose
+// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32, -64 or -128 header whose
 // num_sections names no layout).  The base sections come first: base_sections() of them, then section 17 in a version-32 file, sections 17
-// (when viscous64: a version-64 file that holds it) and 18 in a version-64 file.
+// (when viscous64: a version-64 or -128 file that holds it) and 18 in a version-64 file, 17 and 19 in a version-128 file.
+// the last section of a version whose base sections are followed by an optional section 17 and one setting section
+uint32_t last_section_id(const StateHeader &h) {
+    return h.format_version == kFormatVersionSurfaceTension ? SEC_SURFACE_TENSION : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES : 0u;
+}
 uint32_t base_sections(const StateHeader &h, bool viscous64) {
     if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
-    if (h.format_version == kFormatVersionSurfaceTension) {
+    if (last_section_id(h)) {
         const uint32_t extra = viscous64 ? 2 : 1;
         return h.num_sections >= 13 + extra && h.num_sections <= 16 + extra ? h.num_sections - extra : 0;
     }
@@ -133,18 +147,19 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], bool
                                      {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
                                      {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
-                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)}};
+                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)},
+                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}};
     std::memcpy(out, s, sizeof(s));
     const uint32_t nb = base_sections(h, viscous64);
     if (nb == 0) return 0;
     uint32_t ns = nb;
-    if (h.format_version == kFormatVersionViscosity || (h.format_version == kFormatVersionSurfaceTension && viscous64)) out[ns++] = s[16];
-    if (h.format_version == kFormatVersionSurfaceTension) out[ns++] = s[17];
+    if (h.format_version == kFormatVersionViscosity || (last_section_id(h) && viscous64)) out[ns++] = s[16];
+    if (last_section_id(h)) out[ns++] = s[last_section_id(h) - 1];
     return ns;
 }
-// whether the file has a viscosity section: a version-32 file always, a version-64 file when section 17 follows its base sections
+// whether the file has a viscosity section: a version-32 file always, a version-64 or -128 file when section 17 follows its base sections
 bool has_viscosity_section(const StateHeader &h, bool viscous64) {
-    return h.format_version == kFormatVersionViscosity || (h.format_version == kFormatVersionSurfaceTension && viscous64);
+    return h.format_version == kFormatVersionViscosity || (last_section_id(h) && viscous64);
 }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
@@ -182,8 +197,8 @@ struct File {
     }
 };
 
-// A version-64 file: whether a section 17 lies among the sections after section 13, found by walking their heads with their stored lengths
-// (at most four of them before section 18).  Leaves `f` where it was.  The lengths are checked later, section by section.
+// A version-64 or -128 file: whether a section 17 lies among the sections after section 13, found by walking their heads with their stored
+// lengths (at most four of them before the last section, 18 or 19).  Leaves `f` where it was.  The lengths are checked later, section by section.
 bool version64_viscous(File &f, const StateHeader &h) {
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const uint64_t base[13] = {np, np, np, np, 4 * n, 4 * n, 4 * n, n, 4 * n, 4 * n, 2 * sizeof(PcgScalars), 8ull * h.num_stats[0], 8ull * h.num_stats[1]};
@@ -196,7 +211,7 @@ bool version64_viscous(File &f, const StateHeader &h) {
         f.seek(at);
         f.read(&head, sizeof(head));
         if (head.id == SEC_VISCOSITY) viscous = true;
-        if (head.id == SEC_SURFACE_TENSION || head.length > size) break;
+        if (head.id == last_section_id(h) || head.length > size) break;
         at += sizeof(SectionHead) + head.length + 4;
     }
     f.seek(here);
@@ -244,9 +259,9 @@ StateHeader read_header(File &f, bool &viscous64) {
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
         h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity &&
-        h.format_version != kFormatVersionSurfaceTension)
+        h.format_version != kFormatVersionSurfaceTension && h.format_version != kFormatVersionTagDensities)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32 and 64)");
+                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64 and 128)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -260,7 +275,7 @@ StateHeader read_header(File &f, bool &viscous64) {
         throw ParseError(f.path + ": precond_mode, transfer path or graph replay flag out of range");
     const uint32_t sp = h.solver_path;
     if (sp > 6 || sp == 3 || sp == 5 || (sp == 2 && d[0] % 128)) throw ParseError(f.path + ": solver path out of range");
-    viscous64 = h.format_version == kFormatVersionSurfaceTension && version64_viscous(f, h);
+    viscous64 = last_section_id(h) && version64_viscous(f, h);
     Section sec[kNumSections];
     const uint32_t ns = expected_sections(h, sec, viscous64);
     if (h.num_sections != ns)
@@ -486,6 +501,23 @@ float surface_tension_of(const SurfaceTensionSection &s, const std::string &path
     return s.surface_tension;
 }
 
+// The table of section 19, checked with the rules of set_tag_densities; a version-128 file has a table, precond_mode 0 and no floating bodies.
+std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const StateHeader &h, bool viscous64, const std::string &path) {
+    if (h.precond_mode != 0) throw ParseError(path + ": section 19: a tag density table needs precond_mode 0");
+    if (base_sections(h, viscous64) >= 15) throw ParseError(path + ": section 19: a tag density table is not supported with floating bodies");
+    if (s.count == 0 || s.count > 16) throw ParseError(path + ": section 19 must hold 1 to 16 entries");
+    if (s.reserved != 0u) throw ParseError(path + ": section 19: reserved must be 0");
+    try {
+        check_tag_densities(s.entry, s.count);
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": section 19: " + e.what());
+    }
+    const BlubTagDensity zero{};
+    for (uint32_t k = s.count; k < 16; ++k)
+        if (std::memcmp(&s.entry[k], &zero, sizeof(zero)) != 0) throw ParseError(path + ": section 19: the unused entries must be zero");
+    return std::vector<BlubTagDensity>(s.entry, s.entry + s.count);
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
@@ -518,10 +550,14 @@ StateInfo read_state_info(const std::string &path) {
         read_section(f, sec[next++], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&v) + off, data, n); });
         viscosity_of(v, f.path);
     }
-    if (next < ns) {
+    if (next < ns && sec[next].id == SEC_SURFACE_TENSION) {
         SurfaceTensionSection s{};
         read_section(f, sec[next], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&s) + off, data, n); });
         surface_tension_of(s, f.path);
+    } else if (next < ns) {
+        TagDensitySection s{};
+        read_section(f, sec[next], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&s) + off, data, n); });
+        tag_densities_of(s, h, viscous64, f.path);
     }
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
@@ -543,8 +579,8 @@ void HybridFluid::save_state(const std::string &path) {
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
     const bool with_bodies = num_bodies_ > 0;
-    const bool viscous = viscosity_.kinematic_viscosity > 0.0f, capillary = surface_tension_ > 0.0f;
-    h.format_version = capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool viscous = viscosity_.kinematic_viscosity > 0.0f, capillary = surface_tension_ > 0.0f, densities = !tag_densities_.empty();
+    h.format_version = densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -563,7 +599,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0);
+    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0) + (densities ? 1 : 0);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -608,7 +644,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities ? sizeof(tagged) : sizeof(fl));
         }
         if (with_bodies) {
             BodySection bs{};
@@ -652,6 +688,12 @@ void HybridFluid::save_state(const std::string &path) {
         if (capillary) {
             const SurfaceTensionSection sts = {surface_tension_, 0u};
             write_host_section(f, SEC_SURFACE_TENSION, &sts, sizeof(sts));
+        }
+        if (densities) {
+            TagDensitySection tds{};
+            tds.count = (uint32_t)tag_densities_.size();
+            for (uint32_t k = 0; k < tds.count; ++k) tds.entry[k] = tag_densities_[k];
+            write_host_section(f, SEC_TAG_DENSITIES, &tds, sizeof(tds));
         }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
@@ -736,10 +778,15 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         v = viscosity_of(v, f.path);
         x.set_viscosity(&v);
     }
-    if (next < ns) { // the curvature is not state: stage 1 measures it again
+    if (next < ns && sec[next].id == SEC_SURFACE_TENSION) { // the curvature is not state: stage 1 measures it again
         SurfaceTensionSection s{};
         to_host(sec[next], &s);
         x.set_surface_tension(surface_tension_of(s, f.path));
+    } else if (next < ns) { // the coefficients are not state: stage 0 forms them again
+        TagDensitySection s{};
+        to_host(sec[next], &s);
+        const std::vector<BlubTagDensity> t = tag_densities_of(s, h, viscous64, f.path);
+        x.set_tag_densities(t.data(), (uint32_t)t.size());
     }
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;

@@ -41,16 +41,6 @@ inline int blocks_for(int64_t n, int per_block) { return (int)((n + per_block - 
 // particle kernels: at most 128 blocks per SM (small enough for a negligible tail, few enough to launch quickly), a grid-stride loop over the rest
 inline int particle_blocks(uint32_t np_upper) { return min(blocks_for(np_upper, PT), device_sm_count() * 128); }
 
-// The position a transfer sees: clamped so that every face / cell a particle touches exists (a simulated particle is always
-// inside [1.001, dim - 1.001], so this only ever changes particles handed in from outside the domain).  lo = 1.0 for the
-// velocity transfer, 0.5 for the density transfer, 0.0 for binning (which only needs a valid cell).
-__device__ __forceinline__ float3 transfer_position(const GridDim &g, const float4 &p, float lo) {
-    return make_float3(fminf(fmaxf(p.x, lo), (float)g.nx - 1.0f), fminf(fmaxf(p.y, lo), (float)g.ny - 1.0f), fminf(fmaxf(p.z, lo), (float)g.nz - 1.0f));
-}
-__device__ __forceinline__ int cell_of_position(const GridDim &g, const float3 &p) {
-    return lin(g, min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
-}
-
 // ------------------------------------------------------------------------------------------------ cell lists
 // count: cell_count[cell] += 1; the returned value is the particle's (arbitrary) slot inside the cell
 __device__ __forceinline__ void cell_count_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos, float lo,

@@ -25,6 +25,8 @@ STAGES = [
 TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, TAP_P_DEN, TAP_RESIDUAL, TAP_SOLID_VOXELS = range(12)
 # download only: the float32 curvature of the last stage 1; the int64 density accumulator (a diagnostic whose contents may change, see blub_fluid.h)
 TAP_CURVATURE, TAP_DENSITY = 12, 13
+# download only: the float32 relative cell density of the last stage 0 on FLUID cells (zeros without a tag density table)
+TAP_CELL_DENSITY = 14
 
 BLUB_OK = 0
 BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
@@ -37,6 +39,7 @@ LOAD_FORCE_FRAC_BITS = 16       # BLUB_LOAD_FORCE_FRAC_BITS: force sums are sums
 LOAD_TORQUE_FRAC_BITS = 8       # BLUB_LOAD_TORQUE_FRAC_BITS: torque sums are sums of rint(r_b * q * 2^8)
 BODIES_MAX = 16                 # BLUB_BODIES_MAX
 BODY_HISTORY_LENGTH = 1024      # BLUB_BODY_HISTORY_LENGTH: records per body in the device ring
+TAG_DENSITIES_MAX = 16          # BLUB_TAG_DENSITIES_MAX
 
 
 class BlubError(RuntimeError):
@@ -130,6 +133,12 @@ class Viscosity(C.Structure):
     """BlubViscosity: kinematic viscosity in cells^2/s, the solve's absolute tolerance (cells/s) and iteration cap."""
 
     _fields_ = [("kinematic_viscosity", C.c_float), ("error_tolerance", C.c_float), ("max_num_iterations", C.c_int32), ("reserved", C.c_uint32)]
+
+
+class TagDensity(C.Structure):
+    """BlubTagDensity: the density of a tag's particles relative to the reference density."""
+
+    _fields_ = [("tag", C.c_uint32), ("relative_density", C.c_float)]
 
 
 class TimeStepping(C.Structure):
@@ -423,6 +432,9 @@ def lib():
         "blub_fluid_set_surface_tension": (C.c_int, [vp, C.c_float]),
         "blub_fluid_surface_tension": (C.c_int, [vp, C.POINTER(C.c_float)]),
         "blub_scene_surface_tension": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
+        "blub_fluid_set_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32]),
+        "blub_fluid_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
+        "blub_scene_tag_densities": (C.c_int, [C.c_char_p, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
         "blub_fluid_max_particle_velocity": (C.c_int, [vp, f3]),
         "blub_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
         "blub_fluid_plan_substep": (C.c_int, [vp, C.c_uint64, C.POINTER(TimeStepping), C.POINTER(C.c_uint64), f3]),
@@ -598,6 +610,14 @@ def scene_surface_tension(path):
     out = C.c_float(0)
     _check(lib().blub_scene_surface_tension(os.fsencode(path), C.byref(out)))
     return float(out.value)
+
+
+def scene_tag_densities(path):
+    """The scene's fluid.tag_densities as {tag: relative density} in the scene's order ({} without the key; host only)."""
+    count = C.c_uint32(0)
+    arr = (TagDensity * TAG_DENSITIES_MAX)()
+    _check(lib().blub_scene_tag_densities(os.fsencode(path), arr, TAG_DENSITIES_MAX, C.byref(count)))
+    return {int(e.tag): float(e.relative_density) for e in arr[:count.value]}
 
 
 def scene_viscosity(path):
@@ -923,6 +943,25 @@ class HybridFluid:
         out = C.c_float(0)
         _check(self.L.blub_fluid_surface_tension(self.h, C.byref(out)))
         return float(out.value)
+
+    # -- liquids of different densities -------------------------------------------------------
+    def set_tag_densities(self, table):
+        """{tag: relative density} (or pairs in order): the particles of a tag have that density relative to the reference density, tags not
+        in the table 1.  An empty table turns the feature off.  Every step then runs the variable-density velocity solve and projection.  Raises
+        BlubError (and changes nothing) on more than 16 entries, a tag listed twice, a density that is not finite or outside [1/2, 2], floating bodies, surface
+        tension above 0, precond_mode 1, z-slab ranks and a fluid inside a step."""
+        items = list(table.items()) if isinstance(table, dict) else [tuple(e) for e in table]
+        arr = (TagDensity * max(len(items), 1))()
+        for k, (tag, rho) in enumerate(items):
+            arr[k].tag, arr[k].relative_density = int(tag), float(rho)
+        _check(self.L.blub_fluid_set_tag_densities(self.h, arr, len(items)))
+
+    def tag_densities(self):
+        """The current table as {tag: relative density} in the order it was set ({}: off)."""
+        count = C.c_uint32(0)
+        arr = (TagDensity * TAG_DENSITIES_MAX)()
+        _check(self.L.blub_fluid_tag_densities(self.h, arr, TAG_DENSITIES_MAX, C.byref(count)))
+        return {int(e.tag): float(e.relative_density) for e in arr[:count.value]}
 
     # -- moving tanks -------------------------------------------------------------------------
     def set_tank_frame(self, frame):

@@ -408,6 +408,32 @@ int blub_fluid_surface_tension(const BlubFluid *fluid, float *cells3_per_s2);
  * sets it on the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
 int blub_scene_surface_tension(const char *scene_json_path, float *cells3_per_s2);
 
+/* ---- liquids of different densities (not part of the reference surface; rules: DESIGN.md section 8 "Liquids of different densities") ----
+ * A table gives the particles of a tag a density relative to the reference density rho_ref that the velocity solve's pressure p dt / rho_ref,
+ * the bodies' relative densities, the load probes' forces, the viscosity and the surface tension are all defined against.  Tags not in the
+ * table have density 1.  Stage 0 of every step averages the particles' densities per cell (exact integer sums, independent of the particle
+ * order), and the velocity solve of stage 2 and the velocity update of stage 4 become variable-density: a face between the FLUID cells i and
+ * j carries 2 / (rho_i + rho_j), a FLUID-AIR face 1 / rho_i.  The transfer, the divergence, the density correction of stage 10 and the
+ * advection are unchanged.  The table is part of the saved state (format version 128). */
+typedef struct {
+    uint32_t tag;
+    float relative_density; /* finite, in [1/2, 2] */
+} BlubTagDensity;
+#define BLUB_TAG_DENSITIES_MAX 16
+/* Replaces the table; count 0 turns the feature off, and the fluid is then bit for bit a fluid that never had a table.  Stream-ordered;
+ * turning it on or off drops the cached step graphs, a change between two non-empty tables does not.  BLUB_ERR_INVALID_ARGUMENT, changing
+ * nothing: more than 16 entries, a tag listed twice, a density that is not finite or lies outside [1/2, 2], floating bodies (and blub_fluid_set_bodies refuses bodies while a table is
+ * set), a table while the surface tension
+ * is above 0, precond_mode 1 (blub_fluid_set_quirks refuses precond_mode 1 and blub_fluid_set_surface_tension a value above 0 while a table
+ * is set), a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_tag_densities(BlubFluid *fluid, const BlubTagDensity *table, uint32_t count);
+/* the current table in the order it was set: min(count, capacity) entries into out, their number into *count (0: off) */
+int blub_fluid_tag_densities(const BlubFluid *fluid, BlubTagDensity *out, uint32_t capacity, uint32_t *count);
+/* The scene's optional fluid.tag_densities, [{"tag": n, "relative_density": x}]: min(count, capacity) entries into out, their number into
+ * *count (0 without the key).  blub_scene_load sets it on the fluid it creates.  A value the setter would refuse (and a table together with a
+ * surface tension above 0) makes every scene call fail with BLUB_ERR_PARSE. */
+int blub_scene_tag_densities(const char *scene_json_path, BlubTagDensity *out, uint32_t capacity, uint32_t *count);
+
 /* ---- moving tanks (not part of the reference surface; rules: DESIGN.md section 8 "Moving tanks") ----------------------------------
  * The liquid is simulated in the tank's own frame: the grid, the walls, the solid volume, probes, sources and drains are fixed in it, and the
  * fluid feels f = R^T (g - A) - alpha x r - omega x (omega x r) - 2 omega x v with r = x - pivot (all lengths in grid cells).  The library keeps
@@ -604,11 +630,13 @@ enum {
     BLUB_TAP_SOLID_VOXELS = 11, /* the solid volume the step reads: the composite one with bodies, else the borrowed one (download only) */
     BLUB_TAP_CURVATURE = 12,    /* float per cell: the curvature (cells^-1) of the last stage 1 in the surface band, 0 elsewhere; zeros while
                                    surface tension is off (download only) */
-    BLUB_TAP_DENSITY = 13       /* DIAGNOSTIC, not a stable interface: the step's internal scratch density accumulator as the last stage that
+    BLUB_TAP_DENSITY = 13,      /* DIAGNOSTIC, not a stable interface: the step's internal scratch density accumulator as the last stage that
                                    wrote it left it (int64 per cell: the stage-9 splat in 2^-40 particle weights when stage 9 ran without stage 7 in the same call
                                    -- after a whole step it is all zero --, or after a stage 1 with surface
                                    tension the smoothed field phi within 2 cells of FLUID).  Its contents and layout may change with the step's
                                    implementation; it exists so that tests can restate stage 1 bit for bit (download only) */
+    BLUB_TAP_CELL_DENSITY = 14  /* float per cell: the relative density rho_i of the last stage 0 on FLUID cells, 0 elsewhere; zeros while no
+                                   tag density table is set (download only) */
 };
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);
@@ -618,7 +646,8 @@ int blub_fluid_set_particles(BlubFluid *fluid, uint32_t count, const float *pos4
                              const float *vz4);
 /* run stages [from, to) of the 14-stage list of one step (same numbering as oracle/blub_oracle.c:orc_step_stages) */
 int blub_fluid_step_stages(BlubFluid *fluid, double simulation_delta_seconds, int from, int to);
-/* PCG only: solve for the rhs currently in the residual tap with the current markers; warm start from the field */
+/* PCG only: solve for the rhs currently in the residual tap with the current markers; warm start from the field.  With a tag density table
+ * the velocity solve (which 0) is the variable-density one, with the face coefficients of the last stage 0. */
 int blub_fluid_solve_only(BlubFluid *fluid, int which, double simulation_delta_seconds);
 /* viscosity only: applies the viscosity stage to the grid velocity and marker as they are (tap uploads), nothing else;
  * BLUB_ERR_INVALID_ARGUMENT without a viscosity above zero */

@@ -87,6 +87,12 @@ bool tank_frame_rotates(const BlubTankFrame &f);
 // twice or a density that is not finite or outside [1/2, 2]; make_tag_density_block is the device block of a checked table.
 void check_tag_densities(const BlubTagDensity *table, uint32_t count);
 TagDensityBlock make_tag_density_block(const BlubTagDensity *table, uint32_t count);
+// Liquids of different viscosities (tag_density_kernels.cu): check_tag_viscosities throws std::invalid_argument on more than 16 entries, a
+// NULL table with count > 0, a tag listed twice or a viscosity that is negative or not finite; tag_viscosity_scale is nu_scale, the largest
+// of the table's values and the fluid's; make_tag_viscosity_block is the device block of a checked table.
+void check_tag_viscosities(const BlubTagViscosity *table, uint32_t count);
+float tag_viscosity_scale(const BlubTagViscosity *table, uint32_t count, float fluid_nu);
+TagViscosityBlock make_tag_viscosity_block(const BlubTagViscosity *table, uint32_t count, float fluid_nu);
 
 class PressureSolver;
 
@@ -304,15 +310,25 @@ class HybridFluid {
     BlubMeshBodyProperties body_mass_properties(uint32_t body) const;
     bool has_mesh_bodies() const { return !mesh_bodies_.empty(); }
 
-    // Viscous liquids (viscosity_kernels.cu): nullptr or a kinematic viscosity of 0 turns the stage off.  Stream-ordered; the working volumes are
+    // Viscous liquids (viscosity_kernels.cu): nullptr or a kinematic viscosity of 0 turns the stage off while there is no tag viscosity table
+    // (with one, 0 makes the tags not in it inviscid; the tolerance and the cap are kept either way).  Stream-ordered; the working volumes are
     // allocated with the first viscosity above zero, and only a change between off and on drops the step graphs.  Throws std::invalid_argument
     // and changes nothing on a value check_viscosity refuses, a z-slab rank or a fluid inside a step.
     void set_viscosity(const BlubViscosity *v);
     const BlubViscosity &viscosity() const { return viscosity_; }
     // iterations and max |r| per component of the last viscosity solve (synchronises); zeros before the first one
     void last_viscosity_solve(int32_t *iterations, float max_error[3]);
-    // test hook: the viscosity stage on the grid velocity and marker as they are
+    // test hook: the viscosity stage on the grid velocity and marker as they are (with a tag viscosity table, the cell viscosities are first
+    // formed from the particles the fluid holds)
     void viscosity_only(double simulation_delta_seconds);
+    // Liquids of different viscosities (viscosity_kernels.cu): replaces the table, count 0 clears it.  Stream-ordered; the working volumes are
+    // allocated with the first non-empty table, and only a change that turns the table or the stage on or off drops the step graphs.  Throws
+    // std::invalid_argument and changes nothing on a table check_tag_viscosities refuses, a z-slab rank or a fluid inside a step.
+    void set_tag_viscosities(const BlubTagViscosity *table, uint32_t count);
+    const std::vector<BlubTagViscosity> &tag_viscosities() const { return tag_viscosities_; }
+    float *cell_viscosity() const { return tv_.nu; } // nullptr before the first non-empty table
+    // the viscosity stage runs: the fluid's nu or a value of the table is above 0
+    bool viscosity_on() const;
 
     // CFL-limited substeps (cfl_kernels.cu): max |v_c| over the live particles per axis (one kernel, then synchronises), and the next substep
     // of `remaining_ns` by cfl_substep_ns with this fluid's gravity (max_velocity_out, may be nullptr, receives the measurement even when the
@@ -364,6 +380,9 @@ class HybridFluid {
     void free_mesh_bodies();
     BlubViscosity viscosity_ = kViscosityOff;
     ViscosityWork visc_;
+    std::vector<BlubTagViscosity> tag_viscosities_;
+    TagViscosityWork tv_;
+    void ensure_viscosity_work();
     float surface_tension_ = 0.0f;
     SurfaceTensionWork st_;
     void run_viscosity();
@@ -603,6 +622,7 @@ struct SceneConfig {
     float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
     float surface_tension = 0.0f;            // optional fluid.surface_tension: kinematic, m^3/s^2
     std::vector<BlubTagDensity> tag_densities; // optional fluid.tag_densities, checked with the setter's rules
+    std::vector<BlubTagViscosity> tag_viscosities; // optional fluid.tag_viscosities (m^2/s), checked in cells^2/s with the setter's rules
     bool has_tank_motion = false;            // optional fluid.tank_motion (world units, Hz, rad, rad/s; directions and axis normalised)
     BlubTankMotion tank_motion{};
     uint32_t num_static_objects = 0;
@@ -615,6 +635,7 @@ std::vector<BlubLoadProbe> scene_load_probes_grid(const SceneConfig &cfg);
 BlubTankMotion scene_tank_motion_grid(const SceneConfig &cfg);
 // the scene's kinematic viscosity in cells^2/s: viscosity / grid_to_world_scale^2
 float scene_viscosity_grid(const SceneConfig &cfg);
+std::vector<BlubTagViscosity> scene_tag_viscosities_grid(const SceneConfig &cfg); // fluid.tag_viscosities in cells^2/s
 // the scene's kinematic surface tension in cells^3/s^2: surface_tension / grid_to_world_scale^3
 float scene_surface_tension_grid(const SceneConfig &cfg);
 // the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a

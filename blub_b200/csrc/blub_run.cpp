@@ -346,12 +346,22 @@ int main(int argc, char **argv) {
         }
         BlubViscosity visc;
         if (blub_fluid_viscosity(fluid, &visc)) die("cannot read the viscosity");
-        if (visc.kinematic_viscosity > 0.0f) {
+        BlubTagViscosity tv[BLUB_TAG_VISCOSITIES_MAX];
+        uint32_t ntv = 0;
+        if (blub_fluid_tag_viscosities(fluid, tv, BLUB_TAG_VISCOSITIES_MAX, &ntv)) die("cannot read the tag viscosities");
+        if (visc.kinematic_viscosity > 0.0f || ntv > 0) {
             int32_t it = 0;
             float e[3] = {0, 0, 0};
             if (blub_fluid_last_viscosity_solve(fluid, &it, e)) die("cannot read the last viscosity solve");
-            std::fprintf(f, ", \"viscosity\": {\"kinematic_viscosity\": %.9g, \"last_iterations\": %d, \"last_max_error\": [%.9g, %.9g, %.9g]}",
+            std::fprintf(f, ", \"viscosity\": {\"kinematic_viscosity\": %.9g, \"last_iterations\": %d, \"last_max_error\": [%.9g, %.9g, %.9g]",
                          visc.kinematic_viscosity, it, e[0], e[1], e[2]);
+            if (ntv > 0) {
+                std::fprintf(f, ", \"tag_viscosities\": [");
+                for (uint32_t k = 0; k < ntv; ++k)
+                    std::fprintf(f, "%s{\"tag\": %u, \"kinematic_viscosity\": %.9g}", k ? ", " : "", tv[k].tag, tv[k].kinematic_viscosity);
+                std::fprintf(f, "]");
+            }
+            std::fprintf(f, "}");
         }
         float sigma = 0.0f;
         if (blub_fluid_surface_tension(fluid, &sigma)) die("cannot read the surface tension");

@@ -72,6 +72,7 @@ Tap tap_of(BlubFluid *f, int tap) {
     case BLUB_TAP_CURVATURE: return {h.curvature(), n * 4}; // nullptr before the first surface tension above zero: zeros
     case BLUB_TAP_DENSITY: return {h.density_accumulator(), n * 8};
     case BLUB_TAP_CELL_DENSITY: return {h.cell_density(), n * 4}; // nullptr before the first table: zeros
+    case BLUB_TAP_CELL_VISCOSITY: return {h.cell_viscosity(), n * 4}; // nullptr before the first table: zeros
     default: return {nullptr, 0};
     }
 }
@@ -550,6 +551,30 @@ int blub_fluid_tag_densities(const BlubFluid *fluid, BlubTagDensity *out, uint32
     return BLUB_OK;
 }
 
+int blub_fluid_set_tag_viscosities(BlubFluid *fluid, const BlubTagViscosity *table, uint32_t count) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_tag_viscosities(table, count); return BLUB_OK; });
+}
+
+int blub_fluid_tag_viscosities(const BlubFluid *fluid, BlubTagViscosity *out, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    const std::vector<BlubTagViscosity> &t = fluid->impl->tag_viscosities();
+    for (size_t k = 0; k < t.size() && k < capacity; ++k) out[k] = t[k];
+    *count = (uint32_t)t.size();
+    return BLUB_OK;
+}
+
+int blub_scene_tag_viscosities(const char *path, BlubTagViscosity *out, uint32_t capacity, uint32_t *count) {
+    if (!path || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig c = blub::parse_scene_file(path);
+        const std::vector<BlubTagViscosity> t = blub::scene_tag_viscosities_grid(c);
+        for (size_t k = 0; k < t.size() && k < capacity; ++k) out[k] = t[k];
+        *count = (uint32_t)t.size();
+        return BLUB_OK;
+    });
+}
+
 int blub_scene_tag_densities(const char *path, BlubTagDensity *out, uint32_t capacity, uint32_t *count) {
     if (!path || !count || (capacity && !out)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
@@ -682,7 +707,7 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
     if (!fluid || !host_dst) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
-        if ((tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_CELL_DENSITY) && !t.ptr) {
+        if ((tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_CELL_DENSITY || tap == BLUB_TAP_CELL_VISCOSITY) && !t.ptr) {
             if (bytes > (size_t)fluid->impl->grid_dimension().n * 4) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
             std::memset(host_dst, 0, bytes);
             return BLUB_OK;
@@ -697,8 +722,9 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
 
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes) {
     if (!fluid || !host_src) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
-    if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY || tap == BLUB_TAP_CELL_DENSITY)
-        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature, density and cell density taps are download only");
+    if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY || tap == BLUB_TAP_CELL_DENSITY ||
+        tap == BLUB_TAP_CELL_VISCOSITY)
+        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature, density, cell density and cell viscosity taps are download only");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");

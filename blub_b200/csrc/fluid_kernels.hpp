@@ -226,12 +226,45 @@ struct ViscosityWork {
     BlubViscosity *block = nullptr;              // what the kernels read of the setting: a change does not invalidate a captured graph
     ViscositySolveInfo *info = nullptr;
     int blocks = 0;                              // the solve's resident grid
+    int pair_blocks = 0;                         // the same for the per-pair solve (a tag viscosity table; partials are sized for the larger)
 };
-int viscosity_solve_blocks(); // SMs x resident blocks per SM; throws CudaError without cooperative launch
+// SMs x resident blocks per SM of the constant (pairs = false) or the per-pair solve; throws CudaError without cooperative launch
+int viscosity_solve_blocks(bool pairs = false);
+
+// ---- liquids of different viscosities (viscosity_kernels.cu, DESIGN.md §8 "Liquids of different viscosities") ----
+constexpr int TAG_VISCOSITIES_MAX = BLUB_TAG_VISCOSITIES_MAX;
+constexpr int TAG_VISCOSITY_FRAC_BITS = 32; // a particle adds rint(nu_tag / nu_scale * 2^32) to its cell's sum
+// What the kernels read of the table and of the fluid's nu: a change does not invalidate a captured graph.
+struct TagViscosityBlock {
+    uint32_t count;
+    uint32_t tag[TAG_VISCOSITIES_MAX];
+    unsigned long long q[TAG_VISCOSITIES_MAX]; // rint(nu_tag / nu_scale * 2^32), at most 2^32
+    unsigned long long q_default;              // the same for the tags not in the table (the fluid's nu)
+    float nu_scale;                            // the largest of the table's values and the fluid's nu (> 0 while the stage runs)
+    float nu_fluid;                            // the fluid's nu: a FLUID cell without a particle
+};
+// Working memory, allocated with the first non-empty table: 64 bytes per cell.  k[c][i] = (k_{+x}, k_{+y}, k_{+z}, 1 + sum of the face's
+// k_fn) of face i of component c, k_{+d} the pair coefficient k_fn with its +d neighbour face; the -d one is component d of k[c][i - e_d].
+// Written on live faces only.  k[c] = k[0] + c n: the solve addresses them from one pointer.
+struct TagViscosityWork {
+    float4 *k[3] = {};                 // n each
+    unsigned long long *sum = nullptr; // n: sum of the cell's particles' q; zero between stages 0
+    uint32_t *count = nullptr;         // n: the cell's particles; zero between stages 0
+    float *nu = nullptr;               // n: nu_i of the last stage 0 on FLUID cells, 0 elsewhere
+    TagViscosityBlock *block = nullptr;
+};
+
+// Stage 0 of a tag viscosity table, after P2G: the cell viscosities w.nu of the live particles (params->num_particles when device_count, else
+// n_host; np_upper sizes the launch) and the marker.  Leaves sum and count zero.  The scatter is the tag density one (tag_density_kernels.cu).
+void launch_tag_viscosity_cells(cudaStream_t st, const GridDim &g, const StepParams *params, bool device_count, uint32_t n_host, uint32_t np_upper,
+                                const float4 *pos, const int8_t *marker, const TagViscosityWork &w);
 // The whole stage: classify the faces and list the active words from the FLUID bits and the marker, then solve all three components in one
-// cooperative launch; k = block->kinematic_viscosity * params->dt is formed on the device.  Writes live faces of u only.
+// cooperative launch; k = block->kinematic_viscosity * params->dt is formed on the device.  Writes live faces of u only.  With `tag` (a
+// non-empty table), first the cell viscosities of the live particles (params->num_particles when device_count, else n_host; np_upper sizes
+// the launch), then the system with per-pair coefficients k_fn = nu_fn * params->dt.
 void launch_viscosity(cudaStream_t st, const GridDim &g, const StepParams *params, const FluidBits &bits, const int8_t *marker, const uint2 *vox,
-                      float *const u[3], const ViscosityWork &w);
+                      float *const u[3], const ViscosityWork &w, const TagViscosityWork *tag = nullptr, bool device_count = false,
+                      uint32_t n_host = 0, uint32_t np_upper = 0, const float4 *pos = nullptr);
 
 // ---- CFL-limited substeps (cfl_kernels.cu, DESIGN.md §8 "CFL-limited substeps") ----
 // out[c] = the bits of max |v_c| over the particles (params->num_particles when `params` is not null, else n_host; np_upper sizes the launch).

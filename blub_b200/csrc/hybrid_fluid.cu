@@ -50,6 +50,11 @@ void free_work(ViscosityWork &w) {
     cudaFree(w.info);
     w = ViscosityWork{};
 }
+void free_work(TagViscosityWork &w) {
+    cudaFree(w.k[0]); // the one allocation of every volume
+    cudaFree(w.block);
+    w = TagViscosityWork{};
+}
 void free_work(SurfaceTensionWork &w) {
     cudaFree(w.psi);
     cudaFree(w.kappa);
@@ -245,6 +250,7 @@ HybridFluid::~HybridFluid() {
     cudaFree(flow_scratch_.scalars);
     cudaFree(flow_scratch_.counters);
     free_work(visc_);
+    free_work(tv_);
     free_work(st_);
     free_work(td_);
     cudaFree(census_dev_);
@@ -546,7 +552,7 @@ void HybridFluid::run_stage(int stage, float dt) {
             const NvtxScope td_scope("liquids of different densities: cell density");
             launch_tag_density(stream_, grid_, params_dev_, device_count_mode(), num_particles_, np, pos_[cur_], marker_.ptr, td_);
         }
-        if (viscosity_.kinematic_viscosity > 0.0f) run_viscosity();
+        if (viscosity_on()) run_viscosity();
         break;
     case 1: // compute divergence -> PCG residual (:835-840)
         refresh_fluid_bits();
@@ -796,49 +802,105 @@ void check_viscosity(const BlubViscosity &v) {
     if (v.reserved != 0u) throw std::invalid_argument("viscosity: reserved must be 0");
 }
 
+bool HybridFluid::viscosity_on() const {
+    return viscosity_.kinematic_viscosity > 0.0f || tag_viscosity_scale(tag_viscosities_.data(), (uint32_t)tag_viscosities_.size(), 0.0f) > 0.0f;
+}
+
+void HybridFluid::ensure_viscosity_work() {
+    if (visc_.block) return;
+    ViscosityWork w;
+    w.blocks = viscosity_solve_blocks();
+    w.pair_blocks = viscosity_solve_blocks(true);
+    const size_t n = (size_t)grid_.n, words = (size_t)fluid_bits_.wpr * grid_.ny * grid_.nz;
+    try {
+        BLUB_CUDA_CHECK(cudaMalloc(&w.codes, n * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMemsetAsync(w.codes, 0, n * sizeof(uint32_t), stream_));
+        for (int c = 0; c < 3; ++c) {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.r[c], n * sizeof(float)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.s[c], n * sizeof(float)));
+        }
+        BLUB_CUDA_CHECK(cudaMalloc(&w.word_flags, (words + 1) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.words, words * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks((int64_t)words + 1) + 1024) * sizeof(uint32_t)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.partials, 2 * 6 * (size_t)std::max(w.blocks, w.pair_blocks) * sizeof(float)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.barrier, 256));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(BlubViscosity)));
+        BLUB_CUDA_CHECK(cudaMalloc(&w.info, sizeof(ViscositySolveInfo)));
+        BLUB_CUDA_CHECK(cudaMemsetAsync(w.info, 0, sizeof(ViscositySolveInfo), stream_));
+    } catch (...) {
+        cudaStreamSynchronize(stream_); // the memsets may be in flight
+        free_work(w);
+        throw;
+    }
+    visc_ = w;
+}
+
 void HybridFluid::set_viscosity(const BlubViscosity *v) {
     if (slab_world_ > 1) throw std::invalid_argument("set_viscosity: z-slab ranks have no viscosity");
     if (mid_step_) throw std::invalid_argument("set_viscosity: the fluid is inside a step (the last step_stages call did not end at stage 14)");
     const BlubViscosity next = v ? *v : kViscosityOff;
     check_viscosity(next);
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
-    const bool on = next.kinematic_viscosity > 0.0f;
-    if (on && !visc_.block) {
-        ViscosityWork w;
-        w.blocks = viscosity_solve_blocks();
-        const size_t n = (size_t)grid_.n, words = (size_t)fluid_bits_.wpr * grid_.ny * grid_.nz;
+    const bool was_on = viscosity_on();
+    const uint32_t count = (uint32_t)tag_viscosities_.size();
+    if (next.kinematic_viscosity > 0.0f || tag_viscosity_scale(tag_viscosities_.data(), count, 0.0f) > 0.0f) ensure_viscosity_work();
+    // stream-ordered behind the steps already enqueued (the copies stage the values before they return)
+    if (visc_.block) BLUB_CUDA_CHECK(cudaMemcpyAsync(visc_.block, &next, sizeof(next), cudaMemcpyHostToDevice, stream_));
+    if (count) { // the fluid's nu is the value of the tags not in the table, and may be nu_scale
+        const TagViscosityBlock b = make_tag_viscosity_block(tag_viscosities_.data(), count, next.kinematic_viscosity);
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(tv_.block, &b, sizeof(b), cudaMemcpyHostToDevice, stream_));
+    }
+    viscosity_ = next;
+    if (viscosity_on() != was_on) destroy_graphs();
+}
+
+// Liquids of different viscosities (viscosity_kernels.cu).  Not in the reference.  The kernels read the table from a device block, so a new
+// non-empty table replays the captured graphs; turning the table or the stage on or off changes the launches and drops them.
+void HybridFluid::set_tag_viscosities(const BlubTagViscosity *table, uint32_t count) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_tag_viscosities: z-slab ranks have no viscosity");
+    if (mid_step_) throw std::invalid_argument("set_tag_viscosities: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    check_tag_viscosities(table, count);
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const bool was_on = viscosity_on(), had_table = !tag_viscosities_.empty();
+    if (count && !tv_.block) {
+        TagViscosityWork w;
+        const size_t n = (size_t)grid_.n, bytes = n * (sizeof(unsigned long long) + sizeof(uint32_t) + 13 * sizeof(float));
         try {
-            BLUB_CUDA_CHECK(cudaMalloc(&w.codes, n * sizeof(uint32_t)));
-            BLUB_CUDA_CHECK(cudaMemsetAsync(w.codes, 0, n * sizeof(uint32_t), stream_));
-            for (int c = 0; c < 3; ++c) {
-                BLUB_CUDA_CHECK(cudaMalloc(&w.r[c], n * sizeof(float)));
-                BLUB_CUDA_CHECK(cudaMalloc(&w.s[c], n * sizeof(float)));
-            }
-            BLUB_CUDA_CHECK(cudaMalloc(&w.word_flags, (words + 1) * sizeof(uint32_t)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.words, words * sizeof(uint32_t)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks((int64_t)words + 1) + 1024) * sizeof(uint32_t)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.partials, 2 * 6 * (size_t)w.blocks * sizeof(float)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.barrier, 256));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(BlubViscosity)));
-            BLUB_CUDA_CHECK(cudaMalloc(&w.info, sizeof(ViscositySolveInfo)));
-            BLUB_CUDA_CHECK(cudaMemsetAsync(w.info, 0, sizeof(ViscositySolveInfo), stream_));
+            char *mem = nullptr;
+            BLUB_CUDA_CHECK(cudaMalloc(&mem, bytes));
+            w.k[0] = reinterpret_cast<float4 *>(mem);
+            BLUB_CUDA_CHECK(cudaMemsetAsync(mem, 0, bytes, stream_));
+            for (int c = 1; c < 3; ++c) w.k[c] = w.k[0] + c * n;
+            w.sum = reinterpret_cast<unsigned long long *>(w.k[0] + 3 * n);
+            w.count = reinterpret_cast<uint32_t *>(w.sum + n);
+            w.nu = reinterpret_cast<float *>(w.count + n);
+            BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(TagViscosityBlock)));
         } catch (...) {
-            cudaStreamSynchronize(stream_); // the memsets may be in flight
+            cudaStreamSynchronize(stream_); // the memset may be in flight
             free_work(w);
             throw;
         }
-        visc_ = w;
+        tv_ = w;
     }
-    // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
-    if (visc_.block) BLUB_CUDA_CHECK(cudaMemcpyAsync(visc_.block, &next, sizeof(next), cudaMemcpyHostToDevice, stream_));
-    if (on != (viscosity_.kinematic_viscosity > 0.0f)) destroy_graphs();
-    viscosity_ = next;
+    if (count && tag_viscosity_scale(table, count, viscosity_.kinematic_viscosity) > 0.0f) ensure_viscosity_work();
+    if (tv_.block) { // stream-ordered behind the steps already enqueued (the copies stage the values before they return)
+        const TagViscosityBlock b = make_tag_viscosity_block(table, count, viscosity_.kinematic_viscosity);
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(tv_.block, &b, sizeof(b), cudaMemcpyHostToDevice, stream_));
+        if (!count) BLUB_CUDA_CHECK(cudaMemsetAsync(tv_.nu, 0, (size_t)grid_.n * sizeof(float), stream_)); // the tap reads zeros without a table
+    }
+    // the tolerance and the cap of a setting with nu = 0, for a table that turns the stage on
+    if (visc_.block && !was_on) BLUB_CUDA_CHECK(cudaMemcpyAsync(visc_.block, &viscosity_, sizeof(viscosity_), cudaMemcpyHostToDevice, stream_));
+    tag_viscosities_.assign(table, table + count);
+    if (viscosity_on() != was_on || had_table != !tag_viscosities_.empty()) destroy_graphs();
 }
 
 void HybridFluid::run_viscosity() {
     const NvtxScope scope("apply viscosity");
     float *u[3] = {u_[0].ptr, u_[1].ptr, u_[2].ptr};
-    launch_viscosity(stream_, grid_, params_dev_, fluid_bits_, marker_.ptr, solid_volume(), u, visc_);
+    if (tag_viscosities_.empty()) launch_viscosity(stream_, grid_, params_dev_, fluid_bits_, marker_.ptr, solid_volume(), u, visc_);
+    else
+        launch_viscosity(stream_, grid_, params_dev_, fluid_bits_, marker_.ptr, solid_volume(), u, visc_, &tv_, device_count_mode(), num_particles_,
+                         device_count_mode() ? max_num_particles_ : num_particles_, pos_[cur_]);
 }
 
 void HybridFluid::last_viscosity_solve(int32_t *iterations, float max_error[3]) {
@@ -851,7 +913,7 @@ void HybridFluid::last_viscosity_solve(int32_t *iterations, float max_error[3]) 
 }
 
 void HybridFluid::viscosity_only(double simulation_delta_seconds) {
-    if (!(viscosity_.kinematic_viscosity > 0.0f)) throw std::invalid_argument("viscosity_only: the fluid has no viscosity");
+    if (!viscosity_on()) throw std::invalid_argument("viscosity_only: the fluid has no viscosity");
     BLUB_CUDA_CHECK(cudaSetDevice(device_));
     const float dt = (float)simulation_delta_seconds;
     if (!(dt > 0.0f)) throw std::invalid_argument("simulation delta must be positive");
@@ -1438,6 +1500,10 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
         BlubViscosity v = kViscosityOff;
         v.kinematic_viscosity = scene_viscosity_grid(cfg);
         f->set_viscosity(&v);
+    }
+    if (!cfg.tag_viscosities.empty()) {
+        const std::vector<BlubTagViscosity> t = scene_tag_viscosities_grid(cfg);
+        f->set_tag_viscosities(t.data(), (uint32_t)t.size());
     }
     if (cfg.surface_tension > 0.0f) f->set_surface_tension(scene_surface_tension_grid(cfg));
     if (!cfg.tag_densities.empty()) f->set_tag_densities(cfg.tag_densities.data(), (uint32_t)cfg.tag_densities.size());

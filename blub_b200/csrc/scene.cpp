@@ -146,6 +146,11 @@ uint32_t tag_of(const JsonValue &obj, const char *what) {
 } // namespace
 
 float scene_viscosity_grid(const SceneConfig &cfg) { return cfg.viscosity / (cfg.grid_to_world_scale * cfg.grid_to_world_scale); }
+std::vector<BlubTagViscosity> scene_tag_viscosities_grid(const SceneConfig &cfg) {
+    std::vector<BlubTagViscosity> t = cfg.tag_viscosities;
+    for (BlubTagViscosity &e : t) e.kinematic_viscosity /= cfg.grid_to_world_scale * cfg.grid_to_world_scale;
+    return t;
+}
 float scene_surface_tension_grid(const SceneConfig &cfg) {
     return cfg.surface_tension / (cfg.grid_to_world_scale * cfg.grid_to_world_scale * cfg.grid_to_world_scale);
 }
@@ -243,6 +248,23 @@ SceneConfig parse_scene_file(const std::string &path) {
             throw std::runtime_error("scene JSON: `fluid.tag_densities` is not supported together with `fluid.surface_tension` above 0");
         if (!cfg.tag_densities.empty() && fluid.get("bodies") && !fluid.get("bodies")->array.empty())
             throw std::runtime_error("scene JSON: `fluid.tag_densities` is not supported together with `fluid.bodies`");
+    }
+    // liquids of different viscosities (not in the reference): [{"tag": n, "viscosity": m^2/s}], checked in cells^2/s with the setter's rules
+    if (const JsonValue *tv = fluid.get("tag_viscosities")) {
+        if (tv->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.tag_viscosities` is not an array");
+        for (const JsonValue &e : tv->array) {
+            if (e.kind != JsonValue::Object) throw std::runtime_error("scene JSON: a `fluid.tag_viscosities` entry is not an object");
+            BlubTagViscosity v;
+            v.tag = num_u32(need(e, "tag"), "tag_viscosities.tag");
+            v.kinematic_viscosity = num_f32(need(e, "viscosity"), "tag_viscosities.viscosity");
+            cfg.tag_viscosities.push_back(v);
+        }
+        try {
+            const std::vector<BlubTagViscosity> grid = scene_tag_viscosities_grid(cfg);
+            check_tag_viscosities(grid.data(), (uint32_t)grid.size());
+        } catch (const std::invalid_argument &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.tag_viscosities`: ") + e.what());
+        }
     }
     // a moving tank (not in the reference): pivot and amplitudes in world units, frequencies in Hz, phases in rad, the rate in rad/s; checked
     // here against the rules of blub_tank_frame_at

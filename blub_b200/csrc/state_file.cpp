@@ -34,15 +34,19 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // Version 128: a fluid with a tag density table (liquids of different densities, never together with surface tension); the layout it would
 // otherwise have (13 to 16 base sections, then section 17 when it is viscous) plus a last section 19, the table.  Section 17 is found as in
 // version 64.  Versions 65 to 127 are not formats.
+// Version 256: a fluid with a tag viscosity table (liquids of different viscosities); the 13 to 16 base sections as in version 32, then
+// section 17 always (its kinematic_viscosity may be 0: the tags not in the table are inviscid), section 18 when the surface tension is
+// above 0, section 19 when a tag density table is set, and a last section 20, the table.  The reader finds 17, 18 and 19 by walking the
+// section heads as for versions 64 and 128.  Versions 129 to 255 are not formats.
 constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32,
-                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128;
-constexpr uint32_t kNumSections = 19; // at most
+                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128, kFormatVersionTagViscosities = 256;
+constexpr uint32_t kNumSections = 20; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES
+    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES, SEC_TAG_VISCOSITIES
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -91,6 +95,13 @@ struct TagDensitySection {
     BlubTagDensity entry[16];
 };
 static_assert(sizeof(TagDensitySection) == 136 && TAG_DENSITIES_MAX == 16, "tag density section layout");
+// Section 20 (version 256): the tag viscosity table in the order it was set, unused entries zero
+struct TagViscositySection {
+    uint32_t count;
+    uint32_t reserved; // 0
+    BlubTagViscosity entry[16];
+};
+static_assert(sizeof(TagViscositySection) == 136 && TAG_VISCOSITIES_MAX == 16, "tag viscosity section layout");
 
 struct StateHeader {
     char magic[8];
@@ -124,22 +135,24 @@ struct Section {
     uint64_t length;
 };
 
-// The sections of a file in their order, with the lengths its header implies; returns their number (0: a version-32, -64 or -128 header whose
-// num_sections names no layout).  The base sections come first: base_sections() of them, then section 17 in a version-32 file, sections 17
-// (when viscous64: a version-64 or -128 file that holds it) and 18 in a version-64 file, 17 and 19 in a version-128 file.
-// the last section of a version whose base sections are followed by an optional section 17 and one setting section
-uint32_t last_section_id(const StateHeader &h) {
-    return h.format_version == kFormatVersionSurfaceTension ? SEC_SURFACE_TENSION : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES : 0u;
+// The setting sections (17 to 20) that follow the base sections, as a mask of bits 1 << id.  Version 32: 17.  Versions 64, 128 and 256: what
+// the section heads say (settings_in_file), with the sections every file of the version holds: 18 (64), 19 (128), 17 and 20 (256).
+constexpr uint32_t bit(uint32_t id) { return 1u << id; }
+// the versions whose base sections are followed by setting sections the header does not tell apart
+bool walks_settings(const StateHeader &h) {
+    return h.format_version == kFormatVersionSurfaceTension || h.format_version == kFormatVersionTagDensities || h.format_version == kFormatVersionTagViscosities;
 }
-uint32_t base_sections(const StateHeader &h, bool viscous64) {
+uint32_t base_sections(const StateHeader &h, uint32_t settings) {
     if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
-    if (last_section_id(h)) {
-        const uint32_t extra = viscous64 ? 2 : 1;
+    if (walks_settings(h)) {
+        const uint32_t extra = (uint32_t)__builtin_popcount(settings);
         return h.num_sections >= 13 + extra && h.num_sections <= 16 + extra ? h.num_sections - extra : 0;
     }
     return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
 }
-uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], bool viscous64) {
+// The sections of a file in their order, with the lengths its header implies; returns their number (0: a header whose num_sections names no
+// layout).  The base sections come first, base_sections() of them, then the setting sections of `settings` in the order 17, 18, 19, 20.
+uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], uint32_t settings) {
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const Section s[kNumSections] = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
                                      {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
@@ -148,19 +161,17 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], bool
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
                                      {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
                                      {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)},
-                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}};
+                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}, {SEC_TAG_VISCOSITIES, sizeof(TagViscositySection)}};
     std::memcpy(out, s, sizeof(s));
-    const uint32_t nb = base_sections(h, viscous64);
+    const uint32_t nb = base_sections(h, settings);
     if (nb == 0) return 0;
     uint32_t ns = nb;
-    if (h.format_version == kFormatVersionViscosity || (last_section_id(h) && viscous64)) out[ns++] = s[16];
-    if (last_section_id(h)) out[ns++] = s[last_section_id(h) - 1];
+    for (uint32_t id = SEC_VISCOSITY; id <= SEC_TAG_VISCOSITIES; ++id)
+        if (settings & bit(id)) out[ns++] = s[id - 1];
     return ns;
 }
-// whether the file has a viscosity section: a version-32 file always, a version-64 or -128 file when section 17 follows its base sections
-bool has_viscosity_section(const StateHeader &h, bool viscous64) {
-    return h.format_version == kFormatVersionViscosity || (last_section_id(h) && viscous64);
-}
+// whether the file has a viscosity section
+bool has_viscosity_section(uint32_t settings) { return (settings & bit(SEC_VISCOSITY)) != 0; }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
 
@@ -197,25 +208,32 @@ struct File {
     }
 };
 
-// A version-64 or -128 file: whether a section 17 lies among the sections after section 13, found by walking their heads with their stored
-// lengths (at most four of them before the last section, 18 or 19).  Leaves `f` where it was.  The lengths are checked later, section by section.
-bool version64_viscous(File &f, const StateHeader &h) {
+// The setting sections of a file (see base_sections).  Versions 64, 128 and 256: the ids 17 to 19 found among the sections after section 13 by
+// walking their heads with their stored lengths (at most six of them before the last section, 18, 19 or 20), plus the sections the version
+// always holds.  Leaves `f` where it was.  The lengths are checked later, section by section.
+uint32_t settings_in_file(File &f, const StateHeader &h) {
+    if (h.format_version == kFormatVersionViscosity) return bit(SEC_VISCOSITY);
+    if (!walks_settings(h)) return 0u;
+    const uint32_t last = h.format_version == kFormatVersionSurfaceTension ? SEC_SURFACE_TENSION
+                          : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES : SEC_TAG_VISCOSITIES;
+    // what the walk may find: 17 in versions 64 and 128, 18 and 19 in version 256 (17 is always there)
+    const uint32_t optional = last == SEC_TAG_VISCOSITIES ? bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) : bit(SEC_VISCOSITY);
+    uint32_t settings = bit(last) | (last == SEC_TAG_VISCOSITIES ? bit(SEC_VISCOSITY) : 0u);
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const uint64_t base[13] = {np, np, np, np, 4 * n, 4 * n, 4 * n, n, 4 * n, 4 * n, 2 * sizeof(PcgScalars), 8ull * h.num_stats[0], 8ull * h.num_stats[1]};
     const uint64_t here = f.tell(), size = f.size();
     uint64_t at = here;
     for (uint64_t len : base) at += sizeof(SectionHead) + len + 4;
-    bool viscous = false;
-    for (int k = 0; k < 5 && at + sizeof(SectionHead) <= size; ++k) {
+    for (int k = 0; k < 7 && at + sizeof(SectionHead) <= size; ++k) {
         SectionHead head;
         f.seek(at);
         f.read(&head, sizeof(head));
-        if (head.id == SEC_VISCOSITY) viscous = true;
-        if (head.id == last_section_id(h) || head.length > size) break;
+        if (head.id >= SEC_VISCOSITY && head.id < 32 && (optional & bit(head.id))) settings |= bit(head.id);
+        if (head.id == last || head.length > size) break;
         at += sizeof(SectionHead) + head.length + 4;
     }
     f.seek(here);
-    return viscous;
+    return settings;
 }
 
 // Staging memory of the array sections: pinned halves with an event each when the arrays come from / go to the device, plain host memory
@@ -249,9 +267,9 @@ struct Staging {
     }
 };
 
-// Header checks: everything a reader needs to trust before it allocates anything.  Leaves `f` at the first section.  viscous64: whether a
-// version-64 file holds section 17 (false for every other version).
-StateHeader read_header(File &f, bool &viscous64) {
+// Header checks: everything a reader needs to trust before it allocates anything.  Leaves `f` at the first section.  settings: the setting
+// sections the file holds (settings_in_file).
+StateHeader read_header(File &f, uint32_t &settings) {
     StateHeader h;
     const uint64_t size = f.size();
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
@@ -259,9 +277,10 @@ StateHeader read_header(File &f, bool &viscous64) {
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
         h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity &&
-        h.format_version != kFormatVersionSurfaceTension && h.format_version != kFormatVersionTagDensities)
+        h.format_version != kFormatVersionSurfaceTension && h.format_version != kFormatVersionTagDensities &&
+        h.format_version != kFormatVersionTagViscosities)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64 and 128)");
+                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64, 128 and 256)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -275,16 +294,17 @@ StateHeader read_header(File &f, bool &viscous64) {
         throw ParseError(f.path + ": precond_mode, transfer path or graph replay flag out of range");
     const uint32_t sp = h.solver_path;
     if (sp > 6 || sp == 3 || sp == 5 || (sp == 2 && d[0] % 128)) throw ParseError(f.path + ": solver path out of range");
-    viscous64 = last_section_id(h) && version64_viscous(f, h);
+    settings = settings_in_file(f, h);
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, viscous64);
+    const uint32_t ns = expected_sections(h, sec, settings);
+    const uint32_t extra = (uint32_t)__builtin_popcount(settings);
     if (h.num_sections != ns)
         throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(h.format_version) + " has " +
-                         (ns ? std::to_string(ns) : viscous64 ? std::string("15 to 18") : std::string("14 to 17")));
+                         (ns ? std::to_string(ns) : std::to_string(13 + extra) + " to " + std::to_string(16 + extra)));
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
     // version 16: section 16 holds at least its count and one mesh body record
-    if (base_sections(h, viscous64) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
+    if (base_sections(h, settings) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
         throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
 }
@@ -292,10 +312,10 @@ StateHeader read_header(File &f, bool &viscous64) {
 // Reads one section whose id and length must be `s`, in chunks of at most one staging half; sink(slot, data, bytes, offset) receives
 // every chunk (it must be done with the half `slot` before that half's event is waited on again), then the CRC is checked.
 // the length of section 16 when the file has one: what the file holds beyond section 15, its head and its CRC
-uint64_t mesh_section_length(File &f, const StateHeader &h, bool viscous64) {
-    if (base_sections(h, viscous64) != 16) return 0;
+uint64_t mesh_section_length(File &f, const StateHeader &h, uint32_t settings) {
+    if (base_sections(h, settings) != 16) return 0;
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, viscous64);
+    const uint32_t ns = expected_sections(h, sec, settings);
     uint64_t total = sizeof(StateHeader);
     for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4; // section 16 counted empty
     return f.size() - total;
@@ -483,14 +503,16 @@ std::vector<BlubBody> mesh_body_set_of(const BodySection &bs, const std::vector<
     return set;
 }
 
-// The setting of section 17, checked with the rules of set_viscosity; a version-32 file has viscosity.
-BlubViscosity viscosity_of(const BlubViscosity &v, const std::string &path) {
+// The setting of section 17, checked with the rules of set_viscosity; below version 256 it holds a viscosity above 0 (a version-256 file's
+// may hold 0: the tags not in its table are inviscid).
+BlubViscosity viscosity_of(const BlubViscosity &v, const StateHeader &h, const std::string &path) {
     try {
         check_viscosity(v);
     } catch (const std::invalid_argument &e) {
         throw ParseError(path + ": section 17: " + e.what());
     }
-    if (!(v.kinematic_viscosity > 0.0f)) throw ParseError(path + ": section 17: a version-32 or -64 file's section 17 holds a viscosity above 0");
+    if (h.format_version != kFormatVersionTagViscosities && !(v.kinematic_viscosity > 0.0f))
+        throw ParseError(path + ": section 17: a version-32, -64 or -128 file's section 17 holds a viscosity above 0");
     return v;
 }
 
@@ -502,9 +524,10 @@ float surface_tension_of(const SurfaceTensionSection &s, const std::string &path
 }
 
 // The table of section 19, checked with the rules of set_tag_densities; a version-128 file has a table, precond_mode 0 and no floating bodies.
-std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const StateHeader &h, bool viscous64, const std::string &path) {
+std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const StateHeader &h, uint32_t settings, const std::string &path) {
     if (h.precond_mode != 0) throw ParseError(path + ": section 19: a tag density table needs precond_mode 0");
-    if (base_sections(h, viscous64) >= 15) throw ParseError(path + ": section 19: a tag density table is not supported with floating bodies");
+    if (settings & bit(SEC_SURFACE_TENSION)) throw ParseError(path + ": section 19: a tag density table is not supported with surface tension");
+    if (base_sections(h, settings) >= 15) throw ParseError(path + ": section 19: a tag density table is not supported with floating bodies");
     if (s.count == 0 || s.count > 16) throw ParseError(path + ": section 19 must hold 1 to 16 entries");
     if (s.reserved != 0u) throw ParseError(path + ": section 19: reserved must be 0");
     try {
@@ -518,14 +541,59 @@ std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const S
     return std::vector<BlubTagDensity>(s.entry, s.entry + s.count);
 }
 
+// The table of section 20, checked with the rules of set_tag_viscosities; a version-256 file has a table.
+std::vector<BlubTagViscosity> tag_viscosities_of(const TagViscositySection &s, const std::string &path) {
+    if (s.count == 0 || s.count > 16) throw ParseError(path + ": section 20 must hold 1 to 16 entries");
+    if (s.reserved != 0u) throw ParseError(path + ": section 20: reserved must be 0");
+    try {
+        check_tag_viscosities(s.entry, s.count);
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": section 20: " + e.what());
+    }
+    const BlubTagViscosity zero{};
+    for (uint32_t k = s.count; k < 16; ++k)
+        if (std::memcmp(&s.entry[k], &zero, sizeof(zero)) != 0) throw ParseError(path + ": section 20: the unused entries must be zero");
+    return std::vector<BlubTagViscosity>(s.entry, s.entry + s.count);
+}
+
+// The setting sections after the base sections, read in their order: read(section, destination) fills a host struct.
+struct Settings {
+    bool has_viscosity = false, has_surface_tension = false, has_densities = false, has_viscosities = false;
+    BlubViscosity viscosity{};
+    SurfaceTensionSection surface_tension{};
+    TagDensitySection densities{};
+    TagViscositySection viscosities{};
+};
+template <class Read> Settings read_settings(const StateHeader &h, uint32_t settings, const Section *sec, uint32_t next, const std::string &path, Read read) {
+    Settings out;
+    if ((out.has_viscosity = has_viscosity_section(settings))) {
+        read(sec[next++], &out.viscosity);
+        out.viscosity = viscosity_of(out.viscosity, h, path);
+    }
+    if ((out.has_surface_tension = (settings & bit(SEC_SURFACE_TENSION)) != 0)) {
+        read(sec[next++], &out.surface_tension);
+        surface_tension_of(out.surface_tension, path);
+    }
+    if ((out.has_densities = (settings & bit(SEC_TAG_DENSITIES)) != 0)) {
+        read(sec[next++], &out.densities);
+        tag_densities_of(out.densities, h, settings, path);
+    }
+    if ((out.has_viscosities = (settings & bit(SEC_TAG_VISCOSITIES)) != 0)) {
+        read(sec[next++], &out.viscosities);
+        tag_viscosities_of(out.viscosities, path);
+    }
+    return out;
+}
+
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
     File f(path, "rb");
-    bool viscous64 = false;
-    const StateHeader h = read_header(f, viscous64);
+    uint32_t settings = 0;
+    const StateHeader h = read_header(f, settings);
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, viscous64), nb = base_sections(h, viscous64);
+    expected_sections(h, sec, settings);
+    const uint32_t nb = base_sections(h, settings);
     Staging st(false);
     for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
     if (nb >= 14) {
@@ -538,27 +606,15 @@ StateInfo read_state_info(const std::string &path) {
         read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
         if (nb == 15) body_set_of(bs, h, f.path);
         else {
-            std::vector<char> bytes(mesh_section_length(f, h, viscous64));
+            std::vector<char> bytes(mesh_section_length(f, h, settings));
             read_section(f, {SEC_MESH_BODIES, bytes.size()}, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(bytes.data() + off, data, n); });
             std::vector<MeshBodyHost> meshes;
             mesh_body_set_of(bs, bytes, h, f.path, meshes);
         }
     }
-    uint32_t next = nb;
-    if (has_viscosity_section(h, viscous64)) {
-        BlubViscosity v{};
-        read_section(f, sec[next++], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&v) + off, data, n); });
-        viscosity_of(v, f.path);
-    }
-    if (next < ns && sec[next].id == SEC_SURFACE_TENSION) {
-        SurfaceTensionSection s{};
-        read_section(f, sec[next], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&s) + off, data, n); });
-        surface_tension_of(s, f.path);
-    } else if (next < ns) {
-        TagDensitySection s{};
-        read_section(f, sec[next], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&s) + off, data, n); });
-        tag_densities_of(s, h, viscous64, f.path);
-    }
+    read_settings(h, settings, sec, nb, f.path, [&](const Section &s, void *dst) {
+        read_section(f, s, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(static_cast<char *>(dst) + off, data, n); });
+    });
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
     info.max_num_particles = h.max_num_particles;
@@ -579,8 +635,9 @@ void HybridFluid::save_state(const std::string &path) {
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
     const bool with_bodies = num_bodies_ > 0;
-    const bool viscous = viscosity_.kinematic_viscosity > 0.0f, capillary = surface_tension_ > 0.0f, densities = !tag_densities_.empty();
-    h.format_version = densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool capillary = surface_tension_ > 0.0f, densities = !tag_densities_.empty(), viscosities = !tag_viscosities_.empty();
+    const bool viscous = viscosity_.kinematic_viscosity > 0.0f || viscosities; // version 256 always holds section 17
+    h.format_version = viscosities ? kFormatVersionTagViscosities : densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -599,7 +656,8 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0) + (densities ? 1 : 0);
+    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0) + (densities ? 1 : 0) +
+                     (viscosities ? 1 : 0);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -644,7 +702,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities || viscosities ? sizeof(tagged) : sizeof(fl));
         }
         if (with_bodies) {
             BodySection bs{};
@@ -695,6 +753,12 @@ void HybridFluid::save_state(const std::string &path) {
             for (uint32_t k = 0; k < tds.count; ++k) tds.entry[k] = tag_densities_[k];
             write_host_section(f, SEC_TAG_DENSITIES, &tds, sizeof(tds));
         }
+        if (viscosities) {
+            TagViscositySection tvs{};
+            tvs.count = (uint32_t)tag_viscosities_.size();
+            for (uint32_t k = 0; k < tvs.count; ++k) tvs.entry[k] = tag_viscosities_[k];
+            write_host_section(f, SEC_TAG_VISCOSITIES, &tvs, sizeof(tvs));
+        }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
         f.f = nullptr;
@@ -708,10 +772,11 @@ void HybridFluid::save_state(const std::string &path) {
 
 std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, int device, cudaStream_t stream) {
     File f(path, "rb");
-    bool viscous64 = false;
-    const StateHeader h = read_header(f, viscous64); // every size is checked before anything is allocated
+    uint32_t settings = 0;
+    const StateHeader h = read_header(f, settings); // every size is checked before anything is allocated
     Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, viscous64), nb = base_sections(h, viscous64);
+    expected_sections(h, sec, settings);
+    const uint32_t nb = base_sections(h, settings);
     std::unique_ptr<HybridFluid> fluid(
         new HybridFluid(h.grid_dimension[0], h.grid_dimension[1], h.grid_dimension[2], h.max_num_particles, device, stream));
     HybridFluid &x = *fluid;
@@ -764,30 +829,20 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
         to_host(sec[14], &bs);
         if (nb == 15) x.restore_bodies(body_set_of(bs, h, f.path));
         else {
-            std::vector<char> bytes(mesh_section_length(f, h, viscous64));
+            std::vector<char> bytes(mesh_section_length(f, h, settings));
             to_host({SEC_MESH_BODIES, bytes.size()}, bytes.data());
             std::vector<MeshBodyHost> meshes;
             const std::vector<BlubBody> set = mesh_body_set_of(bs, bytes, h, f.path, meshes);
             x.restore_bodies(set, std::move(meshes));
         }
     }
-    uint32_t next = nb;
-    if (has_viscosity_section(h, viscous64)) { // the working volumes and the last solve are not state
-        BlubViscosity v{};
-        to_host(sec[next++], &v);
-        v = viscosity_of(v, f.path);
-        x.set_viscosity(&v);
-    }
-    if (next < ns && sec[next].id == SEC_SURFACE_TENSION) { // the curvature is not state: stage 1 measures it again
-        SurfaceTensionSection s{};
-        to_host(sec[next], &s);
-        x.set_surface_tension(surface_tension_of(s, f.path));
-    } else if (next < ns) { // the coefficients are not state: stage 0 forms them again
-        TagDensitySection s{};
-        to_host(sec[next], &s);
-        const std::vector<BlubTagDensity> t = tag_densities_of(s, h, viscous64, f.path);
-        x.set_tag_densities(t.data(), (uint32_t)t.size());
-    }
+    // the working volumes, the last viscosity solve, the curvature, the cell densities, viscosities and coefficients are not state: the steps
+    // form them again
+    const Settings set = read_settings(h, settings, sec, nb, f.path, to_host);
+    if (set.has_viscosity) x.set_viscosity(&set.viscosity);
+    if (set.has_surface_tension) x.set_surface_tension(set.surface_tension.surface_tension);
+    if (set.has_densities) x.set_tag_densities(set.densities.entry, set.densities.count);
+    if (set.has_viscosities) x.set_tag_viscosities(set.viscosities.entry, set.viscosities.count);
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;
 }

@@ -27,6 +27,8 @@ TAP_POS, TAP_VX, TAP_VY, TAP_VZ, TAP_UX, TAP_UY, TAP_UZ, TAP_MARKER, TAP_P_VEL, 
 TAP_CURVATURE, TAP_DENSITY = 12, 13
 # download only: the float32 relative cell density of the last stage 0 on FLUID cells (zeros without a tag density table)
 TAP_CELL_DENSITY = 14
+# download only: the float32 kinematic cell viscosity of the last stage 0 on FLUID cells (zeros without a tag viscosity table)
+TAP_CELL_VISCOSITY = 15
 
 BLUB_OK = 0
 BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
@@ -40,6 +42,7 @@ LOAD_TORQUE_FRAC_BITS = 8       # BLUB_LOAD_TORQUE_FRAC_BITS: torque sums are su
 BODIES_MAX = 16                 # BLUB_BODIES_MAX
 BODY_HISTORY_LENGTH = 1024      # BLUB_BODY_HISTORY_LENGTH: records per body in the device ring
 TAG_DENSITIES_MAX = 16          # BLUB_TAG_DENSITIES_MAX
+TAG_VISCOSITIES_MAX = 16        # BLUB_TAG_VISCOSITIES_MAX
 
 
 class BlubError(RuntimeError):
@@ -139,6 +142,12 @@ class TagDensity(C.Structure):
     """BlubTagDensity: the density of a tag's particles relative to the reference density."""
 
     _fields_ = [("tag", C.c_uint32), ("relative_density", C.c_float)]
+
+
+class TagViscosity(C.Structure):
+    """BlubTagViscosity: the kinematic viscosity of a tag's particles in cells^2/s."""
+
+    _fields_ = [("tag", C.c_uint32), ("kinematic_viscosity", C.c_float)]
 
 
 class TimeStepping(C.Structure):
@@ -435,6 +444,9 @@ def lib():
         "blub_fluid_set_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32]),
         "blub_fluid_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
         "blub_scene_tag_densities": (C.c_int, [C.c_char_p, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
+        "blub_fluid_set_tag_viscosities": (C.c_int, [vp, C.POINTER(TagViscosity), u32]),
+        "blub_fluid_tag_viscosities": (C.c_int, [vp, C.POINTER(TagViscosity), u32, C.POINTER(u32)]),
+        "blub_scene_tag_viscosities": (C.c_int, [C.c_char_p, C.POINTER(TagViscosity), u32, C.POINTER(u32)]),
         "blub_fluid_max_particle_velocity": (C.c_int, [vp, f3]),
         "blub_cfl_substep_ns": (C.c_int, [C.c_uint64, f3, f3, C.POINTER(TimeStepping), C.POINTER(C.c_uint64)]),
         "blub_fluid_plan_substep": (C.c_int, [vp, C.c_uint64, C.POINTER(TimeStepping), C.POINTER(C.c_uint64), f3]),
@@ -618,6 +630,15 @@ def scene_tag_densities(path):
     arr = (TagDensity * TAG_DENSITIES_MAX)()
     _check(lib().blub_scene_tag_densities(os.fsencode(path), arr, TAG_DENSITIES_MAX, C.byref(count)))
     return {int(e.tag): float(e.relative_density) for e in arr[:count.value]}
+
+
+def scene_tag_viscosities(path):
+    """The scene's fluid.tag_viscosities as {tag: kinematic viscosity in cells^2/s} (m^2/s / grid_to_world_scale^2) in the scene's order
+    ({} without the key; host only)."""
+    count = C.c_uint32(0)
+    arr = (TagViscosity * TAG_VISCOSITIES_MAX)()
+    _check(lib().blub_scene_tag_viscosities(os.fsencode(path), arr, TAG_VISCOSITIES_MAX, C.byref(count)))
+    return {int(e.tag): float(e.kinematic_viscosity) for e in arr[:count.value]}
 
 
 def scene_viscosity(path):
@@ -908,7 +929,8 @@ class HybridFluid:
 
     # -- solid load probes --------------------------------------------------------------------
     def set_viscosity(self, nu, error_tolerance=1e-4, max_num_iterations=200):
-        """Kinematic viscosity in cells^2/s (m^2/s / grid_to_world_scale^2); 0 turns the stage off.  Every step then ends its stage 0 with
+        """Kinematic viscosity in cells^2/s (m^2/s / grid_to_world_scale^2); 0 turns the stage off without a tag viscosity table, and makes
+        the tags not in the table inviscid with one (the tolerance and the cap are kept either way).  Every step then ends its stage 0 with
         the implicit diffusion of the grid velocity, solved to max |residual| <= error_tolerance (cells/s) or max_num_iterations.  Raises
         BlubError (and changes nothing) on a negative or non-finite nu, a tolerance that is not finite and above 0, a cap outside
         [1, 10000], z-slab ranks and a fluid inside a step."""
@@ -928,7 +950,8 @@ class HybridFluid:
         return int(it.value), [float(x) for x in e]
 
     def viscosity_only(self, dt=DT_120HZ):
-        """Test hook: the viscosity stage on the grid velocity and marker as they are (tap uploads), nothing else."""
+        """Test hook: the viscosity stage on the grid velocity and marker as they are (tap uploads), nothing else.  With a tag viscosity
+        table the cell viscosities are first formed from the particles the fluid holds."""
         _check(self.L.blub_fluid_viscosity_only(self.h, dt))
 
     # -- surface tension ----------------------------------------------------------------------
@@ -962,6 +985,25 @@ class HybridFluid:
         arr = (TagDensity * TAG_DENSITIES_MAX)()
         _check(self.L.blub_fluid_tag_densities(self.h, arr, TAG_DENSITIES_MAX, C.byref(count)))
         return {int(e.tag): float(e.relative_density) for e in arr[:count.value]}
+
+    # -- liquids of different viscosities -----------------------------------------------------
+    def set_tag_viscosities(self, table):
+        """{tag: kinematic viscosity in cells^2/s} (or pairs in order): the particles of a tag have that viscosity, tags not in the table the
+        fluid's (set_viscosity, which may be 0).  An empty table clears it.  The viscosity stage runs while any of these values is above 0.
+        Raises BlubError (and changes nothing) on more than 16 entries, a tag listed twice, a viscosity that is negative or not finite,
+        z-slab ranks and a fluid inside a step.  The table is saved with the state (format version 256)."""
+        items = list(table.items()) if isinstance(table, dict) else [tuple(e) for e in table]
+        arr = (TagViscosity * max(len(items), 1))()
+        for k, (tag, nu) in enumerate(items):
+            arr[k].tag, arr[k].kinematic_viscosity = int(tag), float(nu)
+        _check(self.L.blub_fluid_set_tag_viscosities(self.h, arr, len(items)))
+
+    def tag_viscosities(self):
+        """The current table as {tag: kinematic viscosity} in the order it was set ({}: none)."""
+        count = C.c_uint32(0)
+        arr = (TagViscosity * TAG_VISCOSITIES_MAX)()
+        _check(self.L.blub_fluid_tag_viscosities(self.h, arr, TAG_VISCOSITIES_MAX, C.byref(count)))
+        return {int(e.tag): float(e.kinematic_viscosity) for e in arr[:count.value]}
 
     # -- moving tanks -------------------------------------------------------------------------
     def set_tank_frame(self, frame):

@@ -346,7 +346,9 @@ typedef struct {
     int32_t max_num_iterations;
     uint32_t reserved; /* 0 */
 } BlubViscosity;
-/* NULL or kinematic_viscosity == 0 turns the stage off: the step is then the step of a fluid that never had viscosity.  Stream-ordered;
+/* NULL or kinematic_viscosity == 0 turns the stage off while there is no tag viscosity table (blub_fluid_set_tag_viscosities): the step is
+ * then the step of a fluid that never had viscosity.  With a table, 0 makes the tags not in it inviscid.  error_tolerance and
+ * max_num_iterations are kept also with kinematic_viscosity == 0, for a table that turns the stage on.  Stream-ordered;
  * turning it on or off drops the cached step graphs, a change between two positive settings does not.  BLUB_ERR_INVALID_ARGUMENT, changing
  * nothing: a negative or non-finite viscosity, a tolerance that is not finite or not above 0, max_num_iterations outside [1, 10000],
  * reserved != 0, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
@@ -433,6 +435,32 @@ int blub_fluid_tag_densities(const BlubFluid *fluid, BlubTagDensity *out, uint32
  * *count (0 without the key).  blub_scene_load sets it on the fluid it creates.  A value the setter would refuse (and a table together with a
  * surface tension above 0) makes every scene call fail with BLUB_ERR_PARSE. */
 int blub_scene_tag_densities(const char *scene_json_path, BlubTagDensity *out, uint32_t capacity, uint32_t *count);
+
+/* ---- liquids of different viscosities (not part of the reference surface; rules: DESIGN.md section 8 "Liquids of different viscosities")
+ * A table gives the particles of a tag their own kinematic viscosity nu_tag >= 0 in cells^2/s; tags not in it take the fluid's
+ * kinematic_viscosity (blub_fluid_set_viscosity, which may be 0).  The viscosity stage runs while the fluid's value or any of the table's is
+ * above 0, with the fluid's error_tolerance and max_num_iterations.  Stage 0 averages the particles' nu per FLUID cell (exact integer sums
+ * of rint(nu_tag / nu_scale 2^32), nu_scale the largest value, independent of the particle order; a FLUID cell without a particle takes the
+ * fluid's value), and the viscosity solve couples two velocity faces with nu_fn dt, nu_fn the mean of nu over the FLUID cells at the
+ * midpoint of the two faces.  A face whose coefficients are all 0 is not solved and keeps its value.  The viscosity stays kinematic, also
+ * together with a tag density table (then not momentum-conserving across a density interface).  The table is part of the saved state
+ * (format version 256). */
+typedef struct {
+    uint32_t tag;
+    float kinematic_viscosity; /* finite, >= 0, cells^2/s */
+} BlubTagViscosity;
+#define BLUB_TAG_VISCOSITIES_MAX 16
+/* Replaces the table; count 0 clears it, and the fluid is then bit for bit a fluid that never had a table.  Stream-ordered; turning it on or
+ * off drops the cached step graphs, a change between two non-empty tables does not (unless it turns the stage on or off).
+ * BLUB_ERR_INVALID_ARGUMENT, changing nothing: more than 16 entries, a NULL table with count > 0, a tag listed twice, a viscosity that is
+ * negative or not finite, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_tag_viscosities(BlubFluid *fluid, const BlubTagViscosity *table, uint32_t count);
+/* the current table in the order it was set: min(count, capacity) entries into out, their number into *count (0: none) */
+int blub_fluid_tag_viscosities(const BlubFluid *fluid, BlubTagViscosity *out, uint32_t capacity, uint32_t *count);
+/* The scene's optional fluid.tag_viscosities, [{"tag": n, "viscosity": m^2/s}], each value divided by grid_to_world_scale^2:
+ * min(count, capacity) entries into out, their number into *count (0 without the key).  blub_scene_load sets it on the fluid it creates.  A
+ * value the setter would refuse makes every scene call fail with BLUB_ERR_PARSE. */
+int blub_scene_tag_viscosities(const char *scene_json_path, BlubTagViscosity *out, uint32_t capacity, uint32_t *count);
 
 /* ---- moving tanks (not part of the reference surface; rules: DESIGN.md section 8 "Moving tanks") ----------------------------------
  * The liquid is simulated in the tank's own frame: the grid, the walls, the solid volume, probes, sources and drains are fixed in it, and the
@@ -635,8 +663,10 @@ enum {
                                    -- after a whole step it is all zero --, or after a stage 1 with surface
                                    tension the smoothed field phi within 2 cells of FLUID).  Its contents and layout may change with the step's
                                    implementation; it exists so that tests can restate stage 1 bit for bit (download only) */
-    BLUB_TAP_CELL_DENSITY = 14  /* float per cell: the relative density rho_i of the last stage 0 on FLUID cells, 0 elsewhere; zeros while no
+    BLUB_TAP_CELL_DENSITY = 14, /* float per cell: the relative density rho_i of the last stage 0 on FLUID cells, 0 elsewhere; zeros while no
                                    tag density table is set (download only) */
+    BLUB_TAP_CELL_VISCOSITY = 15 /* float per cell: the kinematic viscosity nu_i (cells^2/s) of the last stage 0 on FLUID cells, 0 elsewhere;
+                                    zeros while no tag viscosity table is set (download only) */
 };
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);
@@ -649,8 +679,8 @@ int blub_fluid_step_stages(BlubFluid *fluid, double simulation_delta_seconds, in
 /* PCG only: solve for the rhs currently in the residual tap with the current markers; warm start from the field.  With a tag density table
  * the velocity solve (which 0) is the variable-density one, with the face coefficients of the last stage 0. */
 int blub_fluid_solve_only(BlubFluid *fluid, int which, double simulation_delta_seconds);
-/* viscosity only: applies the viscosity stage to the grid velocity and marker as they are (tap uploads), nothing else;
- * BLUB_ERR_INVALID_ARGUMENT without a viscosity above zero */
+/* viscosity only: applies the viscosity stage to the grid velocity and marker as they are (tap uploads), nothing else; with a tag viscosity
+ * table it first forms the cell viscosities from the particles the fluid holds.  BLUB_ERR_INVALID_ARGUMENT while the stage is off */
 int blub_fluid_viscosity_only(BlubFluid *fluid, double simulation_delta_seconds);
 /* last finished solve of a field, synchronously: max|r| (not multiplied by dt) and iteration count */
 int blub_fluid_last_solve(BlubFluid *fluid, int which, float *max_error, int32_t *iterations);

@@ -349,6 +349,16 @@ class HybridFluid {
     void set_tank_frame(const BlubTankFrame *frame);
     const BlubTankFrame *tank_frame() const { return has_tank_frame_ ? &tank_frame_ : nullptr; }
     float *curvature() const { return st_.kappa; }             // nullptr before the first surface tension above zero
+    // Interfacial tension (surface_tension_kernels.cu): a kinematic tension in cells^3/s^2 between phase B (the particles whose tag is one of
+    // `tags`) and the rest of the liquid, 0 turns it off.  Stream-ordered; the working volumes are allocated with the first value above zero,
+    // and only a change between off and on drops the step graphs.  Throws std::invalid_argument and changes nothing on a value or set
+    // check_interfacial_tension refuses, a z-slab rank or a fluid inside a step.  While it is on, plan_substep holds every substep to the
+    // capillary limit of the larger tension.
+    void set_interfacial_tension(const uint32_t *tags, uint32_t count, float cells3_per_s2);
+    float interfacial_tension() const { return interfacial_tension_; }
+    const std::vector<uint32_t> &interface_tags() const { return interface_tags_; }
+    float *interface_curvature() const { return it_.kappa; } // nullptr before the first interfacial tension above zero
+    long long *interface_field() const { return it_.phi; }   // likewise
     long long *density_accumulator() const { return density_.ptr; }
     // Liquids of different densities (tag_density_kernels.cu): replaces the table, count 0 turns the feature off.  Stream-ordered; the working
     // volumes are allocated with the first non-empty table, and only a change between off and on drops the step graphs.  Throws
@@ -385,6 +395,9 @@ class HybridFluid {
     void ensure_viscosity_work();
     float surface_tension_ = 0.0f;
     SurfaceTensionWork st_;
+    float interfacial_tension_ = 0.0f;
+    std::vector<uint32_t> interface_tags_;
+    InterfacialTensionWork it_;
     void run_viscosity();
     LoadProbeBox *load_probes_dev_ = nullptr; // LOAD_PROBES_MAX boxes and LOAD_PROBES_MAX x LOAD_HISTORY_LENGTH records, allocated with the
     BlubSolidLoad *load_ring_ = nullptr;      // first non-empty set
@@ -518,6 +531,9 @@ void check_time_stepping(const BlubTimeStepping &ts);
 // Brackbill's capillary step limit with dx = 1 cell and the mean of the liquid and air densities: floor(1e9 sqrt(1 / (4 pi s))) ns for a
 // kinematic surface tension s > 0 (cells^3/s^2), saturating at UINT64_MAX.
 uint64_t capillary_limit_ns(float cells3_per_s2);
+// The interfacial tension setter's rules: s finite and >= 0, at most BLUB_INTERFACE_TAGS_MAX tags, none twice, not NULL with count > 0, and
+// at least one tag when s > 0.  Throws std::invalid_argument naming `who`.
+void check_interfacial_tension(const uint32_t *tags, uint32_t count, float s, const char *who);
 uint64_t cfl_substep_ns(uint64_t remaining_ns, const float max_velocity[3], const float gravity_grid[3], const BlubTimeStepping &ts);
 // Moving tanks (tank_kernels.cu, DESIGN.md §8 "Moving tanks"): the host rules of blub_tank_frame_at, blub_tank_step_constants and
 // blub_tank_cfl_substep_ns (frame == nullptr: cfl_substep_ns).
@@ -621,6 +637,8 @@ struct SceneConfig {
     std::vector<SceneBody> bodies;           // optional fluid.bodies (world units, m/s)
     float viscosity = 0.0f;                  // optional fluid.viscosity: kinematic, m^2/s
     float surface_tension = 0.0f;            // optional fluid.surface_tension: kinematic, m^3/s^2
+    float interfacial_tension = 0.0f;        // optional fluid.interfacial_tension: kinematic, m^3/s^2, between the tags below and the rest
+    std::vector<uint32_t> interface_tags;    // checked with the setter's rules
     std::vector<BlubTagDensity> tag_densities; // optional fluid.tag_densities, checked with the setter's rules
     std::vector<BlubTagViscosity> tag_viscosities; // optional fluid.tag_viscosities (m^2/s), checked in cells^2/s with the setter's rules
     bool has_tank_motion = false;            // optional fluid.tank_motion (world units, Hz, rad, rad/s; directions and axis normalised)
@@ -638,6 +656,8 @@ float scene_viscosity_grid(const SceneConfig &cfg);
 std::vector<BlubTagViscosity> scene_tag_viscosities_grid(const SceneConfig &cfg); // fluid.tag_viscosities in cells^2/s
 // the scene's kinematic surface tension in cells^3/s^2: surface_tension / grid_to_world_scale^3
 float scene_surface_tension_grid(const SceneConfig &cfg);
+// the scene's kinematic interfacial tension in cells^3/s^2: interfacial_tension / grid_to_world_scale^3
+float scene_interfacial_tension_grid(const SceneConfig &cfg);
 // the scene's bodies in grid cells and cells/s: (position - world_position) / scale, half extents and velocity / scale, the Euler angles as a
 // quaternion (quat_from_euler_deg_wxyz), the angular velocity unchanged
 std::vector<BlubBody> scene_bodies_grid(const SceneConfig &cfg);

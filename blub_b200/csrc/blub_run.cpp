@@ -366,6 +366,14 @@ int main(int argc, char **argv) {
         float sigma = 0.0f;
         if (blub_fluid_surface_tension(fluid, &sigma)) die("cannot read the surface tension");
         if (sigma > 0.0f) std::fprintf(f, ", \"surface_tension\": %.9g", sigma);
+        uint32_t itags[BLUB_INTERFACE_TAGS_MAX], nit = 0;
+        float sab = 0.0f;
+        if (blub_fluid_interfacial_tension(fluid, itags, BLUB_INTERFACE_TAGS_MAX, &nit, &sab)) die("cannot read the interfacial tension");
+        if (sab > 0.0f) {
+            std::fprintf(f, ", \"interfacial_tension\": {\"tension\": %.9g, \"tags\": [", sab);
+            for (uint32_t k = 0; k < nit; ++k) std::fprintf(f, "%s%u", k ? ", " : "", itags[k]);
+            std::fprintf(f, "]}");
+        }
         if (adaptive) {
             std::fprintf(f, ", \"time_stepping\": {\"cfl\": %.9g, \"interval_ns\": %llu, \"min_dt_ns\": %llu, \"intervals\": [", (double)time_stepping.cfl_number,
                          (unsigned long long)dt_ns, (unsigned long long)time_stepping.min_dt_ns);

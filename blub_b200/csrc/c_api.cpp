@@ -73,6 +73,8 @@ Tap tap_of(BlubFluid *f, int tap) {
     case BLUB_TAP_DENSITY: return {h.density_accumulator(), n * 8};
     case BLUB_TAP_CELL_DENSITY: return {h.cell_density(), n * 4}; // nullptr before the first table: zeros
     case BLUB_TAP_CELL_VISCOSITY: return {h.cell_viscosity(), n * 4}; // nullptr before the first table: zeros
+    case BLUB_TAP_INTERFACE_CURVATURE: return {h.interface_curvature(), n * 4}; // nullptr before the first interfacial tension: zeros
+    case BLUB_TAP_INTERFACE_FIELD: return {h.interface_field(), n * 8};         // likewise
     default: return {nullptr, 0};
     }
 }
@@ -538,6 +540,31 @@ int blub_scene_surface_tension(const char *path, float *cells3_per_s2) {
     return guarded([&] { *cells3_per_s2 = blub::scene_surface_tension_grid(blub::parse_scene_file(path)); return BLUB_OK; });
 }
 
+int blub_fluid_set_interfacial_tension(BlubFluid *fluid, const uint32_t *tags, uint32_t count, float cells3_per_s2) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_interfacial_tension(tags, count, cells3_per_s2); return BLUB_OK; });
+}
+
+int blub_fluid_interfacial_tension(const BlubFluid *fluid, uint32_t *tags, uint32_t capacity, uint32_t *count, float *cells3_per_s2) {
+    if (!fluid || !count || !cells3_per_s2 || (capacity && !tags)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    const std::vector<uint32_t> &t = fluid->impl->interface_tags();
+    for (uint32_t k = 0; k < capacity && k < t.size(); ++k) tags[k] = t[k];
+    *count = (uint32_t)t.size();
+    *cells3_per_s2 = fluid->impl->interfacial_tension();
+    return BLUB_OK;
+}
+
+int blub_scene_interfacial_tension(const char *path, uint32_t *tags, uint32_t capacity, uint32_t *count, float *cells3_per_s2) {
+    if (!path || !count || !cells3_per_s2 || (capacity && !tags)) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig c = blub::parse_scene_file(path);
+        for (uint32_t k = 0; k < capacity && k < c.interface_tags.size(); ++k) tags[k] = c.interface_tags[k];
+        *count = (uint32_t)c.interface_tags.size();
+        *cells3_per_s2 = blub::scene_interfacial_tension_grid(c);
+        return BLUB_OK;
+    });
+}
+
 int blub_fluid_set_tag_densities(BlubFluid *fluid, const BlubTagDensity *table, uint32_t count) {
     if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
     return guarded([&] { fluid->impl->set_tag_densities(table, count); return BLUB_OK; });
@@ -707,8 +734,9 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
     if (!fluid || !host_dst) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
-        if ((tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_CELL_DENSITY || tap == BLUB_TAP_CELL_VISCOSITY) && !t.ptr) {
-            if (bytes > (size_t)fluid->impl->grid_dimension().n * 4) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
+        if ((tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_CELL_DENSITY || tap == BLUB_TAP_CELL_VISCOSITY || tap == BLUB_TAP_INTERFACE_CURVATURE ||
+             tap == BLUB_TAP_INTERFACE_FIELD) && !t.ptr) {
+            if (bytes > (size_t)fluid->impl->grid_dimension().n * (tap == BLUB_TAP_INTERFACE_FIELD ? 8 : 4)) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");
             std::memset(host_dst, 0, bytes);
             return BLUB_OK;
         }
@@ -723,8 +751,9 @@ int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes)
 int blub_fluid_upload(BlubFluid *fluid, int tap, const void *host_src, size_t bytes) {
     if (!fluid || !host_src) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
     if (tap == BLUB_TAP_SOLID_VOXELS || tap == BLUB_TAP_CURVATURE || tap == BLUB_TAP_DENSITY || tap == BLUB_TAP_CELL_DENSITY ||
-        tap == BLUB_TAP_CELL_VISCOSITY)
-        return fail(BLUB_ERR_INVALID_ARGUMENT, "the solid volume, curvature, density, cell density and cell viscosity taps are download only");
+        tap == BLUB_TAP_CELL_VISCOSITY || tap == BLUB_TAP_INTERFACE_CURVATURE || tap == BLUB_TAP_INTERFACE_FIELD)
+        return fail(BLUB_ERR_INVALID_ARGUMENT,
+                    "the solid volume, curvature, density, cell density, cell viscosity, interface curvature and interface field taps are download only");
     return guarded([&] {
         Tap t = tap_of(fluid, tap);
         if (!t.ptr || bytes > t.bytes) return fail(BLUB_ERR_INVALID_ARGUMENT, "bad tap or size");

@@ -295,6 +295,38 @@ void launch_surface_rhs(cudaStream_t st, const GridDim &g, const FluidBits &bits
 void launch_surface_faces(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
                           const SurfaceTensionWork &w, float *const u[3]);
 
+// ---- interfacial tension (surface_tension_kernels.cu, DESIGN.md §8 "Interfacial tension") ----
+constexpr int INTERFACE_TAGS_MAX = BLUB_INTERFACE_TAGS_MAX;
+// What the kernels read of the setting: a change between two values above zero does not invalidate a captured graph.
+struct InterfacialTensionBlock {
+    float s;        // the kinematic interfacial tension (cells^3/s^2)
+    uint32_t count; // phase B: the particles whose tag is one of tag[0, count); the unused entries are 0
+    uint32_t tag[INTERFACE_TAGS_MAX];
+};
+// Working memory, allocated with the first interfacial tension above zero: 20 bytes per cell.
+struct InterfacialTensionWork {
+    long long *phi = nullptr;   // n: the phase-B splat (2^-40), then the smoothed phase field phi (2^-32), valid within 2 cells of FLUID
+    long long *psi = nullptr;   // n: the wall-ruled phase field, valid within 3 cells of FLUID
+    float *kappa = nullptr;     // n: the interface's curvature of the last stage 1 in the band (cells^-1), 0 elsewhere
+    InterfacialTensionBlock *block = nullptr;
+};
+// The phase-B splat: launch_density_scatter of the particles whose tag the block lists into `density` (zeroed first).
+void launch_phase_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density,
+                          const ScatterSchedule &sched, const InterfacialTensionBlock *blk);
+// Stage 1: the phase field of the splat of every particle in `splat_all` and of the phase-B particles in w.phi (launch_phase_scatter), in
+// two parts so that the free surface can reuse `splat_all` in between: launch_interface_psi reads both splats into w.psi, then
+// launch_interface_curvature smooths w.psi into w.phi and measures the curvature into w.kappa.
+void launch_interface_psi(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const long long *splat_all,
+                          const InterfacialTensionWork &w);
+void launch_interface_curvature(cudaStream_t st, const GridDim &g, const FluidBits &bits, const int8_t *marker, const InterfacialTensionWork &w);
+// Stage 1, after the divergence (and the free surface's terms): rhs += +-beta_f g_f over every band cell's interface faces.  `beta`: the
+// density table's face arrays, nullptr without a table (beta_f = 1).
+void launch_interface_rhs(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
+                          const InterfacialTensionWork &w, const float *const *beta, float *rhs);
+// Stage 4, after the projection: the interface faces get the beta_f g_f the solve assumed.
+void launch_interface_faces(cudaStream_t st, const GridDim &g, const FluidBits &bits, const StepParams *params, const int8_t *marker,
+                            const InterfacialTensionWork &w, const float *const *beta, float *const u[3]);
+
 // ---- liquids of different densities (tag_density_kernels.cu, DESIGN.md §8 "Liquids of different densities") ----
 constexpr int TAG_DENSITIES_MAX = BLUB_TAG_DENSITIES_MAX;
 constexpr int TAG_DENSITY_FRAC_BITS = 20; // a particle adds rint(rho * 2^20) to its cell's sum

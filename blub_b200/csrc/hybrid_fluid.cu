@@ -61,6 +61,13 @@ void free_work(SurfaceTensionWork &w) {
     cudaFree(w.sigma);
     w = SurfaceTensionWork{};
 }
+void free_work(InterfacialTensionWork &w) {
+    cudaFree(w.phi);
+    cudaFree(w.psi);
+    cudaFree(w.kappa);
+    cudaFree(w.block);
+    w = InterfacialTensionWork{};
+}
 void free_work(TagDensityWork &w) {
     cudaFree(w.sum);
     cudaFree(w.count);
@@ -252,6 +259,7 @@ HybridFluid::~HybridFluid() {
     free_work(visc_);
     free_work(tv_);
     free_work(st_);
+    free_work(it_);
     free_work(td_);
     cudaFree(census_dev_);
     cudaFree(max_velocity_dev_);
@@ -557,14 +565,26 @@ void HybridFluid::run_stage(int stage, float dt) {
     case 1: // compute divergence -> PCG residual (:835-840)
         refresh_fluid_bits();
         launch_divergence_compute(stream_, grid_, bits, marker_.ptr, u, vox, solver_->residual());
-        if (surface_tension_ > 0.0f) {
+        if (surface_tension_ > 0.0f || interfacial_tension_ > 0.0f) {
             const NvtxScope st_scope("surface tension: curvature");
-            // The density accumulator is free until stage 7 or 9 clears it.  On the scheduled path the splat rewrites sched_.item_box, the boxes
-            // the next P2G reads: harmless, because stage 7 or 9 of this step rewrites them before that P2G.
+            // The density accumulator is free until stage 7 or 9 clears it.  On the scheduled path the splats rewrite sched_.item_box, the
+            // boxes the next P2G reads: harmless, because stage 7 or 9 of this step rewrites them before that P2G.  One splat of every particle
+            // serves both tensions: the interface reads it before the free surface overwrites it with its phi.
             launch_density_scatter(stream_, grid_, params_dev_, np, pos_[cur_], density_.ptr, sched_);
             density_zero_ = false;
-            launch_surface_curvature(stream_, grid_, bits, marker_.ptr, density_.ptr, st_);
-            launch_surface_rhs(stream_, grid_, bits, params_dev_, marker_.ptr, st_, solver_->residual());
+            if (interfacial_tension_ > 0.0f) {
+                launch_phase_scatter(stream_, grid_, params_dev_, np, pos_[cur_], it_.phi, sched_, it_.block);
+                launch_interface_psi(stream_, grid_, bits, marker_.ptr, density_.ptr, it_);
+            }
+            if (surface_tension_ > 0.0f) {
+                launch_surface_curvature(stream_, grid_, bits, marker_.ptr, density_.ptr, st_);
+                launch_surface_rhs(stream_, grid_, bits, params_dev_, marker_.ptr, st_, solver_->residual());
+            }
+            if (interfacial_tension_ > 0.0f) {
+                const NvtxScope it_scope("interfacial tension: curvature");
+                launch_interface_curvature(stream_, grid_, bits, marker_.ptr, it_);
+                launch_interface_rhs(stream_, grid_, bits, params_dev_, marker_.ptr, it_, tag_densities_.empty() ? nullptr : td_.beta, solver_->residual());
+            }
         }
         break;
     case 2: // primary pressure solver (:843-852)
@@ -597,6 +617,10 @@ void HybridFluid::run_stage(int stage, float dt) {
         if (surface_tension_ > 0.0f) {
             const NvtxScope st_scope("surface tension: pressure jump");
             launch_surface_faces(stream_, grid_, bits, params_dev_, marker_.ptr, st_, u);
+        }
+        if (interfacial_tension_ > 0.0f) {
+            const NvtxScope it_scope("interfacial tension: pressure jump");
+            launch_interface_faces(stream_, grid_, bits, params_dev_, marker_.ptr, it_, tag_densities_.empty() ? nullptr : td_.beta, u);
         }
         break;
     case 5: // extrapolate velocity grid (:906-909)
@@ -1099,10 +1123,12 @@ uint64_t HybridFluid::plan_substep(uint64_t remaining_ns, const BlubTimeStepping
     max_particle_velocity(v);
     if (max_velocity_out) std::memcpy(max_velocity_out, v, sizeof(v));
     const uint32_t dim[3] = {(uint32_t)grid_.nx, (uint32_t)grid_.ny, (uint32_t)grid_.nz};
-    if (!(surface_tension_ > 0.0f)) return tank_cfl_substep_ns(remaining_ns, v, gravity_, tank_frame(), dim, ts);
-    const uint64_t cap = capillary_limit_ns(surface_tension_);
+    // the larger of the two tensions: conservative for the interface, whose densities (at least 1/2 each) sum to at least 1
+    const float s = std::max(surface_tension_, interfacial_tension_);
+    if (!(s > 0.0f)) return tank_cfl_substep_ns(remaining_ns, v, gravity_, tank_frame(), dim, ts);
+    const uint64_t cap = capillary_limit_ns(s);
     if (cap < ts.min_dt_ns)
-        throw UnstableError("plan_substep: the capillary step limit of " + std::to_string(cap) + " ns at a surface tension of " + std::to_string(surface_tension_) +
+        throw UnstableError("plan_substep: the capillary step limit of " + std::to_string(cap) + " ns at a surface tension of " + std::to_string(s) +
                             " cells^3/s^2 is below min_dt_ns = " + std::to_string(ts.min_dt_ns) + " ns");
     BlubTimeStepping capped = ts;
     capped.max_dt_ns = std::min(ts.max_dt_ns, cap);
@@ -1156,6 +1182,60 @@ void HybridFluid::set_surface_tension(float s) {
     if (!on && st_.kappa) BLUB_CUDA_CHECK(cudaMemsetAsync(st_.kappa, 0, (size_t)grid_.n * sizeof(float), stream_)); // the tap reads zeros when off
     if (on != (surface_tension_ > 0.0f)) destroy_graphs();
     surface_tension_ = s;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Interfacial tension (surface_tension_kernels.cu).  Not in the reference.  The kernels read the tension and the tag set from a device block,
+// so a change between two settings above zero replays the captured graphs; turning it on or off changes the launches and drops them.
+void check_interfacial_tension(const uint32_t *tags, uint32_t count, float s, const char *who) {
+    const std::string w = who;
+    if (!std::isfinite(s) || s < 0.0f) throw std::invalid_argument(w + ": the interfacial tension must be finite and not negative");
+    if (count > (uint32_t)INTERFACE_TAGS_MAX) throw std::invalid_argument(w + ": more than " + std::to_string(INTERFACE_TAGS_MAX) + " tags");
+    if (count && !tags) throw std::invalid_argument(w + ": NULL tags with count > 0");
+    for (uint32_t a = 0; a < count; ++a)
+        for (uint32_t b = 0; b < a; ++b)
+            if (tags[a] == tags[b]) throw std::invalid_argument(w + ": tag " + std::to_string(tags[a]) + " is listed twice");
+    if (s > 0.0f && !count) throw std::invalid_argument(w + ": an interfacial tension above 0 needs at least one tag");
+}
+
+void HybridFluid::set_interfacial_tension(const uint32_t *tags, uint32_t count, float s) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_interfacial_tension: z-slab ranks have no interfacial tension");
+    if (mid_step_) throw std::invalid_argument("set_interfacial_tension: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    check_interfacial_tension(tags, count, s, "set_interfacial_tension");
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    const bool on = s > 0.0f;
+    if (on && !it_.block) {
+        InterfacialTensionWork w;
+        const size_t n = (size_t)grid_.n;
+        try {
+            BLUB_CUDA_CHECK(cudaMalloc(&w.phi, n * sizeof(long long)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.phi, 0, n * sizeof(long long), stream_));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.psi, n * sizeof(long long)));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.kappa, n * sizeof(float)));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(w.kappa, 0, n * sizeof(float), stream_));
+            BLUB_CUDA_CHECK(cudaMalloc(&w.block, sizeof(InterfacialTensionBlock)));
+        } catch (...) {
+            cudaStreamSynchronize(stream_); // the memsets may be in flight
+            free_work(w);
+            throw;
+        }
+        it_ = w;
+    }
+    if (it_.block) { // stream-ordered behind the steps already enqueued (the copy stages the value before it returns)
+        InterfacialTensionBlock b{};
+        b.s = s;
+        b.count = on ? count : 0u;
+        for (uint32_t k = 0; k < b.count; ++k) b.tag[k] = tags[k];
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(it_.block, &b, sizeof(b), cudaMemcpyHostToDevice, stream_));
+        if (!on) { // the taps read zeros when off
+            BLUB_CUDA_CHECK(cudaMemsetAsync(it_.kappa, 0, (size_t)grid_.n * sizeof(float), stream_));
+            BLUB_CUDA_CHECK(cudaMemsetAsync(it_.phi, 0, (size_t)grid_.n * sizeof(long long), stream_));
+        }
+    }
+    if (on != (interfacial_tension_ > 0.0f)) destroy_graphs();
+    interfacial_tension_ = s;
+    if (on) interface_tags_.assign(tags, tags + count);
+    else interface_tags_.clear();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1507,6 +1587,7 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
     }
     if (cfg.surface_tension > 0.0f) f->set_surface_tension(scene_surface_tension_grid(cfg));
     if (!cfg.tag_densities.empty()) f->set_tag_densities(cfg.tag_densities.data(), (uint32_t)cfg.tag_densities.size());
+    if (cfg.interfacial_tension > 0.0f) f->set_interfacial_tension(cfg.interface_tags.data(), (uint32_t)cfg.interface_tags.size(), scene_interfacial_tension_grid(cfg));
     if (!cfg.load_probes.empty()) {
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);
         f->set_load_probes(probes.data(), (uint32_t)probes.size());

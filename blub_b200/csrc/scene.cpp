@@ -155,6 +155,10 @@ float scene_surface_tension_grid(const SceneConfig &cfg) {
     return cfg.surface_tension / (cfg.grid_to_world_scale * cfg.grid_to_world_scale * cfg.grid_to_world_scale);
 }
 
+float scene_interfacial_tension_grid(const SceneConfig &cfg) {
+    return cfg.interfacial_tension / (cfg.grid_to_world_scale * cfg.grid_to_world_scale * cfg.grid_to_world_scale);
+}
+
 BlubTankMotion scene_tank_motion_grid(const SceneConfig &cfg) {
     const float scale = cfg.grid_to_world_scale;
     BlubTankMotion m = cfg.tank_motion;
@@ -228,6 +232,20 @@ SceneConfig parse_scene_file(const std::string &path) {
         cfg.surface_tension = num_f32(*st, "surface_tension");
         if (!std::isfinite(cfg.surface_tension) || cfg.surface_tension < 0.0f || !std::isfinite(scene_surface_tension_grid(cfg)))
             throw std::runtime_error("scene JSON: `fluid.surface_tension` must be finite and not negative");
+    }
+    // interfacial tension (not in the reference): {"tags": [n, ...], "tension": m^3/s^2}, checked in cells^3/s^2 with the setter's rules
+    if (const JsonValue *it = fluid.get("interfacial_tension")) {
+        if (it->kind != JsonValue::Object) throw std::runtime_error("scene JSON: `fluid.interfacial_tension` is not an object");
+        const JsonValue &tags = need(*it, "tags"), &tension = need(*it, "tension");
+        if (tags.kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.interfacial_tension.tags` is not an array");
+        if (tension.kind != JsonValue::Number) throw std::runtime_error("scene JSON: `fluid.interfacial_tension.tension` is not a number");
+        for (const JsonValue &t : tags.array) cfg.interface_tags.push_back(num_u32(t, "interfacial_tension.tags"));
+        cfg.interfacial_tension = num_f32(tension, "interfacial_tension.tension");
+        try {
+            check_interfacial_tension(cfg.interface_tags.data(), (uint32_t)cfg.interface_tags.size(), scene_interfacial_tension_grid(cfg), "scene");
+        } catch (const std::invalid_argument &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.interfacial_tension`: ") + e.what());
+        }
     }
     // liquids of different densities (not in the reference): [{"tag": n, "relative_density": x}], checked with the setter's rules
     if (const JsonValue *td = fluid.get("tag_densities")) {

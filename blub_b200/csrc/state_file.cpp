@@ -38,15 +38,20 @@ constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
 // section 17 always (its kinematic_viscosity may be 0: the tags not in the table are inviscid), section 18 when the surface tension is
 // above 0, section 19 when a tag density table is set, and a last section 20, the table.  The reader finds 17, 18 and 19 by walking the
 // section heads as for versions 64 and 128.  Versions 129 to 255 are not formats.
+// Version 512: a fluid with an interfacial tension; the layout it would otherwise have (versions 1 to 256: 13 to 16 base sections, then the
+// setting sections 17 to 20 it has) plus a last section 21, the tension and phase B's tags.  The reader finds 17 to 20 by walking the section
+// heads as for versions 64, 128 and 256, and refuses a version-512 file whose walk does not reach a section 21.  Section 17 may hold a
+// viscosity of 0 only together with section 20, as in version 256.  Versions 257 to 511 are not formats.
 constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32,
-                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128, kFormatVersionTagViscosities = 256;
-constexpr uint32_t kNumSections = 20; // at most
+                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128, kFormatVersionTagViscosities = 256,
+                   kFormatVersionInterfacialTension = 512;
+constexpr uint32_t kNumSections = 21; // at most
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES, SEC_TAG_VISCOSITIES
+    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES, SEC_TAG_VISCOSITIES, SEC_INTERFACIAL_TENSION
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -102,6 +107,14 @@ struct TagViscositySection {
     BlubTagViscosity entry[16];
 };
 static_assert(sizeof(TagViscositySection) == 136 && TAG_VISCOSITIES_MAX == 16, "tag viscosity section layout");
+// Section 21 (version 512): the kinematic interfacial tension as set, above 0 (cells^3/s^2), and phase B's tags in the order they were set,
+// unused entries zero
+struct InterfacialTensionSection {
+    float tension;
+    uint32_t count;
+    uint32_t tag[16];
+};
+static_assert(sizeof(InterfacialTensionSection) == 72 && INTERFACE_TAGS_MAX == 16, "interfacial tension section layout");
 
 struct StateHeader {
     char magic[8];
@@ -140,7 +153,8 @@ struct Section {
 constexpr uint32_t bit(uint32_t id) { return 1u << id; }
 // the versions whose base sections are followed by setting sections the header does not tell apart
 bool walks_settings(const StateHeader &h) {
-    return h.format_version == kFormatVersionSurfaceTension || h.format_version == kFormatVersionTagDensities || h.format_version == kFormatVersionTagViscosities;
+    return h.format_version == kFormatVersionSurfaceTension || h.format_version == kFormatVersionTagDensities || h.format_version == kFormatVersionTagViscosities ||
+           h.format_version == kFormatVersionInterfacialTension;
 }
 uint32_t base_sections(const StateHeader &h, uint32_t settings) {
     if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
@@ -161,12 +175,13 @@ uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], uint
                                      {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
                                      {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
                                      {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)},
-                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}, {SEC_TAG_VISCOSITIES, sizeof(TagViscositySection)}};
+                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}, {SEC_TAG_VISCOSITIES, sizeof(TagViscositySection)},
+                                     {SEC_INTERFACIAL_TENSION, sizeof(InterfacialTensionSection)}};
     std::memcpy(out, s, sizeof(s));
     const uint32_t nb = base_sections(h, settings);
     if (nb == 0) return 0;
     uint32_t ns = nb;
-    for (uint32_t id = SEC_VISCOSITY; id <= SEC_TAG_VISCOSITIES; ++id)
+    for (uint32_t id = SEC_VISCOSITY; id <= SEC_INTERFACIAL_TENSION; ++id)
         if (settings & bit(id)) out[ns++] = s[id - 1];
     return ns;
 }
@@ -209,30 +224,37 @@ struct File {
 };
 
 // The setting sections of a file (see base_sections).  Versions 64, 128 and 256: the ids 17 to 19 found among the sections after section 13 by
-// walking their heads with their stored lengths (at most six of them before the last section, 18, 19 or 20), plus the sections the version
+// walking their heads with their stored lengths (at most seven of them before the last section, 18, 19, 20 or 21), plus the sections the version
 // always holds.  Leaves `f` where it was.  The lengths are checked later, section by section.
 uint32_t settings_in_file(File &f, const StateHeader &h) {
     if (h.format_version == kFormatVersionViscosity) return bit(SEC_VISCOSITY);
     if (!walks_settings(h)) return 0u;
     const uint32_t last = h.format_version == kFormatVersionSurfaceTension ? SEC_SURFACE_TENSION
-                          : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES : SEC_TAG_VISCOSITIES;
-    // what the walk may find: 17 in versions 64 and 128, 18 and 19 in version 256 (17 is always there)
-    const uint32_t optional = last == SEC_TAG_VISCOSITIES ? bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) : bit(SEC_VISCOSITY);
+                          : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES
+                          : h.format_version == kFormatVersionTagViscosities ? SEC_TAG_VISCOSITIES : SEC_INTERFACIAL_TENSION;
+    // what the walk may find: 17 in versions 64 and 128, 18 and 19 in version 256 (17 is always there), 17 to 20 in version 512
+    const uint32_t optional = last == SEC_INTERFACIAL_TENSION ? bit(SEC_VISCOSITY) | bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) | bit(SEC_TAG_VISCOSITIES)
+                              : last == SEC_TAG_VISCOSITIES ? bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) : bit(SEC_VISCOSITY);
     uint32_t settings = bit(last) | (last == SEC_TAG_VISCOSITIES ? bit(SEC_VISCOSITY) : 0u);
+    bool found_last = false;
     const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
     const uint64_t base[13] = {np, np, np, np, 4 * n, 4 * n, 4 * n, n, 4 * n, 4 * n, 2 * sizeof(PcgScalars), 8ull * h.num_stats[0], 8ull * h.num_stats[1]};
     const uint64_t here = f.tell(), size = f.size();
     uint64_t at = here;
     for (uint64_t len : base) at += sizeof(SectionHead) + len + 4;
-    for (int k = 0; k < 7 && at + sizeof(SectionHead) <= size; ++k) {
+    for (int k = 0; k < 8 && at + sizeof(SectionHead) <= size; ++k) {
         SectionHead head;
         f.seek(at);
         f.read(&head, sizeof(head));
         if (head.id >= SEC_VISCOSITY && head.id < 32 && (optional & bit(head.id))) settings |= bit(head.id);
+        if (head.id == last) found_last = true;
         if (head.id == last || head.length > size) break;
         at += sizeof(SectionHead) + head.length + 4;
     }
     f.seek(here);
+    // a version-512 header over a layout without the interfacial tension (a version-256 file relabelled, say) is not a version-512 file
+    if (last == SEC_INTERFACIAL_TENSION && !found_last)
+        throw ParseError(f.path + ": format version 512 ends with section 21 (the interfacial tension), the file has none");
     return settings;
 }
 
@@ -278,9 +300,9 @@ StateHeader read_header(File &f, uint32_t &settings) {
     if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
         h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity &&
         h.format_version != kFormatVersionSurfaceTension && h.format_version != kFormatVersionTagDensities &&
-        h.format_version != kFormatVersionTagViscosities)
+        h.format_version != kFormatVersionTagViscosities && h.format_version != kFormatVersionInterfacialTension)
         throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64, 128 and 256)");
+                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64, 128, 256 and 512)");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -504,15 +526,15 @@ std::vector<BlubBody> mesh_body_set_of(const BodySection &bs, const std::vector<
 }
 
 // The setting of section 17, checked with the rules of set_viscosity; below version 256 it holds a viscosity above 0 (a version-256 file's
-// may hold 0: the tags not in its table are inviscid).
-BlubViscosity viscosity_of(const BlubViscosity &v, const StateHeader &h, const std::string &path) {
+// may hold 0: the tags not in its table are inviscid; so may a version-512 file's that has a section 20).
+BlubViscosity viscosity_of(const BlubViscosity &v, const StateHeader &h, uint32_t settings, const std::string &path) {
     try {
         check_viscosity(v);
     } catch (const std::invalid_argument &e) {
         throw ParseError(path + ": section 17: " + e.what());
     }
-    if (h.format_version != kFormatVersionTagViscosities && !(v.kinematic_viscosity > 0.0f))
-        throw ParseError(path + ": section 17: a version-32, -64 or -128 file's section 17 holds a viscosity above 0");
+    if (!(settings & bit(SEC_TAG_VISCOSITIES)) && !(v.kinematic_viscosity > 0.0f))
+        throw ParseError(path + ": section 17: without a section 20 section 17 holds a viscosity above 0");
     return v;
 }
 
@@ -556,19 +578,33 @@ std::vector<BlubTagViscosity> tag_viscosities_of(const TagViscositySection &s, c
     return std::vector<BlubTagViscosity>(s.entry, s.entry + s.count);
 }
 
+// The setting of section 21, checked with the rules of set_interfacial_tension; a version-512 file has an interfacial tension above 0.
+void interfacial_tension_of(const InterfacialTensionSection &s, const std::string &path) {
+    if (!(s.tension > 0.0f)) throw ParseError(path + ": section 21: the interfacial tension must be above 0");
+    if (s.count > 16) throw ParseError(path + ": section 21 must hold 1 to 16 tags");
+    try {
+        check_interfacial_tension(s.tag, s.count, s.tension, "section 21");
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": " + e.what());
+    }
+    for (uint32_t k = s.count; k < 16; ++k)
+        if (s.tag[k] != 0u) throw ParseError(path + ": section 21: the unused entries must be zero");
+}
+
 // The setting sections after the base sections, read in their order: read(section, destination) fills a host struct.
 struct Settings {
-    bool has_viscosity = false, has_surface_tension = false, has_densities = false, has_viscosities = false;
+    bool has_viscosity = false, has_surface_tension = false, has_densities = false, has_viscosities = false, has_interfacial = false;
     BlubViscosity viscosity{};
     SurfaceTensionSection surface_tension{};
     TagDensitySection densities{};
     TagViscositySection viscosities{};
+    InterfacialTensionSection interfacial{};
 };
 template <class Read> Settings read_settings(const StateHeader &h, uint32_t settings, const Section *sec, uint32_t next, const std::string &path, Read read) {
     Settings out;
     if ((out.has_viscosity = has_viscosity_section(settings))) {
         read(sec[next++], &out.viscosity);
-        out.viscosity = viscosity_of(out.viscosity, h, path);
+        out.viscosity = viscosity_of(out.viscosity, h, settings, path);
     }
     if ((out.has_surface_tension = (settings & bit(SEC_SURFACE_TENSION)) != 0)) {
         read(sec[next++], &out.surface_tension);
@@ -581,6 +617,11 @@ template <class Read> Settings read_settings(const StateHeader &h, uint32_t sett
     if ((out.has_viscosities = (settings & bit(SEC_TAG_VISCOSITIES)) != 0)) {
         read(sec[next++], &out.viscosities);
         tag_viscosities_of(out.viscosities, path);
+        if (!has_viscosity_section(settings)) throw ParseError(path + ": section 20 needs a section 17 before it");
+    }
+    if ((out.has_interfacial = (settings & bit(SEC_INTERFACIAL_TENSION)) != 0)) {
+        read(sec[next++], &out.interfacial);
+        interfacial_tension_of(out.interfacial, path);
     }
     return out;
 }
@@ -637,7 +678,8 @@ void HybridFluid::save_state(const std::string &path) {
     const bool with_bodies = num_bodies_ > 0;
     const bool capillary = surface_tension_ > 0.0f, densities = !tag_densities_.empty(), viscosities = !tag_viscosities_.empty();
     const bool viscous = viscosity_.kinematic_viscosity > 0.0f || viscosities; // version 256 always holds section 17
-    h.format_version = viscosities ? kFormatVersionTagViscosities : densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    const bool interfacial = interfacial_tension_ > 0.0f;
+    h.format_version = interfacial ? kFormatVersionInterfacialTension : viscosities ? kFormatVersionTagViscosities : densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -657,7 +699,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
     h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0) + (densities ? 1 : 0) +
-                     (viscosities ? 1 : 0);
+                     (viscosities ? 1 : 0) + (interfacial ? 1 : 0);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -702,7 +744,7 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities || viscosities ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities || viscosities || interfacial ? sizeof(tagged) : sizeof(fl));
         }
         if (with_bodies) {
             BodySection bs{};
@@ -758,6 +800,13 @@ void HybridFluid::save_state(const std::string &path) {
             tvs.count = (uint32_t)tag_viscosities_.size();
             for (uint32_t k = 0; k < tvs.count; ++k) tvs.entry[k] = tag_viscosities_[k];
             write_host_section(f, SEC_TAG_VISCOSITIES, &tvs, sizeof(tvs));
+        }
+        if (interfacial) {
+            InterfacialTensionSection its{};
+            its.tension = interfacial_tension_;
+            its.count = (uint32_t)interface_tags_.size();
+            for (uint32_t k = 0; k < its.count; ++k) its.tag[k] = interface_tags_[k];
+            write_host_section(f, SEC_INTERFACIAL_TENSION, &its, sizeof(its));
         }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
@@ -843,6 +892,7 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     if (set.has_surface_tension) x.set_surface_tension(set.surface_tension.surface_tension);
     if (set.has_densities) x.set_tag_densities(set.densities.entry, set.densities.count);
     if (set.has_viscosities) x.set_tag_viscosities(set.viscosities.entry, set.viscosities.count);
+    if (set.has_interfacial) x.set_interfacial_tension(set.interfacial.tag, set.interfacial.count, set.interfacial.tension);
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;
 }

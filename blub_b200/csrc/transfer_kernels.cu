@@ -1151,10 +1151,11 @@ __global__ void __launch_bounds__(PT) p2g_normalize_kernel(GridDim g, int wpr, c
 // warp-aggregated and tiled like the P2G scatter.
 template <bool MATCH>
 __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, const float3 p,
-                                                             long long *__restrict__ density, const TileWindow &win, uint32_t *__restrict__ tile) {
+                                                             long long *__restrict__ density, const TileWindow &win, uint32_t *__restrict__ tile,
+                                                             bool keep = true) {
     const uint32_t np = params->num_particles;
     if ((i & ~31u) >= np) return; // whole warp beyond the last particle
-    const bool valid = i < np;
+    const bool valid = i < np && keep; // a particle that is not kept still joins the warp's peer groups, with a key of its own
     const int dx = (int)(p.x - 0.5f), dy = (int)(p.y - 0.5f), dz = (int)(p.z - 0.5f);
     const float qx = (float)dx + 0.5f, qy = (float)dy + 0.5f, qz = (float)dz + 0.5f;
     const float wx[2] = {saturatef(1.0f - fabsf(qx - p.x)), saturatef(1.0f - fabsf(qx + 1.0f - p.x))};
@@ -1187,9 +1188,10 @@ __device__ __forceinline__ void density_scatter_kernel_one(uint32_t i, GridDim g
             }
     }
 }
-template <bool MATCH>
-__global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
-                                                             long long *__restrict__ density, ScatterSchedule sched) {
+// The whole scatter: the particles `keep(position)` accepts add their weights (every particle of the fused and unfiltered scatters)
+template <bool MATCH, class Keep>
+__device__ __forceinline__ void density_scatter_all(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
+                                                    long long *__restrict__ density, const ScatterSchedule &sched, Keep keep) {
     __shared__ __align__(16) uint32_t tile[2 * DENSITY_TILE]; // low words, high words
     __shared__ int scratch[PT / 32 + 1][8];
     __shared__ TileWindow shared_win;
@@ -1206,8 +1208,8 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
         __syncthreads();
         for (uint32_t k = w0 + warp; k < w1; k += PT / 32) { // warp-uniform
             const uint32_t i = 32u * sched.warps[k] + lane;
-            const float3 p = transfer_position(g, i < np_ ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
-            density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
+            const float4 q = i < np_ ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f);
+            density_scatter_kernel_one<MATCH>(i, g, params, transfer_position(g, q, 0.5f), density, win, tile, keep(q));
         }
         __syncthreads();
         for (int t = threadIdx.x; t < size; t += PT) { // flush, as in p2g_scatter_kernel
@@ -1221,19 +1223,45 @@ __global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const St
     for (uint32_t b = tail + blockIdx.x * PT; b < np_; b += gridDim.x * PT) { // block-uniform
         const uint32_t i = b + threadIdx.x;
         const bool valid = i < np_;
-        const float3 p = transfer_position(g, valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f), 0.5f);
+        const float4 q = valid ? pos[i] : make_float4(1.5f, 1.5f, 1.5f, 0.0f);
+        const float3 p = transfer_position(g, q, 0.5f);
         const int3 cell = make_int3(min((int)p.x, g.nx - 1), min((int)p.y, g.ny - 1), min((int)p.z, g.nz - 1));
         const TileWindow win = scatter_window<DENSITY_TILE>(b, np_, valid, cell, scratch, &shared_win);
         const int size = win.ex * win.ey * win.ez;
         tile_zero<2, DENSITY_TILE>(tile, size);
         __syncthreads();
-        density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile);
+        density_scatter_kernel_one<MATCH>(i, g, params, p, density, win, tile, keep(q));
         __syncthreads();
         for (int t = threadIdx.x; t < size; t += PT) {
             const long long q = tile_word(tile + t, tile + DENSITY_TILE + t);
             if (q != 0) fixed_add(density + tile_cell(g, win, t), q);
         }
     }
+}
+template <bool MATCH>
+__global__ void __launch_bounds__(PT) density_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
+                                                             long long *__restrict__ density, ScatterSchedule sched) {
+    density_scatter_all<MATCH>(g, params, pos, density, sched, [](const float4 &) { return true; });
+}
+// The interfacial tension's phase-B splat: only the particles whose tag (the fourth word's bits) is in the set add their weights.  The others
+// still take part in the windows and the warp's peer matching, but with a key of their own, so a kept particle's peer group holds only kept
+// particles: where both phases share a cell within a warp, the group sums (and their fixed-point roundings) differ from the all-particle
+// splat's.  The phase field takes any pair of splats (DESIGN.md §8 "Interfacial tension").
+template <bool MATCH>
+__global__ void __launch_bounds__(PT) phase_scatter_kernel(GridDim g, const StepParams *__restrict__ params, const float4 *__restrict__ pos,
+                                                           long long *__restrict__ density, ScatterSchedule sched,
+                                                           const InterfacialTensionBlock *__restrict__ blk) {
+    __shared__ uint32_t set[INTERFACE_TAGS_MAX];
+    const uint32_t count = blk->count;
+    if (threadIdx.x < INTERFACE_TAGS_MAX) set[threadIdx.x] = blk->tag[threadIdx.x];
+    __syncthreads();
+    density_scatter_all<MATCH>(g, params, pos, density, sched, [&](const float4 &q) {
+        const uint32_t t = __float_as_uint(q.w);
+        bool in = false;
+#pragma unroll
+        for (int k = 0; k < INTERFACE_TAGS_MAX; ++k) in |= k < (int)count && set[k] == t;
+        return in;
+    });
 }
 
 // Stage 7 with the density scatter of stage 9 fused in behind it (one GPU): every particle is advected by advect_kernel_one and its new
@@ -1502,6 +1530,14 @@ void launch_density_scatter(cudaStream_t st, const GridDim &g, const StepParams 
     if (np_upper == 0) return;
     const auto kernel = scatter_groups_by_match() ? density_scatter_kernel<true> : density_scatter_kernel<false>;
     BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, density, sched);
+}
+
+void launch_phase_scatter(cudaStream_t st, const GridDim &g, const StepParams *params, uint32_t np_upper, const float4 *pos, long long *density,
+                          const ScatterSchedule &sched, const InterfacialTensionBlock *blk) {
+    BLUB_CUDA_CHECK(cudaMemsetAsync(density, 0, (size_t)g.n * sizeof(long long), st));
+    if (np_upper == 0) return;
+    const auto kernel = scatter_groups_by_match() ? phase_scatter_kernel<true> : phase_scatter_kernel<false>;
+    BLUB_LAUNCH(kernel, particle_blocks(np_upper), PT, 0, st, g, params, pos, density, sched, blk);
 }
 
 void launch_density_finish(cudaStream_t st, const GridDim &g, const StepParams *params, const int8_t *marker, const long long *density, float *rhs) {

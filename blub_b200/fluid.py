@@ -29,6 +29,10 @@ TAP_CURVATURE, TAP_DENSITY = 12, 13
 TAP_CELL_DENSITY = 14
 # download only: the float32 kinematic cell viscosity of the last stage 0 on FLUID cells (zeros without a tag viscosity table)
 TAP_CELL_VISCOSITY = 15
+# download only: the float32 interface curvature of the last stage 1; the int64 phase field phi (a diagnostic whose contents may change, see
+# blub_fluid.h)
+TAP_INTERFACE_CURVATURE, TAP_INTERFACE_FIELD = 16, 17
+INTERFACE_TAGS_MAX = 16
 
 BLUB_OK = 0
 BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
@@ -441,6 +445,9 @@ def lib():
         "blub_fluid_set_surface_tension": (C.c_int, [vp, C.c_float]),
         "blub_fluid_surface_tension": (C.c_int, [vp, C.POINTER(C.c_float)]),
         "blub_scene_surface_tension": (C.c_int, [C.c_char_p, C.POINTER(C.c_float)]),
+        "blub_fluid_set_interfacial_tension": (C.c_int, [vp, C.POINTER(C.c_uint32), C.c_uint32, C.c_float]),
+        "blub_fluid_interfacial_tension": (C.c_int, [vp, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_float)]),
+        "blub_scene_interfacial_tension": (C.c_int, [C.c_char_p, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_float)]),
         "blub_fluid_set_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32]),
         "blub_fluid_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
         "blub_scene_tag_densities": (C.c_int, [C.c_char_p, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
@@ -622,6 +629,15 @@ def scene_surface_tension(path):
     out = C.c_float(0)
     _check(lib().blub_scene_surface_tension(os.fsencode(path), C.byref(out)))
     return float(out.value)
+
+
+def scene_interfacial_tension(path):
+    """The scene's fluid.interfacial_tension as (tension in cells^3/s^2, [tags]): m^3/s^2 / grid_to_world_scale^3, (0.0, []) without the key
+    (host only)."""
+    count, out = C.c_uint32(0), C.c_float(0)
+    arr = (C.c_uint32 * INTERFACE_TAGS_MAX)()
+    _check(lib().blub_scene_interfacial_tension(os.fsencode(path), arr, INTERFACE_TAGS_MAX, C.byref(count), C.byref(out)))
+    return float(out.value), [int(t) for t in arr[:count.value]]
 
 
 def scene_tag_densities(path):
@@ -824,7 +840,7 @@ class HybridFluid:
 
     # -- taps ---------------------------------------------------------------------------------
     def download_grid(self, tap):
-        dt = np.int8 if tap == TAP_MARKER else np.int64 if tap == TAP_DENSITY else np.float32
+        dt = np.int8 if tap == TAP_MARKER else np.int64 if tap in (TAP_DENSITY, TAP_INTERFACE_FIELD) else np.float32
         out = np.empty((self.nz, self.ny, self.nx), dtype=dt)
         _check(self.L.blub_fluid_download(self.h, tap, out.ctypes.data_as(C.c_void_p), out.nbytes))
         return out
@@ -966,6 +982,24 @@ class HybridFluid:
         out = C.c_float(0)
         _check(self.L.blub_fluid_surface_tension(self.h, C.byref(out)))
         return float(out.value)
+
+    # -- interfacial tension -------------------------------------------------------------------
+    def set_interfacial_tension(self, sigma, tags=()):
+        """Kinematic interfacial tension sigma_AB / density in cells^3/s^2 (m^3/s^2 / grid_to_world_scale^3; oil on water: about 3e-5
+        m^3/s^2) between phase B, the particles whose tag is in `tags` (at most 16), and the rest of the liquid; 0 turns it off.  Every step
+        then applies the pressure jump P_B - P_A = sigma_AB kappa across their interface, and plan_substep / advance respect the capillary step
+        limit.  Raises BlubError (and changes nothing) on a negative or non-finite value, more than 16 tags, a tag listed twice, a value above
+        0 without tags, z-slab ranks and a fluid inside a step."""
+        tags = [int(t) for t in tags]
+        arr = (C.c_uint32 * max(len(tags), 1))(*tags)
+        _check(self.L.blub_fluid_set_interfacial_tension(self.h, arr, len(tags), float(sigma)))
+
+    def interfacial_tension(self):
+        """(kinematic interfacial tension in cells^3/s^2, [phase B's tags]) ((0.0, []): off)."""
+        count, out = C.c_uint32(0), C.c_float(0)
+        arr = (C.c_uint32 * INTERFACE_TAGS_MAX)()
+        _check(self.L.blub_fluid_interfacial_tension(self.h, arr, INTERFACE_TAGS_MAX, C.byref(count), C.byref(out)))
+        return float(out.value), [int(t) for t in arr[:count.value]]
 
     # -- liquids of different densities -------------------------------------------------------
     def set_tag_densities(self, table):

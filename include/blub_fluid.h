@@ -410,6 +410,30 @@ int blub_fluid_surface_tension(const BlubFluid *fluid, float *cells3_per_s2);
  * sets it on the fluid it creates.  A value that is not a number, negative or not finite makes every scene call fail with BLUB_ERR_PARSE. */
 int blub_scene_surface_tension(const char *scene_json_path, float *cells3_per_s2);
 
+/* ---- interfacial tension (not part of the reference surface; rules: DESIGN.md section 8 "Interfacial tension") ---------------------
+ * A kinematic interfacial tension s_AB = sigma_AB / rho_ref (cells^3/s^2: m^3/s^2 divided by grid_to_world_scale^3; oil on water is about
+ * 3e-5 m^3/s^2) between two phases of the liquid: phase B, the particles whose tag is in a set of at most 16 tags, and phase A, every other
+ * particle.  The interface carries P_B - P_A = sigma_AB kappa, kappa = div n with n pointing from B into A (+2/R for a drop of B).  Stage 1
+ * of every step splats all particles and the phase-B particles, smooths 2 splat_B - splat_all in integer arithmetic (bit-reproducible) into a
+ * phase field phi (> 0: phase B), measures the curvature on the FLUID cells next to a FLUID cell of the other phase and moves the velocity
+ * solve's right-hand side by the ghost values g = -dt s_AB (kappa_i + kappa_j) / 2 of those faces, times the face coefficient of a tag
+ * density table; stage 4 adds them to the faces.  The matrix is unchanged.  It is independent of the free surface's tension and works with
+ * and without a tag density table.  Walls are neutrally wetting.  While s_AB > 0 blub_fluid_plan_substep holds every substep to the
+ * capillary limit of max(surface tension, s_AB).  The tension and the tags are part of the saved state (format version 512). */
+#define BLUB_INTERFACE_TAGS_MAX 16
+/* Sets s_AB and phase B's tags; s_AB = 0 turns it off (the set is then ignored and may be empty), and the step is then the step of a fluid
+ * that never had an interfacial tension.  Stream-ordered; turning it on or off drops the cached step graphs, a change between two settings
+ * above zero does not.  BLUB_ERR_INVALID_ARGUMENT, changing nothing: a negative or non-finite value, more than 16 tags, a tag listed twice, a
+ * NULL set with count > 0, a value above 0 with an empty set, a z-slab rank, or a fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_interfacial_tension(BlubFluid *fluid, const uint32_t *tags, uint32_t count, float cells3_per_s2);
+/* the current setting: s_AB into *cells3_per_s2 (0: off), min(count, capacity) tags into tags (may be NULL with capacity 0), their number
+ * into *count */
+int blub_fluid_interfacial_tension(const BlubFluid *fluid, uint32_t *tags, uint32_t capacity, uint32_t *count, float *cells3_per_s2);
+/* The scene's optional fluid.interfacial_tension, {"tags": [n, ...], "tension": m^3/s^2}, the tension divided by grid_to_world_scale^3 (0
+ * and no tags without the key).  blub_scene_load sets it on the fluid it creates.  A value the setter would refuse makes every scene call
+ * fail with BLUB_ERR_PARSE. */
+int blub_scene_interfacial_tension(const char *scene_json_path, uint32_t *tags, uint32_t capacity, uint32_t *count, float *cells3_per_s2);
+
 /* ---- liquids of different densities (not part of the reference surface; rules: DESIGN.md section 8 "Liquids of different densities") ----
  * A table gives the particles of a tag a density relative to the reference density rho_ref that the velocity solve's pressure p dt / rho_ref,
  * the bodies' relative densities, the load probes' forces, the viscosity and the surface tension are all defined against.  Tags not in the
@@ -665,8 +689,16 @@ enum {
                                    implementation; it exists so that tests can restate stage 1 bit for bit (download only) */
     BLUB_TAP_CELL_DENSITY = 14, /* float per cell: the relative density rho_i of the last stage 0 on FLUID cells, 0 elsewhere; zeros while no
                                    tag density table is set (download only) */
-    BLUB_TAP_CELL_VISCOSITY = 15 /* float per cell: the kinematic viscosity nu_i (cells^2/s) of the last stage 0 on FLUID cells, 0 elsewhere;
+    BLUB_TAP_CELL_VISCOSITY = 15, /* float per cell: the kinematic viscosity nu_i (cells^2/s) of the last stage 0 on FLUID cells, 0 elsewhere;
                                     zeros while no tag viscosity table is set (download only) */
+    BLUB_TAP_INTERFACE_CURVATURE = 16, /* float per cell: the interface's curvature (cells^-1) of the last stage 1 on the FLUID cells next to
+                                          a FLUID cell of the other phase, 0 elsewhere; zeros while the interfacial tension is off (download
+                                          only) */
+    BLUB_TAP_INTERFACE_FIELD = 17      /* DIAGNOSTIC, not a stable interface: int64 per cell, the smoothed phase field phi (2^-32 particle
+                                          weights, > 0 in phase B) of the last stage 1, valid within 2 cells of FLUID; elsewhere whatever an
+                                          earlier step left.  Zeros while the interfacial tension is off.  Its contents and layout may change
+                                          with the step's implementation; it exists so that tests can restate stage 1 bit for bit (download
+                                          only) */
 };
 /* synchronous copies between host memory and the tapped array (bytes must not exceed the array) */
 int blub_fluid_download(BlubFluid *fluid, int tap, void *host_dst, size_t bytes);

@@ -21,31 +21,12 @@ namespace {
 static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the state file is little-endian and written as the host lays it out");
 
 constexpr char kMagic[8] = {'B', 'L', 'U', 'B', 'S', 'T', 'A', 'T'};
-// version 1: a fluid without sources or drains, 13 sections; version 2: the same plus section 14, the flow set and its counters; version 4:
-// section 14 followed by the sources' particle tags (written only when one of them is not 0).  Version 3 is not a format: no build writes
-// it and readers refuse it.  Version 8: a fluid with floating bodies; the version-4 layout (section 14 may describe an empty flow set) plus
-// section 15, the bodies.  Versions 3, 5, 6 and 7 are not formats either.  Version 16: a fluid with at least one mesh body; the version-8
-// layout plus section 16, the mesh bodies' geometry and mass properties (its length is what the file holds beyond section 15).  Version 32: a
-// fluid with viscosity; the layout it would otherwise have, promoted to 13 sections, or 14 (section 14 in its version-4 form, possibly an empty
-// set), 15 or 16, plus a last section 17, the viscosity setting: num_sections (14 to 17) tells which.  Versions 17 to 31 are not formats.
-// Version 64: a fluid with surface tension; the layout it would otherwise have (13 to 16 base sections as in version 32, then section 17 when
-// it is viscous) plus a last section 18, the setting.  The header cannot tell 13 + 17 + 18 from 14 + 18 apart: the reader walks the section
-// heads (their stored lengths) after section 13 and finds section 17 by its id.  Versions 33 to 63 are not formats.
-// Version 128: a fluid with a tag density table (liquids of different densities, never together with surface tension); the layout it would
-// otherwise have (13 to 16 base sections, then section 17 when it is viscous) plus a last section 19, the table.  Section 17 is found as in
-// version 64.  Versions 65 to 127 are not formats.
-// Version 256: a fluid with a tag viscosity table (liquids of different viscosities); the 13 to 16 base sections as in version 32, then
-// section 17 always (its kinematic_viscosity may be 0: the tags not in the table are inviscid), section 18 when the surface tension is
-// above 0, section 19 when a tag density table is set, and a last section 20, the table.  The reader finds 17, 18 and 19 by walking the
-// section heads as for versions 64 and 128.  Versions 129 to 255 are not formats.
-// Version 512: a fluid with an interfacial tension; the layout it would otherwise have (versions 1 to 256: 13 to 16 base sections, then the
-// setting sections 17 to 20 it has) plus a last section 21, the tension and phase B's tags.  The reader finds 17 to 20 by walking the section
-// heads as for versions 64, 128 and 256, and refuses a version-512 file whose walk does not reach a section 21.  Section 17 may hold a
-// viscosity of 0 only together with section 20, as in version 256.  Versions 257 to 511 are not formats.
-constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4, kFormatVersionBodies = 8, kFormatVersionMeshBodies = 16, kFormatVersionViscosity = 32,
-                   kFormatVersionSurfaceTension = 64, kFormatVersionTagDensities = 128, kFormatVersionTagViscosities = 256,
-                   kFormatVersionInterfacialTension = 512;
-constexpr uint32_t kNumSections = 21; // at most
+// The layout rule (DESIGN.md §8): a header, sections 1 to 13 at the lengths the header implies, then a strictly ascending selection of the
+// optional sections 14 to 21 of kOptional.  Section 15 needs 14 and 16 needs 15, so num_sections, which counts every section, tells how many of
+// 14, 15 and 16 a file holds; the sections from 17 on are found by their ids.  format_version is the largest version that introduced one of the
+// file's sections, or 1 when it has none; section 14 counts as version 4 when a source tag is not 0, and it is 992 bytes long in a version-2
+// file only.  Every other version number is not a format.  The rules between sections are checked with the payloads.
+constexpr uint32_t kFormatVersionFlow = 2, kFormatVersionSourceTags = 4;
 constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while the other one is copied
 
 enum : uint32_t {
@@ -148,45 +129,40 @@ struct Section {
     uint64_t length;
 };
 
-// The setting sections (17 to 20) that follow the base sections, as a mask of bits 1 << id.  Version 32: 17.  Versions 64, 128 and 256: what
-// the section heads say (settings_in_file), with the sections every file of the version holds: 18 (64), 19 (128), 17 and 20 (256).
+// The optional sections in id order: the format version that introduced each one and its payload length.
+struct OptionalSection {
+    uint32_t id, version;
+    uint64_t length; // section 14: in every version but 2 (fixed_length); section 16: 0, its length is what the file holds beyond the others
+    const char *name;
+};
+constexpr OptionalSection kOptional[] = {
+    {SEC_FLOW, kFormatVersionFlow, sizeof(FlowSectionTagged), "the flow set"},
+    {SEC_BODIES, 8, sizeof(BodySection), "the bodies"},
+    {SEC_MESH_BODIES, 16, 0, "the mesh bodies"},
+    {SEC_VISCOSITY, 32, sizeof(BlubViscosity), "the viscosity"},
+    {SEC_SURFACE_TENSION, 64, sizeof(SurfaceTensionSection), "the surface tension"},
+    {SEC_TAG_DENSITIES, 128, sizeof(TagDensitySection), "the tag densities"},
+    {SEC_TAG_VISCOSITIES, 256, sizeof(TagViscositySection), "the tag viscosities"},
+    {SEC_INTERFACIAL_TENSION, 512, sizeof(InterfacialTensionSection), "the interfacial tension"},
+};
+constexpr uint32_t kLastSection = SEC_INTERFACIAL_TENSION;
+static_assert(sizeof(kOptional) / sizeof(kOptional[0]) == kLastSection - SEC_FLOW + 1, "one row per optional section");
+const OptionalSection &optional_section(uint32_t id) { return kOptional[id - SEC_FLOW]; }
+
 constexpr uint32_t bit(uint32_t id) { return 1u << id; }
-// the versions whose base sections are followed by setting sections the header does not tell apart
-bool walks_settings(const StateHeader &h) {
-    return h.format_version == kFormatVersionSurfaceTension || h.format_version == kFormatVersionTagDensities || h.format_version == kFormatVersionTagViscosities ||
-           h.format_version == kFormatVersionInterfacialTension;
+
+// The payload length of a section the rule fixes: sections 14, 15 and 17 to 21.
+uint64_t fixed_length(uint32_t id, uint32_t version) {
+    return id == SEC_FLOW && version == kFormatVersionFlow ? sizeof(FlowSection) : optional_section(id).length;
 }
-uint32_t base_sections(const StateHeader &h, uint32_t settings) {
-    if (h.format_version == kFormatVersionViscosity) return h.num_sections >= 14 && h.num_sections <= 17 ? h.num_sections - 1 : 0;
-    if (walks_settings(h)) {
-        const uint32_t extra = (uint32_t)__builtin_popcount(settings);
-        return h.num_sections >= 13 + extra && h.num_sections <= 16 + extra ? h.num_sections - extra : 0;
-    }
-    return h.format_version == kFormatVersionMeshBodies ? 16 : h.format_version == kFormatVersionBodies ? 15 : h.format_version >= kFormatVersionFlow ? 14 : 13;
+
+// The format version of a file with the sections `sections` (bits 1 << id); source_tags: section 14 holds a source tag that is not 0.
+uint32_t format_version_of(uint32_t sections, bool source_tags) {
+    uint32_t v = 1;
+    for (const OptionalSection &s : kOptional)
+        if (sections & bit(s.id)) v = std::max(v, s.id == SEC_FLOW && source_tags ? kFormatVersionSourceTags : s.version);
+    return v;
 }
-// The sections of a file in their order, with the lengths its header implies; returns their number (0: a header whose num_sections names no
-// layout).  The base sections come first, base_sections() of them, then the setting sections of `settings` in the order 17, 18, 19, 20.
-uint32_t expected_sections(const StateHeader &h, Section out[kNumSections], uint32_t settings) {
-    const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
-    const Section s[kNumSections] = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
-                                     {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
-                                     {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
-                                     {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]},
-                                     {SEC_FLOW, h.format_version >= kFormatVersionSourceTags ? sizeof(FlowSectionTagged) : sizeof(FlowSection)},
-                                     {SEC_BODIES, sizeof(BodySection)}, {SEC_MESH_BODIES, 0}, // section 16: the file's bytes beyond the others
-                                     {SEC_VISCOSITY, sizeof(BlubViscosity)}, {SEC_SURFACE_TENSION, sizeof(SurfaceTensionSection)},
-                                     {SEC_TAG_DENSITIES, sizeof(TagDensitySection)}, {SEC_TAG_VISCOSITIES, sizeof(TagViscositySection)},
-                                     {SEC_INTERFACIAL_TENSION, sizeof(InterfacialTensionSection)}};
-    std::memcpy(out, s, sizeof(s));
-    const uint32_t nb = base_sections(h, settings);
-    if (nb == 0) return 0;
-    uint32_t ns = nb;
-    for (uint32_t id = SEC_VISCOSITY; id <= SEC_INTERFACIAL_TENSION; ++id)
-        if (settings & bit(id)) out[ns++] = s[id - 1];
-    return ns;
-}
-// whether the file has a viscosity section
-bool has_viscosity_section(uint32_t settings) { return (settings & bit(SEC_VISCOSITY)) != 0; }
 
 uint32_t crc_of(const void *p, size_t n, uint32_t crc = 0) { return (uint32_t)crc32_z(crc, static_cast<const Bytef *>(p), n); }
 
@@ -223,41 +199,6 @@ struct File {
     }
 };
 
-// The setting sections of a file (see base_sections).  Versions 64, 128 and 256: the ids 17 to 19 found among the sections after section 13 by
-// walking their heads with their stored lengths (at most seven of them before the last section, 18, 19, 20 or 21), plus the sections the version
-// always holds.  Leaves `f` where it was.  The lengths are checked later, section by section.
-uint32_t settings_in_file(File &f, const StateHeader &h) {
-    if (h.format_version == kFormatVersionViscosity) return bit(SEC_VISCOSITY);
-    if (!walks_settings(h)) return 0u;
-    const uint32_t last = h.format_version == kFormatVersionSurfaceTension ? SEC_SURFACE_TENSION
-                          : h.format_version == kFormatVersionTagDensities ? SEC_TAG_DENSITIES
-                          : h.format_version == kFormatVersionTagViscosities ? SEC_TAG_VISCOSITIES : SEC_INTERFACIAL_TENSION;
-    // what the walk may find: 17 in versions 64 and 128, 18 and 19 in version 256 (17 is always there), 17 to 20 in version 512
-    const uint32_t optional = last == SEC_INTERFACIAL_TENSION ? bit(SEC_VISCOSITY) | bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) | bit(SEC_TAG_VISCOSITIES)
-                              : last == SEC_TAG_VISCOSITIES ? bit(SEC_SURFACE_TENSION) | bit(SEC_TAG_DENSITIES) : bit(SEC_VISCOSITY);
-    uint32_t settings = bit(last) | (last == SEC_TAG_VISCOSITIES ? bit(SEC_VISCOSITY) : 0u);
-    bool found_last = false;
-    const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
-    const uint64_t base[13] = {np, np, np, np, 4 * n, 4 * n, 4 * n, n, 4 * n, 4 * n, 2 * sizeof(PcgScalars), 8ull * h.num_stats[0], 8ull * h.num_stats[1]};
-    const uint64_t here = f.tell(), size = f.size();
-    uint64_t at = here;
-    for (uint64_t len : base) at += sizeof(SectionHead) + len + 4;
-    for (int k = 0; k < 8 && at + sizeof(SectionHead) <= size; ++k) {
-        SectionHead head;
-        f.seek(at);
-        f.read(&head, sizeof(head));
-        if (head.id >= SEC_VISCOSITY && head.id < 32 && (optional & bit(head.id))) settings |= bit(head.id);
-        if (head.id == last) found_last = true;
-        if (head.id == last || head.length > size) break;
-        at += sizeof(SectionHead) + head.length + 4;
-    }
-    f.seek(here);
-    // a version-512 header over a layout without the interfacial tension (a version-256 file relabelled, say) is not a version-512 file
-    if (last == SEC_INTERFACIAL_TENSION && !found_last)
-        throw ParseError(f.path + ": format version 512 ends with section 21 (the interfacial tension), the file has none");
-    return settings;
-}
-
 // Staging memory of the array sections: pinned halves with an event each when the arrays come from / go to the device, plain host memory
 // for the host-only reader.
 struct Staging {
@@ -289,20 +230,22 @@ struct Staging {
     }
 };
 
-// Header checks: everything a reader needs to trust before it allocates anything.  Leaves `f` at the first section.  settings: the setting
-// sections the file holds (settings_in_file).
-StateHeader read_header(File &f, uint32_t &settings) {
+// Header checks: everything a reader needs to trust before it walks the sections.  Leaves `f` at the first section.
+StateHeader read_header(File &f) {
     StateHeader h;
     const uint64_t size = f.size();
     if (size < sizeof(StateHeader)) throw ParseError(f.path + ": truncated state file (" + std::to_string(size) + " bytes)");
     f.read(&h, sizeof(h));
     if (std::memcmp(h.magic, kMagic, sizeof(kMagic)) != 0) throw ParseError(f.path + ": not a blub state file (bad magic)");
-    if (h.format_version != 1 && h.format_version != kFormatVersionFlow && h.format_version != kFormatVersionSourceTags &&
-        h.format_version != kFormatVersionBodies && h.format_version != kFormatVersionMeshBodies && h.format_version != kFormatVersionViscosity &&
-        h.format_version != kFormatVersionSurfaceTension && h.format_version != kFormatVersionTagDensities &&
-        h.format_version != kFormatVersionTagViscosities && h.format_version != kFormatVersionInterfacialTension)
-        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) +
-                         " is not supported (this library reads versions 1, 2, 4, 8, 16, 32, 64, 128, 256 and 512)");
+    std::string versions = "1";
+    bool known = h.format_version == 1 || h.format_version == kFormatVersionSourceTags;
+    for (const OptionalSection &s : kOptional) {
+        versions += (s.id == kLastSection ? " and " : ", ") + std::to_string(s.version) + (s.id == SEC_FLOW ? ", 4" : "");
+        known = known || h.format_version == s.version;
+    }
+    if (!known)
+        throw ParseError(f.path + ": state format version " + std::to_string(h.format_version) + " is not supported (this library reads versions " +
+                         versions + ")");
     if (crc_of(&h, offsetof(StateHeader, header_crc)) != h.header_crc) throw ParseError(f.path + ": header checksum mismatch");
     const uint32_t *d = h.grid_dimension;
     if (d[0] == 0 || d[1] == 0 || d[2] == 0 || d[0] % 8 || d[1] % 8 || d[2] % 8)
@@ -316,33 +259,70 @@ StateHeader read_header(File &f, uint32_t &settings) {
         throw ParseError(f.path + ": precond_mode, transfer path or graph replay flag out of range");
     const uint32_t sp = h.solver_path;
     if (sp > 6 || sp == 3 || sp == 5 || (sp == 2 && d[0] % 128)) throw ParseError(f.path + ": solver path out of range");
-    settings = settings_in_file(f, h);
-    Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, settings);
-    const uint32_t extra = (uint32_t)__builtin_popcount(settings);
-    if (h.num_sections != ns)
-        throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(h.format_version) + " has " +
-                         (ns ? std::to_string(ns) : std::to_string(13 + extra) + " to " + std::to_string(16 + extra)));
-    uint64_t total = sizeof(StateHeader);
-    for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4;
-    // version 16: section 16 holds at least its count and one mesh body record
-    if (base_sections(h, settings) == 16 ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
-        throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
     return h;
+}
+
+// The sections of the file in their order with the lengths the rule gives them, checked against the header and the file size before anything
+// is allocated.  Sections 1 to 13 take the lengths the header implies.  The walk then reads the heads after section 13 in ascending-id order and
+// ends at the first one that is not a later section the format version may hold.  It advances over each section by the rule's length, over
+// section 16 by its stored one, so a wrong stored length of another section is reported as that section's length error and does not end the
+// walk early.  The sections from 17 on are the walk's; num_sections tells how many of 14, 15 and 16 precede them.  Leaves `f` at the first
+// section.
+std::vector<Section> layout_of(File &f, const StateHeader &h) {
+    const uint32_t v = h.format_version;
+    const uint64_t np = (uint64_t)h.num_particles * 16, n = (uint64_t)h.grid_dimension[0] * h.grid_dimension[1] * h.grid_dimension[2];
+    std::vector<Section> sec = {{SEC_POSITIONS, np}, {SEC_VELOCITY_X, np}, {SEC_VELOCITY_Y, np}, {SEC_VELOCITY_Z, np},
+                                {SEC_GRID_VELOCITY_X, 4 * n}, {SEC_GRID_VELOCITY_Y, 4 * n}, {SEC_GRID_VELOCITY_Z, 4 * n}, {SEC_MARKER, n},
+                                {SEC_PRESSURE_VELOCITY, 4 * n}, {SEC_PRESSURE_DENSITY, 4 * n}, {SEC_SOLVER_SCALARS, 2 * sizeof(PcgScalars)},
+                                {SEC_STATS_VELOCITY, 8ull * h.num_stats[0]}, {SEC_STATS_DENSITY, 8ull * h.num_stats[1]}};
+    const uint64_t first = f.tell(), size = f.size();
+    uint64_t at = first;
+    for (const Section &s : sec) at += sizeof(SectionHead) + s.length + 4;
+    std::vector<Section> settings;
+    for (uint32_t last = SEC_STATS_DENSITY; at + sizeof(SectionHead) <= size;) {
+        SectionHead head;
+        f.seek(at);
+        f.read(&head, sizeof(head));
+        if (head.id <= last || head.id > kLastSection || optional_section(head.id).version > v) break;
+        // 18 and 19 never go together: a version-128 file has no section 18, and in later versions the check of section 19 refuses the pair
+        if (head.id == SEC_SURFACE_TENSION && v == optional_section(SEC_TAG_DENSITIES).version) break;
+        const uint64_t length = head.id == SEC_MESH_BODIES ? head.length : fixed_length(head.id, v);
+        if (length > size - at) break;
+        if (head.id >= SEC_VISCOSITY) settings.push_back({head.id, length});
+        last = head.id;
+        at += sizeof(SectionHead) + length + 4;
+    }
+    f.seek(first);
+    // of 14, 15 and 16 the file holds those up to the last one its version may hold, or, in a version that introduced a setting section, fewer
+    uint32_t hi = SEC_STATS_DENSITY;
+    while (hi < SEC_MESH_BODIES && optional_section(hi + 1).version <= v) ++hi;
+    const uint32_t lo = v >= optional_section(SEC_VISCOSITY).version ? SEC_STATS_DENSITY : hi, extra = (uint32_t)settings.size();
+    if (h.num_sections < lo + extra || h.num_sections > hi + extra)
+        throw ParseError(f.path + ": " + std::to_string(h.num_sections) + " sections, format version " + std::to_string(v) + " has " +
+                         std::to_string(lo + extra) + (lo == hi ? "" : " to " + std::to_string(hi + extra)));
+    const uint32_t base = h.num_sections - extra;
+    for (uint32_t id = SEC_FLOW; id <= base; ++id) sec.push_back({id, id == SEC_MESH_BODIES ? 0 : fixed_length(id, v)});
+    sec.insert(sec.end(), settings.begin(), settings.end());
+    uint64_t total = sizeof(StateHeader);
+    for (const Section &s : sec) total += sizeof(SectionHead) + s.length + 4;
+    // section 16 holds at least its count and one mesh body record
+    if (base == SEC_MESH_BODIES ? size < total + 8 + sizeof(MeshBodyRecordHead) : size != total)
+        throw ParseError(f.path + ": the file has " + std::to_string(size) + " bytes, its header describes " + std::to_string(total));
+    if (base == SEC_MESH_BODIES) sec[SEC_MESH_BODIES - 1].length = size - total;
+    // the walk took no section newer than the version and the count placed 14, 15 and 16: only the version's own setting section can be
+    // missing (section 14 of a version-4 file counts as version 4)
+    uint32_t ids = 0;
+    for (const Section &s : sec) ids |= bit(s.id);
+    if (format_version_of(ids, v == kFormatVersionSourceTags) != v) {
+        const OptionalSection &own = *std::find_if(std::begin(kOptional), std::end(kOptional), [&](const OptionalSection &s) { return s.version == v; });
+        throw ParseError(f.path + ": format version " + std::to_string(v) + " ends with section " + std::to_string(own.id) + " (" + own.name +
+                         "), the file has none");
+    }
+    return sec;
 }
 
 // Reads one section whose id and length must be `s`, in chunks of at most one staging half; sink(slot, data, bytes, offset) receives
 // every chunk (it must be done with the half `slot` before that half's event is waited on again), then the CRC is checked.
-// the length of section 16 when the file has one: what the file holds beyond section 15, its head and its CRC
-uint64_t mesh_section_length(File &f, const StateHeader &h, uint32_t settings) {
-    if (base_sections(h, settings) != 16) return 0;
-    Section sec[kNumSections];
-    const uint32_t ns = expected_sections(h, sec, settings);
-    uint64_t total = sizeof(StateHeader);
-    for (uint32_t k = 0; k < ns; ++k) total += sizeof(SectionHead) + sec[k].length + 4; // section 16 counted empty
-    return f.size() - total;
-}
-
 template <class Sink> void read_section(File &f, const Section &s, Staging &st, Sink sink) {
     SectionHead head;
     f.read(&head, sizeof(head));
@@ -396,9 +376,9 @@ void write_host_section(File &f, uint32_t id, const void *src, uint64_t bytes) {
 }
 
 // The flow set of section 14, checked with the rules of set_flow: the corners must be what clamping them again gives.  tags: the sources'
-// particle tags (version 4), or nullptr.  Versions 8, 16 and 32 may describe an empty set.
+// particle tags (version 4), or nullptr.  From version 8 on it may describe an empty set.
 FlowSet flow_set_of(const FlowSection &fl, const uint32_t *tags, const StateHeader &h, const std::string &path) {
-    if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version < kFormatVersionBodies))
+    if (fl.num_sources > 16 || fl.num_drains > 16 || (fl.num_sources + fl.num_drains == 0 && h.format_version < optional_section(SEC_BODIES).version))
         throw ParseError(path + ": section 14 must hold at most 16 boxes of each kind and at least one box");
     std::vector<BlubFluidSource> src(fl.num_sources);
     std::vector<BlubFluidDrain> drn(fl.num_drains);
@@ -525,15 +505,15 @@ std::vector<BlubBody> mesh_body_set_of(const BodySection &bs, const std::vector<
     return set;
 }
 
-// The setting of section 17, checked with the rules of set_viscosity; below version 256 it holds a viscosity above 0 (a version-256 file's
-// may hold 0: the tags not in its table are inviscid; so may a version-512 file's that has a section 20).
-BlubViscosity viscosity_of(const BlubViscosity &v, const StateHeader &h, uint32_t settings, const std::string &path) {
+// The setting of section 17, checked with the rules of set_viscosity; it holds a viscosity above 0 unless the file has a section 20 (the tags
+// not in that table are inviscid).  sections: the file's section ids, bits 1 << id.
+BlubViscosity viscosity_of(const BlubViscosity &v, uint32_t sections, const std::string &path) {
     try {
         check_viscosity(v);
     } catch (const std::invalid_argument &e) {
         throw ParseError(path + ": section 17: " + e.what());
     }
-    if (!(settings & bit(SEC_TAG_VISCOSITIES)) && !(v.kinematic_viscosity > 0.0f))
+    if (!(sections & bit(SEC_TAG_VISCOSITIES)) && !(v.kinematic_viscosity > 0.0f))
         throw ParseError(path + ": section 17: without a section 20 section 17 holds a viscosity above 0");
     return v;
 }
@@ -545,11 +525,11 @@ float surface_tension_of(const SurfaceTensionSection &s, const std::string &path
     return s.surface_tension;
 }
 
-// The table of section 19, checked with the rules of set_tag_densities; a version-128 file has a table, precond_mode 0 and no floating bodies.
-std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const StateHeader &h, uint32_t settings, const std::string &path) {
+// The table of section 19, checked with the rules of set_tag_densities: precond_mode 0, no surface tension and no floating bodies.
+std::vector<BlubTagDensity> tag_densities_of(const TagDensitySection &s, const StateHeader &h, uint32_t sections, const std::string &path) {
     if (h.precond_mode != 0) throw ParseError(path + ": section 19: a tag density table needs precond_mode 0");
-    if (settings & bit(SEC_SURFACE_TENSION)) throw ParseError(path + ": section 19: a tag density table is not supported with surface tension");
-    if (base_sections(h, settings) >= 15) throw ParseError(path + ": section 19: a tag density table is not supported with floating bodies");
+    if (sections & bit(SEC_SURFACE_TENSION)) throw ParseError(path + ": section 19: a tag density table is not supported with surface tension");
+    if (sections & bit(SEC_BODIES)) throw ParseError(path + ": section 19: a tag density table is not supported with floating bodies");
     if (s.count == 0 || s.count > 16) throw ParseError(path + ": section 19 must hold 1 to 16 entries");
     if (s.reserved != 0u) throw ParseError(path + ": section 19: reserved must be 0");
     try {
@@ -591,71 +571,93 @@ void interfacial_tension_of(const InterfacialTensionSection &s, const std::strin
         if (s.tag[k] != 0u) throw ParseError(path + ": section 21: the unused entries must be zero");
 }
 
-// The setting sections after the base sections, read in their order: read(section, destination) fills a host struct.
-struct Settings {
-    bool has_viscosity = false, has_surface_tension = false, has_densities = false, has_viscosities = false, has_interfacial = false;
+// What a state file holds besides its header and its ten arrays, checked with the setters' rules.
+struct StateContents {
+    uint32_t sections = 0; // the file's section ids, bits 1 << id
+    PcgScalars scalars[2];
+    std::vector<SolverStatisticSample> stats[2];
+    FlowSet flow{};
+    uint64_t flow_counters[3] = {0, 0, 0};
+    std::vector<BlubBody> bodies;
+    std::vector<MeshBodyHost> meshes;
     BlubViscosity viscosity{};
     SurfaceTensionSection surface_tension{};
     TagDensitySection densities{};
     TagViscositySection viscosities{};
     InterfacialTensionSection interfacial{};
 };
-template <class Read> Settings read_settings(const StateHeader &h, uint32_t settings, const Section *sec, uint32_t next, const std::string &path, Read read) {
-    Settings out;
-    if ((out.has_viscosity = has_viscosity_section(settings))) {
-        read(sec[next++], &out.viscosity);
-        out.viscosity = viscosity_of(out.viscosity, h, settings, path);
+
+// Reads the sections of `layout` (layout_of) in their order, `f` at the first one.  The ten array sections go to
+// to_array(id, slot, data, bytes, offset), which is read_section's sink with the section id in front; the others are checked and returned.
+template <class ArraySink>
+StateContents read_sections(File &f, const StateHeader &h, const std::vector<Section> &layout, Staging &st, ArraySink to_array) {
+    StateContents c;
+    for (const Section &s : layout) c.sections |= bit(s.id);
+    auto to_host = [&](const Section &s, void *dst) {
+        read_section(f, s, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(static_cast<char *>(dst) + off, data, n); });
+    };
+    FlowSectionTagged fl{};
+    BodySection bs{};
+    std::vector<char> mesh_bytes;
+    for (const Section &s : layout) {
+        switch (s.id) {
+        case SEC_SOLVER_SCALARS: to_host(s, c.scalars); break;
+        case SEC_STATS_VELOCITY:
+        case SEC_STATS_DENSITY: {
+            std::vector<SolverStatisticSample> &stats = c.stats[s.id - SEC_STATS_VELOCITY];
+            stats.resize(s.length / sizeof(SolverStatisticSample));
+            to_host(s, stats.data());
+            break;
+        }
+        case SEC_FLOW:
+            to_host(s, &fl);
+            c.flow = flow_set_of(fl.flow, fl.source_tags, h, f.path);
+            std::memcpy(c.flow_counters, fl.flow.counters, sizeof(c.flow_counters));
+            break;
+        case SEC_BODIES:
+            to_host(s, &bs);
+            if (!(c.sections & bit(SEC_MESH_BODIES))) c.bodies = body_set_of(bs, h, f.path);
+            break;
+        case SEC_MESH_BODIES:
+            mesh_bytes.resize(s.length);
+            to_host(s, mesh_bytes.data());
+            c.bodies = mesh_body_set_of(bs, mesh_bytes, h, f.path, c.meshes);
+            break;
+        case SEC_VISCOSITY:
+            to_host(s, &c.viscosity);
+            viscosity_of(c.viscosity, c.sections, f.path);
+            break;
+        case SEC_SURFACE_TENSION:
+            to_host(s, &c.surface_tension);
+            surface_tension_of(c.surface_tension, f.path);
+            break;
+        case SEC_TAG_DENSITIES:
+            to_host(s, &c.densities);
+            tag_densities_of(c.densities, h, c.sections, f.path);
+            break;
+        case SEC_TAG_VISCOSITIES:
+            to_host(s, &c.viscosities);
+            tag_viscosities_of(c.viscosities, f.path);
+            if (!(c.sections & bit(SEC_VISCOSITY))) throw ParseError(f.path + ": section 20 needs a section 17 before it");
+            break;
+        case SEC_INTERFACIAL_TENSION:
+            to_host(s, &c.interfacial);
+            interfacial_tension_of(c.interfacial, f.path);
+            break;
+        default: read_section(f, s, st, [&](int k, const char *data, size_t n, uint64_t off) { to_array(s.id, k, data, n, off); });
+        }
     }
-    if ((out.has_surface_tension = (settings & bit(SEC_SURFACE_TENSION)) != 0)) {
-        read(sec[next++], &out.surface_tension);
-        surface_tension_of(out.surface_tension, path);
-    }
-    if ((out.has_densities = (settings & bit(SEC_TAG_DENSITIES)) != 0)) {
-        read(sec[next++], &out.densities);
-        tag_densities_of(out.densities, h, settings, path);
-    }
-    if ((out.has_viscosities = (settings & bit(SEC_TAG_VISCOSITIES)) != 0)) {
-        read(sec[next++], &out.viscosities);
-        tag_viscosities_of(out.viscosities, path);
-        if (!has_viscosity_section(settings)) throw ParseError(path + ": section 20 needs a section 17 before it");
-    }
-    if ((out.has_interfacial = (settings & bit(SEC_INTERFACIAL_TENSION)) != 0)) {
-        read(sec[next++], &out.interfacial);
-        interfacial_tension_of(out.interfacial, path);
-    }
-    return out;
+    return c;
 }
 
 } // namespace
 
 StateInfo read_state_info(const std::string &path) {
     File f(path, "rb");
-    uint32_t settings = 0;
-    const StateHeader h = read_header(f, settings);
-    Section sec[kNumSections];
-    expected_sections(h, sec, settings);
-    const uint32_t nb = base_sections(h, settings);
+    const StateHeader h = read_header(f);
+    const std::vector<Section> layout = layout_of(f, h);
     Staging st(false);
-    for (uint32_t k = 0; k < 13; ++k) read_section(f, sec[k], st, [](int, const char *, size_t, uint64_t) {});
-    if (nb >= 14) {
-        FlowSectionTagged fl{};
-        read_section(f, sec[13], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&fl) + off, data, n); });
-        flow_set_of(fl.flow, fl.source_tags, h, f.path);
-    }
-    if (nb >= 15) {
-        BodySection bs{};
-        read_section(f, sec[14], st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(reinterpret_cast<char *>(&bs) + off, data, n); });
-        if (nb == 15) body_set_of(bs, h, f.path);
-        else {
-            std::vector<char> bytes(mesh_section_length(f, h, settings));
-            read_section(f, {SEC_MESH_BODIES, bytes.size()}, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(bytes.data() + off, data, n); });
-            std::vector<MeshBodyHost> meshes;
-            mesh_body_set_of(bs, bytes, h, f.path, meshes);
-        }
-    }
-    read_settings(h, settings, sec, nb, f.path, [&](const Section &s, void *dst) {
-        read_section(f, s, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(static_cast<char *>(dst) + off, data, n); });
-    });
+    read_sections(f, h, layout, st, [](uint32_t, int, const char *, size_t, uint64_t) {});
     StateInfo info;
     std::memcpy(info.grid_dimension, h.grid_dimension, sizeof(info.grid_dimension));
     info.max_num_particles = h.max_num_particles;
@@ -675,11 +677,18 @@ void HybridFluid::save_state(const std::string &path) {
     std::memcpy(h.magic, kMagic, sizeof(kMagic));
     bool source_tags = false;
     for (int b = 0; b < flow_.num_sources; ++b) source_tags = source_tags || flow_.tag[b] != 0u;
+    // the sections the fluid writes, bits 1 << id: 1 to 13 always, then the optional ones its features need
+    uint32_t sections = bit(SEC_FLOW) - bit(SEC_POSITIONS);
     const bool with_bodies = num_bodies_ > 0;
-    const bool capillary = surface_tension_ > 0.0f, densities = !tag_densities_.empty(), viscosities = !tag_viscosities_.empty();
-    const bool viscous = viscosity_.kinematic_viscosity > 0.0f || viscosities; // version 256 always holds section 17
-    const bool interfacial = interfacial_tension_ > 0.0f;
-    h.format_version = interfacial ? kFormatVersionInterfacialTension : viscosities ? kFormatVersionTagViscosities : densities ? kFormatVersionTagDensities : capillary ? kFormatVersionSurfaceTension : viscous ? kFormatVersionViscosity : has_mesh_bodies() ? kFormatVersionMeshBodies : with_bodies ? kFormatVersionBodies : !flow_active_ ? 1 : source_tags ? kFormatVersionSourceTags : kFormatVersionFlow;
+    if (flow_active_ || with_bodies) sections |= bit(SEC_FLOW); // a fluid with bodies writes a flow section, possibly of an empty set
+    if (with_bodies) sections |= bit(SEC_BODIES);
+    if (has_mesh_bodies()) sections |= bit(SEC_MESH_BODIES);
+    if (viscosity_.kinematic_viscosity > 0.0f || !tag_viscosities_.empty()) sections |= bit(SEC_VISCOSITY); // section 20 needs section 17
+    if (surface_tension_ > 0.0f) sections |= bit(SEC_SURFACE_TENSION);
+    if (!tag_densities_.empty()) sections |= bit(SEC_TAG_DENSITIES);
+    if (!tag_viscosities_.empty()) sections |= bit(SEC_TAG_VISCOSITIES);
+    if (interfacial_tension_ > 0.0f) sections |= bit(SEC_INTERFACIAL_TENSION);
+    h.format_version = format_version_of(sections, source_tags);
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
     h.grid_dimension[1] = (uint32_t)grid_.ny;
@@ -698,8 +707,7 @@ void HybridFluid::save_state(const std::string &path) {
     h.graph_replay = use_graph ? 1 : 0;
     h.num_stats[0] = (uint32_t)field_velocity_->stats.size();
     h.num_stats[1] = (uint32_t)field_density_->stats.size();
-    h.num_sections = (has_mesh_bodies() ? 16 : with_bodies ? 15 : flow_active_ ? 14 : 13) + (viscous ? 1 : 0) + (capillary ? 1 : 0) + (densities ? 1 : 0) +
-                     (viscosities ? 1 : 0) + (interfacial ? 1 : 0);
+    h.num_sections = (uint32_t)__builtin_popcount(sections);
     h.header_crc = crc_of(&h, offsetof(StateHeader, header_crc));
 
     PcgScalars scalars[2];
@@ -725,7 +733,7 @@ void HybridFluid::save_state(const std::string &path) {
         write_host_section(f, SEC_SOLVER_SCALARS, scalars, sizeof(scalars));
         write_host_section(f, SEC_STATS_VELOCITY, stats[0].data(), stats[0].size() * sizeof(SolverStatisticSample));
         write_host_section(f, SEC_STATS_DENSITY, stats[1].data(), stats[1].size() * sizeof(SolverStatisticSample));
-        if (flow_active_ || with_bodies) {
+        if (sections & bit(SEC_FLOW)) {
             FlowSectionTagged tagged{};
             FlowSection &fl = tagged.flow;
             fl.num_sources = (uint32_t)flow_.num_sources;
@@ -744,14 +752,14 @@ void HybridFluid::save_state(const std::string &path) {
                     }
                 }
             flow_counters(fl.counters);
-            write_host_section(f, SEC_FLOW, &tagged, source_tags || with_bodies || viscous || capillary || densities || viscosities || interfacial ? sizeof(tagged) : sizeof(fl));
+            write_host_section(f, SEC_FLOW, &tagged, fixed_length(SEC_FLOW, h.format_version));
         }
-        if (with_bodies) {
+        if (sections & bit(SEC_BODIES)) {
             BodySection bs{};
             bs.num_bodies = bodies(bs.body, BODIES_MAX);
             write_host_section(f, SEC_BODIES, &bs, sizeof(bs));
         }
-        if (has_mesh_bodies()) {
+        if (sections & bit(SEC_MESH_BODIES)) {
             std::vector<char> bytes(8, 0);
             uint32_t count = 0;
             for (const MeshBodyHost &m : mesh_bodies_) count += m.vertices.empty() ? 0 : 1;
@@ -784,24 +792,24 @@ void HybridFluid::save_state(const std::string &path) {
             }
             write_host_section(f, SEC_MESH_BODIES, bytes.data(), bytes.size());
         }
-        if (viscous) write_host_section(f, SEC_VISCOSITY, &viscosity_, sizeof(viscosity_));
-        if (capillary) {
+        if (sections & bit(SEC_VISCOSITY)) write_host_section(f, SEC_VISCOSITY, &viscosity_, sizeof(viscosity_));
+        if (sections & bit(SEC_SURFACE_TENSION)) {
             const SurfaceTensionSection sts = {surface_tension_, 0u};
             write_host_section(f, SEC_SURFACE_TENSION, &sts, sizeof(sts));
         }
-        if (densities) {
+        if (sections & bit(SEC_TAG_DENSITIES)) {
             TagDensitySection tds{};
             tds.count = (uint32_t)tag_densities_.size();
             for (uint32_t k = 0; k < tds.count; ++k) tds.entry[k] = tag_densities_[k];
             write_host_section(f, SEC_TAG_DENSITIES, &tds, sizeof(tds));
         }
-        if (viscosities) {
+        if (sections & bit(SEC_TAG_VISCOSITIES)) {
             TagViscositySection tvs{};
             tvs.count = (uint32_t)tag_viscosities_.size();
             for (uint32_t k = 0; k < tvs.count; ++k) tvs.entry[k] = tag_viscosities_[k];
             write_host_section(f, SEC_TAG_VISCOSITIES, &tvs, sizeof(tvs));
         }
-        if (interfacial) {
+        if (sections & bit(SEC_INTERFACIAL_TENSION)) {
             InterfacialTensionSection its{};
             its.tension = interfacial_tension_;
             its.count = (uint32_t)interface_tags_.size();
@@ -821,11 +829,8 @@ void HybridFluid::save_state(const std::string &path) {
 
 std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, int device, cudaStream_t stream) {
     File f(path, "rb");
-    uint32_t settings = 0;
-    const StateHeader h = read_header(f, settings); // every size is checked before anything is allocated
-    Section sec[kNumSections];
-    expected_sections(h, sec, settings);
-    const uint32_t nb = base_sections(h, settings);
+    const StateHeader h = read_header(f);
+    const std::vector<Section> layout = layout_of(f, h); // every size is checked before anything is allocated
     std::unique_ptr<HybridFluid> fluid(
         new HybridFluid(h.grid_dimension[0], h.grid_dimension[1], h.grid_dimension[2], h.max_num_particles, device, stream));
     HybridFluid &x = *fluid;
@@ -843,56 +848,30 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     x.use_graph = h.graph_replay != 0;
 
     Staging st(true);
-    auto to_device = [&](const Section &s, void *dst) {
-        read_section(f, s, st, [&](int k, const char *data, size_t n, uint64_t off) {
-            BLUB_CUDA_CHECK(cudaMemcpyAsync(static_cast<char *>(dst) + off, data, n, cudaMemcpyHostToDevice, x.stream_));
-            BLUB_CUDA_CHECK(cudaEventRecord(st.done[k], x.stream_));
-        });
-    };
     x.cur_ = 0;
     void *const arrays[10] = {x.pos_[0], x.row_[0], x.row_[1], x.row_[2], x.u_[0].ptr, x.u_[1].ptr, x.u_[2].ptr, x.marker_.ptr,
                               x.field_velocity_->pressure(), x.field_density_->pressure()};
-    for (int k = 0; k < 10; ++k) to_device(sec[k], arrays[k]);
-    auto to_host = [&](const Section &s, void *dst) {
-        read_section(f, s, st, [&](int, const char *data, size_t n, uint64_t off) { std::memcpy(static_cast<char *>(dst) + off, data, n); });
-    };
-    PcgScalars scalars[2];
-    to_host(sec[10], scalars);
-    BLUB_CUDA_CHECK(cudaMemcpyAsync(x.field_velocity_->scalars, &scalars[0], sizeof(PcgScalars), cudaMemcpyHostToDevice, x.stream_));
-    BLUB_CUDA_CHECK(cudaMemcpyAsync(x.field_density_->scalars, &scalars[1], sizeof(PcgScalars), cudaMemcpyHostToDevice, x.stream_));
-    for (int which = 0; which < 2; ++which) {
-        std::vector<SolverStatisticSample> samples(h.num_stats[which]);
-        to_host(sec[11 + which], samples.data());
-        x.field(which).stats.assign(samples.begin(), samples.end());
-    }
+    StateContents c = read_sections(f, h, layout, st, [&](uint32_t id, int k, const char *data, size_t n, uint64_t off) {
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(static_cast<char *>(arrays[id - SEC_POSITIONS]) + off, data, n, cudaMemcpyHostToDevice, x.stream_));
+        BLUB_CUDA_CHECK(cudaEventRecord(st.done[k], x.stream_));
+    });
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(x.field_velocity_->scalars, &c.scalars[0], sizeof(PcgScalars), cudaMemcpyHostToDevice, x.stream_));
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(x.field_density_->scalars, &c.scalars[1], sizeof(PcgScalars), cudaMemcpyHostToDevice, x.stream_));
+    for (int which = 0; which < 2; ++which) x.field(which).stats.assign(c.stats[which].begin(), c.stats[which].end());
     x.fluid_bits_stale_ = true; // rebuilt from the restored marker volume before the next grid pass that reads it
-    if (nb >= 14) {
-        FlowSectionTagged fl{};
-        to_host(sec[13], &fl);
-        const FlowSet fs = flow_set_of(fl.flow, fl.source_tags, h, f.path);
+    if (c.sections & bit(SEC_FLOW)) {
         BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
-        if (fs.num_sources + fs.num_drains > 0) x.restore_flow(fs, fl.flow.counters); // the device takes over the restored count
+        if (c.flow.num_sources + c.flow.num_drains > 0) x.restore_flow(c.flow, c.flow_counters); // the device takes over the restored count
     }
-    if (nb >= 15) { // the history ring is not state: a loaded fluid starts with an empty one
-        BodySection bs{};
-        to_host(sec[14], &bs);
-        if (nb == 15) x.restore_bodies(body_set_of(bs, h, f.path));
-        else {
-            std::vector<char> bytes(mesh_section_length(f, h, settings));
-            to_host({SEC_MESH_BODIES, bytes.size()}, bytes.data());
-            std::vector<MeshBodyHost> meshes;
-            const std::vector<BlubBody> set = mesh_body_set_of(bs, bytes, h, f.path, meshes);
-            x.restore_bodies(set, std::move(meshes));
-        }
-    }
+    // the history ring is not state: a loaded fluid starts with an empty one
+    if (c.sections & bit(SEC_BODIES)) x.restore_bodies(c.bodies, std::move(c.meshes));
     // the working volumes, the last viscosity solve, the curvature, the cell densities, viscosities and coefficients are not state: the steps
     // form them again
-    const Settings set = read_settings(h, settings, sec, nb, f.path, to_host);
-    if (set.has_viscosity) x.set_viscosity(&set.viscosity);
-    if (set.has_surface_tension) x.set_surface_tension(set.surface_tension.surface_tension);
-    if (set.has_densities) x.set_tag_densities(set.densities.entry, set.densities.count);
-    if (set.has_viscosities) x.set_tag_viscosities(set.viscosities.entry, set.viscosities.count);
-    if (set.has_interfacial) x.set_interfacial_tension(set.interfacial.tag, set.interfacial.count, set.interfacial.tension);
+    if (c.sections & bit(SEC_VISCOSITY)) x.set_viscosity(&c.viscosity);
+    if (c.sections & bit(SEC_SURFACE_TENSION)) x.set_surface_tension(c.surface_tension.surface_tension);
+    if (c.sections & bit(SEC_TAG_DENSITIES)) x.set_tag_densities(c.densities.entry, c.densities.count);
+    if (c.sections & bit(SEC_TAG_VISCOSITIES)) x.set_tag_viscosities(c.viscosities.entry, c.viscosities.count);
+    if (c.sections & bit(SEC_INTERFACIAL_TENSION)) x.set_interfacial_tension(c.interfacial.tag, c.interfacial.count, c.interfacial.tension);
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;
 }

@@ -11,11 +11,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libblubcore.so")
-SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu", "load_kernels.cu", "body_kernels.cu", "viscosity_kernels.cu", "cfl_kernels.cu", "surface_tension_kernels.cu", "tank_kernels.cu", "tag_density_kernels.cu", "mesh_body.cpp", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
+SOURCES = ["pcg.cu", "fluid_kernels.cu", "transfer_kernels.cu", "flow_kernels.cu", "load_kernels.cu", "body_kernels.cu", "viscosity_kernels.cu", "cfl_kernels.cu", "surface_tension_kernels.cu", "tank_kernels.cu", "tag_density_kernels.cu", "whitewater_kernels.cu", "mesh_body.cpp", "hybrid_fluid.cu", "slab.cu", "solids.cu", "mesh_voxelizer.cu", "scene.cpp", "state_file.cpp",
            "c_api.cpp"]
 # the mesh voxelizer shares its arithmetic with a host twin and a NumPy restatement, the curvatures of the free surface and of the
-# interfacial tension with NumPy restatements: no FMA contraction, so that they agree bit for bit
-EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"], "surface_tension_kernels.cu": ["-fmad=false"]}
+# interfacial tension and the whitewater pass with NumPy restatements: no FMA contraction, so that they agree bit for bit
+EXTRA_FLAGS = {"mesh_voxelizer.cu": ["-fmad=false"], "surface_tension_kernels.cu": ["-fmad=false"], "whitewater_kernels.cu": ["-fmad=false"]}
 HEADERS = ["common.cuh", "blub_core.hpp", "fluid_kernels.hpp", "advect.cuh", "voxelize_core.hpp", "xoshiro.hpp", "grid_words.cuh", "grid_reduce.cuh", os.path.join("..", "..", "include", "blub_fluid.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [

@@ -41,39 +41,14 @@ __device__ __forceinline__ void trilerp3(const Corners &c, const float ix[3], co
     }
 }
 
-// advect_particles.comp:35-194.  Writes position + the three APIC rows, marks the new cell FLUID (:175-178); the
-// linked-list rebuild of :179-181 has no counterpart (the density pass scatters).
-// MIGRATE (z-slab ranks): instead of writing back in place, the kernel itself sorts its results -- stayers are compacted
-// into the spare arrays, particles that left the slab go straight to the neighbour (see MigrateOut) -- so that migration
-// costs one warp-aggregated atomic per warp instead of an extra pass over all particles.
-// Returns the new position (tag included) -- for a particle beyond the last one the stand-in (1.5, 1.5, 1.5) the scatters give such lanes.
-template <bool MIGRATE>
-__device__ __forceinline__ float4 advect_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, float4 *__restrict__ pos,
-                                                    float4 *__restrict__ rowx, float4 *__restrict__ rowy, float4 *__restrict__ rowz,
-                                                    const float *__restrict__ ux, const float *__restrict__ uy,
-                                                    const float *__restrict__ uz, const uint2 *__restrict__ vox,
-                                                    int8_t *__restrict__ marker, MigrateOut mig) {
-    if (i >= params->num_particles) return make_float4(1.5f, 1.5f, 1.5f, 0.0f);
-    const float dt = params->dt;
-    const float4 p4 = pos[i];
-    float x0[3] = {p4.x, p4.y, p4.z};
+// The MAC trilinear sample of the grid velocity at x0 (advect_particles.comp:73-92): per component c the eight faces around x0 into
+// cn.v[..][c] and the interpolants into ix[c], iy[c], iz[c]; trilerp3(cn, ix, iy, iz) is then the velocity there.  Advection and the
+// whitewater pass (whitewater_kernels.cu) both sample with it.
+__device__ __forceinline__ void mac_corners(const GridDim &g, const float x0[3], const float *const U[3], Corners &cn, float ix[3], float iy[3],
+                                            float iz[3]) {
     const int S[3] = {g.nx, g.ny, g.nz};
-    if (vox != nullptr) { // :45-64 particle "eaten" by a moving wall
-        const Voxel s = voxel_point_clamp(g, vox, x0[0], x0[1], x0[2]);
-        if (s.w > 0.0f) {
-            const float ax = fabsf(s.x), ay = fabsf(s.y), az = fabsf(s.z);
-            if (ax > ay) {
-                if (ax > az) x0[0] += signf(s.x); else x0[2] += signf(s.z);
-            } else {
-                if (ay > az) x0[1] += signf(s.y); else x0[2] += signf(s.z);
-            }
-        }
-    }
-    Corners cn;
-    float ix[3], iy[3], iz[3];
-    const float *const U[3] = {ux, uy, uz};
 #pragma unroll
-    for (int c = 0; c < 3; ++c) { // :73-92
+    for (int c = 0; c < 3; ++c) {
         float op[3];
         int lo[3], hi[3];
 #pragma unroll
@@ -90,6 +65,39 @@ __device__ __forceinline__ float4 advect_kernel_one(uint32_t i, GridDim g, const
         cn.v[6][c] = u[lin(g, lo[0], hi[1], hi[2])]; cn.v[7][c] = u[lin(g, hi[0], hi[1], hi[2])];
         ix[c] = fractf(op[0]); iy[c] = fractf(op[1]); iz[c] = fractf(op[2]);
     }
+}
+
+// advect_particles.comp:35-194.  Writes position + the three APIC rows, marks the new cell FLUID (:175-178); the
+// linked-list rebuild of :179-181 has no counterpart (the density pass scatters).
+// MIGRATE (z-slab ranks): instead of writing back in place, the kernel itself sorts its results -- stayers are compacted
+// into the spare arrays, particles that left the slab go straight to the neighbour (see MigrateOut) -- so that migration
+// costs one warp-aggregated atomic per warp instead of an extra pass over all particles.
+// Returns the new position (tag included) -- for a particle beyond the last one the stand-in (1.5, 1.5, 1.5) the scatters give such lanes.
+template <bool MIGRATE>
+__device__ __forceinline__ float4 advect_kernel_one(uint32_t i, GridDim g, const StepParams *__restrict__ params, float4 *__restrict__ pos,
+                                                    float4 *__restrict__ rowx, float4 *__restrict__ rowy, float4 *__restrict__ rowz,
+                                                    const float *__restrict__ ux, const float *__restrict__ uy,
+                                                    const float *__restrict__ uz, const uint2 *__restrict__ vox,
+                                                    int8_t *__restrict__ marker, MigrateOut mig) {
+    if (i >= params->num_particles) return make_float4(1.5f, 1.5f, 1.5f, 0.0f);
+    const float dt = params->dt;
+    const float4 p4 = pos[i];
+    float x0[3] = {p4.x, p4.y, p4.z};
+    if (vox != nullptr) { // :45-64 particle "eaten" by a moving wall
+        const Voxel s = voxel_point_clamp(g, vox, x0[0], x0[1], x0[2]);
+        if (s.w > 0.0f) {
+            const float ax = fabsf(s.x), ay = fabsf(s.y), az = fabsf(s.z);
+            if (ax > ay) {
+                if (ax > az) x0[0] += signf(s.x); else x0[2] += signf(s.z);
+            } else {
+                if (ay > az) x0[1] += signf(s.y); else x0[2] += signf(s.z);
+            }
+        }
+    }
+    Corners cn;
+    float ix[3], iy[3], iz[3];
+    const float *const U[3] = {ux, uy, uz};
+    mac_corners(g, x0, U, cn, ix, iy, iz);
     float nv[3], cx[3], cy[3], cz[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { // :96-112

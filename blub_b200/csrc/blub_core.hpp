@@ -369,7 +369,23 @@ class HybridFluid {
     bool has_tag_densities() const { return !tag_densities_.empty(); }
     float *cell_density() const { return td_.rho; } // nullptr before the first non-empty table
 
+    // Whitewater (whitewater_kernels.cu): nullptr or a capacity of 0 turns it off, frees its memory and stores an all-zero setting.  A new
+    // capacity starts from no particles and zero counters (its storage is allocated before the old one is freed), another change keeps them;
+    // every change drops the step graphs.  Throws std::invalid_argument and changes nothing on a
+    // setting check_whitewater refuses, a z-slab rank or a fluid inside a step.
+    void set_whitewater(const BlubWhitewater *s);
+    const BlubWhitewater &whitewater() const { return whitewater_; }
+    bool whitewater_on() const { return whitewater_.max_num_particles > 0; }
+    // {live, emitted, removed, refused}, zeros while off (synchronises)
+    void whitewater_counters(uint64_t out[4]);
+    // the live particles, at most `capacity` of them (pos4 / vel4: 4 floats each); returns the live count (synchronises)
+    uint32_t download_whitewater(float *pos4, float *vel4, uint32_t capacity);
+
   private:
+    BlubWhitewater whitewater_{};
+    WhitewaterWork ww_;
+    // a state file's whitewater: the setting, the counters {emitted, removed, refused} and `count` particles (4 + 4 floats each, host memory)
+    void restore_whitewater(const BlubWhitewater &s, const uint64_t counters[3], uint32_t count, const float *particles);
     std::vector<BlubTagDensity> tag_densities_;
     TagDensityWork td_;
     const TagDensityWork *solve_weights() const { return tag_densities_.empty() ? nullptr : &td_; }
@@ -581,6 +597,9 @@ void quat_from_euler_deg_wxyz(const float deg[3], float q[4]);
 // that does not depend on the fluid.  source_tags may be nullptr (all 0).
 FlowSet make_flow_set(const uint32_t dim[3], const BlubFluidSource *sources, const uint32_t *source_tags, uint32_t num_sources, const BlubFluidDrain *drains,
                       uint32_t num_drains);
+// The whitewater setter's rules (DESIGN.md §8 "Whitewater"); throws std::invalid_argument naming `who` and the field.  A capacity of 0 is off
+// and passes whatever the other fields hold.
+void check_whitewater(const BlubWhitewater &s, const char *who);
 // Host only: reads and validates the whole state file (header, every section length and checksum).
 StateInfo read_state_info(const std::string &path);
 
@@ -641,6 +660,8 @@ struct SceneConfig {
     std::vector<uint32_t> interface_tags;    // checked with the setter's rules
     std::vector<BlubTagDensity> tag_densities; // optional fluid.tag_densities, checked with the setter's rules
     std::vector<BlubTagViscosity> tag_viscosities; // optional fluid.tag_viscosities (m^2/s), checked in cells^2/s with the setter's rules
+    bool has_whitewater = false;             // optional fluid.whitewater, in grid units (the energy range / grid_to_world_scale^2), checked
+    BlubWhitewater whitewater{};
     bool has_tank_motion = false;            // optional fluid.tank_motion (world units, Hz, rad, rad/s; directions and axis normalised)
     BlubTankMotion tank_motion{};
     uint32_t num_static_objects = 0;

@@ -13,6 +13,7 @@
 //   --record FPS PREFIX   the controller's "recording with fixed frame length" (simulation_controller.rs:80-82,174-176): the render
 //                  clock advances by 1 / FPS per frame, the simulation runs the steps that belong to the frame (Timer::simulation_frame_loop),
 //                  and instead of a screenshot the particle positions are written to PREFIX00000.f32, PREFIX00001.f32, ...
+//                  With fluid.whitewater each frame also writes PREFIX%05d.whitewater.f32: its live whitewater particles, 8 floats each.
 //   --save-state FILE  the fluid's complete state after the last step (blub_fluid_save_state); --checkpoint-every N also rewrites FILE every
 //                  N steps at batch boundaries.  --load-state FILE resumes such a file instead of seeding the scene's fluid cubes: the scene
 //                  still provides scale, origin and static objects, and the simulation clock restarts at step_count * dt.
@@ -33,6 +34,7 @@
 //                  the clock of a resumed adaptive run is not step_count * dt.
 //   fluid.tank_motion  a moving tank (not in the reference): before every step (and every --cfl substep) the runner sets the tank frame at the
 //                  time the static objects are voxelized at (blub_tank_frame_at); a --load-state run continues the clock at step_count * dt.
+#include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -237,6 +239,26 @@ int main(int argc, char **argv) {
         std::fclose(f);
         return n;
     };
+    // with whitewater on: its live particles, each a position float4 (w: lifetime) then a velocity float4 (w: the kind's bits)
+    auto write_whitewater = [&](const std::string &path) {
+        BlubWhitewater ww;
+        if (blub_fluid_whitewater(fluid, &ww)) die("cannot read the whitewater setting");
+        if (ww.max_num_particles == 0) return;
+        uint64_t c[4];
+        if (blub_fluid_whitewater_counters(fluid, c)) die("cannot read the whitewater counters");
+        const uint32_t live = (uint32_t)c[0]; // buffers for the live particles only: nothing steps in between
+        std::vector<float> pos((size_t)live * 4), vel((size_t)live * 4);
+        uint32_t n = 0;
+        if (blub_fluid_download_whitewater(fluid, pos.data(), vel.data(), live, &n)) die("whitewater download failed");
+        n = std::min(n, live);
+        FILE *f = std::fopen(path.c_str(), "wb");
+        if (!f) { std::perror("blub_run: cannot write whitewater"); std::exit(1); }
+        for (uint32_t i = 0; i < n; ++i) {
+            std::fwrite(&pos[4 * (size_t)i], sizeof(float), 4, f);
+            std::fwrite(&vel[4 * (size_t)i], sizeof(float), 4, f);
+        }
+        std::fclose(f);
+    };
 
     // every record of every probe, collected at batch / frame boundaries (the ring holds the newest BLUB_LOAD_HISTORY_LENGTH steps)
     std::vector<std::vector<BlubSolidLoad>> loads(num_probes);
@@ -301,6 +323,8 @@ int main(int argc, char **argv) {
             char name[32];
             std::snprintf(name, sizeof(name), "%05d.f32", frame);
             write_particles(record_prefix + name);
+            std::snprintf(name, sizeof(name), "%05d.whitewater.f32", frame);
+            write_whitewater(record_prefix + name);
             collect_loads();
             collect_bodies();
             std::printf("frame %d: %u step(s), simulated %.6f s\n", frame, n, (double)blub_duration_as_secs_f32(simulated_ns));
@@ -366,6 +390,14 @@ int main(int argc, char **argv) {
         float sigma = 0.0f;
         if (blub_fluid_surface_tension(fluid, &sigma)) die("cannot read the surface tension");
         if (sigma > 0.0f) std::fprintf(f, ", \"surface_tension\": %.9g", sigma);
+        BlubWhitewater ww;
+        if (blub_fluid_whitewater(fluid, &ww)) die("cannot read the whitewater setting");
+        if (ww.max_num_particles) {
+            uint64_t c[4];
+            if (blub_fluid_whitewater_counters(fluid, c)) die("cannot read the whitewater counters");
+            std::fprintf(f, ", \"whitewater\": {\"live\": %llu, \"emitted\": %llu, \"removed\": %llu, \"refused\": %llu}", (unsigned long long)c[0],
+                         (unsigned long long)c[1], (unsigned long long)c[2], (unsigned long long)c[3]);
+        }
         uint32_t itags[BLUB_INTERFACE_TAGS_MAX], nit = 0;
         float sab = 0.0f;
         if (blub_fluid_interfacial_tension(fluid, itags, BLUB_INTERFACE_TAGS_MAX, &nit, &sab)) die("cannot read the interfacial tension");

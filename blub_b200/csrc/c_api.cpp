@@ -565,6 +565,37 @@ int blub_scene_interfacial_tension(const char *path, uint32_t *tags, uint32_t ca
     });
 }
 
+int blub_fluid_set_whitewater(BlubFluid *fluid, const BlubWhitewater *settings) {
+    if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
+    return guarded([&] { fluid->impl->set_whitewater(settings); return BLUB_OK; });
+}
+
+int blub_fluid_whitewater(const BlubFluid *fluid, BlubWhitewater *out) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    *out = fluid->impl->whitewater();
+    return BLUB_OK;
+}
+
+int blub_fluid_whitewater_counters(BlubFluid *fluid, uint64_t out[4]) {
+    if (!fluid || !out) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { fluid->impl->whitewater_counters(out); return BLUB_OK; });
+}
+
+int blub_fluid_download_whitewater(BlubFluid *fluid, float *pos4, float *vel4, uint32_t capacity, uint32_t *count) {
+    if (!fluid || !count || (capacity && (!pos4 || !vel4))) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] { *count = fluid->impl->download_whitewater(pos4, vel4, capacity); return BLUB_OK; });
+}
+
+int blub_scene_whitewater(const char *path, BlubWhitewater *out, int32_t *has) {
+    if (!path || !out || !has) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL argument");
+    return guarded([&] {
+        const blub::SceneConfig c = blub::parse_scene_file(path);
+        *has = c.has_whitewater ? 1 : 0;
+        *out = c.whitewater;
+        return BLUB_OK;
+    });
+}
+
 int blub_fluid_set_tag_densities(BlubFluid *fluid, const BlubTagDensity *table, uint32_t count) {
     if (!fluid) return fail(BLUB_ERR_INVALID_ARGUMENT, "NULL fluid");
     return guarded([&] { fluid->impl->set_tag_densities(table, count); return BLUB_OK; });

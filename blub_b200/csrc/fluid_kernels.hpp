@@ -353,4 +353,28 @@ struct TagDensityWork {
 void launch_tag_density(cudaStream_t st, const GridDim &g, const StepParams *params, bool device_count, uint32_t n_host, uint32_t np_upper,
                         const float4 *pos, const int8_t *marker, const TagDensityWork &w);
 
+// ---- whitewater (whitewater_kernels.cu, DESIGN.md §8 "Whitewater") ----
+// Xored into the (step << 32 | cell) seed of a cell's emission draws.  The low half has bit 31 set and a cell index is below 2^31, so no
+// whitewater seed equals a seed of the flow prologue's emission.
+constexpr uint64_t WHITEWATER_SEED_KEY = 0xD1B54A32D192ED03ull;
+// The device counters: cumulative emitted, removed and refused for capacity; the live count; the survivors of the running update.
+struct WhitewaterCounters {
+    unsigned long long emitted, removed, refused;
+    uint32_t count, survivors;
+};
+// Storage, allocated by the setter with a capacity above zero: 64 bytes per particle and 4 per cell.  pos[0] / vel[0] hold the live particles
+// between steps (position xyz and lifetime in s; velocity xyz in cells/s and the kind's bits), pos[1] / vel[1] what the update made of them.
+struct WhitewaterWork {
+    float4 *pos[2] = {nullptr, nullptr}, *vel[2] = {nullptr, nullptr};
+    uint32_t *flags = nullptr;       // capacity + 1: "the particle survives", then their exclusive scan
+    uint32_t *cell_counts = nullptr; // n + 1: the particles each cell emits, then their exclusive scan
+    uint32_t *scan_sums = nullptr;   // block sums of both scans
+    WhitewaterCounters *counters = nullptr;
+    uint32_t capacity = 0;
+};
+// The pass at the end of stage 5 (update, stable compaction, emission from the surface band), reading the projected and extrapolated u, the
+// marker of this step's P2G and its FLUID bits, and the solid volume `vox` (may be nullptr).  Writes only w.
+void launch_whitewater(cudaStream_t st, const GridDim &g, const StepParams *params, const FluidBits &bits, const int8_t *marker, float *const u[3],
+                       const uint2 *vox, const BlubWhitewater &s, const WhitewaterWork &w);
+
 } // namespace blub

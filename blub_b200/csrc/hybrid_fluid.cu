@@ -68,6 +68,17 @@ void free_work(InterfacialTensionWork &w) {
     cudaFree(w.block);
     w = InterfacialTensionWork{};
 }
+void free_work(WhitewaterWork &w) {
+    for (int k = 0; k < 2; ++k) {
+        cudaFree(w.pos[k]);
+        cudaFree(w.vel[k]);
+    }
+    cudaFree(w.flags);
+    cudaFree(w.cell_counts);
+    cudaFree(w.scan_sums);
+    cudaFree(w.counters);
+    w = WhitewaterWork{};
+}
 void free_work(TagDensityWork &w) {
     cudaFree(w.sum);
     cudaFree(w.count);
@@ -261,6 +272,7 @@ HybridFluid::~HybridFluid() {
     free_work(st_);
     free_work(it_);
     free_work(td_);
+    free_work(ww_);
     cudaFree(census_dev_);
     cudaFree(max_velocity_dev_);
     cudaFree(load_probes_dev_);
@@ -629,6 +641,10 @@ void HybridFluid::run_stage(int stage, float dt) {
         if (shard) {
             const SlabHaloItem items[3] = {{u[0], sizeof(float), 2}, {u[1], sizeof(float), 2}, {u[2], sizeof(float), 2}};
             slab_halo_exchange(items, 3); // X2
+        }
+        if (whitewater_on()) { // u is projected and extrapolated, the marker is this step's P2G marker: stage 6 clears it
+            const NvtxScope ww_scope("whitewater");
+            launch_whitewater(stream_, grid_, params_dev_, bits, marker_.ptr, u, vox, whitewater_, ww_);
         }
         break;
     case 6: // clear marker (& linked list) grids (:911-916)
@@ -1239,6 +1255,113 @@ void HybridFluid::set_interfacial_tension(const uint32_t *tags, uint32_t count, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Whitewater (whitewater_kernels.cu).  Not in the reference.  The setting reaches the kernels by value, so every change drops the step graphs.
+void check_whitewater(const BlubWhitewater &s, const char *who) {
+    const std::string w = who;
+    if (s.max_num_particles == 0) return;
+    if (s.max_num_particles > BLUB_WHITEWATER_MAX_PARTICLES)
+        throw std::invalid_argument(w + ": max_num_particles above " + std::to_string(BLUB_WHITEWATER_MAX_PARTICLES));
+    const float values[] = {s.trapped_air_rate, s.wave_crest_rate, s.trapped_air_range[0], s.trapped_air_range[1], s.wave_crest_range[0],
+                            s.wave_crest_range[1], s.energy_range[0], s.energy_range[1], s.lifetime_lo, s.lifetime_hi, s.buoyancy, s.drag};
+    for (float v : values)
+        if (!std::isfinite(v)) throw std::invalid_argument(w + ": every value must be finite");
+    if (s.trapped_air_rate < 0.0f || s.wave_crest_rate < 0.0f) throw std::invalid_argument(w + ": a rate is negative");
+    if (!(s.trapped_air_range[0] < s.trapped_air_range[1])) throw std::invalid_argument(w + ": trapped_air_range needs lo < hi");
+    if (!(s.wave_crest_range[0] < s.wave_crest_range[1])) throw std::invalid_argument(w + ": wave_crest_range needs lo < hi");
+    if (!(s.energy_range[0] < s.energy_range[1])) throw std::invalid_argument(w + ": energy_range needs lo < hi");
+    if (s.lifetime_lo < 0.0f || !(s.lifetime_lo < s.lifetime_hi)) throw std::invalid_argument(w + ": the lifetime needs 0 <= lo < hi");
+    if (!(s.drag >= 0.0f && s.drag <= 1.0f)) throw std::invalid_argument(w + ": drag must lie in [0, 1]");
+    if (s.spray_below > s.bubble_from) throw std::invalid_argument(w + ": spray_below is above bubble_from");
+    if (s.bubble_from > 27u) throw std::invalid_argument(w + ": bubble_from is above 27");
+    if (s.max_per_cell > 16u) throw std::invalid_argument(w + ": max_per_cell is above 16");
+}
+
+void HybridFluid::set_whitewater(const BlubWhitewater *setting) {
+    if (slab_world_ > 1) throw std::invalid_argument("set_whitewater: z-slab ranks have no whitewater");
+    if (mid_step_) throw std::invalid_argument("set_whitewater: the fluid is inside a step (the last step_stages call did not end at stage 14)");
+    check_whitewater(setting ? *setting : BlubWhitewater{}, "set_whitewater");
+    const BlubWhitewater s = setting && setting->max_num_particles ? *setting : BlubWhitewater{}; // off is stored as all zero
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    if (s.max_num_particles != ww_.capacity) {
+        // the new storage first: a failed allocation throws with the fluid, its particles and its graphs as they were
+        WhitewaterWork w;
+        if (s.max_num_particles) {
+            const size_t cap = s.max_num_particles, n = (size_t)grid_.n;
+            try {
+                for (int k = 0; k < 2; ++k) {
+                    BLUB_CUDA_CHECK(cudaMalloc(&w.pos[k], cap * sizeof(float4)));
+                    BLUB_CUDA_CHECK(cudaMalloc(&w.vel[k], cap * sizeof(float4)));
+                }
+                BLUB_CUDA_CHECK(cudaMalloc(&w.flags, (cap + 1) * sizeof(uint32_t)));
+                BLUB_CUDA_CHECK(cudaMalloc(&w.cell_counts, (n + 1) * sizeof(uint32_t)));
+                const int64_t longest = std::max<int64_t>((int64_t)cap + 1, (int64_t)n + 1);
+                BLUB_CUDA_CHECK(cudaMalloc(&w.scan_sums, ((size_t)exclusive_scan_blocks(longest) + 1024) * sizeof(uint32_t)));
+                BLUB_CUDA_CHECK(cudaMalloc(&w.counters, sizeof(WhitewaterCounters)));
+                BLUB_CUDA_CHECK(cudaMemsetAsync(w.counters, 0, sizeof(WhitewaterCounters), stream_));
+            } catch (...) {
+                cudaStreamSynchronize(stream_); // the memset may be in flight
+                free_work(w);
+                throw;
+            }
+            w.capacity = s.max_num_particles;
+        }
+        if (ww_.counters) {
+            BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // the enqueued steps may still use the old storage
+            free_work(ww_);
+        }
+        ww_ = w;
+    }
+    whitewater_ = s;
+    destroy_graphs();
+}
+
+void HybridFluid::whitewater_counters(uint64_t out[4]) {
+    BLUB_CUDA_CHECK(cudaSetDevice(device_));
+    out[0] = out[1] = out[2] = out[3] = 0;
+    if (!ww_.counters) return;
+    WhitewaterCounters c;
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(&c, ww_.counters, sizeof(c), cudaMemcpyDeviceToHost, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    out[0] = c.count;
+    out[1] = c.emitted;
+    out[2] = c.removed;
+    out[3] = c.refused;
+}
+
+uint32_t HybridFluid::download_whitewater(float *pos4, float *vel4, uint32_t capacity) {
+    uint64_t c[4];
+    whitewater_counters(c);
+    const uint32_t count = (uint32_t)c[0], n = std::min(count, capacity);
+    if (n) {
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(pos4, ww_.pos[0], (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(vel4, ww_.vel[0], (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, stream_));
+        BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    }
+    return count;
+}
+
+void HybridFluid::restore_whitewater(const BlubWhitewater &s, const uint64_t counters[3], uint32_t count, const float *particles) {
+    set_whitewater(&s);
+    if (count > ww_.capacity) throw std::invalid_argument("restore_whitewater: more particles than the capacity");
+    std::vector<float4> pos(count), vel(count);
+    for (uint32_t i = 0; i < count; ++i) {
+        std::memcpy(&pos[i], particles + 8ull * i, sizeof(float4));
+        std::memcpy(&vel[i], particles + 8ull * i + 4, sizeof(float4));
+    }
+    WhitewaterCounters c{};
+    c.emitted = counters[0];
+    c.removed = counters[1];
+    c.refused = counters[2];
+    c.count = count;
+    if (count) {
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(ww_.pos[0], pos.data(), (size_t)count * sizeof(float4), cudaMemcpyHostToDevice, stream_));
+        BLUB_CUDA_CHECK(cudaMemcpyAsync(ww_.vel[0], vel.data(), (size_t)count * sizeof(float4), cudaMemcpyHostToDevice, stream_));
+    }
+    BLUB_CUDA_CHECK(cudaMemcpyAsync(ww_.counters, &c, sizeof(c), cudaMemcpyHostToDevice, stream_));
+    BLUB_CUDA_CHECK(cudaStreamSynchronize(stream_)); // the host copies are pageable
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Liquids of different densities (tag_density_kernels.cu).  Not in the reference.  The kernels read the table from a device block, so a new
 // non-empty table replays the captured graphs; turning the feature on or off changes the launches and drops them.
 void HybridFluid::set_tag_densities(const BlubTagDensity *table, uint32_t count) {
@@ -1587,6 +1710,7 @@ std::unique_ptr<HybridFluid> create_fluid_from_config(const SceneConfig &cfg, in
     }
     if (cfg.surface_tension > 0.0f) f->set_surface_tension(scene_surface_tension_grid(cfg));
     if (!cfg.tag_densities.empty()) f->set_tag_densities(cfg.tag_densities.data(), (uint32_t)cfg.tag_densities.size());
+    if (cfg.has_whitewater) f->set_whitewater(&cfg.whitewater);
     if (cfg.interfacial_tension > 0.0f) f->set_interfacial_tension(cfg.interface_tags.data(), (uint32_t)cfg.interface_tags.size(), scene_interfacial_tension_grid(cfg));
     if (!cfg.load_probes.empty()) {
         const std::vector<BlubLoadProbe> probes = scene_load_probes_grid(cfg);

@@ -247,6 +247,42 @@ SceneConfig parse_scene_file(const std::string &path) {
             throw std::runtime_error(std::string("scene JSON: `fluid.interfacial_tension`: ") + e.what());
         }
     }
+    // whitewater (not in the reference): every field of BlubWhitewater, ranges as [lo, hi] and the lifetime as "lifetime": [lo, hi], the energy
+    // range in m^2/s^2; converted to grid units here and checked with the setter's rules
+    if (const JsonValue *ww = fluid.get("whitewater")) {
+        if (ww->kind != JsonValue::Object) throw std::runtime_error("scene JSON: `fluid.whitewater` is not an object");
+        BlubWhitewater &w = cfg.whitewater;
+        auto pair = [&](const char *key, float out[2]) {
+            const JsonValue &v = need(*ww, key);
+            if (v.kind != JsonValue::Array || v.array.size() != 2)
+                throw std::runtime_error(std::string("scene JSON: `fluid.whitewater.") + key + "` is not a pair [lo, hi]");
+            out[0] = num_f32(v.array[0], key);
+            out[1] = num_f32(v.array[1], key);
+        };
+        w.max_num_particles = num_u32(need(*ww, "max_num_particles"), "whitewater.max_num_particles");
+        w.trapped_air_rate = num_f32(need(*ww, "trapped_air_rate"), "whitewater.trapped_air_rate");
+        w.wave_crest_rate = num_f32(need(*ww, "wave_crest_rate"), "whitewater.wave_crest_rate");
+        pair("trapped_air_range", w.trapped_air_range);
+        pair("wave_crest_range", w.wave_crest_range);
+        pair("energy_range", w.energy_range);
+        float life[2];
+        pair("lifetime", life);
+        w.lifetime_lo = life[0];
+        w.lifetime_hi = life[1];
+        w.buoyancy = num_f32(need(*ww, "buoyancy"), "whitewater.buoyancy");
+        w.drag = num_f32(need(*ww, "drag"), "whitewater.drag");
+        w.spray_below = num_u32(need(*ww, "spray_below"), "whitewater.spray_below");
+        w.bubble_from = num_u32(need(*ww, "bubble_from"), "whitewater.bubble_from");
+        w.max_per_cell = num_u32(need(*ww, "max_per_cell"), "whitewater.max_per_cell");
+        const float s2 = cfg.grid_to_world_scale * cfg.grid_to_world_scale;
+        for (float &e : w.energy_range) e /= s2;
+        try {
+            check_whitewater(w, "scene");
+        } catch (const std::invalid_argument &e) {
+            throw std::runtime_error(std::string("scene JSON: `fluid.whitewater`: ") + e.what());
+        }
+        cfg.has_whitewater = true;
+    }
     // liquids of different densities (not in the reference): [{"tag": n, "relative_density": x}], checked with the setter's rules
     if (const JsonValue *td = fluid.get("tag_densities")) {
         if (td->kind != JsonValue::Array) throw std::runtime_error("scene JSON: `fluid.tag_densities` is not an array");

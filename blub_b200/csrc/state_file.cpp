@@ -32,7 +32,7 @@ constexpr size_t kStagingBytes = 64u << 20; // two halves: one is filled while t
 enum : uint32_t {
     SEC_POSITIONS = 1, SEC_VELOCITY_X, SEC_VELOCITY_Y, SEC_VELOCITY_Z, SEC_GRID_VELOCITY_X, SEC_GRID_VELOCITY_Y, SEC_GRID_VELOCITY_Z,
     SEC_MARKER, SEC_PRESSURE_VELOCITY, SEC_PRESSURE_DENSITY, SEC_SOLVER_SCALARS, SEC_STATS_VELOCITY, SEC_STATS_DENSITY, SEC_FLOW, SEC_BODIES,
-    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES, SEC_TAG_VISCOSITIES, SEC_INTERFACIAL_TENSION
+    SEC_MESH_BODIES, SEC_VISCOSITY, SEC_SURFACE_TENSION, SEC_TAG_DENSITIES, SEC_TAG_VISCOSITIES, SEC_INTERFACIAL_TENSION, SEC_WHITEWATER
 };
 
 // Section 14 (version 2): the flow set as clamped integer cell corners [lo, hi), unused slots zero, and the cumulative counters.
@@ -96,6 +96,14 @@ struct InterfacialTensionSection {
     uint32_t tag[16];
 };
 static_assert(sizeof(InterfacialTensionSection) == 72 && INTERFACE_TAGS_MAX == 16, "interfacial tension section layout");
+// Section 22 (version 1024): this head, then `count` particles of 32 bytes each (the position float4, then the velocity float4)
+struct WhitewaterSectionHead {
+    BlubWhitewater setting;    // as set, capacity above 0
+    uint64_t counters[3];      // emitted, removed, refused for capacity
+    uint32_t count;            // live particles, at most the capacity
+};
+static_assert(sizeof(BlubWhitewater) == 64 && offsetof(WhitewaterSectionHead, count) == 88, "whitewater section layout");
+constexpr uint64_t kWhitewaterHeadBytes = 92; // the head without its tail padding
 
 struct StateHeader {
     char magic[8];
@@ -132,7 +140,7 @@ struct Section {
 // The optional sections in id order: the format version that introduced each one and its payload length.
 struct OptionalSection {
     uint32_t id, version;
-    uint64_t length; // section 14: in every version but 2 (fixed_length); section 16: 0, its length is what the file holds beyond the others
+    uint64_t length; // section 14: in every version but 2 (fixed_length); sections 16 and 22: 0, their length is stored
     const char *name;
 };
 constexpr OptionalSection kOptional[] = {
@@ -144,14 +152,15 @@ constexpr OptionalSection kOptional[] = {
     {SEC_TAG_DENSITIES, 128, sizeof(TagDensitySection), "the tag densities"},
     {SEC_TAG_VISCOSITIES, 256, sizeof(TagViscositySection), "the tag viscosities"},
     {SEC_INTERFACIAL_TENSION, 512, sizeof(InterfacialTensionSection), "the interfacial tension"},
+    {SEC_WHITEWATER, 1024, 0, "the whitewater"},
 };
-constexpr uint32_t kLastSection = SEC_INTERFACIAL_TENSION;
+constexpr uint32_t kLastSection = SEC_WHITEWATER;
 static_assert(sizeof(kOptional) / sizeof(kOptional[0]) == kLastSection - SEC_FLOW + 1, "one row per optional section");
 const OptionalSection &optional_section(uint32_t id) { return kOptional[id - SEC_FLOW]; }
 
 constexpr uint32_t bit(uint32_t id) { return 1u << id; }
 
-// The payload length of a section the rule fixes: sections 14, 15 and 17 to 21.
+// The payload length of a section the rule fixes: sections 14, 15 and 17 to 21.  Sections 16 and 22 are as long as they say.
 uint64_t fixed_length(uint32_t id, uint32_t version) {
     return id == SEC_FLOW && version == kFormatVersionFlow ? sizeof(FlowSection) : optional_section(id).length;
 }
@@ -286,7 +295,7 @@ std::vector<Section> layout_of(File &f, const StateHeader &h) {
         if (head.id <= last || head.id > kLastSection || optional_section(head.id).version > v) break;
         // 18 and 19 never go together: a version-128 file has no section 18, and in later versions the check of section 19 refuses the pair
         if (head.id == SEC_SURFACE_TENSION && v == optional_section(SEC_TAG_DENSITIES).version) break;
-        const uint64_t length = head.id == SEC_MESH_BODIES ? head.length : fixed_length(head.id, v);
+        const uint64_t length = head.id == SEC_MESH_BODIES || head.id == SEC_WHITEWATER ? head.length : fixed_length(head.id, v);
         if (length > size - at) break;
         if (head.id >= SEC_VISCOSITY) settings.push_back({head.id, length});
         last = head.id;
@@ -319,6 +328,27 @@ std::vector<Section> layout_of(File &f, const StateHeader &h) {
                          "), the file has none");
     }
     return sec;
+}
+
+// The whitewater of section 22, checked with the rules of set_whitewater: a capacity above 0, at most that many particles, and a length that
+// holds exactly them.  particles: count x 8 floats.
+WhitewaterSectionHead whitewater_of(const std::vector<char> &bytes, std::vector<float> &particles, const std::string &path) {
+    WhitewaterSectionHead w{};
+    if (bytes.size() < kWhitewaterHeadBytes) throw ParseError(path + ": section 22 is shorter than its head");
+    std::memcpy(&w, bytes.data(), kWhitewaterHeadBytes);
+    if (w.setting.max_num_particles == 0) throw ParseError(path + ": section 22: the capacity must be above 0");
+    try {
+        check_whitewater(w.setting, "section 22");
+    } catch (const std::invalid_argument &e) {
+        throw ParseError(path + ": " + e.what());
+    }
+    if (w.count > w.setting.max_num_particles) throw ParseError(path + ": section 22 holds more particles than its capacity");
+    if (bytes.size() != kWhitewaterHeadBytes + 32ull * w.count)
+        throw ParseError(path + ": section 22 has " + std::to_string(bytes.size()) + " bytes, " + std::to_string(w.count) + " particles take " +
+                         std::to_string(kWhitewaterHeadBytes + 32ull * w.count));
+    particles.resize(8ull * w.count);
+    if (w.count) std::memcpy(particles.data(), bytes.data() + kWhitewaterHeadBytes, 32ull * w.count);
+    return w;
 }
 
 // Reads one section whose id and length must be `s`, in chunks of at most one staging half; sink(slot, data, bytes, offset) receives
@@ -585,6 +615,8 @@ struct StateContents {
     TagDensitySection densities{};
     TagViscositySection viscosities{};
     InterfacialTensionSection interfacial{};
+    WhitewaterSectionHead whitewater{};
+    std::vector<float> whitewater_particles;
 };
 
 // Reads the sections of `layout` (layout_of) in their order, `f` at the first one.  The ten array sections go to
@@ -644,6 +676,12 @@ StateContents read_sections(File &f, const StateHeader &h, const std::vector<Sec
             to_host(s, &c.interfacial);
             interfacial_tension_of(c.interfacial, f.path);
             break;
+        case SEC_WHITEWATER: {
+            std::vector<char> bytes(s.length);
+            to_host(s, bytes.data());
+            c.whitewater = whitewater_of(bytes, c.whitewater_particles, f.path);
+            break;
+        }
         default: read_section(f, s, st, [&](int k, const char *data, size_t n, uint64_t off) { to_array(s.id, k, data, n, off); });
         }
     }
@@ -688,6 +726,7 @@ void HybridFluid::save_state(const std::string &path) {
     if (!tag_densities_.empty()) sections |= bit(SEC_TAG_DENSITIES);
     if (!tag_viscosities_.empty()) sections |= bit(SEC_TAG_VISCOSITIES);
     if (interfacial_tension_ > 0.0f) sections |= bit(SEC_INTERFACIAL_TENSION);
+    if (whitewater_on()) sections |= bit(SEC_WHITEWATER);
     h.format_version = format_version_of(sections, source_tags);
     std::strncpy(h.library_version, blub_version(), sizeof(h.library_version) - 1);
     h.grid_dimension[0] = (uint32_t)grid_.nx;
@@ -816,6 +855,23 @@ void HybridFluid::save_state(const std::string &path) {
             for (uint32_t k = 0; k < its.count; ++k) its.tag[k] = interface_tags_[k];
             write_host_section(f, SEC_INTERFACIAL_TENSION, &its, sizeof(its));
         }
+        if (sections & bit(SEC_WHITEWATER)) {
+            uint64_t counters[4];
+            whitewater_counters(counters);
+            WhitewaterSectionHead wh{};
+            wh.setting = whitewater_;
+            for (int k = 0; k < 3; ++k) wh.counters[k] = counters[1 + k];
+            wh.count = (uint32_t)counters[0];
+            std::vector<char> bytes(kWhitewaterHeadBytes + 32ull * wh.count);
+            std::memcpy(bytes.data(), &wh, kWhitewaterHeadBytes);
+            std::vector<float> pos(4ull * wh.count), vel(4ull * wh.count);
+            download_whitewater(pos.data(), vel.data(), wh.count);
+            for (uint32_t i = 0; i < wh.count; ++i) {
+                std::memcpy(bytes.data() + kWhitewaterHeadBytes + 32ull * i, &pos[4ull * i], 16);
+                std::memcpy(bytes.data() + kWhitewaterHeadBytes + 32ull * i + 16, &vel[4ull * i], 16);
+            }
+            write_host_section(f, SEC_WHITEWATER, bytes.data(), bytes.size());
+        }
         if (std::fflush(f.f) != 0 || fsync(fileno(f.f)) != 0) throw IoError("cannot flush " + tmp + ": " + errno_text());
         FILE *raw = f.f;
         f.f = nullptr;
@@ -872,6 +928,8 @@ std::unique_ptr<HybridFluid> HybridFluid::load_state(const std::string &path, in
     if (c.sections & bit(SEC_TAG_DENSITIES)) x.set_tag_densities(c.densities.entry, c.densities.count);
     if (c.sections & bit(SEC_TAG_VISCOSITIES)) x.set_tag_viscosities(c.viscosities.entry, c.viscosities.count);
     if (c.sections & bit(SEC_INTERFACIAL_TENSION)) x.set_interfacial_tension(c.interfacial.tag, c.interfacial.count, c.interfacial.tension);
+    if (c.sections & bit(SEC_WHITEWATER))
+        x.restore_whitewater(c.whitewater.setting, c.whitewater.counters, c.whitewater.count, c.whitewater_particles.data());
     BLUB_CUDA_CHECK(cudaStreamSynchronize(x.stream_));
     return fluid;
 }

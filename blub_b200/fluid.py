@@ -33,6 +33,8 @@ TAP_CELL_VISCOSITY = 15
 # blub_fluid.h)
 TAP_INTERFACE_CURVATURE, TAP_INTERFACE_FIELD = 16, 17
 INTERFACE_TAGS_MAX = 16
+WHITEWATER_SPRAY, WHITEWATER_FOAM, WHITEWATER_BUBBLE = 0, 1, 2  # BLUB_WHITEWATER_*: a whitewater particle's kind
+WHITEWATER_MAX_PARTICLES = 1 << 26                              # BLUB_WHITEWATER_MAX_PARTICLES
 
 BLUB_OK = 0
 BLUB_ERR_UNSTABLE = 6  # a CFL substep that cannot be planned: a non-finite particle velocity, or a step below min_dt_ns
@@ -140,6 +142,40 @@ class Viscosity(C.Structure):
     """BlubViscosity: kinematic viscosity in cells^2/s, the solve's absolute tolerance (cells/s) and iteration cap."""
 
     _fields_ = [("kinematic_viscosity", C.c_float), ("error_tolerance", C.c_float), ("max_num_iterations", C.c_int32), ("reserved", C.c_uint32)]
+
+
+class Whitewater(C.Structure):
+    """BlubWhitewater, grid units: capacity (0: off), emission rates (particles per cell and second), the potentials' [lo, hi] ramps (|curl u| in
+    1/s, AIR neighbours of a crest cell, 0.5 |u|^2 in cells^2/s^2), lifetimes (s), bubble buoyancy and drag, and the classification thresholds."""
+
+    _fields_ = [("max_num_particles", C.c_uint32), ("trapped_air_rate", C.c_float), ("wave_crest_rate", C.c_float),
+                ("trapped_air_range", C.c_float * 2), ("wave_crest_range", C.c_float * 2), ("energy_range", C.c_float * 2),
+                ("lifetime_lo", C.c_float), ("lifetime_hi", C.c_float), ("buoyancy", C.c_float), ("drag", C.c_float),
+                ("spray_below", C.c_uint32), ("bubble_from", C.c_uint32), ("max_per_cell", C.c_uint32)]
+
+    def to_dict(self):
+        d = {}
+        for name, _ in self._fields_:
+            v = getattr(self, name)
+            d[name] = tuple(float(x) for x in v) if name.endswith("_range") else (float(v) if isinstance(v, float) else int(v))
+        return d
+
+    @classmethod
+    def from_dict(cls, d):
+        w = cls()
+        for name, _ in cls._fields_:
+            v = d[name]
+            if name.endswith("_range"):
+                getattr(w, name)[:] = [float(x) for x in v]
+            else:
+                setattr(w, name, v)
+        return w
+
+
+# The defaults of HybridFluid.set_whitewater (grid units, tuned on the 128 x 64 x 64 dam break at 120 Hz)
+WHITEWATER_DEFAULTS = {"trapped_air_rate": 120.0, "wave_crest_rate": 120.0, "trapped_air_range": (5.0, 20.0), "wave_crest_range": (6.0, 18.0),
+                       "energy_range": (50.0, 5000.0), "lifetime_lo": 1.0, "lifetime_hi": 3.0, "buoyancy": 2.0, "drag": 0.5, "spray_below": 6,
+                       "bubble_from": 20, "max_per_cell": 4}
 
 
 class TagDensity(C.Structure):
@@ -448,6 +484,11 @@ def lib():
         "blub_fluid_set_interfacial_tension": (C.c_int, [vp, C.POINTER(C.c_uint32), C.c_uint32, C.c_float]),
         "blub_fluid_interfacial_tension": (C.c_int, [vp, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_float)]),
         "blub_scene_interfacial_tension": (C.c_int, [C.c_char_p, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_float)]),
+        "blub_fluid_set_whitewater": (C.c_int, [vp, C.POINTER(Whitewater)]),
+        "blub_fluid_whitewater": (C.c_int, [vp, C.POINTER(Whitewater)]),
+        "blub_fluid_whitewater_counters": (C.c_int, [vp, C.POINTER(C.c_uint64)]),
+        "blub_fluid_download_whitewater": (C.c_int, [vp, vp, vp, u32, C.POINTER(u32)]),
+        "blub_scene_whitewater": (C.c_int, [C.c_char_p, C.POINTER(Whitewater), C.POINTER(C.c_int32)]),
         "blub_fluid_set_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32]),
         "blub_fluid_tag_densities": (C.c_int, [vp, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
         "blub_scene_tag_densities": (C.c_int, [C.c_char_p, C.POINTER(TagDensity), u32, C.POINTER(u32)]),
@@ -638,6 +679,14 @@ def scene_interfacial_tension(path):
     arr = (C.c_uint32 * INTERFACE_TAGS_MAX)()
     _check(lib().blub_scene_interfacial_tension(os.fsencode(path), arr, INTERFACE_TAGS_MAX, C.byref(count), C.byref(out)))
     return float(out.value), [int(t) for t in arr[:count.value]]
+
+
+def scene_whitewater(path):
+    """The scene's fluid.whitewater as a dict of grid-unit settings (see Whitewater; the energy range / grid_to_world_scale^2), None without
+    the key (host only)."""
+    out, has = Whitewater(), C.c_int32(0)
+    _check(lib().blub_scene_whitewater(os.fsencode(path), C.byref(out), C.byref(has)))
+    return out.to_dict() if has.value else None
 
 
 def scene_tag_densities(path):
@@ -1188,6 +1237,46 @@ class HybridFluid:
         out = (C.c_uint64 * 3)()
         _check(self.L.blub_fluid_flow_counters(self.h, out))
         return {"emitted": int(out[0]), "drained": int(out[1]), "refused": int(out[2])}
+
+    # -- whitewater ----------------------------------------------------------------------------
+    def set_whitewater(self, max_num_particles, **params):
+        """Spray, foam and bubble particles, stepped at the end of stage 5 of every step; they never act on the liquid.  max_num_particles = 0
+        turns them off and frees their memory.  `params` override WHITEWATER_DEFAULTS (grid units; see Whitewater).  A new capacity starts
+        from no particles and zero counters.  Raises BlubError (changing nothing) on a setting the library refuses."""
+        unknown = set(params) - set(WHITEWATER_DEFAULTS)
+        if unknown:
+            raise TypeError(f"unknown whitewater parameters: {sorted(unknown)}")
+        d = dict(WHITEWATER_DEFAULTS, **params, max_num_particles=int(max_num_particles))
+        w = Whitewater.from_dict(d) if max_num_particles else None
+        _check(self.L.blub_fluid_set_whitewater(self.h, C.byref(w) if w is not None else None))
+
+    def whitewater(self):
+        """The current setting as a dict (max_num_particles 0: off)."""
+        out = Whitewater()
+        _check(self.L.blub_fluid_whitewater(self.h, C.byref(out)))
+        return out.to_dict()
+
+    @property
+    def whitewater_counters(self):
+        """{"live", "emitted", "removed", "refused"} whitewater particle counts (the last three cumulative; synchronises)."""
+        out = (C.c_uint64 * 4)()
+        _check(self.L.blub_fluid_whitewater_counters(self.h, out))
+        return {"live": int(out[0]), "emitted": int(out[1]), "removed": int(out[2]), "refused": int(out[3])}
+
+    def whitewater_raw(self):
+        """The live whitewater particles as two (n, 4) float32 arrays: positions (w = lifetime) and velocities (w = the kind's bits)."""
+        live = self.whitewater_counters["live"]  # buffers for the live particles only: nothing steps in between
+        pos, vel = np.empty((live, 4), dtype=np.float32), np.empty((live, 4), dtype=np.float32)
+        count = C.c_uint32(0)
+        _check(self.L.blub_fluid_download_whitewater(self.h, pos.ctypes.data_as(C.c_void_p), vel.ctypes.data_as(C.c_void_p), live, C.byref(count)))
+        n = min(count.value, live)
+        return pos[:n], vel[:n]
+
+    def whitewater_particles(self):
+        """The live whitewater particles: {"position": (n, 3) cells, "velocity": (n, 3) cells/s, "lifetime": (n,) s, "kind": (n,) uint32
+        WHITEWATER_SPRAY / FOAM / BUBBLE} (synchronises)."""
+        pos, vel = self.whitewater_raw()
+        return {"position": pos[:, :3].copy(), "velocity": vel[:, :3].copy(), "lifetime": pos[:, 3].copy(), "kind": vel[:, 3].view(np.uint32).copy()}
 
     def set_transfer_path(self, scatter):
         """True / "scatter" (default): warp-aggregated atomic scatter; False / "gather": deterministic gather P2G over per-step cell lists."""

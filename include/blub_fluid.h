@@ -434,6 +434,54 @@ int blub_fluid_interfacial_tension(const BlubFluid *fluid, uint32_t *tags, uint3
  * fail with BLUB_ERR_PARSE. */
 int blub_scene_interfacial_tension(const char *scene_json_path, uint32_t *tags, uint32_t capacity, uint32_t *count, float *cells3_per_s2);
 
+/* ---- whitewater (not part of the reference surface; rules: DESIGN.md section 8 "Whitewater") --------------------------------------
+ * Spray, foam and bubble particles (Ihmsen et al. 2012), stepped at the end of stage 5 of every step from the projected grid velocity and
+ * this step's marker.  They never act on the liquid: every liquid tap, dump and saved liquid section is what it is without them.  A live
+ * particle is classified by the FLUID cells among the 27 around its cell (fewer than spray_below: spray; its own cell FLUID and at least
+ * bubble_from: bubble; else foam), then spray falls ballistically, a bubble rises by buoyancy * -g and is pulled towards u by `drag` per
+ * step, foam moves with u and ages; particles leaving [1, dim - 1), entering a SOLID cell or the solid volume, or out of lifetime are removed.
+ * FLUID cells with an AIR neighbour emit dt (trapped_air_rate I_ta + wave_crest_rate I_wc) I_k particles, at most max_per_cell, with the
+ * potentials I ramps of the curl's magnitude (1/s), of the AIR neighbour count on a crest moving outwards and of 0.5 |u|^2 (cells^2/s^2).
+ * All in grid units.  Bit-reproducible.  Part of the saved state (format version 1024). */
+#define BLUB_WHITEWATER_MAX_PARTICLES (1u << 26)
+typedef struct BlubWhitewater {
+    uint32_t max_num_particles;   /* capacity, at most BLUB_WHITEWATER_MAX_PARTICLES; 0: off */
+    float trapped_air_rate;       /* particles per cell and second at full potential, >= 0 */
+    float wave_crest_rate;        /* >= 0 */
+    float trapped_air_range[2];   /* |curl u| in 1/s: the ramp's lo < hi */
+    float wave_crest_range[2];    /* AIR neighbours of a crest cell (0 to 26): lo < hi */
+    float energy_range[2];        /* 0.5 |u|^2 in cells^2/s^2: lo < hi */
+    float lifetime_lo, lifetime_hi; /* seconds, a new particle's lifetime is uniform in [lo, hi): 0 <= lo < hi */
+    float buoyancy;               /* a bubble accelerates by -buoyancy g */
+    float drag;                   /* in [0, 1]: the share of u - v a bubble takes on per step */
+    uint32_t spray_below;         /* spray_below <= bubble_from <= 27 */
+    uint32_t bubble_from;
+    uint32_t max_per_cell;        /* at most 16 particles a cell emits per step */
+} BlubWhitewater;
+/* NULL or max_num_particles 0 turns whitewater off, frees its memory and leaves an all-zero setting; a fluid that never turned it on
+ * allocates and launches nothing for it.  A new capacity starts from no particles and zero counters; another change keeps them.  The new
+ * storage is allocated before the old one is freed: a failed allocation returns its error and leaves the fluid as it was.  Every change drops the cached step graphs.
+ * BLUB_ERR_INVALID_ARGUMENT, changing nothing: a non-finite value, a range or lifetime with lo >= hi, a negative rate or lifetime, drag outside
+ * [0, 1], spray_below > bubble_from, bubble_from > 27, max_per_cell > 16, a capacity above BLUB_WHITEWATER_MAX_PARTICLES, a z-slab rank, or a
+ * fluid left inside a step by blub_fluid_step_stages. */
+int blub_fluid_set_whitewater(BlubFluid *fluid, const BlubWhitewater *settings);
+/* the current setting (all zero: off) */
+int blub_fluid_whitewater(const BlubFluid *fluid, BlubWhitewater *out);
+/* {live, emitted, removed, refused for capacity}; the last three are cumulative since the setting that allocated the capacity.  Zeros while
+ * off.  Synchronises. */
+int blub_fluid_whitewater_counters(BlubFluid *fluid, uint64_t out[4]);
+/* The live particles in their order: min(count, capacity) float4 positions (xyz in cells, w = remaining lifetime in s) into pos4 and
+ * velocities (xyz in cells/s, w = the raw bits of the kind: 0 spray, 1 foam, 2 bubble) into vel4; the live count into *count.  pos4 / vel4
+ * may be NULL with capacity 0.  Synchronises. */
+#define BLUB_WHITEWATER_SPRAY 0
+#define BLUB_WHITEWATER_FOAM 1
+#define BLUB_WHITEWATER_BUBBLE 2
+int blub_fluid_download_whitewater(BlubFluid *fluid, float *pos4, float *vel4, uint32_t capacity, uint32_t *count);
+/* The scene's optional fluid.whitewater in grid units (*has = 0 and a zeroed setting without the key): the same fields in world units, the
+ * energy range in m^2/s^2 divided by grid_to_world_scale^2, the curl's range in 1/s, rates in 1/s, lifetimes in s as they are.
+ * blub_scene_load sets it on the fluid it creates.  A value the setter would refuse makes every scene call fail with BLUB_ERR_PARSE. */
+int blub_scene_whitewater(const char *scene_json_path, BlubWhitewater *out, int32_t *has);
+
 /* ---- liquids of different densities (not part of the reference surface; rules: DESIGN.md section 8 "Liquids of different densities") ----
  * A table gives the particles of a tag a density relative to the reference density rho_ref that the velocity solve's pressure p dt / rho_ref,
  * the bodies' relative densities, the load probes' forces, the viscosity and the surface tension are all defined against.  Tags not in the
